@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the north-star hot path (per-layer Conv2D / depthwise / pool / FC inference) on B200.
+"""bench.py — frames/sec of the north-star hot path (per-layer Conv2D / depthwise / pool / FC inference) on H100.
 
-  python bench.py --gpus N --steps K --warmup W            our arm (libsnn_b200.so, hand-written sm_100a CUDA)
+  python bench.py --gpus N --steps K --warmup W            our arm (libsnn_b200.so, hand-written sm_90a CUDA)
   python bench.py --impl reference --gpus N ...            the reference's CPU operator path on the host cores
 
 A "step" is one forward pass over one batch of synthetic images. Workload at N=1 = BASELINE.json configs[1]: ResNet-18 (the
@@ -18,6 +18,9 @@ arena is broadcast once over NCCL at init. One JSON line on stdout (rank 0):
   cpu_baseline  the oracle (C++ restatement of the reference's operators, OpenMP, fixed thread team) on the same full batch,
              plus the parity of THIS run's output against it (max relative error, top-1 mismatches, distinct classes)
   workloads / precision_modes   the other BASELINE.json configurations and the opt-in fast modes, measured briefly
+With --dump-outputs DIR the arrays the timed path computed in its last step (the model's outputs; a detector's two head tensors)
+are written as DIR/<name>.npy in float32, a fixed seeded sample of at most 64 MB in all; the inputs depend only on the arguments,
+so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -51,7 +54,8 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA's H100 SXM data sheet (700 W): dense fp16/bf16 and HBM3 bandwidth; not reached figures, only the denominators
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet (not measured)"}
 
 
 def layer_work(layers, shapes, batch):
@@ -85,9 +89,9 @@ def layer_work(layers, shapes, batch):
     return work
 
 
-# HBM bandwidth by direction, measured on this pool's B200 with tools/hbm_rw_probe.py (profiles/r02_hbm_rw.txt): the copy figure is
-# the roofline denominator of MEASURED_PEAKS.json; a write-dominated layer cannot beat the fill figure
-HBM_WRITE_GBS, HBM_READ_GBS = 3930.0, 6126.0
+# HBM bandwidth by direction: not measured on the H100, so both directions take the data sheet's copy figure (a write-dominated
+# layer may in fact be bounded lower)
+HBM_WRITE_GBS, HBM_READ_GBS = 3350.0, 3350.0
 WRITE_BYTES = {}
 
 
@@ -98,7 +102,7 @@ def hbm_dir_floor(i, by, pk):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -366,7 +370,7 @@ def kernel_roofline(wl, work, pk, terms, step_ms, reps=5):
     roof["per_layer_roofline_frac"] = tmin / (dms * 1e-3)
     roof["per_layer_ceiling_frac"] = tceil / (dms * 1e-3)
     roof["per_layer_achievable_frac"] = tach / (dms * 1e-3)
-    roof["achievable_note"] = "ceiling + direction-aware HBM floor: this GPU writes at most %.0f GB/s and reads %.0f GB/s alone (tools/hbm_rw_probe.py), %.0f only as a copy" % (
+    roof["achievable_note"] = "ceiling + direction-aware HBM floor: writes at %.0f GB/s, reads at %.0f GB/s, %.0f as a copy (data-sheet figures, not measured)" % (
         HBM_WRITE_GBS, HBM_READ_GBS, pk["hbm_gbs"])
     roof["ceiling_note"] = ("a product costs %d fp16 MMAs (snnb.h SNNB_PRECISION_*): the tensor-bound layers' ceiling is peak / %d; per_layer_ceiling_frac measures against "
                             "that achievable bound, per_layer_roofline_frac / frac against SURVEY 8d's algorithmic roofline" % (terms, terms))
@@ -375,17 +379,6 @@ def kernel_roofline(wl, work, pk, terms, step_ms, reps=5):
     roof["timing"] = "CUDA-event pairs around every layer of an eager pass on the engine's stream, %d repetitions; the CUDA-graph step is %.3f ms against %.3f ms eager" % (
         reps, step_ms, float(lt.sum()))
     roof["traffic"] = None
-    prof = os.path.join(ROOT, "profiles", "r02_%s_kernels.csv" % wl.key)
-    if os.path.exists(prof):
-        import csv
-        rows = list(csv.reader(open(prof)))
-        col = {n.split("[")[0]: i for i, n in enumerate(rows[0])}
-        sel = [r for r in rows[1:] if dom in r[col["kernel"]]]
-        if sel and "dram_read_MB" in col:
-            mb = [float(r[col["dram_read_MB"]]) + float(r[col["dram_write_MB"]]) for r in sel]
-            roof["traffic"] = sum(mb) / len(mb) * 1e6
-            roof["traffic_note"] = "mean dram__bytes_read.sum + dram__bytes_write.sum per launch over %d profiled %s launches (%s); algorithmic bytes per launch %.1f MB" % (
-                len(sel), dom, os.path.basename(prof), dby / dn / 1e6)
     # whole-graph lower bounds: every reference layer's bytes (fused-away Add / Pad included) and the launched kernels' only
     t_unf = sum(max(by / (pk["hbm_gbs"] * 1e9), fl / (peak_t * 1e12)) for (_, fl, by) in work)
     t_fus = 0.0
@@ -405,7 +398,7 @@ def layer_table(desc, batch, work, lt, kernels, pk, terms, step_ms, out):
     out.write("# %s, batch %d per GPU; per-layer event pairs (eager pass). roofline%% = max(bytes/HBM, flops/peak) / t with the algorithmic work of SURVEY 8d (fp32\n"
               "# bytes, 2*MAC flops; peak = measured sustained dense fp16/bf16); ceiling%% = the same with flops x %d (a product is %d fp16 MMAs): the achievable bound\n"
               % (desc, batch, terms, terms))
-    out.write("# achievable%% = against max(ceiling, the direction-aware HBM floor: written bytes / %.0f GB/s write-only, read / %.0f read-only - tools/hbm_rw_probe.py)\n"
+    out.write("# achievable%% = against max(ceiling, the direction-aware HBM floor: written bytes / %.0f GB/s write-only, read / %.0f read-only)\n"
               % (HBM_WRITE_GBS, HBM_READ_GBS))
     out.write("# %-3s %-18s %-26s %8s %8s %8s %8s %8s %6s %9s %9s %11s\n" % ("id", "layer", "kernel", "ms", "GFLOP", "MB", "TF/s", "GB/s", "bound", "roofline%", "ceiling%",
                                                                                "achievable%"))
@@ -417,6 +410,31 @@ def layer_table(desc, batch, work, lt, kernels, pk, terms, step_ms, out):
                   (i, t, kn, ms_l, fl / 1e9, by / 1e6, fl / ms_l / 1e9, by / ms_l / 1e6, "tensor" if t_t > t_h else "hbm",
                    100 * max(t_h, t_t) / (ms_l * 1e-3), 100 * max(t_h, terms * t_t) / (ms_l * 1e-3), 100 * max(hbm_dir_floor(i, by, pk), terms * t_t) / (ms_l * 1e-3)))
     out.write("# total eager %.3f ms; CUDA-graph step %.3f ms\n" % (float(lt.sum()), step_ms))
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(wl, out_dir):
+    """What the timed path computed in its last step, as a caller of it receives it: the model's outputs (a detector's two YOLO head
+    tensors, whose boxes are decoded on the host). Arrays over their share of 64 MB are replaced by a fixed seeded sample of their
+    flattened elements, with the sampled indices beside them in <name>_index.npy (float64, exact)."""
+    os.makedirs(out_dir, exist_ok=True)
+    m = wl.model
+    if wl.detector:
+        yi = [i for i, l in enumerate(wl.layers) if l["type"] == "YOLO"][0]
+        arrays = [("head%d" % k, m.layer_output(j)) for k, j in enumerate(wl.layers[yi]["inputId"])]
+    else:
+        arrays = [("output%d" % i, m.get_output(i)) for i in range(m.num_outputs)]
+    share = DUMP_LIMIT_BYTES // len(arrays)
+    for name, a in arrays:
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        if a.nbytes > share:
+            keep = share // 12  # 4 bytes of value + 8 bytes of index per kept element
+            idx = np.sort(np.random.default_rng(20240917).choice(a.size, keep, replace=False))
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def main():
@@ -437,6 +455,7 @@ def main():
     ap.add_argument("--precision", default="fp32x3", choices=["fp32x3", "fp16w", "fp16"],
                     help="product form of the tensor-core path (snnb.h SNNB_PRECISION_*); the headline is fp32x3")
     ap.add_argument("--batch", type=int, default=0, help="override the workload's batch per GPU (the metric's config is the default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs to DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -479,6 +498,8 @@ def main():
         wl.ctx.sync()
     dev_ms, launches, region = wl.device_loop(args.steps, args.warmup, lib, check)
     clocks = sampler.stop(region)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(wl, args.dump_outputs)
 
     # ---- end to end through the C-ABI with host buffers ("e2e") ----
     u8_ms = wl.e2e_loop(args.steps, True)
@@ -552,7 +573,7 @@ def main():
         "data": "synthetic",
         "config": {"workload": desc, "model": key, "input_hw": list(hw), "batch_per_gpu": batch, "global_batch": batch * world, "parallelism": "dp%d" % world,
                    "precision": args.precision, "conv_algo": args.algo, "cuda_graph": not args.no_graph, "fused": not args.no_fuse, "weights_broadcast_bytes": arena_bytes,
-                   "l2": "per-step working set (~%.1f GB of activations) exceeds the 126 MB L2; no explicit flush" % (sum(b for _, _, b in work) / 1e9)},
+                   "l2": "per-step working set (~%.1f GB of activations) exceeds the 50 MB L2; no explicit flush" % (sum(b for _, _, b in work) / 1e9)},
         "clocks": clocks,
         "e2e": {"value": frames / (u8_ms * 1e-3), "unit": "frames/s", "ms_per_step": u8_ms / args.steps, "h2d_bytes_per_step": in_elems, "d2h_bytes_per_step": wl.d2h_bytes(),
                 "api": "snnb_model_submit_u8/snnb_model_wait (double-buffered; pinned host 8-bit NHWC images in, normalised on the device as the reference's ImageTexture "

@@ -1,5 +1,5 @@
 /*
- * snnb.h — C-ABI of libsnn_b200.so: the B200 (sm_100a) backend for ShaderNN's operator / graph API.
+ * snnb.h — C-ABI of libsnn_b200.so: the H100 (sm_90a) backend for ShaderNN's operator / graph API.
  *
  * This is the drop-in boundary (SURVEY.md §8b): plain C, opaque handles, plain pointers and sizes,
  * `int` status (0 = ok, non-zero = error, message via snnb_last_error()), never throws or aborts
@@ -14,7 +14,7 @@
  * reference's own texture layout "C4HW4" (core/inc/snn/imageTexture.h; element (x,y,c) at
  * (((c/4)*H + y)*W + x)*4 + c%4, demo/common/shaderUnitTest.cpp:87-131). Device storage is private:
  * two fp16 planes (hi, lo = value - hi) in NHWC with the channel pitch padded to 8 — an fp32-faithful
- * (22 significant bits, range +-65504) format that TMA can feed straight to tcgen05 tensor cores (see DESIGN.md).
+ * (22 significant bits, range +-65504) format that TMA can feed straight to the tensor cores (wgmma, see DESIGN.md).
  */
 #ifndef SNNB_H_
 #define SNNB_H_
@@ -38,7 +38,7 @@ typedef struct snnb_timer snnb_timer;     /* replaces snn::DeviceTimer (core/inc
 enum { SNNB_ACT_NONE = 0, SNNB_ACT_RELU = 1, SNNB_ACT_RELU6 = 2, SNNB_ACT_TANH = 3, SNNB_ACT_SIGMOID = 4, SNNB_ACT_LEAKY_RELU = 5, SNNB_ACT_SILU = 6, SNNB_ACT_SOFTMAX = 7 };
 /* Padding modes = conv2dVulkan.cpp:73-80 (0 = unset: out-of-range taps read 0, same as constant). */
 enum { SNNB_PAD_NONE = 0, SNNB_PAD_CONSTANT = 1, SNNB_PAD_REPLICATE = 2, SNNB_PAD_REFLECT = 3 };
-/* Kernel selection for convolutions. AUTO picks the tcgen05 implicit-GEMM path when the shape allows. TCGEN05_STREAMK also lets the
+/* Kernel selection for convolutions. AUTO picks the tensor-core (wgmma) implicit-GEMM path when the shape allows. TCGEN05_STREAMK also lets the
  * planner cut the K loops of the last partial wave of tiles across all SMs (stream-K; measured slower than whole tiles on ResNet-18's
  * shapes - DESIGN.md 3.4 - so it is not part of AUTO; environment SNNB_SK=1 enables it for every launch). */
 enum { SNNB_ALGO_AUTO = 0, SNNB_ALGO_SIMT = 1, SNNB_ALGO_TCGEN05 = 2, SNNB_ALGO_TCGEN05_STREAMK = 3 };

@@ -1,7 +1,7 @@
-"""Build libsnn_b200.so (hand-written sm_100a CUDA + C++ host engine) in-tree with nvcc.
+"""Build libsnn_b200.so (hand-written sm_90a CUDA + C++ host engine) in-tree with nvcc.
 
 Objects are cached under shadernn_b200/csrc/build/ keyed on source mtime; the shared library lands at
-shadernn_b200/libsnn_b200.so (git-ignored, travels to the GPU box with the gpurun snapshot).
+shadernn_b200/libsnn_b200.so (git-ignored build product).
 """
 import os
 import shutil
@@ -28,7 +28,7 @@ SOURCES = [
 ]
 HEADERS = ["snnb_internal.h", "engine/engine.h", "engine/json.h", "../../include/snnb.h"]
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-pthread", "-Xcompiler", "-Wall", "-I", os.path.join(ROOT, "include"), "-I", CSRC]
 
 
@@ -70,7 +70,7 @@ def _compile_one(nvcc, src, hdr_mtime, verbose):
 
 
 def build(verbose=False, force=False):
-    """Compile every source for sm_100a and link libsnn_b200.so. Returns the library path."""
+    """Compile every source for sm_90a and link libsnn_b200.so. Returns the library path."""
     os.makedirs(BUILD, exist_ok=True)
     nvcc = _nvcc()
     hdr = _newest_header_mtime()

@@ -102,7 +102,8 @@ int snnb_context_create(int device, snnb_context** out) {
     SNNB_CUDA_OK(cudaSetDevice(device));
     cudaDeviceProp prop;
     SNNB_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-    SNNB_REQUIRE(prop.major == 10, "snnb_context_create: device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major, prop.minor);
+    SNNB_REQUIRE(prop.major == 9 && prop.minor == 0, "snnb_context_create: device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major,
+                 prop.minor);
     auto ctx      = std::make_unique<snnb_context>();
     ctx->device   = device;
     ctx->sm_count = prop.multiProcessorCount;
@@ -295,7 +296,7 @@ int snnb_conv2d_launch(snnb_context* ctx, const snnb_conv_desc* d, const snnb_we
     ConvArgs a {in, residual, out, w, d->kernel, d->stride, d->pad_x, d->pad_y, d->pad_mode, d->activation, d->leaky_alpha};
     a.stream_k = d->algo == SNNB_ALGO_TCGEN05_STREAMK;
     if (d->algo == SNNB_ALGO_TCGEN05 || d->algo == SNNB_ALGO_TCGEN05_STREAMK) {
-        SNNB_REQUIRE(conv2d_umma_supported(a), "snnb_conv2d_launch: the tcgen05 path does not support this shape (IC=%d OC=%d k=%d s=%d pad_mode=%d)", in->c, out->c,
+        SNNB_REQUIRE(conv2d_umma_supported(a), "snnb_conv2d_launch: the tensor-core path does not support this shape (IC=%d OC=%d k=%d s=%d pad_mode=%d)", in->c, out->c,
                      d->kernel, d->stride, d->pad_mode);
         return launch_conv2d_umma(ctx, a);
     }

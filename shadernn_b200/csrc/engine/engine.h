@@ -170,7 +170,7 @@ public:
     Conv2DDesc _desc;
     int algo = SNNB_ALGO_AUTO;
     // Replicate / reflect padding on the tensor path: the TMA unit can only zero-fill, so the engine materialises the
-    // padded input once (pad kernel, vk_pad.comp semantics) and runs the tcgen05 kernel over it with zero padding.
+    // padded input once (pad kernel, vk_pad.comp semantics) and runs the tensor-core kernel over it with zero padding.
     snnb_tensor* prepadded = nullptr;
     // Stride-2 stem with <= 4 input channels reading a model input: the input tensor carries a compact 4-channel copy
     // (snnb_tensor::feed_hi) and the weights get the matching K order (FeedPlan, kernels_umma.cu conv_rowwin_kernel feed mode).

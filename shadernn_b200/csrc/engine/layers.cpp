@@ -121,7 +121,7 @@ int Conv2DLayer::run(snnb_context* ctx, const ExecOptions& opt) {
     const int want = algo != SNNB_ALGO_AUTO ? algo : opt.convAlgo;
     if (want != SNNB_ALGO_SIMT && conv2d_umma_supported(a)) return launch_conv2d_umma(ctx, a);
     if (want == SNNB_ALGO_TCGEN05) {
-        set_error("%s: tcgen05 path requested but unsupported for this shape", name.c_str());
+        set_error("%s: tensor-core path requested but unsupported for this shape", name.c_str());
         return 2;
     }
     return launch_conv2d_simt(ctx, a);

@@ -1,4 +1,4 @@
-// CUDA-core (SIMT) kernels for sm_100a: the HBM-bound operators (depthwise, pooling, add, norms, layout ops)
+// CUDA-core (SIMT) kernels for sm_90a: the HBM-bound operators (depthwise, pooling, add, norms, layout ops)
 // and the generic direct/implicit-GEMM fp32 convolution used where the tcgen05 path does not apply
 // (IC = 3 stems, 1-channel ESPCN layers, reflect/replicate padding).
 //

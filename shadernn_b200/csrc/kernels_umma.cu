@@ -1,17 +1,15 @@
-// Conv2D (1x1 and k x k, stride 1 and 2) as an implicit GEMM on Blackwell's 5th-generation tensor
-// cores, hand-written for sm_100a: TMA (cp.async.bulk.tensor) stages NHWC activation tiles and packed weights from HBM
-// into 128B-swizzled shared memory, one elected thread issues tcgen05.mma, accumulators live in TMEM and are read back
-// with tcgen05.ld by the epilogue warps (bias + residual + activation + split-fp16 store).
+// Conv2D (1x1 and k x k, stride 1 and 2) as an implicit GEMM on Hopper's tensor cores, hand-written for sm_90a: TMA
+// (cp.async.bulk.tensor) stages NHWC activation tiles and packed weights from HBM into 128B-swizzled shared memory, two
+// consumer warpgroups run wgmma.mma_async on them with fp32 accumulators in registers and then the epilogue of their rows
+// (bias + residual + activation + split-fp16, staged in swizzled shared memory and written with one TMA store per slab).
 //
 //   D[M = 128 output pixels, N = n_blk <= 128 output channels] += A[M, K] * B[N, K]^T,   K = (tap, 64-channel block)
 //
 // fp32-faithful arithmetic out of fp16 tensor cores: activations and weights are stored as hi + lo fp16 pairs
-// (snnb_internal.h); every K block accumulates into fp32 TMEM, template parameter TERMS:
-//   3:  A_hi*B_hi + A_lo*B_hi + A_hi*B_lo   (the dropped A_lo*B_lo term is ~2^-24 relative): ~22 mantissa bits per operand. Issued
-//       as TWO instructions per K=16 step: A_hi x [B_hi ; B_lo] (N = 2 n_blk, two accumulator column blocks) and A_lo x B_hi
-//       (onto the first block); the epilogue adds the blocks. n_blk <= 128.
-//   2:  (A_hi + A_lo) * B_hi: the weights rounded ONCE to fp16 (<= 2^-12 relative per weight, measured per-layer error vs the
-//       oracle ~1e-4 of the tensor's range - inside the 1e-3 budget), two instructions, ONE accumulator block, n_blk <= 256.
+// (snnb_internal.h); every K step accumulates into the same fp32 accumulator, template parameter TERMS:
+//   3:  A_hi*B_hi + A_hi*B_lo + A_lo*B_hi  (the dropped A_lo*B_lo term is ~2^-24 relative): ~22 mantissa bits per operand.
+//   2:  (A_hi + A_lo) * B_hi: the weights rounded ONCE to fp16 (<= 2^-12 relative per weight, per-layer error vs the oracle
+//       ~1e-4 of the tensor's range - inside the 1e-3 budget).
 //   1:  A_hi * B_hi: the half-precision storage mode (the reference's RGBA16F), no lo planes anywhere.
 //
 // A tile = a (tw x th x tn)-pixel box of the OUTPUT grid (tw*th*tn <= 128): for filter tap (ky,kx) the producer issues
@@ -19,12 +17,12 @@
 // zero-filled by the TMA unit, which is exactly the reference's constant padding (vk_conv2d.comp:168-172), and the
 // channel tail (c >= IC) is zero-filled too, so no im2col buffer and no boundary code exist anywhere.
 //
-// Roles (320 threads, persistent CTAs, one per SM): warp 0 = TMA producer (also draws work items from a global counter),
-// warp 1 = TMEM allocator + one thread that owns the MMA issue loop, warps 2-9 = epilogue (TMEM -> registers -> swizzled smem
-// -> TMA bulk store). Pipelines: smem full/empty ring and a double-buffered TMEM accumulator (tmem_full/tmem_empty), so the
-// epilogue of tile i overlaps the mainloop of tile i+1. Layers with few tiles split K over several CTAs (fp32 partials, last
-// arriver reduces); layers with a short K loop use two independent epilogue groups. Also in this file: the row-window kernel
-// for small-channel stems and the TMA-staged depthwise kernel. DESIGN.md section 3 has the measurements behind each choice.
+// Roles (384 threads, persistent CTAs, one per SM): warpgroup 0 = TMA producer (one thread issues), warpgroups 1 and 2 =
+// consumers, each owning 64 of the tile's 128 rows: one m64 wgmma per K step and product term, then the epilogue of those
+// rows. The operand ring (full/empty mbarriers) is as deep as shared memory allows for the launch's n_blk, so the producer
+// runs several K blocks ahead. Layers with few tiles split K over several CTAs (fp32 partials, last arriver reduces), or,
+// on request, use a stream-K decomposition. Also in this file: the row-window kernel for small-channel stems and the
+// TMA-staged depthwise kernel.
 //
 // Reference semantics: shadertemplate_vk_conv2d.comp:148-347, vk_conv2d_1x1.comp:68-211 (+ fused vk_add.comp:41-90).
 #include <cuda.h>
@@ -38,42 +36,30 @@
 namespace snnb {
 
 constexpr int UM_BLOCK_M     = 128;
-constexpr int UM_BLOCK_K     = 64; // fp16 elements: 128 bytes = one SWIZZLE_128B row
-constexpr int UM_MAX_N       = 128; // 3-term product: the accumulator holds two column blocks of n_blk
-constexpr int UM_MAX_N2      = 256; // 2-term (fp16 weights) and 1-term (fp16 storage) products: one column block
-constexpr int UM_STAGES      = 3;
+constexpr int UM_BLOCK_K     = 64;  // fp16 elements: 128 bytes = one SWIZZLE_128B row
+constexpr int UM_MAX_N       = 128; // widest output-channel tile: 64 fp32 accumulator registers per consumer thread
 constexpr int UM_A_BYTES     = UM_BLOCK_M * 128;
-constexpr int UM_B_BYTES     = UM_MAX_N * 128;
-constexpr int UM_STAGE_BYTES = 2 * UM_A_BYTES + 2 * UM_B_BYTES; // A_hi, A_lo, then [B_hi ; B_lo] (3-term) or one B plane of up to 256 rows = 64 KB
-constexpr int UM_EPI_WARPS   = 8;                       // two warps per TMEM lane quarter, interleaved over 16-column chunks
-constexpr int UM_THREADS     = 64 + 32 * UM_EPI_WARPS; // warp 0 TMA, warp 1 MMA, warps 2.. epilogue
-constexpr int UM_ACC_COLS    = 2 * UM_MAX_N; // one accumulator buffer: [A_hi.B_hi + A_lo.B_hi | A_hi.B_lo], up to 2 x 128 fp32 columns
-constexpr int UM_TMEM_COLS   = 2 * UM_ACC_COLS; // double-buffered: all 512 columns
-constexpr int UM_STG_BYTES   = 2 * UM_BLOCK_M * 128; // epilogue staging: one 64-channel slab, hi + lo planes (32 KB)
-constexpr int UM_SCHED_SLOTS = 8;                        // ring of work-item ids handed from the producer warp to the MMA / epilogue warps
-constexpr int UM_SMEM_BYTES  = UM_STAGES * UM_STAGE_BYTES + UM_STG_BYTES + 1024 /*alignment slack*/ + 320 /*barriers + scheduler ring*/;
-constexpr int UM_SMEM_BYTES_SPLIT = (UM_STAGES - 1) * UM_STAGE_BYTES + 2 * UM_STG_BYTES + 1024 + 320; // two epilogue groups, one ring stage less
+constexpr int UM_CONSUMERS   = 2;                          // consumer warpgroups, 64 tile rows each
+constexpr int UM_THREADS     = 128 * (1 + UM_CONSUMERS);   // warpgroup 0 = producer
+constexpr int UM_EPI_THREADS = 128 * UM_CONSUMERS;
+constexpr int UM_STG_BYTES   = 2 * UM_BLOCK_M * 128;       // epilogue staging: one 64-channel slab, hi + lo planes (32 KB)
+constexpr int UM_SMEM_LIMIT  = 227 * 1024;                 // opt-in shared memory per block on sm_90
+constexpr int UM_BAR_BYTES   = 256;
 
-// ---- halo mode (3x3, stride 1): the A operand of all nine taps comes from ONE (8+2) x (16+2)-pixel halo tile per 64-channel
-// block, loaded once by TMA; tap (ky,kx) is the same shared memory read through a descriptor whose start address is shifted
-// by (ky * 10 + kx) pixels and whose 8-row group stride (SBO) is the halo's row pitch, 10 pixels = 1280 B. Legal because both
-// the TMA unit and the tensor core apply SWIZZLE_128B to absolute shared-memory address bits (tools/umma_desc_probe.cu), so a
-// pixel row is found where TMA put it whatever the descriptor's phase. L2 -> SM traffic of A drops from 9 x 32 KB to 46 KB per
-// tile and channel block (the r01 kernel moved 363-389 MB per 56x56x64 launch against 51.5 MB algorithmic: it was bound by
-// the ~72 B/clk/SM the SM can ingest, not by the tensor pipe). The weights (one K block per tap) keep their own ring.
-constexpr int HL_TW = 8, HL_TH = 16, HL_W = HL_TW + 2, HL_H = HL_TH + 2;
-constexpr int HL_PLANE         = (HL_W * HL_H * 128 + 1023) / 1024 * 1024; // 23 552 B: one plane of the halo tile, 1024-aligned
-constexpr int HL_A_STAGES      = 2;
-constexpr int HL_A_STAGE_BYTES = 2 * HL_PLANE;
-constexpr int HL_B_STAGES      = 6;              // == the STAGES template argument of the halo instantiations (barrier slots)
-constexpr int HL_B_RING_BYTES  = 6 * UM_B_BYTES; // 96 KB of weight stages: 3 x 32 KB ([B_hi ; B_lo] of 128 rows / one plane of 256 rows) or 6 x 16 KB
-constexpr int HL_SMEM_BYTES    = HL_A_STAGES * HL_A_STAGE_BYTES + HL_B_RING_BYTES + UM_STG_BYTES + 1024 + 384;
+// Shared-memory carve-up of conv_umma_kernel<TERMS, NB>: [ring: STAGES x (A_hi, A_lo, B_hi, B_lo)] [staging] [barriers]. A stage
+// holds only the planes the product reads, and the ring takes whatever shared memory the staging buffer leaves (at most 8 stages).
+template <int TERMS, int NB> struct UmGeom {
+    static constexpr int A_PLANES    = TERMS == 1 ? 1 : 2;
+    static constexpr int B_PLANES    = TERMS == 3 ? 2 : 1;
+    static constexpr int B_BYTES     = NB * 128; // one plane: NB rows of 64 K columns (a multiple of 1024 B: SWIZZLE_128B alignment)
+    static constexpr int STAGE_BYTES = A_PLANES * UM_A_BYTES + B_PLANES * B_BYTES;
+    static constexpr int FIT         = (UM_SMEM_LIMIT - 1024 - UM_BAR_BYTES - UM_STG_BYTES) / STAGE_BYTES;
+    static constexpr int STAGES      = FIT > 8 ? 8 : FIT;
+    static constexpr int SMEM_BYTES  = STAGES * STAGE_BYTES + UM_STG_BYTES + 1024 /*alignment slack*/ + UM_BAR_BYTES;
+    static_assert(STAGES >= 2, "operand ring needs two stages");
+};
 
 struct UmmaParams {
-    __half* out_hi;
-    __half* out_lo;
-    const __half* res_hi;
-    const __half* res_lo;
     const float* bias;
     int N, OH, OW, OC, OCp;
     int tw, th, tn, rows_used;
@@ -87,20 +73,16 @@ struct UmmaParams {
     // dumps its fp32 partial tile to `partials`, bumps the tile's arrival counter, and the LAST arriver sums all partials
     // in split order (deterministic) and runs the normal epilogue.
     int ksplit, kb_per_split;
-    int* sched_counter; // dynamic work distribution: next work item = gridDim.x + atomicAdd(counter, 1); zero between launches
     float* partials; // [tile][split][128 rows][n_blk]
     int* counters;   // [tile], zero between launches (the last arriver resets it)
-    long long* trace; // profiling aid (env SNNB_UMMA_TRACE): CTA 0 writes clock64 stamps per role, [6][256]
-    int ablate; // profiling aid (env SNNB_UMMA_ABLATE, results are WRONG when set): 1 skip epilogue work, 2 skip TMA loads, 4 skip MMAs
-    int has_lo; // the output tensor has a lo plane (0 in the fp16 storage mode)
-    // Stream-K (sk != 0, plain mode): the first sk_dp tiles (a multiple of the grid) are whole-tile work items, CTA b taking tiles
+    int has_lo;      // the output tensor has a lo plane (0 in the fp16 storage mode)
+    // Stream-K (sk != 0): the first sk_dp tiles (a multiple of the grid) are whole-tile work items, CTA b taking tiles
     // b, b + grid, ...; the K-block units of the remaining tiles (sk_units = tiles x K blocks, laid end to end) are cut into sk_ctas
     // equal ranges, CTA b < sk_ctas taking range b - which covers the tail of one tile and the head of the next. A tile cut into
     // pieces is finished like a split-K tile (fp32 partials, last arriver sums them in piece order). Work ids: [0, sk_dp) tiles,
-    // sk_dp + 4 c + j = the j-th piece of CTA c's range; the schedule is static (no draw from sched_counter): pieces first, then tiles.
+    // sk_dp + 4 c + j = the j-th piece of CTA c's range; the schedule is static: pieces first, then tiles.
     int sk, sk_dp, sk_ctas;
     long long sk_units;
-    int b_stages, b_stage_bytes; // halo mode: depth and stage size of the weight ring (3 x 32 KB, or 6 x 16 KB when a stage fits)
 };
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -124,22 +106,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) { // never suspends
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-// Progress word of every CTA's producer warp (debugging aid: printed when a wait times out)
-__device__ unsigned int g_producer_progress[1024];
-__device__ __forceinline__ void producer_progress(int lane, unsigned int code) {
-    if (lane == 0) *reinterpret_cast<volatile unsigned int*>(&g_producer_progress[blockIdx.x & 1023]) = code;
-}
 // Bounded wait: a broken descriptor or protocol bug must surface as a trapped kernel, never as a hung GPU.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
@@ -150,24 +116,20 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         if (dt > 4000000000LL && !reported) {
             uint32_t dyn;
             asm volatile("mov.u32 %0, %%dynamic_smem_size;" : "=r"(dyn));
-            printf("tcgen05 kernel (dynamic smem %u B): mbarrier wait timed out (block %d thread %d bar 0x%x parity %u, producer progress 0x%x)\n", dyn, blockIdx.x,
-                   threadIdx.x, bar, parity, *reinterpret_cast<volatile unsigned int*>(&g_producer_progress[blockIdx.x & 1023]));
+            printf("tensor-core kernel (dynamic smem %u B): mbarrier wait timed out (block %d thread %d bar 0x%x parity %u)\n", dyn, blockIdx.x, threadIdx.x, bar, parity);
             reported = true;
         }
         if (dt > 4040000000LL) __trap(); // ~20 ms after the first report: every stuck thread gets to print
     }
 }
-// One lane of a CONVERGED warp. Unlike `lane == 0` the compiler knows a single thread is active in the guarded region, so
-// descriptors stay in uniform registers and each tcgen05.mma / TMA issue is one predicated instruction rather than an
-// ELECT + BRA.U.ANY waterfall loop (ncu r01: the issuing warp spent 77% of its time in that scalar code, not waiting).
+// One lane of a CONVERGED warp: the compiler knows a single thread is active in the guarded region, so the TMA issue is
+// one predicated instruction rather than a loop over the active lanes.
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) { asm volatile("prefetch.tensormap [%0];" ::"l"(m) : "memory"); }
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3) {
@@ -175,41 +137,16 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* m, 
                  "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                  : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst), "l"(m), "r"(bar),
+                 "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst), "l"(m), "r"(bar),
                  "r"(c0), "r"(c1)
                  : "memory");
 }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16 inputs, fp32 accumulate; issued by ONE thread for the whole CTA.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed (implicitly fences).
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-                   "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3) {
     asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(m), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                  : "memory");
@@ -220,27 +157,66 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); } // all but the newest group
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
-// Shared-memory matrix descriptor, K-major operand, SWIZZLE_128B (cute::UMMA::SmemDescriptor layout):
+// wgmma shared-memory matrix descriptor (sm_90), K-major operand, SWIZZLE_128B:
 //   [0,14) start address >> 4 | [16,30) LBO >> 4 (= 1, unused for swizzled K-major) | [32,46) SBO >> 4 (= 1024 B: 8 rows x 128 B)
-//   [46,48) version = 1 (Blackwell) | [61,64) layout type = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-    return (uint64_t) ((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+//   [62,64) layout type = 1 (SWIZZLE_128B). A K step of 16 fp16 (32 B) inside the 128-byte row adds 2 to the address field.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
+    return (uint64_t) ((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// Same with an arbitrary stride between 8-row groups (halo mode: the halo tile's row pitch, not a multiple of 1024 B)
-__device__ __forceinline__ uint64_t make_smem_desc_sbo(uint32_t saddr, uint32_t sbo_bytes) {
-    return (uint64_t) ((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t) (sbo_bytes >> 4) << 32) | (1ull << 46) | (2ull << 61);
+// Un-swizzled K-major descriptor with an overlapping K stride (row-window kernel): LBO = 16 B (next 16-byte K chunk = next
+// pixel), SBO = 128 B (8 rows x 16 B), layout type 0.
+__device__ __forceinline__ uint64_t gmma_desc_window(uint32_t saddr) { return (uint64_t) ((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (8ull << 32); }
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x N] (fp32 registers) (+)= A[64 x 16] * B[N x 16]^T, both fp16 K-major operands in shared memory, issued by a whole
+// warpgroup; accumulate = 0 overwrites D. Fragment of thread t (warp w = t / 32 of the warpgroup, lane l): d[4 j + 2 r + b] = D[16 w + l / 4 + 8 r][8 j + 2 (l % 4) + b].
+template <int N> struct Wgmma;
+template <> struct Wgmma<32> {
+    static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                     : "l"(a), "l"(b), "r"(accumulate));
+    }
+};
+template <> struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                     : "l"(a), "l"(b), "r"(accumulate));
+    }
+};
+template <> struct Wgmma<128> {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t accumulate) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                     : "l"(a), "l"(b), "r"(accumulate));
+    }
+};
+
+template <int NACC> __device__ __forceinline__ void acc_fence(float (&d)[NACC]) {
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// Instruction descriptor for kind::f16 (cute::UMMA::InstrDescriptor): c_format F32 (bit 4), a/b format at bits 7 / 10,
-// both operands K-major, N >> 3 at bit 17, M >> 4 at bit 24.
-// a_format / b_format (bits [7,10) / [10,13)): 0 = F16 for both operands. (kind::f16 refuses a BF16 A with an F16 B operand:
-// "illegal instruction", tools/umma_desc_probe.cu - which is why the storage format is an fp16 pair, not round 1's bf16 pair.)
-__device__ __forceinline__ uint32_t make_idesc(int M, int N) {
-    return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t) (N >> 3) << 17) | ((uint32_t) (M >> 4) << 24);
+// Two-level accumulation: every K block (every ring stage) is summed by the tensor core into a FRESH accumulator, which is then
+// added to the tile's fp32 sum with round-to-nearest FADDs. The tensor core's own accumulation chain is thus one K block long
+// whatever the layer's K, and a tile's result does not depend on how its K range was split over CTAs beyond the order in which
+// whole-block sums are added.
+template <int NACC> __device__ __forceinline__ void acc_promote(float (&sum)[NACC], float (&d)[NACC]) {
+    acc_fence(d);
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) sum[i] += d[i];
 }
+__device__ __forceinline__ void regs_dealloc_40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void regs_alloc_232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
 // transcendental activations only (tanh / sigmoid / SiLU): rare, kept out of line so the hot epilogue stays small
 __device__ __noinline__ float umma_act(float v, int act, float alpha) {
@@ -268,270 +244,96 @@ __device__ __forceinline__ void um_split2(float a, float b, uint32_t& h, uint32_
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Epilogue of one output tile, shared by both tensor-core kernels: TMEM -> registers -> +bias (+residual) -> activation
-// -> split-fp16 -> SHARED MEMORY (128B-swizzled, bank-conflict-free) -> ONE TMA bulk store per plane and 64-channel slab.
-//
-// Why through smem + TMA: each thread owns one output pixel (TMEM lane), so direct global stores are 32 scattered
-// 16-byte pieces per warp instruction = 32 L1 wavefronts each; at 128 rows x n_blk channels that is 8-16 k wavefronts
-// per tile, MORE than the tile's MMA time - the first version of both kernels was bound by exactly that (their run time
-// did not move across five different producer designs). The TMA store writes full 128-byte lines, clips rows/channels
-// that fall outside the tensor by itself, and costs one instruction. The fused residual (Conv2D -> Add) comes in the same
-// way: a TMA box load of the residual tile into the staging buffer, read back with swizzled LDS.
+// Epilogue of one output tile, shared by both tensor-core kernels and run by the 256 consumer threads: accumulator registers
+// -> +bias (+residual) -> activation -> split-fp16 -> SHARED MEMORY (128B-swizzled for full 64-channel slabs) -> ONE TMA bulk
+// store per plane and slab. The TMA store writes full 128-byte lines and clips rows / channels that fall outside the tensor
+// by itself. The fused residual (Conv2D -> Add) comes in the same way: a TMA box load of the residual slab into the staging
+// buffer, read back by each thread at exactly the place it then overwrites.
 // ---------------------------------------------------------------------------------------------------------------
 struct EpiArgs {
-    const CUtensorMap *o_hi64, *o_lo64, *o_hiT, *o_loT; // output maps: 64-channel slab (SWIZZLE_128B) and tail slab (dense)
+    const CUtensorMap *o_hi64, *o_lo64, *o_hiT, *o_loT; // output maps: 64-channel slab (SWIZZLE_128B) and narrow slab (dense)
     const CUtensorMap *r_hi64, *r_lo64, *r_hiT, *r_loT; // residual maps, same geometry
     const float* bias;
-    int n_blk, OC, act, has_res, rows_box; // 3-term: the A_hi.B_lo partial sums sit n_blk columns after the main block
-    int has_lo;                            // write (and read, for the residual) the lo plane; 0 in the fp16 storage mode
+    int OC, act, has_res, rows_box;
+    int has_lo;     // write (and read, for the residual) the lo plane; 0 in the fp16 storage mode
     float alpha;
-    uint32_t stg;       // staging smem (hi plane; lo plane at + UM_BLOCK_M * 128)
-    uint32_t res_bar;   // mbarrier for the residual TMA load
-    uint32_t tmem_empty;
-    int bar_id;         // named barrier of this epilogue group (1, or 1 + group when two groups work on alternate tiles)
-    // split-K finalisation: accumulator values come from `part_splits` fp32 partial tiles [128][n_blk] in global memory
-    // (summed in split order) instead of TMEM
-    const float* part_src;
-    int part_splits;
-    long long* trace; // profiling aid: leader warp stamps the phases of its first slabs into [4][64 + 8 * slab_seq ...]
-    int trace_seq;
-    bool no_store = false; // profiling aid (SNNB_UMMA_ABLATE & 8, row-window kernel): everything but the TMA store of the tile
-    // Two staging buffers used on alternate tiles (row-window kernel, one slab per tile): only the store of the tile BEFORE the previous
-    // one must have finished reading. The TMA store drains shared memory at ~20 B/clk per SM (1.6 k clk for a 32 KB tile,
-    // profiles/r02_trace_mobilenetv2_1x1.txt); with one buffer that sat in series with the tile's arithmetic.
-    bool two_stagings = false;
+    uint32_t stg;     // staging smem (hi plane; lo plane at + UM_BLOCK_M * 128)
+    uint32_t res_bar; // mbarrier of the residual TMA load
+    bool issuer;      // the one consumer thread that issues (and later waits for) the bulk stores and residual loads
 };
 
-// Fused residual (Conv2D -> Add): TMA box load of the residual tile's slab into the staging buffer. The previous bulk store
-// must have finished READING the buffer. Called for slab 0 BEFORE the wait for the accumulator, so the load's latency
-// hides behind the tile's MMAs. `leader` is warp-uniform: the whole leader warp calls, one lane issues.
-__device__ __forceinline__ void epilogue_residual_load(const EpiArgs& e, int sl, int oc0, int c1, int c2, int c3, bool leader) {
-    if (!leader) return;
-    const int w          = min(64, e.n_blk - sl * 64);
-    const bool sw        = w == 64;
-    const uint32_t pitch = sw ? 128u : (uint32_t) w * 2u;
-    if (elect_one()) {
-        bulk_wait_read0();
-        mbar_expect_tx(e.res_bar, (e.has_lo ? 2u : 1u) * (uint32_t) e.rows_box * pitch); // the box has rows_box rows (<= 128)
-        tma_load_4d(e.stg, sw ? e.r_hi64 : e.r_hiT, e.res_bar, oc0 + sl * 64, c1, c2, c3);
-        if (e.has_lo) tma_load_4d(e.stg + UM_BLOCK_M * 128, sw ? e.r_lo64 : e.r_loT, e.res_bar, oc0 + sl * 64, c1, c2, c3);
+// acc: this thread's fragment of its warpgroup's 64 x NB accumulator; row0 = the tile row of its d[0] (16 w + l / 4 within the
+// warpgroup's rows), q = l % 4.
+template <int NB>
+__device__ __forceinline__ void epilogue_tile(const EpiArgs& e, const float (&acc)[NB / 2], int oc0, int c1, int c2, int c3, int row0, int q, uint32_t& res_phase) {
+    constexpr int W      = NB < 64 ? NB : 64; // slab width in channels
+    constexpr bool SW    = W == 64;            // full slab: 128-byte rows, SWIZZLE_128B
+    constexpr uint32_t PITCH = SW ? 128u : (uint32_t) W * 2u;
+    const bool fast_act  = e.act == SNNB_ACT_NONE || e.act == SNNB_ACT_RELU || e.act == SNNB_ACT_RELU6 || e.act == SNNB_ACT_LEAKY_RELU;
+    const float slope    = (e.act == SNNB_ACT_RELU || e.act == SNNB_ACT_RELU6) ? 0.0f : (e.act == SNNB_ACT_LEAKY_RELU ? e.alpha : 1.0f);
+    const float hi_clip  = e.act == SNNB_ACT_RELU6 ? 6.0f : __int_as_float(0x7f800000);
+    const uint32_t lo_off = UM_BLOCK_M * 128;
+#pragma unroll
+    for (int sl = 0; sl < NB / W; ++sl) {
+        // the staging buffer is free once the previous slab's (or tile's) bulk store has finished reading it
+        if (e.issuer) bulk_wait_read0();
+        named_bar_sync(1, UM_EPI_THREADS);
+        if (e.has_res) {
+            if (e.issuer) {
+                mbar_expect_tx(e.res_bar, (e.has_lo ? 2u : 1u) * (uint32_t) e.rows_box * PITCH);
+                tma_load_4d(e.stg, SW ? e.r_hi64 : e.r_hiT, e.res_bar, oc0 + sl * 64, c1, c2, c3);
+                if (e.has_lo) tma_load_4d(e.stg + lo_off, SW ? e.r_lo64 : e.r_loT, e.res_bar, oc0 + sl * 64, c1, c2, c3);
+            }
+            mbar_wait(e.res_bar, res_phase);
+            res_phase ^= 1u;
+        }
+#pragma unroll
+        for (int j = 0; j < W / 8; ++j) {
+            const int c = sl * 64 + 8 * j + 2 * q; // channel of the pair within the tile
+            const int oc = oc0 + c;
+            const float b0 = oc < e.OC ? __ldg(e.bias + oc) : 0.0f, b1 = oc + 1 < e.OC ? __ldg(e.bias + oc + 1) : 0.0f;
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int row = row0 + 8 * r;
+                const uint32_t a = e.stg + (uint32_t) row * PITCH + (SW ? ((((uint32_t) j) ^ (uint32_t) (row & 7)) << 4) : (uint32_t) j * 16u) + (uint32_t) q * 4u;
+                float v0 = acc[(sl * 8 + j) * 4 + 2 * r] + b0, v1 = acc[(sl * 8 + j) * 4 + 2 * r + 1] + b1;
+                if (e.has_res) {
+                    uint32_t hh, ll = 0u;
+                    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(hh) : "r"(a));
+                    if (e.has_lo) asm volatile("ld.shared.b32 %0, [%1];" : "=r"(ll) : "r"(a + lo_off));
+                    const float2 rh = um_h2f(hh), rl = um_h2f(ll);
+                    v0 += rh.x + rl.x;
+                    v1 += rh.y + rl.y;
+                }
+                if (e.act == SNNB_ACT_RELU) {
+                    v0 = fmaxf(v0, 0.0f), v1 = fmaxf(v1, 0.0f);
+                } else if (e.act == SNNB_ACT_NONE) {
+                } else if (fast_act) {
+                    v0 = fminf(fmaxf(v0, v0 * slope), hi_clip), v1 = fminf(fmaxf(v1, v1 * slope), hi_clip);
+                } else {
+                    v0 = umma_act(v0, e.act, e.alpha), v1 = umma_act(v1, e.act, e.alpha); // out-of-line call
+                }
+                if (oc >= e.OC) v0 = 0.0f; // channels [OC, Cp) stay zero
+                if (oc + 1 >= e.OC) v1 = 0.0f;
+                uint32_t h, l;
+                um_split2(v0, v1, h, l);
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(h) : "memory");
+                if (e.has_lo) asm volatile("st.shared.b32 [%0], %1;" ::"r"(a + lo_off), "r"(l) : "memory");
+            }
+        }
+        fence_async_smem(); // generic-proxy smem writes -> visible to the TMA (async proxy)
+        named_bar_sync(1, UM_EPI_THREADS);
+        if (e.issuer) {
+            tma_store_4d(SW ? e.o_hi64 : e.o_hiT, e.stg, oc0 + sl * 64, c1, c2, c3);
+            if (e.has_lo) tma_store_4d(SW ? e.o_lo64 : e.o_loT, e.stg + lo_off, oc0 + sl * 64, c1, c2, c3);
+            bulk_commit();
+        }
     }
-    __syncwarp();
 }
 
-template <int NWARPS, int TERMS>
-__device__ __forceinline__ void epilogue_tile(const EpiArgs& e, uint32_t taddr, int oc0, int c1, int c2, int c3, int row, int half, bool leader, int lane,
-                                              uint32_t& res_phase) {
-    constexpr int MAXC  = NWARPS == 8 ? 2 : 4; // 16-column chunks of one 64-column slab owned by this warp
-    const bool fast_act = e.act == SNNB_ACT_NONE || e.act == SNNB_ACT_RELU || e.act == SNNB_ACT_RELU6 || e.act == SNNB_ACT_LEAKY_RELU;
-    const float slope   = (e.act == SNNB_ACT_RELU || e.act == SNNB_ACT_RELU6) ? 0.0f : (e.act == SNNB_ACT_LEAKY_RELU ? e.alpha : 1.0f);
-    const float hi_clip = e.act == SNNB_ACT_RELU6 ? 6.0f : __int_as_float(0x7f800000);
-    const int nslabs    = (e.n_blk + 63) >> 6;
-#define EPI_STAMP(k)                                                                                      \
-    do {                                                                                                  \
-        if (e.trace && leader && lane == 0 && blockIdx.x == 0 && tseq < 16) e.trace[4 * 256 + 64 + 8 * tseq + (k)] = clock64(); \
-    } while (0)
-    for (int sl = 0; sl < nslabs; ++sl) {
-        const int tseq     = e.trace_seq * nslabs + sl;
-        EPI_STAMP(0);
-        const int w        = min(64, e.n_blk - sl * 64); // slab width in channels (multiple of 16)
-        const bool sw      = w == 64;                    // full slab: 128-byte rows, SWIZZLE_128B
-        const uint32_t pitch = sw ? 128u : (uint32_t) w * 2u;
-        const uint32_t srow  = e.stg + (uint32_t) row * pitch;
-        const uint32_t xr    = sw ? (uint32_t) (row & 7) : 0u;
-        const int slab_oc    = oc0 + sl * 64;
-        if (e.has_res && sl > 0) epilogue_residual_load(e, sl, oc0, c1, c2, c3, leader); // slab 0's was issued before the accumulator wait
-        // ---- phase 1: TMEM -> registers -> bias (+ residual) -> activation -> packed split-fp16, nothing written yet ----
-        bool res_ready = false;
-#pragma unroll
-        for (int k0 = 0; k0 < MAXC; k0 += 2) { // two chunks at a time: their four TMEM loads are in flight together
-            uint32_t oh[2][8], ol[2][8];
-            uint32_t r[2][16], r2[2][16];
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {
-                const int ci = NWARPS == 8 ? half + 2 * (k0 + kk) : k0 + kk;
-                if (ci < (w >> 4)) {
-                    const int c = sl * 64 + ci * 16;
-                    if (e.part_src) {
-                        // all loads of the chunk are issued before the first add (L2 latency once, not once per split);
-                        // summed in split order: the result does not depend on which CTA arrived last
-                        float4 t[4][4];
-#pragma unroll
-                        for (int sp = 0; sp < 4; ++sp) {
-                            // partial tile layout [chunk][j4][row][4 floats]: a warp's 32 rows are 512 contiguous bytes per access
-                            const float4* src = reinterpret_cast<const float4*>(e.part_src + (size_t) sp * UM_BLOCK_M * e.n_blk) + (size_t) (c >> 4) * 4 * UM_BLOCK_M + row;
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4)
-                                t[sp][j4] = sp < e.part_splits ? __ldcg(src + j4 * UM_BLOCK_M) : make_float4(0.f, 0.f, 0.f, 0.f); // L2: written by other SMs
-                        }
-                        float a16[16];
-#pragma unroll
-                        for (int j4 = 0; j4 < 4; ++j4) {
-                            a16[4 * j4] = t[0][j4].x, a16[4 * j4 + 1] = t[0][j4].y, a16[4 * j4 + 2] = t[0][j4].z, a16[4 * j4 + 3] = t[0][j4].w;
-#pragma unroll
-                            for (int sp = 1; sp < 4; ++sp)
-                                if (sp < e.part_splits) a16[4 * j4] += t[sp][j4].x, a16[4 * j4 + 1] += t[sp][j4].y, a16[4 * j4 + 2] += t[sp][j4].z, a16[4 * j4 + 3] += t[sp][j4].w;
-                        }
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) r[kk][j] = __float_as_uint(a16[j]), r2[kk][j] = 0u;
-                    } else {
-                        tmem_ld16(taddr + (uint32_t) c, r[kk]);
-                        if (TERMS == 3) {
-                            tmem_ld16(taddr + (uint32_t) (e.n_blk + c), r2[kk]);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 16; ++j) r2[kk][j] = 0u; // one column block: folded away by the compiler
-                        }
-                    }
-                }
-            }
-            if (!e.part_src) tmem_ld_wait();
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {
-                const int k = k0 + kk, ci = NWARPS == 8 ? half + 2 * k : k;
-                if (ci < (w >> 4)) {
-                    const int c = sl * 64 + ci * 16;
-                    float v[16];
-#pragma unroll
-                    for (int j4 = 0; j4 < 4; ++j4) { // the bias slice of a tile stays L1-resident across the CTA's tiles
-                        const float4 b = __ldg(reinterpret_cast<const float4*>(e.bias + oc0 + c) + j4);
-                        v[4 * j4 + 0] = (__uint_as_float(r[kk][4 * j4 + 0]) + __uint_as_float(r2[kk][4 * j4 + 0])) + b.x;
-                        v[4 * j4 + 1] = (__uint_as_float(r[kk][4 * j4 + 1]) + __uint_as_float(r2[kk][4 * j4 + 1])) + b.y;
-                        v[4 * j4 + 2] = (__uint_as_float(r[kk][4 * j4 + 2]) + __uint_as_float(r2[kk][4 * j4 + 2])) + b.z;
-                        v[4 * j4 + 3] = (__uint_as_float(r[kk][4 * j4 + 3]) + __uint_as_float(r2[kk][4 * j4 + 3])) + b.w;
-                    }
-                    if (e.has_res) {
-                        if (!res_ready) {
-                            mbar_wait(e.res_bar, res_phase);
-                            res_ready = true;
-                        }
-#pragma unroll
-                        for (int g = 0; g < 2; ++g) { // this thread later overwrites exactly the 16-byte pieces it reads here
-                            const uint32_t a = srow + ((((uint32_t) (ci * 2 + g)) ^ xr) << 4);
-                            uint32_t hh[4], ll[4];
-                            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(hh[0]), "=r"(hh[1]), "=r"(hh[2]), "=r"(hh[3]) : "r"(a));
-                            if (e.has_lo) {
-                                asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(ll[0]), "=r"(ll[1]), "=r"(ll[2]), "=r"(ll[3]) : "r"(a + UM_BLOCK_M * 128));
-                            } else {
-                                ll[0] = ll[1] = ll[2] = ll[3] = 0u;
-                            }
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const float2 rh = um_h2f(hh[j]), rl = um_h2f(ll[j]);
-                                v[g * 8 + 2 * j] += rh.x + rl.x;
-                                v[g * 8 + 2 * j + 1] += rh.y + rl.y;
-                            }
-                        }
-                    }
-                    if (e.act == SNNB_ACT_RELU) { // the common cases one instruction per element (the epilogue is issue-bound on short-K layers)
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.0f);
-                    } else if (e.act == SNNB_ACT_NONE) {
-                    } else if (e.act == SNNB_ACT_RELU6) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] = fminf(fmaxf(v[j], 0.0f), 6.0f);
-                    } else if (fast_act) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] = fminf(fmaxf(v[j], v[j] * slope), hi_clip);
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] = (oc0 + c + j < e.OC) ? umma_act(v[j], e.act, e.alpha) : 0.0f; // out-of-line call
-                    }
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) um_split2(v[2 * j], v[2 * j + 1], oh[kk][j], ol[kk][j]);
-                }
-            }
-            if (k0 + 2 >= MAXC) { // the slab's last chunk pair is in registers
-                EPI_STAMP(1);     // phase 1 done
-                if (e.has_res && !res_ready) mbar_wait(e.res_bar, res_phase); // warps without a chunk in this slab still consume the phase
-                if (e.has_res) res_phase ^= 1u;
-                if (sl == nslabs - 1 && !e.part_src) { // last tcgen05.ld of the tile issued: the accumulator buffer may be reused
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(e.tmem_empty);
-                }
-            }
-            // ---- staging buffer. The previous slab's / tile's bulk store has had the whole first chunk pair (and usually the
-            // wait for the next accumulator) to finish READING the buffer; only now does anyone wait for it. ----
-            if (k0 == 0) {
-                if (!e.has_res) {
-                    if (leader) {
-                        if (elect_one()) {
-                            if (e.two_stagings) bulk_wait_read1();
-                            else bulk_wait_read0();
-                        }
-                        __syncwarp();
-                    }
-                    EPI_STAMP(2); // leader's wait for the previous store's reads
-                    named_bar_sync(e.bar_id, NWARPS * 32);
-                }
-                EPI_STAMP(3); // bar A
-            }
-#pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {
-                const int k = k0 + kk, ci = NWARPS == 8 ? half + 2 * k : k;
-                if (ci < (w >> 4)) {
-#pragma unroll
-                    for (int g = 0; g < 2; ++g) {
-                        const uint32_t a = srow + ((((uint32_t) (ci * 2 + g)) ^ xr) << 4);
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(oh[kk][4 * g]), "r"(oh[kk][4 * g + 1]), "r"(oh[kk][4 * g + 2]), "r"(oh[kk][4 * g + 3])
-                                     : "memory");
-                        if (e.has_lo)
-                            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a + UM_BLOCK_M * 128), "r"(ol[kk][4 * g]), "r"(ol[kk][4 * g + 1]), "r"(ol[kk][4 * g + 2]),
-                                         "r"(ol[kk][4 * g + 3])
-                                         : "memory");
-                    }
-                }
-            }
-        }
-        EPI_STAMP(4); // STS issued
-        fence_async_smem();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
-        EPI_STAMP(5); // fence
-        named_bar_sync(e.bar_id, NWARPS * 32);
-        EPI_STAMP(6); // bar B
-        if (leader) {
-            if (!e.no_store && elect_one()) {
-                tma_store_4d(sw ? e.o_hi64 : e.o_hiT, e.stg, slab_oc, c1, c2, c3);
-                if (e.has_lo) tma_store_4d(sw ? e.o_lo64 : e.o_loT, e.stg + UM_BLOCK_M * 128, slab_oc, c1, c2, c3);
-                bulk_commit();
-            }
-            __syncwarp();
-        }
-        EPI_STAMP(7); // store issued
-    }
-#undef EPI_STAMP
-}
-// Split-K: write this work item's raw fp32 accumulator tile (both column blocks added) to global memory, laid out
-// [16-column chunk][float4 index][row][4 floats] so that every warp access is 512 contiguous bytes.
-template <int NWARPS, int TERMS>
-__device__ __forceinline__ void epilogue_dump_partial(const EpiArgs& e, uint32_t taddr, float* dst, int row, int half, int lane) {
-    for (int c = (NWARPS == 8 ? half : 0) * 16; c < e.n_blk; c += (NWARPS == 8 ? 32 : 16)) {
-        uint32_t r[16], r2[16];
-        tmem_ld16(taddr + (uint32_t) c, r);
-        if (TERMS == 3) {
-            tmem_ld16(taddr + (uint32_t) (e.n_blk + c), r2);
-        } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) r2[j] = 0u;
-        }
-        tmem_ld_wait();
-        float4* d = reinterpret_cast<float4*>(dst) + (size_t) (c >> 4) * 4 * UM_BLOCK_M + row; // [chunk][j4][row][4 floats]
-#pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4)
-            d[j4 * UM_BLOCK_M] = make_float4(__uint_as_float(r[4 * j4]) + __uint_as_float(r2[4 * j4]), __uint_as_float(r[4 * j4 + 1]) + __uint_as_float(r2[4 * j4 + 1]),
-                                __uint_as_float(r[4 * j4 + 2]) + __uint_as_float(r2[4 * j4 + 2]), __uint_as_float(r[4 * j4 + 3]) + __uint_as_float(r2[4 * j4 + 3]));
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(e.tmem_empty);
-}
-
-// After the last tile: the leader's bulk stores must have completed before the CTA (and its shared memory) goes away.
-__device__ __forceinline__ void epilogue_drain(bool leader) {
-    if (leader) {
-        if (elect_one()) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-        __syncwarp();
-    }
+// After the last tile: the issuer's bulk stores must have completed before the CTA (and its shared memory) goes away.
+__device__ __forceinline__ void epilogue_drain(bool issuer) {
+    if (issuer) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -542,7 +344,7 @@ __device__ __forceinline__ void epilogue_drain(bool leader) {
 struct WorkItem {
     int tile, kb0, kb1, piece, pieces, slot;
 };
-template <bool SK> // compile-time: the stream-K arithmetic (64-bit divisions) stays out of every other instantiation's issue loops
+template <bool SK> // compile-time: the stream-K arithmetic (64-bit divisions) stays out of every other instantiation
 __host__ __device__ __forceinline__ WorkItem decode_work(const UmmaParams& p, int work, int total_tiles, int num_kb) {
     WorkItem w;
     if constexpr (!SK) {
@@ -578,549 +380,212 @@ __host__ __device__ __forceinline__ int sk_first_work(const UmmaParams& p, int c
     return cta < p.sk_ctas ? p.sk_dp + 4 * cta : (cta < p.sk_dp ? cta : end);
 }
 
-#define UM_TRACE(role, idx)                                                                          \
-    do {                                                                                             \
-        if (p.trace && blockIdx.x == 0 && lane == 0 && (idx) < 256) p.trace[(role) * 256 + (idx)] = clock64(); \
-    } while (0)
-
-// STAGES: depth of the operand ring. SPLIT_EPI: the eight epilogue warps work as TWO independent groups of four, group g
-// owning accumulator buffer g (tiles alternate between the buffers) with its own staging buffer, named barrier, residual
-// barrier and bulk-store queue, so one group's barrier / TMA-store latencies overlap the other group's arithmetic. Used for
-// layers with a short K loop (1x1 convolutions), which run at the speed of the epilogue; pays for the second staging buffer
-// with one ring stage (2 instead of 3).
-// TERMS: how the fp32-faithful product is formed. 3 = A_hi x [B_hi ; B_lo] + A_lo x B_hi (fp16 weight pair, accumulator of two
-// column blocks, n_blk <= 128); 2 = (A_hi + A_lo) x B16 with ONE fp16 weight plane (one column block, n_blk <= 256);
-// 1 = A_hi x B_hi only (fp16 storage mode: no lo planes anywhere).
-template <int STAGES, bool SPLIT_EPI, int TERMS, bool HALO, bool SK = false> // SK: stream-K work decomposition (UmmaParams::sk)
+// TERMS: how the fp32-faithful product is formed (see the top of the file). NB: output channels per tile (= UmmaParams::n_blk).
+// SK: stream-K work decomposition (UmmaParams::sk); otherwise CTA b takes work items b, b + grid, ...
+template <int TERMS, int NB, bool SK>
 __global__ void __launch_bounds__(UM_THREADS, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo, const __grid_constant__ CUtensorMap tmB_hi,
                  const __grid_constant__ CUtensorMap tmB_lo, const __grid_constant__ CUtensorMap tmO_hi64, const __grid_constant__ CUtensorMap tmO_lo64,
                  const __grid_constant__ CUtensorMap tmO_hiT, const __grid_constant__ CUtensorMap tmO_loT, const __grid_constant__ CUtensorMap tmR_hi64,
                  const __grid_constant__ CUtensorMap tmR_lo64, const __grid_constant__ CUtensorMap tmR_hiT, const __grid_constant__ CUtensorMap tmR_loT,
                  const UmmaParams p) {
+    using G = UmGeom<TERMS, NB>;
+    constexpr int STAGES = G::STAGES;
     extern __shared__ uint8_t smem_raw[];
-    constexpr bool ONE_BLOCK = TERMS != 3 || SPLIT_EPI; // the accumulator is one column block of n_blk (else [hi.hi + lo.hi | hi.lo])
-    constexpr int EPI_TERMS  = ONE_BLOCK ? 2 : 3;       // what the epilogue templates need to know: one block or two
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u; // SWIZZLE_128B tiles need 1024-byte alignment
-    // HALO: [A ring: HL_A_STAGES x (hi plane, lo plane)] [B ring: STAGES x 32 KB] [staging]; else [ring: STAGES x 64 KB] [staging]
-    const uint32_t b_ring    = smem_base + (HALO ? HL_A_STAGES * HL_A_STAGE_BYTES : 0);
-    const uint32_t stg       = HALO ? b_ring + HL_B_RING_BYTES : smem_base + STAGES * UM_STAGE_BYTES; // epilogue staging (1024-aligned), one buffer per epilogue group
-    const uint32_t bar_base  = stg + (SPLIT_EPI ? 2 : 1) * UM_STG_BYTES;
-    // barrier slots (8 bytes each): full[0..S), empty[S..2S), tmem_full[2S..2S+2), tmem_empty[2S+2..2S+4), TMEM base slot, residual barrier
-    auto full_bar       = [&](int s) { return bar_base + 8u * s; };
-    auto empty_bar      = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    auto tmem_full_bar  = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-    auto tmem_empty_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-    const uint32_t res_bar   = bar_base + 8u * (2 * STAGES + 5); // SPLIT_EPI: group 1 uses the slot after the split-K flag (+16)
-    // Dynamic work distribution. CTA b starts with work item b; every further item is drawn from a global counter by the
-    // producer warp (persistent CTAs on a statically striped grid finished up to 17 % apart on store-heavy layers) and handed
-    // to the MMA thread and the epilogue warps through this ring: id in sched_id[slot], full/empty mbarriers per slot.
-    const uint32_t sched_base = bar_base + 8u * (2 * STAGES + 8); // behind the slots above (2 * STAGES + 8 of them)
-    auto sched_full  = [&](int s) { return sched_base + 8u * s; };
-    auto sched_empty = [&](int s) { return sched_base + 64u + 8u * s; };
-    auto sched_id    = [&](int s) { return sched_base + 128u + 4u * s; };
-    auto a_full_bar  = [&](int s) { return sched_base + 160u + 8u * s; }; // HALO: the halo-tile ring
-    auto a_empty_bar = [&](int s) { return sched_base + 176u + 8u * s; };
-    // consumer side: wait for sequence number `seq`, read its work id, release the slot (one arrive per consuming warp)
-    auto sched_take = [&](int seq, bool arrive) {
-        const int slot = seq & (UM_SCHED_SLOTS - 1);
-        mbar_wait(sched_full(slot), (uint32_t) (seq / UM_SCHED_SLOTS) & 1u);
-        int w;
-        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(sched_id(slot)) : "memory");
-        if (arrive) mbar_arrive(sched_empty(slot));
-        return w;
-    };
+    const uint32_t stg       = smem_base + STAGES * G::STAGE_BYTES;
+    const uint32_t bar_base  = stg + UM_STG_BYTES;
+    // barrier slots (8 bytes each): full[0..S), empty[S..2S), residual barrier, split-K "arrived last" flag
+    auto full_bar  = [&](int s) { return bar_base + 8u * s; };
+    auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+    const uint32_t res_bar   = bar_base + 8u * (2 * STAGES);
+    const uint32_t last_flag = bar_base + 8u * (2 * STAGES + 1);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     pdl_trigger(); // the next kernel may start launching; it waits for this grid's completion before touching memory
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         mbar_init(res_bar, 1);
-        mbar_init(res_bar + 16u, 1);
-        tma_prefetch_desc(&tmO_hi64);
-        tma_prefetch_desc(&tmO_lo64);
         tma_prefetch_desc(&tmA_hi);
         tma_prefetch_desc(&tmA_lo);
         tma_prefetch_desc(&tmB_hi);
         tma_prefetch_desc(&tmB_lo);
+        tma_prefetch_desc(&tmO_hi64);
+        tma_prefetch_desc(&tmO_lo64);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        if (HALO)
-            for (int s = 0; s < HL_A_STAGES; ++s) {
-                mbar_init(a_full_bar(s), 1);
-                mbar_init(a_empty_bar(s), 1);
-            }
-        for (int s = 0; s < UM_SCHED_SLOTS; ++s) {
-            mbar_init(sched_full(s), 1);
-            mbar_init(sched_empty(s), 1 + UM_EPI_WARPS); // the MMA thread + one lane of every epilogue warp
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tmem_full_bar(a), 1);
-            mbar_init(tmem_empty_bar(a), SPLIT_EPI ? UM_EPI_WARPS / 2 : UM_EPI_WARPS); // one arrive per epilogue warp that drains the buffer
+            mbar_init(empty_bar(s), UM_EPI_THREADS / 32); // one arrive per consumer warp
         }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, UM_TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-    // The WEIGHTS of this CTA's first work item do not depend on the previous kernel: their loads go out before the dependency wait
-    // (plain mode: the first K block's; halo mode: the first three taps'), so only the activations' latency is left after it.
-    const int pre_total_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_oc;
-    const int pre_num_kb      = p.ksize * p.ksize * p.cblocks;
-    const int pre_end         = SK ? p.sk_dp + 4 * p.sk_ctas : pre_total_tiles * p.ksplit; // one past the last work id
-    const int first_work      = SK ? sk_first_work(p, (int) blockIdx.x, pre_end) : (int) blockIdx.x;
-    const bool pre_b          = (p.ablate & (2 | 16)) == 0 && first_work < pre_end; // ablate 16: no early weight loads (results stay correct)
-    if (warp == 0 && pre_b && elect_one()) {
-        const WorkItem w0 = decode_work<SK>(p, first_work, pre_total_tiles, pre_num_kb);
-        const int tile    = w0.tile;
-        const int oc0  = (tile / (p.tiles_x * p.tiles_y * p.tiles_n)) * p.n_blk;
-        const uint32_t b_lo_off = (uint32_t) p.n_blk * 128u;
-        if (HALO) {
-            for (int tap = 0; tap < 3; ++tap) {
-                const uint32_t sB = b_ring + tap * p.b_stage_bytes, fb = full_bar(tap);
-                mbar_expect_tx(fb, (TERMS == 3 ? 2u : 1u) * (uint32_t) p.n_blk * 128u);
-                tma_load_2d(sB, &tmB_hi, fb, tap * p.ICp, oc0);
-                if (TERMS == 3) tma_load_2d(sB + b_lo_off, &tmB_lo, fb, tap * p.ICp, oc0);
-            }
-        } else {
-            const int kb0 = w0.kb0, cb = kb0 % p.cblocks, tap0 = kb0 / p.cblocks;
-            const uint32_t fb = full_bar(0);
-            mbar_expect_tx(fb, (TERMS == 1 ? 1u : 2u) * (uint32_t) p.rows_used * 128u + (TERMS == 3 ? 2u : 1u) * (uint32_t) p.n_blk * 128u);
-            tma_load_2d(smem_base + 2 * UM_A_BYTES, &tmB_hi, fb, tap0 * p.ICp + cb * UM_BLOCK_K, oc0);
-            if (TERMS == 3) tma_load_2d(smem_base + 2 * UM_A_BYTES + b_lo_off, &tmB_lo, fb, tap0 * p.ICp + cb * UM_BLOCK_K, oc0);
-        }
-    }
-    pdl_wait(); // everything above (barriers, TMEM, tensor-map prefetch, first weights) overlapped with the previous kernel's tail
-    if (warp == 0) UM_TRACE(5, 0); // kernel entry (after the dependency wait)
-    if (p.trace && threadIdx.x == 0) { // wall-clock (ns) envelope over ALL CTAs: [5][8] = earliest entry, [5][9] = latest exit, [5][10..11] CTA 0's own
-        unsigned long long g;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
-        atomicMin(reinterpret_cast<unsigned long long*>(p.trace) + 5 * 256 + 8, g);
-        if (blockIdx.x == 0) p.trace[5 * 256 + 10] = (long long) g;
-    }
-
-    if (warp == 0) UM_TRACE(5, 1); // setup done
+    pdl_wait(); // barrier set-up and tensor-map prefetch overlapped with the previous kernel's tail
 
     const int m_tiles     = p.tiles_x * p.tiles_y * p.tiles_n;
     const int total_tiles = m_tiles * p.tiles_oc;
     const int num_kb      = p.ksize * p.ksize * p.cblocks;
-    const int total_work  = SK ? p.sk_dp + 4 * p.sk_ctas : total_tiles * p.ksplit; // work item = (tile, K range); one past the last work id
+    const int total_work  = SK ? p.sk_dp + 4 * p.sk_ctas : total_tiles * p.ksplit; // one past the last work id
+    auto next_work = [&](int work) { return SK ? sk_next_work(p, work, (int) blockIdx.x, (int) gridDim.x, num_kb, total_work) : work + (int) gridDim.x; };
+    const int first_work = SK ? sk_first_work(p, (int) blockIdx.x, total_work) : (int) blockIdx.x;
 
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        {
-            int stage = 0, hstage = 0;
-            uint32_t phase = 0, hphase = 0;
-            (void) hstage, (void) hphase;
-            const uint32_t tx_bytes = (TERMS == 1 ? 1u : 2u) * (uint32_t) p.rows_used * 128u + (TERMS == 3 ? 2u : 1u) * (uint32_t) p.n_blk * 128u;
-            const int ks = p.ksize, cbs = p.cblocks, icp = p.ICp;
-            const bool skip_tma = (p.ablate & 2) != 0;
-            const uint32_t b_lo_off = (uint32_t) p.n_blk * 128u; // B_lo rows follow B_hi's: one [2 n_blk x 64] operand
-            int tr = 0;
-            const int draws_total = max(0, total_work - (int) gridDim.x) + (int) gridDim.x; // every CTA's last draw is past the end
-            int work = first_work;
-            for (int seq = 0;; ++seq) {
-                if (p.ablate & 32) producer_progress(lane, ((unsigned) seq << 16) | 0x01u); // SNNB_UMMA_ABLATE=32: leave a trail for the time-out report
-                {   // publish this sequence number's work id
-                    const int slot = seq & (UM_SCHED_SLOTS - 1);
-                    mbar_wait(sched_empty(slot), ((uint32_t) (seq / UM_SCHED_SLOTS) & 1u) ^ 1u);
-                    if (elect_one()) {
-                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sched_id(slot)), "r"(work) : "memory");
-                        mbar_arrive(sched_full(slot));
-                    }
-                }
-                if (p.ablate & 32) producer_progress(lane, ((unsigned) seq << 16) | 0x02u);
-                if (work >= total_work) break;
-                // The next work item is drawn NOW but its result is not touched until this item's loads are issued: 148 CTAs hit the same
-                // counter at kernel start (a ~1.3 k clk round trip). r01 tested the result right away (`if (c == last) reset`), which put that
-                // round trip in front of every item's first load - the producer's whole run-ahead margin (r02 trace: first load 2.3-5.4 k clk
-                // after kernel entry, ~1.3 k clk of bubble at every tile boundary).
-                int drawn = 0;
-                if (!SK && elect_one()) drawn = atomicAdd(p.sched_counter, 1);
-                auto take_next = [&]() { // consumes the draw: next work id for all lanes; the launch's last draw re-zeroes the counter
-                    if constexpr (SK) return sk_next_work(p, work, (int) blockIdx.x, (int) gridDim.x, num_kb, total_work); // static schedule
-                    const int c = __shfl_sync(0xffffffffu, drawn, 0); // elect.sync picks lane 0 of the converged warp
-                    if (lane == 0 && c == draws_total - 1) *p.sched_counter = 0;
-                    return (int) gridDim.x + c;
-                };
-                const WorkItem wi = decode_work<SK>(p, work, total_tiles, num_kb);
-                const int tile = wi.tile;
-                const int m_idx = tile % m_tiles, oc_idx = tile / m_tiles;
-                const int bx = m_idx % p.tiles_x, by = (m_idx / p.tiles_x) % p.tiles_y, bn = m_idx / (p.tiles_x * p.tiles_y);
-                const int ix0 = bx * p.tw * p.stride - p.pad_x, iy0 = by * p.th * p.stride - p.pad_y, n0 = bn * p.tn;
-                const int oc0 = oc_idx * p.n_blk;
-                const int kb0 = wi.kb0, kb1 = wi.kb1;
-                // Keep this loop lean: it runs once per K block and every stall here delays the whole pipeline (no divisions,
-                // no parameter loads: ncu r01 showed ~60 dependent scalar instructions/iteration bounding the kernel).
-                // K block kb = (ky * ks + kx) * cbs + cb; the counters are decoded once per work item and then stepped.
-                if constexpr (HALO) {
-                    // K order (cb, tap): one halo tile per channel block, then the nine taps' weights. The halo tile of the NEXT
-                    // unit (next channel block, or the next work item's first) is requested one unit ahead, after this unit's first
-                    // weight stages are in flight: its ~1 us latency used to sit exposed at every tile boundary (r02 trace: ~2 k clk
-                    // of 7.5 k per 56x56x64 tile).
-                    auto issue_halo = [&](int w, int cb) {
-                        const int tile_ = w % total_tiles, m_ = tile_ % m_tiles;
-                        const int bx_ = m_ % p.tiles_x, by_ = (m_ / p.tiles_x) % p.tiles_y, bn_ = m_ / (p.tiles_x * p.tiles_y);
-                        mbar_wait(a_empty_bar(hstage), hphase ^ 1u);
-                        if (elect_one()) {
-                            const uint32_t sA = smem_base + hstage * HL_A_STAGE_BYTES, fb = a_full_bar(hstage);
-                            if (skip_tma) {
-                                mbar_arrive(fb);
-                            } else {
-                                mbar_expect_tx(fb, (TERMS == 1 ? 1u : 2u) * (uint32_t) (HL_W * HL_H * 128));
-                                tma_load_4d(sA, &tmA_hi, fb, cb * UM_BLOCK_K, bx_ * HL_TW - p.pad_x, by_ * HL_TH - p.pad_y, bn_);
-                                if (TERMS >= 2) tma_load_4d(sA + HL_PLANE, &tmA_lo, fb, cb * UM_BLOCK_K, bx_ * HL_TW - p.pad_x, by_ * HL_TH - p.pad_y, bn_);
-                            }
-                        }
-                        __syncwarp();
-                        if (++hstage == HL_A_STAGES) hstage = 0, hphase ^= 1u;
-                    };
-                    if (seq == 0) issue_halo(work, 0); // prologue: every later unit's tile is requested by its predecessor
-                    int nwork = total_work;           // next work item, known once the atomic draw above has returned
-                    for (int cb = 0; cb < cbs; ++cb) {
-                        int wk = cb * UM_BLOCK_K;
-                        for (int tap = 0; tap < 9; ++tap, wk += icp) {
-                            if (tap == 3) { // three weight stages are in flight: now the next unit's halo tile
-                                if (cb + 1 < cbs) {
-                                    issue_halo(work, cb + 1);
-                                } else {
-                                    nwork = take_next();
-                                    if (nwork < total_work) issue_halo(nwork, 0);
-                                }
-                            }
-                            // This CTA's first three weight stages went out before the dependency wait. They must not be waited for either:
-                            // the MMA thread may already have consumed such a stage and committed its empty barrier, and a wait for
-                            // "the phase before the first" would then block for ever (seen as a rare hang of the first launches, when
-                            // the producer was slow to get here: cold instruction cache).
-                            const bool pre_stage = seq == 0 && cb == 0 && tap < 3 && pre_b;
-                            if (!pre_stage) mbar_wait(empty_bar(stage), phase ^ 1u);
-                            UM_TRACE(0, tr);
-                            ++tr;
-                            if (pre_stage) {
-                            } else if (elect_one()) {
-                                const uint32_t sB = b_ring + stage * p.b_stage_bytes, fb = full_bar(stage);
-                                if (skip_tma) {
-                                    mbar_arrive(fb);
-                                } else {
-                                    mbar_expect_tx(fb, (TERMS == 3 ? 2u : 1u) * (uint32_t) p.n_blk * 128u);
-                                    tma_load_2d(sB, &tmB_hi, fb, wk, oc0);
-                                    if (TERMS == 3) tma_load_2d(sB + b_lo_off, &tmB_lo, fb, wk, oc0);
-                                }
-                            }
-                            if (++stage == p.b_stages) stage = 0, phase ^= 1u;
-                        }
-                    }
-                    work = nwork;
-                    continue;
-                }
-                int cb = kb0 % cbs, tap0 = kb0 / cbs;
-                int kx = tap0 % ks, ky = tap0 / ks;
-                int wk = tap0 * icp; // K coordinate into the packed weights = tap * ICp + cb * 64
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(empty_bar(stage), phase ^ 1u);
-                    UM_TRACE(0, tr);
-                    ++tr;
-                    if (elect_one()) {
-                        const uint32_t sA = smem_base + stage * UM_STAGE_BYTES, fb = full_bar(stage);
-                        if (skip_tma) {
-                            mbar_arrive(fb);
-                        } else {
-                            const bool pre = seq == 0 && kb == kb0 && pre_b; // expect_tx + the weights went out before the dependency wait
-                            if (!pre) mbar_expect_tx(fb, tx_bytes);
-                            tma_load_4d(sA, &tmA_hi, fb, cb * UM_BLOCK_K, ix0 + kx, iy0 + ky, n0);
-                            if (TERMS >= 2) tma_load_4d(sA + UM_A_BYTES, &tmA_lo, fb, cb * UM_BLOCK_K, ix0 + kx, iy0 + ky, n0);
-                            if (!pre) {
-                                tma_load_2d(sA + 2 * UM_A_BYTES, &tmB_hi, fb, wk + cb * UM_BLOCK_K, oc0);
-                                if (TERMS == 3) tma_load_2d(sA + 2 * UM_A_BYTES + b_lo_off, &tmB_lo, fb, wk + cb * UM_BLOCK_K, oc0);
-                            }
-                        }
-                    }
-                    if (++stage == STAGES) stage = 0, phase ^= 1u;
-                    if (++cb == cbs) {
-                        cb = 0, wk += icp;
-                        if (++kx == ks) kx = 0, ++ky;
-                    }
-                }
-                work = take_next();
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
+    if (wg == 0) {
+        // ===================== TMA producer (one thread) =====================
+        regs_dealloc_40(); // the consumers' two accumulator sets need the registers
+        if (warp != 0) return;
+        const uint32_t tx_bytes = (uint32_t) G::A_PLANES * (uint32_t) p.rows_used * 128u + (uint32_t) G::B_PLANES * (uint32_t) G::B_BYTES;
+        const int ks = p.ksize, cbs = p.cblocks, icp = p.ICp;
         int stage = 0;
         uint32_t phase = 0;
-        // 3-term split product with TWO MMAs per K step: A_hi x [B_hi ; B_lo] (N = 2 n_blk, two column blocks) and
-        // A_lo x B_hi (N = n_blk, onto the first block); the epilogue adds the blocks. Same math as three N = n_blk MMAs, but
-        // A_hi is fetched from shared memory once instead of twice and there are 8 instead of 12 issues per K block.
-        const uint32_t idesc_cat = TERMS == 3 ? make_idesc(UM_BLOCK_M, 2 * p.n_blk) : 0u;
-        const uint32_t idesc     = make_idesc(UM_BLOCK_M, p.n_blk);
-        // Descriptor of stage 0's A_hi tile; every other operand is this plus a constant in the 16-byte address field (all of
-        // shared memory is < 256 KB, so the 14-bit field never carries). Keeps the per-K-block preamble to a couple of adds:
-        // the issue of tcgen05.mma does not run ahead of the tensor pipe, so every scalar clock here is a lost MMA clock.
-        const uint64_t desc0 = make_smem_desc(smem_base);
-        // ONE thread runs the whole issue loop. Issuing tcgen05.mma stalls the thread while the tensor pipe's short queue is
-        // full, so scalar work placed BETWEEN the MMAs of a K block overlaps with them, while work between K blocks is lost
-        // tensor time: the look-ahead test of the next stage's barrier and the bookkeeping sit before the last two MMAs.
-        if (elect_one()) {
-            int it = 0, tr = 0, hstage = 0;
-            uint32_t hphase = 0;
-            (void) hstage, (void) hphase;
-            bool ready = false; // full_bar(stage) already observed complete by the look-ahead
-            const bool no_mma = (p.ablate & 4) != 0;
-            for (;; ++it) {
-                const int work = sched_take(it, true);
-                if (work >= total_work) break;
-                const int acc = it & 1;
-                const uint32_t acc_phase = (uint32_t) (it >> 1) & 1u;
-                mbar_wait(tmem_empty_bar(acc), acc_phase ^ 1u); // epilogue has drained this accumulator buffer
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t) (acc * UM_ACC_COLS);
-                if constexpr (HALO) {
-                    const uint64_t bdesc0 = make_smem_desc(b_ring);
-                    for (int cb = 0; cb < p.cblocks; ++cb) {
-                        mbar_wait(a_full_bar(hstage), hphase); // this channel block's halo tile has landed
-                        // SBO = the halo's row pitch (10 pixels): 8-row group g of tap (ky,kx) starts (g + ky) * 10 + kx pixels into the tile
-                        const uint64_t halo = make_smem_desc_sbo(smem_base + hstage * HL_A_STAGE_BYTES, HL_W * 128);
-                        int tap_off = 0; // (ky * HL_W + kx) * 128 B, in 16-byte units
-                        for (int tap = 0; tap < 9; ++tap) {
-                            if (!ready) mbar_wait(full_bar(stage), phase); // this tap's weights have landed
-                            tc_fence_after();
-                            UM_TRACE(1, tr);
-                            const uint64_t a_hi = halo + (uint64_t) (uint32_t) tap_off, a_lo = a_hi + (HL_PLANE >> 4);
-                            const uint64_t b_cat = bdesc0 + (uint64_t) (uint32_t) (stage * (p.b_stage_bytes >> 4));
-                            const uint32_t first = (cb > 0 || tap > 0) ? 1u : 0u;
-                            // First K step, then the look-ahead test of the next stage's barrier (its ~150 clk latency hides behind
-                            // the six MMAs still to be issued: behind only two, as in r01, the pipe ran dry ~180 clk per K block),
-                            // then the rest.
-                            if (!no_mma) {
-                                umma_f16(d_tmem, a_hi, b_cat, TERMS == 3 ? idesc_cat : idesc, first);
-                                if (TERMS == 2) umma_f16(d_tmem, a_lo, b_cat, idesc, 1u);
-                            }
-                            const int cur         = stage;
-                            const uint32_t nphase = phase ^ (stage == p.b_stages - 1 ? 1u : 0u);
-                            stage                 = stage == p.b_stages - 1 ? 0 : stage + 1;
-                            phase                 = nphase;
-                            ready                 = mbar_test_wait(full_bar(stage), phase); // non-blocking look-ahead
-                            if (!no_mma) {
-                                if (TERMS == 3) {
-#pragma unroll
-                                    for (int j = 1; j < UM_BLOCK_K / 16; ++j) umma_f16(d_tmem, a_hi + 2u * j, b_cat + 2u * j, idesc_cat, 1u);
-#pragma unroll
-                                    for (int j = 0; j < UM_BLOCK_K / 16; ++j) umma_f16(d_tmem, a_lo + 2u * j, b_cat + 2u * j, idesc, 1u);
-                                } else if (TERMS == 2) {
-#pragma unroll
-                                    for (int j = 1; j < UM_BLOCK_K / 16; ++j) {
-                                        umma_f16(d_tmem, a_hi + 2u * j, b_cat + 2u * j, idesc, 1u);
-                                        umma_f16(d_tmem, a_lo + 2u * j, b_cat + 2u * j, idesc, 1u);
-                                    }
-                                } else {
-#pragma unroll
-                                    for (int j = 1; j < UM_BLOCK_K / 16; ++j) umma_f16(d_tmem, a_hi + 2u * j, b_cat + 2u * j, idesc, 1u);
-                                }
-                            }
-                            umma_commit(empty_bar(cur)); // weight slot free once these MMAs retire
-                            UM_TRACE(2, tr);
-                            ++tr;
-                            tap_off += (tap % 3 == 2) ? ((HL_W - 2) * 128 >> 4) : (128 >> 4); // next tap: +1 pixel, or to the next halo row
-                        }
-                        umma_commit(a_empty_bar(hstage)); // halo tile free once all nine taps have retired
-                        if (++hstage == HL_A_STAGES) hstage = 0, hphase ^= 1u;
-                    }
-                    umma_commit(tmem_full_bar(acc)); // accumulator complete -> epilogue
-                    continue;
-                }
-                const WorkItem wi = decode_work<SK>(p, work, total_tiles, num_kb);
-                const int kb0 = wi.kb0, kb1 = wi.kb1;
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    if (!ready) mbar_wait(full_bar(stage), phase); // TMA bytes have landed
-                    tc_fence_after();
-                    UM_TRACE(1, tr);
-                    const uint64_t a_hi = desc0 + (uint64_t) (uint32_t) (stage * (UM_STAGE_BYTES >> 4)), a_lo = a_hi + (UM_A_BYTES >> 4);
-                    const uint64_t b_cat = a_hi + (2 * UM_A_BYTES >> 4); // rows [0, n_blk) = B_hi, [n_blk, 2 n_blk) = B_lo
-                    // UMMA_K = 16 fp16 = 32 bytes: K step j advances the start address by 2 (x16 B)
-                    const uint32_t first = kb > kb0 ? 1u : 0u;
-                    // ONE_BLOCK (short-K layers, 3-term): all three products go to the SAME accumulator block as separate N = n_blk MMAs
-                    // (12 instead of 8 per K block, A_hi fetched twice) - these layers run at the speed of their epilogue, not of the
-                    // tensor pipe, and this way the epilogue reads one TMEM block instead of two and adds nothing.
-                    const uint64_t b_lo = b_cat + (uint64_t) ((uint32_t) p.n_blk * 8u); // B_lo rows follow B_hi's (n_blk x 128 B)
-                    // first K step | look-ahead test of the next stage (latency hidden behind the remaining MMAs) | the rest
-                    if (!no_mma) {
-                        umma_f16(d_tmem, a_hi, b_cat, (TERMS == 3 && !ONE_BLOCK) ? idesc_cat : idesc, first);
-                        if (TERMS == 2) umma_f16(d_tmem, a_lo, b_cat, idesc, 1u);
-                        if (TERMS == 3 && ONE_BLOCK) umma_f16(d_tmem, a_hi, b_lo, idesc, 1u);
-                    }
-                    const int cur         = stage;
-                    const uint32_t nphase = phase ^ (stage == STAGES - 1 ? 1u : 0u);
-                    stage                 = stage == STAGES - 1 ? 0 : stage + 1;
-                    phase                 = nphase;
-                    ready                 = mbar_test_wait(full_bar(stage), phase); // non-blocking
-                    if (!no_mma) {
-                        if (TERMS == 3 && ONE_BLOCK) {
-#pragma unroll
-                            for (int j = 1; j < UM_BLOCK_K / 16; ++j) {
-                                umma_f16(d_tmem, a_hi + 2u * j, b_cat + 2u * j, idesc, 1u);
-                                umma_f16(d_tmem, a_hi + 2u * j, b_lo + 2u * j, idesc, 1u);
-                            }
-#pragma unroll
-                            for (int j = 0; j < UM_BLOCK_K / 16; ++j) umma_f16(d_tmem, a_lo + 2u * j, b_cat + 2u * j, idesc, 1u);
-                        } else if (TERMS == 3) {
-#pragma unroll
-                            for (int j = 1; j < UM_BLOCK_K / 16; ++j) umma_f16(d_tmem, a_hi + 2u * j, b_cat + 2u * j, idesc_cat, 1u);
-#pragma unroll
-                            for (int j = 0; j < UM_BLOCK_K / 16; ++j) umma_f16(d_tmem, a_lo + 2u * j, b_cat + 2u * j, idesc, 1u);
-                        } else if (TERMS == 2) {
-#pragma unroll
-                            for (int j = 1; j < UM_BLOCK_K / 16; ++j) {
-                                umma_f16(d_tmem, a_hi + 2u * j, b_cat + 2u * j, idesc, 1u);
-                                umma_f16(d_tmem, a_lo + 2u * j, b_cat + 2u * j, idesc, 1u);
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 1; j < UM_BLOCK_K / 16; ++j) umma_f16(d_tmem, a_hi + 2u * j, b_cat + 2u * j, idesc, 1u);
-                        }
-                    }
-                    umma_commit(empty_bar(cur));                           // smem slot free once these MMAs retire
-                    if (kb == kb1 - 1) umma_commit(tmem_full_bar(acc)); // accumulator complete -> epilogue
-                    UM_TRACE(2, tr);
-                    ++tr;
-                }
-            }
-        }
-        __syncwarp();
-    } else {
-        // ===================== epilogue (8 warps): see epilogue_tile =====================
-        const int q    = warp & 3;        // TMEM lane quarter this warp may access
-        const int half = (warp - 2) >> 2; // which interleaved set of 16-column chunks this warp owns
-        const int row  = q * 32 + lane;
-        EpiArgs e;
-        e.o_hi64 = &tmO_hi64, e.o_lo64 = &tmO_lo64, e.o_hiT = &tmO_hiT, e.o_loT = &tmO_loT;
-        e.r_hi64 = &tmR_hi64, e.r_lo64 = &tmR_lo64, e.r_hiT = &tmR_hiT, e.r_loT = &tmR_loT;
-        e.bias = p.bias, e.n_blk = p.n_blk, e.OC = p.OC, e.act = p.act, e.has_res = p.has_res, e.rows_box = p.rows_used, e.alpha = p.alpha;
-        e.has_lo = p.has_lo;
-        const int grp = SPLIT_EPI ? half : 0;                 // epilogue group of this warp
-        const bool leader = warp == (SPLIT_EPI ? 2 + 4 * grp : 2); // the group's TMA-issuing warp
-        e.stg = stg + grp * UM_STG_BYTES, e.res_bar = res_bar + 16u * grp, e.bar_id = 1 + grp;
-        e.part_src = nullptr, e.part_splits = 0;
-        const uint32_t last_flag = bar_base + 8u * (2 * STAGES + 6); // split-K: "this CTA arrived last" broadcast slot
-        uint32_t res_phase = 0;
-        int it = 0;
-        for (;; ++it) {
-            const int work = sched_take(it, lane == 0);
-            if (work >= total_work) break;
+        for (int work = first_work; work < total_work; work = next_work(work)) {
             const WorkItem wi = decode_work<SK>(p, work, total_tiles, num_kb);
-            const int tile = wi.tile;
-            const int acc = it & 1;
-            const uint32_t acc_phase = (uint32_t) (it >> 1) & 1u;
-            if (SPLIT_EPI && acc != grp) continue; // the other group's accumulator buffer
-            const int m_idx = tile % m_tiles, oc_idx = tile / m_tiles;
+            const int m_idx = wi.tile % m_tiles, oc_idx = wi.tile / m_tiles;
             const int bx = m_idx % p.tiles_x, by = (m_idx / p.tiles_x) % p.tiles_y, bn = m_idx / (p.tiles_x * p.tiles_y);
-            if (p.has_res && wi.pieces == 1 && !(p.ablate & 1)) epilogue_residual_load(e, 0, oc_idx * p.n_blk, bx * p.tw, by * p.th, bn * p.tn, leader);
-            mbar_wait(tmem_full_bar(acc), acc_phase);
-            tc_fence_after();
-            if (leader) UM_TRACE(3, it);
-            e.tmem_empty = tmem_empty_bar(acc);
-            e.trace = p.trace, e.trace_seq = it;
-            const uint32_t taddr = tmem_base + ((uint32_t) (q * 32) << 16) + (uint32_t) (acc * UM_ACC_COLS);
-            if (p.ablate & 1) {
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(e.tmem_empty);
-                continue;
-            }
-            if (wi.pieces > 1) {
-                float* tile_parts = p.partials + (size_t) wi.slot * (SK ? 4 : p.ksplit) * (UM_BLOCK_M * p.n_blk);
-                epilogue_dump_partial<UM_EPI_WARPS, EPI_TERMS>(e, taddr, tile_parts + (size_t) wi.piece * (UM_BLOCK_M * p.n_blk), row, half, lane);
-                __threadfence(); // partial tile visible device-wide before the arrival is counted
-                named_bar_sync(1, UM_EPI_WARPS * 32);
-                if (warp == 2 && lane == 0) {
-                    const int old  = atomicAdd(p.counters + wi.slot, 1);
-                    const int last = old == wi.pieces - 1;
-                    if (last) p.counters[wi.slot] = 0; // every piece has arrived: leave the counter ready for the next launch
-                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(last_flag), "r"(last) : "memory");
+            const int ix0 = bx * p.tw * p.stride - p.pad_x, iy0 = by * p.th * p.stride - p.pad_y, n0 = bn * p.tn;
+            const int oc0 = oc_idx * NB;
+            // K block kb = (ky * ks + kx) * cbs + cb; the counters are decoded once per work item and then stepped
+            int cb = wi.kb0 % cbs, tap0 = wi.kb0 / cbs;
+            int kx = tap0 % ks, ky = tap0 / ks;
+            int wk = tap0 * icp; // K coordinate into the packed weights = tap * ICp + cb * 64
+            for (int kb = wi.kb0; kb < wi.kb1; ++kb) {
+                mbar_wait(empty_bar(stage), phase ^ 1u);
+                if (elect_one()) {
+                    const uint32_t sA = smem_base + stage * G::STAGE_BYTES, sB = sA + G::A_PLANES * UM_A_BYTES, fb = full_bar(stage);
+                    mbar_expect_tx(fb, tx_bytes);
+                    tma_load_4d(sA, &tmA_hi, fb, cb * UM_BLOCK_K, ix0 + kx, iy0 + ky, n0);
+                    if (TERMS >= 2) tma_load_4d(sA + UM_A_BYTES, &tmA_lo, fb, cb * UM_BLOCK_K, ix0 + kx, iy0 + ky, n0);
+                    tma_load_2d(sB, &tmB_hi, fb, wk + cb * UM_BLOCK_K, oc0);
+                    if (TERMS == 3) tma_load_2d(sB + G::B_BYTES, &tmB_lo, fb, wk + cb * UM_BLOCK_K, oc0);
                 }
-                named_bar_sync(1, UM_EPI_WARPS * 32);
-                int last;
-                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(last) : "r"(last_flag) : "memory");
-                if (!last) continue;
-                __threadfence();
-                e.part_src = tile_parts, e.part_splits = wi.pieces;
-                if (p.has_res) epilogue_residual_load(e, 0, oc_idx * p.n_blk, bx * p.tw, by * p.th, bn * p.tn, leader);
+                __syncwarp();
+                if (++stage == STAGES) stage = 0, phase ^= 1u;
+                if (++cb == cbs) {
+                    cb = 0, wk += icp;
+                    if (++kx == ks) kx = 0, ++ky;
+                }
             }
-            if (SPLIT_EPI)
-                epilogue_tile<UM_EPI_WARPS / 2, EPI_TERMS>(e, taddr, oc_idx * p.n_blk, bx * p.tw, by * p.th, bn * p.tn, row, 0, leader, lane, res_phase);
-            else
-                epilogue_tile<UM_EPI_WARPS, EPI_TERMS>(e, taddr, oc_idx * p.n_blk, bx * p.tw, by * p.th, bn * p.tn, row, half, leader, lane, res_phase);
-            e.part_src = nullptr;
-            if (leader) UM_TRACE(4, it);
         }
-        epilogue_drain(leader);
+        return;
     }
 
-    if (warp == 0) UM_TRACE(5, 2); // producer done
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) UM_TRACE(5, 3); // all roles done
-    if (p.trace && threadIdx.x == 0) {
-        unsigned long long g;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
-        atomicMax(reinterpret_cast<unsigned long long*>(p.trace) + 5 * 256 + 9, g);
-        if (blockIdx.x == 0) p.trace[5 * 256 + 11] = (long long) g;
+    // ===================== consumers: wgmma main loop + epilogue =====================
+    regs_alloc_232();
+    const int cw  = wg - 1;                                // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
+    const int wq  = warp & 3;                              // warp within the warpgroup
+    const int row0 = 64 * cw + 16 * wq + (lane >> 2);      // tile row of d[0]; d[2] is row0 + 8
+    const int q    = lane & 3;
+    EpiArgs e;
+    e.o_hi64 = &tmO_hi64, e.o_lo64 = &tmO_lo64, e.o_hiT = &tmO_hiT, e.o_loT = &tmO_loT;
+    e.r_hi64 = &tmR_hi64, e.r_lo64 = &tmR_lo64, e.r_hiT = &tmR_hiT, e.r_loT = &tmR_loT;
+    e.bias = p.bias, e.OC = p.OC, e.act = p.act, e.has_res = p.has_res, e.rows_box = p.rows_used, e.alpha = p.alpha;
+    e.has_lo = p.has_lo, e.stg = stg, e.res_bar = res_bar, e.issuer = threadIdx.x == 128;
+    uint32_t res_phase = 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[NB / 2], blk[NB / 2];
+    for (int work = first_work; work < total_work; work = next_work(work)) {
+        const WorkItem wi = decode_work<SK>(p, work, total_tiles, num_kb);
+#pragma unroll
+        for (int i = 0; i < NB / 2; ++i) acc[i] = 0.0f;
+        for (int kb = wi.kb0; kb < wi.kb1; ++kb) {
+            mbar_wait(full_bar(stage), phase); // TMA bytes have landed
+            const uint32_t sA = smem_base + stage * G::STAGE_BYTES, sB = sA + G::A_PLANES * UM_A_BYTES;
+            const uint64_t a_hi = gmma_desc_sw128(sA + cw * 64 * 128), a_lo = gmma_desc_sw128(sA + UM_A_BYTES + cw * 64 * 128);
+            const uint64_t b_hi = gmma_desc_sw128(sB), b_lo = gmma_desc_sw128(sB + G::B_BYTES);
+            wg_fence();
+#pragma unroll
+            for (int k = 0; k < UM_BLOCK_K / 16; ++k) {
+                Wgmma<NB>::mma(blk, a_hi + 2u * k, b_hi + 2u * k, k > 0 ? 1u : 0u);
+                if (TERMS == 3) Wgmma<NB>::mma(blk, a_hi + 2u * k, b_lo + 2u * k, 1u);
+                if (TERMS >= 2) Wgmma<NB>::mma(blk, a_lo + 2u * k, b_hi + 2u * k, 1u);
+            }
+            wg_commit();
+            wg_wait<0>(); // this K block's wgmmas have retired: its stage goes back to the producer
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(stage));
+            acc_promote(acc, blk);
+            if (++stage == STAGES) stage = 0, phase ^= 1u;
+        }
+        const int m_idx = wi.tile % m_tiles, oc_idx = wi.tile / m_tiles;
+        const int bx = m_idx % p.tiles_x, by = (m_idx / p.tiles_x) % p.tiles_y, bn = m_idx / (p.tiles_x * p.tiles_y);
+        if (wi.pieces > 1) {
+            // fp32 partial tile [row][NB]; the last of the tile's pieces to arrive sums them in piece order (deterministic)
+            float* tile_parts = p.partials + (size_t) wi.slot * (SK ? 4 : p.ksplit) * (UM_BLOCK_M * NB);
+            float* mine       = tile_parts + (size_t) wi.piece * (UM_BLOCK_M * NB);
+#pragma unroll
+            for (int j = 0; j < NB / 8; ++j)
+#pragma unroll
+                for (int r = 0; r < 2; ++r)
+                    __stcg(reinterpret_cast<float2*>(mine + (size_t) (row0 + 8 * r) * NB + 8 * j + 2 * q), make_float2(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]));
+            __threadfence(); // partial tile visible device-wide before the arrival is counted
+            named_bar_sync(1, UM_EPI_THREADS);
+            if (e.issuer) {
+                const int old  = atomicAdd(p.counters + wi.slot, 1);
+                const int last = old == wi.pieces - 1;
+                if (last) p.counters[wi.slot] = 0; // every piece has arrived: leave the counter ready for the next launch
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(last_flag), "r"(last) : "memory");
+            }
+            named_bar_sync(1, UM_EPI_THREADS);
+            int last;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(last) : "r"(last_flag) : "memory");
+            if (!last) continue;
+            __threadfence();
+#pragma unroll
+            for (int j = 0; j < NB / 8; ++j)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const float* src = tile_parts + (size_t) (row0 + 8 * r) * NB + 8 * j + 2 * q;
+                    float2 s = __ldcg(reinterpret_cast<const float2*>(src));
+                    for (int sp = 1; sp < wi.pieces; ++sp) {
+                        const float2 t = __ldcg(reinterpret_cast<const float2*>(src + (size_t) sp * (UM_BLOCK_M * NB)));
+                        s.x += t.x, s.y += t.y;
+                    }
+                    acc[4 * j + 2 * r] = s.x, acc[4 * j + 2 * r + 1] = s.y;
+                }
+        }
+        epilogue_tile<NB>(e, acc, oc_idx * NB, bx * p.tw, by * p.th, bn * p.tn, row0, q, res_phase);
     }
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, UM_TMEM_COLS);
-    }
+    epilogue_drain(e.issuer);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Small-input-channel convolution (IC <= 8: the 7x7 / 3x3 RGB stems, ESPCN's 1-channel 5x5) on the same tensor cores,
 // with a ZERO-COPY sliding-window A operand.
 //
-// With C padded to 8 fp16 one pixel is ONE 16-byte vector per plane = exactly one K "chunk" of a tcgen05 K-major
-// operand. In the un-swizzled (SWIZZLE_NONE) canonical layout row m / chunk c of A is read from
+// With C padded to 8 fp16 one pixel is ONE 16-byte vector per plane = exactly one K "core matrix" column of a wgmma K-major
+// operand. In the un-swizzled canonical layout row m / chunk c of A is read from
 //        start + (m/8)*SBO + (m%8)*16 B + c*LBO,
 // and nothing stops LBO from being 16 B: chunk c of row m is then simply pixel m + c of a dense pixel row in shared
-// memory - the convolution's sliding window, expressed in the descriptor (probed on B200: tools/umma_desc_probe.cu).
+// memory - the convolution's sliding window, expressed in the descriptor.
 // So for every filter row ky the producer TMA-loads ONE dense row segment per column parity (for stride 2 the even and
 // odd input columns are de-interleaved by the tensor map's 32-byte pixel stride; out-of-image pixels are zero-filled =
-// constant padding) and the MMA warp issues one K=16 step per pair of taps: no im2col, no producer warps, no copies.
+// constant padding) and the consumers issue one K=16 step per pair of taps: no im2col, no copies.
 // L2 -> SM traffic per 128-pixel tile: kh * s * ~136 * 16 B * 2 planes (61 KB for the 7x7 stem) instead of 224 KB of
 // gathered 16-byte requests. The weight panel [kh][n_blk][64] (hi + lo, K columns in RowPlan order) is loaded once per
 // persistent CTA and stays resident. Tiles = up to 128 consecutive output pixels of one output row.
 //
-// FEED mode (r02; stride 2, <= 4 input channels = the RGB stems): the input kernels also write a compact copy of the image with
+// FEED mode (stride 2, <= 4 input channels = the RGB stems): the input kernels also write a compact copy of the image with
 // FOUR channels per pixel and zero margins (snnb_tensor::feed_hi). With 8-byte pixels one 16-byte K chunk is a PAIR of adjacent
 // pixels, and for stride 2 the window of output pixel m starts at pixel 2 m = 16 m bytes: the plain dense row is already the
 // canonical operand (row pitch 16 B, LBO 16 B) - no parity de-interleave, half the K (7 taps x 4 channels + 1 pad tap = 32 instead of
 // 64), one contiguous bulk copy per plane and filter row, real zeros instead of out-of-bounds fill (FeedPlan, snnb_internal.h).
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int RW_MAX_STAGES    = 16;                           // ring depth is chosen per launch: whatever shared memory is left, see RowWinParams::stages
-constexpr int RW_EPI_WARPS     = 8;
-constexpr int RW_THREADS       = 64 + 32 * RW_EPI_WARPS;
+constexpr int RW_THREADS       = UM_THREADS;
 constexpr int RW_MAX_N         = 64;
 constexpr int RW_BOXW          = 144;                          // 128 tile pixels + up to 8 of window overhang, padded
 constexpr int RW_ARR_BYTES     = RW_BOXW * 16;                 // one (plane, parity) pixel row segment
-constexpr int RW_SMEM_BYTES    = 227 * 1024;                   // everything: resident weight panels | epilogue staging | A ring | barriers
+constexpr int RW_SMEM_BYTES    = UM_SMEM_LIMIT;                // everything: resident weight panels | epilogue staging | A ring | barriers
 constexpr int RW_BAR_BYTES     = 512;
 constexpr int RW_B_MAX_BYTES   = RW_SMEM_BYTES - 1024 - RW_BAR_BYTES - UM_STG_BYTES - 4 * 4 * RW_ARR_BYTES; // weights must leave room for >= 4 stages
 
 struct RowWinParams {
-    __half* out_hi;
-    __half* out_lo;
     const float* bias;
-    int N, OH, OW, OC, OCp, n_blk, ocr;
+    int N, OH, OW, OC, OCp, n_blk;
     int kh, stride, pad_y;
     int tiles_x;
     int parities, dmin[2];
     int ksteps, panels, ks_parity[8], ks_erel[8]; // panels = ceil(ksteps / 4) weight panels of 64 K columns per filter row
     int act;
     float alpha;
-    long long* trace; // profiling aid, see UmmaParams
-    int ablate;       // profiling aid (SNNB_UMMA_ABLATE, results WRONG when set): 1 skip the epilogue work, 2 the activation loads, 4 the MMAs, 8 the TMA stores
     // FEED mode (stride 2, <= 4 input channels; FeedPlan in snnb_internal.h): the A rows come from the input tensor's compact
     // 4-channel copy, one contiguous segment per plane and filter row (a plain bulk copy, the margins are real zeros)
     const __half* feed_hi;
@@ -1129,138 +594,107 @@ struct RowWinParams {
     uint32_t feed_seg_bytes; // 0 = not in feed mode
     // shared-memory carve-up (host-computed): the weight panels take b_bytes (multiple of 1024), the ring gets `stages` stages of
     // stage_bytes = planes x parities x RW_ARR_BYTES; the lo plane's arrays follow the hi plane's at lo_off. The ring is as deep as
-    // shared memory allows: a stage is only ~2-9 KB, and the cycle load -> MMA -> commit -> producer wake-up is ~2.5 k clk long, so a
-    // 5-deep ring ran the 7x7 stem at one stage per ~560 clk whatever the stage's own work was (profiles/r02_stem_ablation.txt).
+    // shared memory allows: a stage is only ~2-9 KB and holds little work, so the producer has to run far ahead.
     int stages;
     uint32_t stage_bytes, lo_off, b_bytes;
-    // FEED mode: a stage holds `rows_per_stage` filter rows (row_bytes each: hi segment, lo segment), released by ONE tcgen05.commit -
-    // a commit costs the issuing thread ~52 clk and a stage boundary ~100 more, against 224 clk of MMAs per filter row of the 7x7 stem
+    // FEED mode: a stage holds `rows_per_stage` filter rows (row_bytes each: hi segment, lo segment), released together
     int rows_per_stage;
     uint32_t row_bytes;
-    int stg_bufs; // epilogue staging buffers (2: alternate tiles, see EpiArgs::two_stagings)
     int feed_prows; // feed mode: 128-byte weight rows per output channel = ceil(kh / FeedPlan::rows_per_panel)
 };
 
-// SWIZZLE_NONE K-major descriptor with an overlapping K stride: LBO = 16 B (next chunk = next pixel), SBO = 128 B
-// (8 rows x 16 B), version 1, layout type 0.
-__device__ __forceinline__ uint64_t make_window_desc(uint32_t saddr) { return (uint64_t) ((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (8ull << 32) | (1ull << 46); }
-
-// FKS > 0: FEED mode with FKS K steps per filter row (see RowWinParams::feed_hi). Its producer and MMA-issue loops are written out
-// separately and kept to a few dozen instructions per stage: both run in ONE thread, a stage of the 7x7 stem holds only four MMAs
-// (224 clk of tensor time), and the generic loops below cost ~290 SASS instructions = ~400 clk per stage whatever the stage's work
-// was (profiles/r02_stem_ablation.txt: with loads, MMAs and epilogue all ablated the kernel still took 48 of its 75 us).
-template <int TERMS, int FKS> // TERMS: see conv_umma_kernel
+// FKS > 0: FEED mode with FKS K steps per filter row (see RowWinParams::feed_hi). NB: n_blk (output channels, 32 or 64).
+template <int TERMS, int FKS, int NB>
 __global__ void __launch_bounds__(RW_THREADS, 1)
 conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_constant__ CUtensorMap tmA_hi1, const __grid_constant__ CUtensorMap tmA_lo0,
                    const __grid_constant__ CUtensorMap tmA_lo1, const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
                    const __grid_constant__ CUtensorMap tmO_hi, const __grid_constant__ CUtensorMap tmO_lo, const RowWinParams p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t sB = smem_base; // weight panel: per kernel row ky, [n_blk rows of B_hi ; n_blk rows of B_lo] x 128 B
+    const uint32_t sB = smem_base; // weight panel: per (filter row, panel), [NB rows of B_hi ; NB rows of B_lo] x 128 B
     const uint32_t stg      = smem_base + p.b_bytes; // epilogue staging (1024-aligned)
-    const uint32_t sA0      = stg + (uint32_t) p.stg_bufs * UM_STG_BYTES;
+    const uint32_t sA0      = stg + (uint32_t) UM_STG_BYTES;
     const uint32_t bar_base = sA0 + (uint32_t) p.stages * p.stage_bytes;
     const int RW_STAGES     = p.stages;
     auto full_bar       = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar      = [&](int s) { return bar_base + 8u * (RW_MAX_STAGES + s); };
-    auto tmem_full_bar  = [&](int a) { return bar_base + 8u * (2 * RW_MAX_STAGES + a); };
-    auto tmem_empty_bar = [&](int a) { return bar_base + 8u * (2 * RW_MAX_STAGES + 2 + a); };
-    const uint32_t b_bar     = bar_base + 8u * (2 * RW_MAX_STAGES + 4);
-    const uint32_t tmem_slot = bar_base + 8u * (2 * RW_MAX_STAGES + 5);
+    const uint32_t b_bar = bar_base + 8u * (2 * RW_MAX_STAGES);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     pdl_trigger();
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA_hi0);
         tma_prefetch_desc(&tmA_lo0);
         tma_prefetch_desc(&tmB_hi);
         tma_prefetch_desc(&tmB_lo);
         for (int s = 0; s < RW_STAGES; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tmem_full_bar(a), 1);
-            mbar_init(tmem_empty_bar(a), RW_EPI_WARPS);
+            mbar_init(empty_bar(s), UM_EPI_THREADS / 32);
         }
         mbar_init(b_bar, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 4 * RW_MAX_N); // two accumulator buffers of 2 x (<= 64) columns
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    uint32_t tmem_base;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
     pdl_wait();
-    if (warp == 0) UM_TRACE(5, 0);
-    if (p.trace && threadIdx.x == 0) {
-        unsigned long long g;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
-        atomicMin(reinterpret_cast<unsigned long long*>(p.trace) + 5 * 256 + 8, g);
-        if (blockIdx.x == 0) p.trace[5 * 256 + 10] = (long long) g;
-    }
 
     const int total_tiles = p.N * p.OH * p.tiles_x;
+    constexpr uint32_t B_PLANE = (uint32_t) NB * 128u; // one weight plane of a panel
 
-    if (warp == 0) {
-        {
-            // weight panel: once per CTA
-            if (elect_one()) {
-                const int vrows = FKS > 0 ? p.feed_prows : p.kh * p.panels; // (filter row, panel); feed mode: several filter rows per weight row
-                mbar_expect_tx(b_bar, (TERMS == 3 ? 2u : 1u) * (uint32_t) vrows * (uint32_t) p.n_blk * 128u);
-                for (int v = 0; v < vrows; ++v) {
-                    if (TERMS == 3) {
-                        tma_load_2d(sB + (2 * v) * p.n_blk * 128, &tmB_hi, b_bar, 0, v * p.ocr);
-                        tma_load_2d(sB + (2 * v + 1) * p.n_blk * 128, &tmB_lo, b_bar, 0, v * p.ocr);
-                    } else {
-                        tma_load_2d(sB + v * p.n_blk * 128, &tmB_hi, b_bar, 0, v * p.ocr); // one plane
-                    }
+    if (wg == 0) {
+        regs_dealloc_40();
+        if (warp != 0) return;
+        // weight panels: once per CTA, [filter row][panel][plane] (feed mode: several filter rows share one 128-byte weight row)
+        if (elect_one()) {
+            const int vrows = FKS > 0 ? p.feed_prows : p.kh * p.panels;
+            mbar_expect_tx(b_bar, (TERMS == 3 ? 2u : 1u) * (uint32_t) vrows * B_PLANE);
+            for (int v = 0; v < vrows; ++v) {
+                if (TERMS == 3) {
+                    tma_load_3d(sB + (2 * v) * B_PLANE, &tmB_hi, b_bar, 0, 0, v);
+                    tma_load_3d(sB + (2 * v + 1) * B_PLANE, &tmB_lo, b_bar, 0, 0, v);
+                } else {
+                    tma_load_3d(sB + v * B_PLANE, &tmB_hi, b_bar, 0, 0, v); // one plane
                 }
             }
-            __syncwarp();
-            // activation row segments
-            int stage = 0;
-            uint32_t phase = 0;
-            const uint32_t tx_bytes = (TERMS == 1 ? 1u : 2u) * (p.feed_seg_bytes ? p.feed_seg_bytes : (uint32_t) p.parities * RW_ARR_BYTES);
-            if constexpr (FKS > 0) {
-                // one contiguous segment per plane and filter row; running pointers, no per-stage address arithmetic
-                const uint32_t seg  = p.feed_seg_bytes;
-                const size_t pitch  = (size_t) p.feed_w * 4; // fp16 elements per feed row
-                const int per_image = p.OH * p.tiles_x;
-                int rem = (int) blockIdx.x % per_image, n = (int) blockIdx.x / per_image;
-                uint32_t sA = sA0;
-                for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                    const int oy = p.tiles_x == 1 ? rem : rem / p.tiles_x, xt = p.tiles_x == 1 ? 0 : rem % p.tiles_x;
-                    const size_t off = (((size_t) n * p.feed_h + (oy * 2 - p.pad_y + p.feed_py)) * p.feed_w + 2 * xt * UM_BLOCK_M) * 4;
-                    const __half* src_hi = p.feed_hi + off;
-                    const __half* src_lo = p.feed_lo + off;
-                    for (int ky0 = 0; ky0 < p.kh; ky0 += p.rows_per_stage) {
-                        const int rows = min(p.rows_per_stage, p.kh - ky0); // this stage's group of filter rows
-                        mbar_wait(empty_bar(stage), phase ^ 1u);
-                        if (elect_one()) {
-                            if (p.ablate & 2) {
-                                mbar_arrive(full_bar(stage));
-                            } else {
-                                mbar_expect_tx(full_bar(stage), tx_bytes * (uint32_t) rows);
-                                const __half* sh = src_hi;
-                                const __half* sl = src_lo;
-                                uint32_t dst     = sA;
-                                for (int r = 0; r < rows; ++r, dst += p.row_bytes, sh += pitch, sl += pitch) {
-                                    bulk_load_1d(dst, sh, seg, full_bar(stage));
-                                    if (TERMS >= 2) bulk_load_1d(dst + RW_ARR_BYTES, sl, seg, full_bar(stage));
-                                }
-                            }
+        }
+        __syncwarp();
+        // activation row segments
+        int stage = 0;
+        uint32_t phase = 0;
+        const uint32_t tx_bytes = (TERMS == 1 ? 1u : 2u) * (p.feed_seg_bytes ? p.feed_seg_bytes : (uint32_t) p.parities * RW_ARR_BYTES);
+        if constexpr (FKS > 0) {
+            // one contiguous segment per plane and filter row; running pointers, no per-stage address arithmetic
+            const uint32_t seg  = p.feed_seg_bytes;
+            const size_t pitch  = (size_t) p.feed_w * 4; // fp16 elements per feed row
+            const int per_image = p.OH * p.tiles_x;
+            int rem = (int) blockIdx.x % per_image, n = (int) blockIdx.x / per_image;
+            uint32_t sA = sA0;
+            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+                const int oy = p.tiles_x == 1 ? rem : rem / p.tiles_x, xt = p.tiles_x == 1 ? 0 : rem % p.tiles_x;
+                const size_t off = (((size_t) n * p.feed_h + (oy * 2 - p.pad_y + p.feed_py)) * p.feed_w + 2 * xt * UM_BLOCK_M) * 4;
+                const __half* src_hi = p.feed_hi + off;
+                const __half* src_lo = p.feed_lo + off;
+                for (int ky0 = 0; ky0 < p.kh; ky0 += p.rows_per_stage) {
+                    const int rows = min(p.rows_per_stage, p.kh - ky0); // this stage's group of filter rows
+                    mbar_wait(empty_bar(stage), phase ^ 1u);
+                    if (elect_one()) {
+                        mbar_expect_tx(full_bar(stage), tx_bytes * (uint32_t) rows);
+                        const __half* sh = src_hi;
+                        const __half* sl = src_lo;
+                        uint32_t dst     = sA;
+                        for (int r = 0; r < rows; ++r, dst += p.row_bytes, sh += pitch, sl += pitch) {
+                            bulk_load_1d(dst, sh, seg, full_bar(stage));
+                            if (TERMS >= 2) bulk_load_1d(dst + RW_ARR_BYTES, sl, seg, full_bar(stage));
                         }
-                        __syncwarp();
-                        src_hi += pitch * rows, src_lo += pitch * rows;
-                        sA += p.stage_bytes;
-                        if (++stage == RW_STAGES) stage = 0, phase ^= 1u, sA = sA0;
                     }
-                    rem += (int) gridDim.x;
-                    while (rem >= per_image) rem -= per_image, ++n;
+                    __syncwarp();
+                    src_hi += pitch * rows, src_lo += pitch * rows;
+                    sA += p.stage_bytes;
+                    if (++stage == RW_STAGES) stage = 0, phase ^= 1u, sA = sA0;
                 }
-            } else
+                rem += (int) gridDim.x;
+                while (rem >= per_image) rem -= per_image, ++n;
+            }
+        } else {
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int xt = tile % p.tiles_x, oy = (tile / p.tiles_x) % p.OH, n = tile / (p.tiles_x * p.OH);
                 const int ox0 = xt * UM_BLOCK_M;
@@ -1269,16 +703,12 @@ conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_con
                     mbar_wait(empty_bar(stage), phase ^ 1u);
                     if (elect_one()) {
                         const uint32_t sA = sA0 + stage * p.stage_bytes;
-                        if (p.ablate & 2) {
-                            mbar_arrive(full_bar(stage));
-                        } else {
-                            mbar_expect_tx(full_bar(stage), tx_bytes);
-                            tma_load_4d(sA, &tmA_hi0, full_bar(stage), 0, ox0 + p.dmin[0], iy, n);
-                            if (TERMS >= 2) tma_load_4d(sA + p.lo_off, &tmA_lo0, full_bar(stage), 0, ox0 + p.dmin[0], iy, n);
-                            if (p.parities == 2) {
-                                tma_load_4d(sA + RW_ARR_BYTES, &tmA_hi1, full_bar(stage), 0, ox0 + p.dmin[1], iy, n);
-                                if (TERMS >= 2) tma_load_4d(sA + p.lo_off + RW_ARR_BYTES, &tmA_lo1, full_bar(stage), 0, ox0 + p.dmin[1], iy, n);
-                            }
+                        mbar_expect_tx(full_bar(stage), tx_bytes);
+                        tma_load_4d(sA, &tmA_hi0, full_bar(stage), 0, ox0 + p.dmin[0], iy, n);
+                        if (TERMS >= 2) tma_load_4d(sA + p.lo_off, &tmA_lo0, full_bar(stage), 0, ox0 + p.dmin[0], iy, n);
+                        if (p.parities == 2) {
+                            tma_load_4d(sA + RW_ARR_BYTES, &tmA_hi1, full_bar(stage), 0, ox0 + p.dmin[1], iy, n);
+                            if (TERMS >= 2) tma_load_4d(sA + p.lo_off + RW_ARR_BYTES, &tmA_lo1, full_bar(stage), 0, ox0 + p.dmin[1], iy, n);
                         }
                     }
                     __syncwarp();
@@ -1286,212 +716,95 @@ conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_con
                 }
             }
         }
-    } else if (warp == 1) {
-        mbar_wait(b_bar, 0);
-        // see conv_umma_kernel: 3-term = A_hi x [B_hi ; B_lo] + A_lo x B_hi; 2-term = (A_hi + A_lo) x B16; 1-term = A_hi x B_hi
-        const uint32_t idesc_cat = TERMS == 3 ? make_idesc(UM_BLOCK_M, 2 * p.n_blk) : make_idesc(UM_BLOCK_M, p.n_blk);
-        const uint32_t idesc     = make_idesc(UM_BLOCK_M, p.n_blk);
-        if (elect_one()) { // one thread owns the issue loop (see conv_umma_kernel)
-            // window descriptor (16-byte address field) offsets of the K steps, relative to the stage's hi plane
-            uint32_t koff[8];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) koff[q] = q < p.ksteps ? (((uint32_t) p.ks_parity[q] * RW_ARR_BYTES + (uint32_t) p.ks_erel[q] * 16u) >> 4) : 0u;
-            const uint64_t wdesc0 = make_window_desc(sA0), bdesc0 = make_smem_desc(sB);
-            const uint32_t b_panel = (uint32_t) ((TERMS == 3 ? 2 : 1) * p.n_blk * 128) >> 4;  // one [B_hi ; B_lo] (or single-plane) panel (64 K columns)
-            const uint32_t b_ky    = b_panel * (uint32_t) p.panels;         // one filter row
-            const int last_q      = p.ksteps - 1;
-            const uint32_t koff_last = ((uint32_t) p.ks_parity[last_q] * RW_ARR_BYTES + (uint32_t) p.ks_erel[last_q] * 16u) >> 4;
-            int stage = 0, it = 0, tr = 0;
-            uint32_t phase = 0;
-            bool ready     = false;
-            const bool no_mma = (p.ablate & 4) != 0;
-            const uint64_t lo_off16 = (uint64_t) (p.lo_off >> 4);
-            if constexpr (FKS > 0) {
-                // FEED mode: K step q of a stage = window start + 2 q pixels pairs (32 B), weights columns 16 q ..; everything a constant offset
-                constexpr uint32_t LO16 = RW_ARR_BYTES >> 4;
-                constexpr int RPP       = FKS == 1 ? 4 : (FKS == 2 ? 2 : 1); // FeedPlan::rows_per_panel
-                const uint32_t stage16  = p.stage_bytes >> 4, row16 = p.row_bytes >> 4;
-                const bool tracing      = p.trace != nullptr && blockIdx.x == 0;
-                uint64_t a_cur = wdesc0;
-                for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-                    const int acc = it & 1;
-                    mbar_wait(tmem_empty_bar(acc), ((uint32_t) (it >> 1) & 1u) ^ 1u);
-                    tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t) (acc * 2 * RW_MAX_N);
-                    uint64_t b_cat = bdesc0;
-                    int b_sub      = 0;
-                    for (int ky0 = 0; ky0 < p.kh; ky0 += p.rows_per_stage) {
-                        const int rows = min(p.rows_per_stage, p.kh - ky0); // the group of filter rows this stage holds
-                        if (!ready) mbar_wait(full_bar(stage), phase);
-                        tc_fence_after();
-                        if (tracing && tr < 256) p.trace[1 * 256 + tr] = clock64();
-                        if (!no_mma) { // first K step of the group, then the look-ahead test, then the rest
-                            umma_f16(d_tmem, a_cur, b_cat, idesc_cat, ky0 > 0 ? 1u : 0u);
-                            if (TERMS >= 2) umma_f16(d_tmem, a_cur + LO16, b_cat, idesc, 1u);
-                        }
-                        const int cur        = stage;
-                        const bool wrap      = stage == RW_STAGES - 1;
-                        uint64_t a_row       = a_cur;
-                        phase ^= wrap ? 1u : 0u;
-                        stage = wrap ? 0 : stage + 1;
-                        a_cur = wrap ? wdesc0 : a_cur + stage16;
-                        ready = mbar_test_wait(full_bar(stage), phase); // look-ahead, overlaps with the MMAs already queued
-                        for (int r = 0; r < rows; ++r, a_row += row16) {
-                            // weights of the next filter row: the next K-column group of the same 128-byte rows, or the next panel
-                            const uint64_t b_now = b_cat;
-                            if (++b_sub == RPP) b_sub = 0, b_cat += b_panel - (RPP - 1) * (8 / RPP);
-                            else b_cat += 8 / RPP;
-                            if (no_mma) continue;
-#pragma unroll
-                            for (int q = 0; q < FKS; ++q) {
-                                if (r == 0 && q == 0) continue; // issued above
-                                umma_f16(d_tmem, a_row + 2u * q, b_now + 2u * q, idesc_cat, 1u);
-                                if (TERMS >= 2) umma_f16(d_tmem, a_row + LO16 + 2u * q, b_now + 2u * q, idesc, 1u);
-                            }
-                        }
-                        umma_commit(empty_bar(cur));
-                        if (ky0 + rows == p.kh) umma_commit(tmem_full_bar(acc));
-                        if (tracing && tr < 256) p.trace[2 * 256 + tr] = clock64();
-                        ++tr;
-                    }
-                }
-            } else
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-                const int acc = it & 1;
-                const uint32_t acc_phase = (uint32_t) (it >> 1) & 1u;
-                mbar_wait(tmem_empty_bar(acc), acc_phase ^ 1u);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t) (acc * 2 * RW_MAX_N);
-                uint64_t b_cat = bdesc0;
-                for (int ky = 0; ky < p.kh; ++ky, b_cat += b_ky) {
-                    if (!ready) mbar_wait(full_bar(stage), phase);
-                    tc_fence_after();
-                    UM_TRACE(1, tr);
-                    const uint64_t a0 = wdesc0 + (uint64_t) ((uint32_t) stage * (p.stage_bytes >> 4));
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) { // K step q lives in weight panel q / 4, columns 16 (q % 4) ..
-                        if (q < last_q && !no_mma) {
-                            const uint64_t bq = b_cat + (uint64_t) ((q >> 2) * b_panel + 2u * (q & 3));
-                            umma_f16(d_tmem, a0 + koff[q], bq, idesc_cat, (ky > 0 || q > 0) ? 1u : 0u);           // -> [hi.hi | hi.lo]
-                            if (TERMS >= 2) umma_f16(d_tmem, a0 + lo_off16 + koff[q], bq, idesc, 1u); // lo.hi onto the first block
-                        }
-                    }
-                    const uint64_t b_last = b_cat + (uint64_t) ((last_q >> 2) * b_panel + 2u * (last_q & 3));
-                    const int cur = stage;
-                    phase ^= (stage == RW_STAGES - 1) ? 1u : 0u;
-                    stage = stage == RW_STAGES - 1 ? 0 : stage + 1;
-                    ready = mbar_test_wait(full_bar(stage), phase); // look-ahead, overlaps with the MMAs already queued
-                    if (!no_mma) {
-                        umma_f16(d_tmem, a0 + koff_last, b_last, idesc_cat, (ky > 0 || last_q > 0) ? 1u : 0u);
-                        if (TERMS >= 2) umma_f16(d_tmem, a0 + lo_off16 + koff_last, b_last, idesc, 1u);
-                    }
-                    umma_commit(empty_bar(cur));
-                    if (ky == p.kh - 1) umma_commit(tmem_full_bar(acc));
-                    UM_TRACE(2, tr);
-                    ++tr;
-                }
-            }
-        }
-        __syncwarp();
-    } else {
-        // ---- epilogue: 8 warps, TMEM lane quarter = warp % 4, two interleaved sets of 16-column chunks (see epilogue_tile) ----
-        const int q    = warp & 3;
-        const int half = (warp - 2) >> 2;
-        const int row  = q * 32 + lane;
-        EpiArgs e;
-        // a 64-channel slab uses the swizzled map, a narrower one the dense map: the host encodes the right one into both slots
-        e.o_hi64 = &tmO_hi, e.o_lo64 = &tmO_lo, e.o_hiT = &tmO_hi, e.o_loT = &tmO_lo;
-        e.r_hi64 = e.r_lo64 = e.r_hiT = e.r_loT = &tmO_hi;
-        e.bias = p.bias, e.n_blk = p.n_blk, e.OC = p.OC, e.act = p.act, e.has_res = 0, e.rows_box = UM_BLOCK_M, e.alpha = p.alpha;
-        e.has_lo = TERMS >= 2;
-        e.stg = stg, e.res_bar = 0, e.bar_id = 1;
-        e.part_src = nullptr, e.part_splits = 0;
-        e.no_store = (p.ablate & 8) != 0;
-        e.two_stagings = p.stg_bufs == 2;
-        uint32_t res_phase = 0;
-        int it = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-            const int acc = it & 1;
-            const uint32_t acc_phase = (uint32_t) (it >> 1) & 1u;
-            const int xt = tile % p.tiles_x, oy = (tile / p.tiles_x) % p.OH, n = tile / (p.tiles_x * p.OH);
-            mbar_wait(tmem_full_bar(acc), acc_phase);
-            tc_fence_after();
-            if (warp == 2) UM_TRACE(3, it);
-            e.tmem_empty = tmem_empty_bar(acc);
-            e.trace = p.trace, e.trace_seq = it;
-            const uint32_t taddr = tmem_base + ((uint32_t) (q * 32) << 16) + (uint32_t) (acc * 2 * RW_MAX_N);
-            if (p.ablate & 1) {
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(e.tmem_empty);
-                continue;
-            }
-            e.stg = stg + (uint32_t) ((it & 1) & (p.stg_bufs - 1)) * UM_STG_BYTES;
-            epilogue_tile<RW_EPI_WARPS, TERMS>(e, taddr, 0, xt * UM_BLOCK_M, oy, n, row, half, warp == 2, lane, res_phase);
-            if (warp == 2) UM_TRACE(4, it);
-        }
-        epilogue_drain(warp == 2);
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) UM_TRACE(5, 3);
-    if (p.trace && threadIdx.x == 0) {
-        unsigned long long g;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
-        atomicMax(reinterpret_cast<unsigned long long*>(p.trace) + 5 * 256 + 9, g);
-        if (blockIdx.x == 0) p.trace[5 * 256 + 11] = (long long) g;
+    // ===================== consumers =====================
+    regs_alloc_232();
+    const int cw   = wg - 1;
+    const int row0 = 64 * cw + 16 * (warp & 3) + (lane >> 2);
+    const int q    = lane & 3;
+    EpiArgs e;
+    // a 64-channel slab uses the swizzled map, a narrower one the dense map: the host encodes the right one into both slots
+    e.o_hi64 = &tmO_hi, e.o_lo64 = &tmO_lo, e.o_hiT = &tmO_hi, e.o_loT = &tmO_lo;
+    e.r_hi64 = e.r_lo64 = e.r_hiT = e.r_loT = &tmO_hi;
+    e.bias = p.bias, e.OC = p.OC, e.act = p.act, e.has_res = 0, e.rows_box = UM_BLOCK_M, e.alpha = p.alpha;
+    e.has_lo = TERMS >= 2, e.stg = stg, e.res_bar = 0, e.issuer = threadIdx.x == 128;
+    uint32_t res_phase = 0;
+    mbar_wait(b_bar, 0);
+    // window descriptor of this warpgroup's 64 rows (64 pixels x 16 B further into the row segment)
+    const uint64_t wdesc0 = gmma_desc_window(sA0 + (uint32_t) cw * 64u * 16u), bdesc0 = gmma_desc_sw128(sB);
+    const uint32_t b_panel = (uint32_t) ((TERMS == 3 ? 2 : 1) * NB * 128) >> 4; // one [B_hi ; B_lo] (or single-plane) panel (64 K columns)
+    const uint32_t b_lo16  = B_PLANE >> 4;
+    const uint64_t lo16    = (uint64_t) (p.lo_off >> 4);
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[NB / 2], blk[NB / 2];
+    // one K=16 step of the product into the stage's fresh accumulator: A window at `a` (hi plane; lo plane at + alo), weights at `b`
+    auto kstep = [&](uint64_t a, uint64_t alo, uint64_t b, uint32_t accumulate) {
+        Wgmma<NB>::mma(blk, a, b, accumulate);
+        if (TERMS == 3) Wgmma<NB>::mma(blk, a, b + b_lo16, 1u);
+        if (TERMS >= 2) Wgmma<NB>::mma(blk, a + alo, b, 1u);
+    };
+    // the stage's wgmmas have retired: hand the stage back to the producer, add the stage's sum to the tile's
+    auto finish_stage = [&]() {
+        wg_commit();
+        wg_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar(stage));
+        acc_promote(acc, blk);
+        if (++stage == RW_STAGES) stage = 0, phase ^= 1u;
+    };
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int xt = tile % p.tiles_x, oy = (tile / p.tiles_x) % p.OH, n = tile / (p.tiles_x * p.OH);
+#pragma unroll
+        for (int i = 0; i < NB / 2; ++i) acc[i] = 0.0f;
+        if constexpr (FKS > 0) {
+            // K step q of a filter row = window start + 2 q pixel pairs (32 B), weight columns 16 q ..
+            constexpr int RPP     = FKS == 1 ? 4 : (FKS == 2 ? 2 : 1); // FeedPlan::rows_per_panel
+            const uint32_t row16  = p.row_bytes >> 4;
+            uint64_t b_cat        = bdesc0;
+            int b_sub             = 0;
+            for (int ky0 = 0; ky0 < p.kh; ky0 += p.rows_per_stage) {
+                const int rows = min(p.rows_per_stage, p.kh - ky0);
+                mbar_wait(full_bar(stage), phase);
+                uint64_t a_row = wdesc0 + (uint64_t) ((uint32_t) stage * (p.stage_bytes >> 4));
+                wg_fence();
+                for (int r = 0; r < rows; ++r, a_row += row16) {
+                    // weights of this filter row: the next K-column group of the same 128-byte rows, or the next panel
+                    const uint64_t b_now = b_cat;
+                    if (++b_sub == RPP) b_sub = 0, b_cat += b_panel - (RPP - 1) * (8 / RPP);
+                    else b_cat += 8 / RPP;
+#pragma unroll
+                    for (int k = 0; k < FKS; ++k) kstep(a_row + 2u * k, (uint64_t) (RW_ARR_BYTES >> 4), b_now + 2u * k, (r > 0 || k > 0) ? 1u : 0u);
+                }
+                finish_stage();
+            }
+        } else {
+            const uint32_t b_ky = b_panel * (uint32_t) p.panels; // one filter row
+            for (int ky = 0; ky < p.kh; ++ky) {
+                mbar_wait(full_bar(stage), phase);
+                const uint64_t a0 = wdesc0 + (uint64_t) ((uint32_t) stage * (p.stage_bytes >> 4));
+                const uint64_t bk = bdesc0 + (uint64_t) ((uint32_t) ky * b_ky);
+                wg_fence();
+#pragma unroll
+                for (int k = 0; k < 8; ++k) { // K step k: parity ks_parity[k], window offset ks_erel[k]; weight panel k / 4, columns 16 (k % 4) ..
+                    if (k < p.ksteps) {
+                        const uint32_t koff = ((uint32_t) p.ks_parity[k] * RW_ARR_BYTES + (uint32_t) p.ks_erel[k] * 16u) >> 4;
+                        kstep(a0 + koff, lo16, bk + (uint64_t) ((k >> 2) * b_panel + 2u * (k & 3)), k > 0 ? 1u : 0u);
+                    }
+                }
+                finish_stage();
+            }
+        }
+        epilogue_tile<NB>(e, acc, 0, xt * UM_BLOCK_M, oy, n, row0, q, res_phase);
     }
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 4 * RW_MAX_N);
-    }
+    epilogue_drain(e.issuer);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Host side: tile-shape selection, tensor maps, launch
 // ---------------------------------------------------------------------------------------------------------------
-// ---- SNNB_UMMA_TRACE: per-launch timeline of CTA 0 (eager mode only: synchronises around every launch) ----
-static bool trace_enabled() {
-    static const bool on = getenv("SNNB_UMMA_TRACE") != nullptr;
-    return on;
-}
-static int trace_begin(snnb_context* ctx, long long** out) {
-    static long long* d_trace = nullptr;
-    if (!d_trace) SNNB_CUDA_OK(cudaMalloc(&d_trace, 6 * 256 * sizeof(long long)));
-    SNNB_CUDA_OK(cudaMemsetAsync(d_trace, 0, 6 * 256 * sizeof(long long), ctx->stream));
-    const long long big = 0x7fffffffffffffffLL;
-    SNNB_CUDA_OK(cudaMemcpyAsync(d_trace + 5 * 256 + 8, &big, sizeof(big), cudaMemcpyHostToDevice, ctx->stream));
-    SNNB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
-    *out = d_trace;
-    return 0;
-}
-static int trace_end(snnb_context* ctx, const long long* d_trace, const char* header) {
-    std::vector<long long> h(6 * 256);
-    SNNB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
-    SNNB_CUDA_OK(cudaMemcpy(h.data(), d_trace, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-    const long long t0 = h[5 * 256];
-    fprintf(stderr, "TRACE %s\n", header);
-    fprintf(stderr, "  wallclock_ns   all-CTA span %lld | CTA0 entry +%lld exit +%lld\n", h[5 * 256 + 9] - h[5 * 256 + 8], h[5 * 256 + 10] - h[5 * 256 + 8],
-            h[5 * 256 + 11] - h[5 * 256 + 8]);
-    fprintf(stderr, "  epi_phases (start, +phase1, +wait_read, +barA, +STS, +fence, +barB, +store) per slab:");
-    for (int sq = 0; sq < 16 && h[4 * 256 + 64 + 8 * sq]; ++sq) {
-        fprintf(stderr, " [");
-        for (int k = 1; k < 8; ++k) fprintf(stderr, "%lld ", h[4 * 256 + 64 + 8 * sq + k] ? h[4 * 256 + 64 + 8 * sq + k] - h[4 * 256 + 64 + 8 * sq] : -1);
-        fprintf(stderr, "]");
-    }
-    fprintf(stderr, "\n");
-    h[4 * 256 + 64] = 0;
-    h[5 * 256 + 4]  = 0; // terminate the clock64 row before the wall-clock slots
-    const char* names[6] = {"prod_got_empty", "mma_got_full", "mma_issued", "epi_got_full", "epi_done", "entry_setup_proddone_alldone"};
-    for (int r = 0; r < 6; ++r) {
-        fprintf(stderr, "  %-14s", names[r]);
-        for (int i = 0; i < 256 && (h[r * 256 + i] || (r == 5 && i == 0)); ++i) fprintf(stderr, " %lld", h[r * 256 + i] - t0);
-        fprintf(stderr, "\n");
-    }
-    return 0;
-}
-
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
@@ -1548,11 +861,6 @@ static TilePlan plan_tiles(int N, int OH, int OW, int stride) {
     return best;
 }
 
-// Output-channel tile width and K split. Measured (profiles/r01_umma_timeline_trace.txt): a K block costs
-// max(bytes loaded / ~72 B per clk of L2->SM ingest, MMA issue ~310 clk at n_blk <= 64 / ~420 clk above) and a work item
-// another ~7 k clk of ramp-up + last epilogue. A layer takes rounds x that, rounds = ceil(work items / SMs). A narrower
-// n_blk re-reads A for more oc tiles but fills more SMs; splitting K (work item = tile x K range, fp32 partials reduced by
-// the last arriver, +~9 k clk) fills the GPU when a layer has few tiles and a long K (7x7x512: 128 tiles x 72 K blocks).
 // Stream-K split of `tiles` tiles of `num_kb` K blocks over `sms` CTAs: dp whole tiles (full waves), the K blocks of the rest (`units`)
 // in `ctas` equal ranges of at least a third of a tile each, so that no tile is cut into more than 4 pieces. False: nothing to cut.
 static bool streamk_split(long long tiles, int num_kb, int sms, int& dp, long long& units, int& ctas) {
@@ -1571,44 +879,38 @@ struct OcPlan {
     int sk = 0, sk_dp = 0, sk_ctas = 0;
     long long sk_units = 0;
 };
-// Tensor-pipe time of one M = 128 tcgen05.mma with N columns (tools/umma_microbench.cu: operand fetch from shared memory, A 4 KB +
-// B N x 32 B at 128 B/clk, bounds the narrow shapes): N <= 64: 48 clk, N = 128: 64, N = 256: 128.
-static double mma_clk(int n) { return std::max(48.0, n * 0.5); }
-static OcPlan plan_oc_ksplit(int OC, int m_tiles, int rows_used, int tile_w, int num_kb, int sm_count, int terms, bool halo = false, bool stream_k = false) {
+// Output-channel tile width (32, 64 or 128: one kernel instantiation each) and K split. Cost model of a launch, in SM clocks: a K
+// block costs the larger of its operand bytes over ~64 B/clk of L2 -> SM ingest and its tensor time (a Hopper SM retires 4096 dense
+// fp16 FLOP/clk: 4 x n_blk x terms clk for 128 rows x 64 K), a work item another ~7 k clk of ramp-up and epilogue, and a layer takes
+// rounds x that, rounds = ceil(work items / SMs). A narrower n_blk re-reads A for more oc tiles but fills more SMs; splitting K (work
+// item = tile x K range, fp32 partials reduced by the last arriver, +~9 k clk) fills the GPU when a layer has few tiles and a long K
+// (7x7x512: 128 tiles x 72 K blocks).
+static OcPlan plan_oc_ksplit(int OC, int m_tiles, int rows_used, int num_kb, int sm_count, int terms, bool stream_k) {
     OcPlan best;
     double best_cost = 1e300;
     static const int no_split = getenv("SNNB_NO_SPLITK") != nullptr;
-    const int max_n = terms == 3 ? UM_MAX_N : UM_MAX_N2;
-    const int t_min = (OC + max_n - 1) / max_n, t_max = (OC + 15) / 16;
-    for (int t = t_min; t <= t_max; ++t) {
-        const int blk = std::min(max_n, round_up((OC + t - 1) / t, 16));
-        if (blk * t < OC) continue;
-        // boxes narrower than 8 pixels (7x7 maps) move ~20 % fewer bytes per clock through the TMA unit (measured 59 vs 74-77 B/clk)
-        const double ingest  = tile_w < 8 ? 58.0 : 72.0;
-        // Measured K-block cadences (r02 traces, 3-term): plain 650 clk at n_blk 64 / 811-830 at 128 (the load ring keeps ~3 x 48-64 KB in
-        // flight: ~76 B/clk per SM), halo 630 / 890 (tensor-pipe time + ~125 clk: its weight ring runs only a few K blocks ahead). The
-        // halo mode therefore wins where the plain mode is ring-bound (n_blk 64) and loses a little where it is MMA-bound (n_blk 128).
+    static const int env_sk   = getenv("SNNB_SK") != nullptr;
+    for (int blk : {UM_MAX_N, 64, 32}) {
+        if (blk > 32 && blk / 2 >= OC) continue; // the next narrower tile already holds every channel
+        const int t          = (OC + blk - 1) / blk;
         const double a_bytes = (terms == 1 ? 1.0 : 2.0) * rows_used * 128.0, b_bytes = (terms == 3 ? 2.0 : 1.0) * blk * 128;
-        const double mma     = terms == 3 ? 4.0 * (mma_clk(2 * blk) + mma_clk(blk)) : 4.0 * terms * mma_clk(blk); // per 64-wide K block
-        const double kb_cost = halo ? mma + 125.0 : std::max((a_bytes + b_bytes) / (ingest * 1.05), mma + 45.0);
-        for (int sp = 1; sp <= ((no_split || halo) ? 1 : 4); ++sp) {
+        const double kb_cost = std::max((a_bytes + b_bytes) / 64.0, 4.0 * blk * terms + 40.0);
+        for (int sp = 1; sp <= (no_split ? 1 : 4); ++sp) {
             if (sp > 1 && (num_kb < 8 * sp)) break; // not worth a reduction for short K
-            const int kbps          = (num_kb + sp - 1) / sp;
+            const int kbps = (num_kb + sp - 1) / sp;
             if ((sp - 1) * kbps >= num_kb) continue; // an empty split
-            const long long items = (long long) m_tiles * t * sp;
+            const long long items  = (long long) m_tiles * t * sp;
             const long long rounds = (items + sm_count - 1) / sm_count;
             const double cost      = (double) rounds * (kbps * kb_cost + 7000.0 + (sp > 1 ? 9000.0 : 0.0));
             if (cost < best_cost * (sp > 1 ? 0.93 : 1.0) - 1e-9) // split only for a clear win
                 best_cost = cost, best.cost = cost, best.n_blk = blk, best.tiles_oc = t, best.ksplit = sp, best.kb_per_split = kbps, best.sk = 0;
         }
         // Stream-K: full waves of whole tiles, then the K blocks of the last partial wave's tiles shared evenly by all CTAs (each tile cut
-        // into at most 4 pieces, reduced by its last arriver) - instead of a last round that leaves most SMs idle.
-        // Opt-in (SNNB_ALGO_TCGEN05_STREAMK / SNNB_SK=1): on ResNet-18's 28x28 and 7x7 layers it measured 3-8 % SLOWER than whole tiles /
-        // uniform split-K - the partial dump, the arrival round trip and the last arriver's 3-4 x 64 KB reduction cost more than
-        // the idle SMs of the last wave (profiles/README.md).
-        static const int env_sk = getenv("SNNB_SK") != nullptr;
+        // into at most 4 pieces, reduced by its last arriver) - instead of a last round that leaves most SMs idle. Opt-in
+        // (SNNB_ALGO_TCGEN05_STREAMK / SNNB_SK=1): the partial dump, the arrival round trip and the last arriver's reduction can cost more
+        // than the idle SMs of the last wave.
         const long long tiles = (long long) m_tiles * t;
-        if ((stream_k || env_sk) && !no_split && !halo && num_kb >= 6 && tiles % sm_count != 0) {
+        if ((stream_k || env_sk) && !no_split && num_kb >= 6 && tiles % sm_count != 0) {
             int dp = 0, ctas = 0;
             long long units = 0;
             if (streamk_split(tiles, num_kb, sm_count, dp, units, ctas)) {
@@ -1619,7 +921,6 @@ static OcPlan plan_oc_ksplit(int OC, int m_tiles, int rows_used, int tile_w, int
                     best.sk_ctas = ctas, best.sk_units = units;
             }
         }
-        if (blk <= 16) break;
     }
     return best;
 }
@@ -1651,6 +952,8 @@ static int conv_terms(const snnb_context* ctx, const ConvArgs& a) {
     return prec == SNNB_PRECISION_FP16W ? 2 : (prec == SNNB_PRECISION_FP16 ? 1 : 3);
 }
 
+static int rowwin_nblk(int oc) { return oc <= 32 ? 32 : 64; }
+
 static bool feed_usable(const ConvArgs& a, FeedPlan& fp);
 static bool rowwin_supported(const ConvArgs& a) {
     // small-C stems: IC <= 8 (one 16-byte vector per pixel), stride 1 or 2, <= 8 K steps per filter row, weights packed
@@ -1661,7 +964,7 @@ static bool rowwin_supported(const ConvArgs& a) {
         return false;
     FeedPlan fp;
     const int wrows = feed_usable(a, fp) ? (a.k + fp.rows_per_panel - 1) / fp.rows_per_panel : a.k * ((rp.ksteps + 3) / 4); // 128-byte weight rows per channel
-    return wrows * 2 * round_up(a.out->c, 16) * 128 <= RW_B_MAX_BYTES;
+    return wrows * 2 * rowwin_nblk(a.out->c) * 128 <= RW_B_MAX_BYTES;
 }
 
 bool conv2d_umma_supported(const ConvArgs& a) {
@@ -1675,20 +978,46 @@ bool conv2d_umma_supported(const ConvArgs& a) {
     return true;
 }
 
-enum { ATTR_UMMA = 1u, ATTR_ROWWIN = 2u, ATTR_DW1 = 4u, ATTR_DW2 = 8u }; // bits of snnb_context::func_attr_mask
+// Bits of snnb_context::func_attr_mask (cudaFuncSetAttribute applies per device): one per kernel instantiation
+enum { ATTR_UMMA0 = 0, ATTR_ROWWIN0 = 18, ATTR_DW1 = 48, ATTR_DW2 = 49 };
+static int ensure_smem_attr(snnb_context* ctx, const void* kernel, int bit, int bytes) {
+    const uint64_t m = 1ull << bit;
+    if (!(ctx->func_attr_mask & m)) {
+        SNNB_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        ctx->func_attr_mask |= m;
+    }
+    return 0;
+}
+
+typedef void (*UmmaKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+                           const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const UmmaParams);
+struct UmmaChoice {
+    UmmaKernel kernel;
+    int smem, bit;
+};
+template <int TERMS, int NB> static UmmaChoice umma_choice_nb(bool sk, int nbi) {
+    return {sk ? conv_umma_kernel<TERMS, NB, true> : conv_umma_kernel<TERMS, NB, false>, UmGeom<TERMS, NB>::SMEM_BYTES, ATTR_UMMA0 + ((TERMS - 1) * 3 + nbi) * 2 + (sk ? 1 : 0)};
+}
+template <int TERMS> static UmmaChoice umma_choice_t(int nb, bool sk) {
+    return nb == 32 ? umma_choice_nb<TERMS, 32>(sk, 0) : (nb == 64 ? umma_choice_nb<TERMS, 64>(sk, 1) : umma_choice_nb<TERMS, 128>(sk, 2));
+}
+static UmmaChoice umma_choice(int terms, int nb, bool sk) { return terms == 3 ? umma_choice_t<3>(nb, sk) : (terms == 2 ? umma_choice_t<2>(nb, sk) : umma_choice_t<1>(nb, sk)); }
 
 typedef void (*RowWinKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
                              const CUtensorMap, const RowWinParams);
-template <int TERMS> static RowWinKernel rowwin_kernel_fks(int fks) {
+template <int TERMS, int NB> static RowWinKernel rowwin_kernel_fks(int fks) {
     switch (fks) {
-    case 1: return conv_rowwin_kernel<TERMS, 1>;
-    case 2: return conv_rowwin_kernel<TERMS, 2>;
-    case 3: return conv_rowwin_kernel<TERMS, 3>;
-    case 4: return conv_rowwin_kernel<TERMS, 4>;
-    default: return conv_rowwin_kernel<TERMS, 0>;
+    case 1: return conv_rowwin_kernel<TERMS, 1, NB>;
+    case 2: return conv_rowwin_kernel<TERMS, 2, NB>;
+    case 3: return conv_rowwin_kernel<TERMS, 3, NB>;
+    case 4: return conv_rowwin_kernel<TERMS, 4, NB>;
+    default: return conv_rowwin_kernel<TERMS, 0, NB>;
     }
 }
-static RowWinKernel rowwin_kernel_of(int terms, int fks) { return terms == 3 ? rowwin_kernel_fks<3>(fks) : (terms == 2 ? rowwin_kernel_fks<2>(fks) : rowwin_kernel_fks<1>(fks)); }
+template <int TERMS> static RowWinKernel rowwin_kernel_t(int fks, int nb) { return nb == 32 ? rowwin_kernel_fks<TERMS, 32>(fks) : rowwin_kernel_fks<TERMS, 64>(fks); }
+static RowWinKernel rowwin_kernel_of(int terms, int fks, int nb) {
+    return terms == 3 ? rowwin_kernel_t<3>(fks, nb) : (terms == 2 ? rowwin_kernel_t<2>(fks, nb) : rowwin_kernel_t<1>(fks, nb));
+}
 
 // FEED mode: the input tensor carries the compact 4-channel copy this layer's weights were packed for, and it is large enough
 static bool feed_usable(const ConvArgs& a, FeedPlan& fp) {
@@ -1714,33 +1043,28 @@ static int launch_conv2d_rowwin(snnb_context* ctx, const ConvArgs& a, EncodeTile
     }
     ctx->last_kernel = feed ? "conv_rowwin_kernel<feed>" : "conv_rowwin_kernel";
     RowWinParams p;
-    p.out_hi = out->hi, p.out_lo = out->lo, p.bias = a.w->bias;
+    p.bias = a.w->bias;
     p.N = out->n, p.OH = out->h, p.OW = out->w, p.OC = out->c, p.OCp = out->cp;
-    p.n_blk = round_up(out->c, 16), p.ocr = a.w->ocr;
+    p.n_blk = rowwin_nblk(out->c);
     p.kh = a.k, p.stride = a.stride, p.pad_y = a.pad_y;
     p.tiles_x  = (out->w + UM_BLOCK_M - 1) / UM_BLOCK_M;
     p.parities = rp.parities, p.dmin[0] = rp.dmin[0], p.dmin[1] = rp.dmin[1];
     p.ksteps   = rp.ksteps, p.panels = (rp.ksteps + 3) / 4;
     for (int q = 0; q < 8; ++q) p.ks_parity[q] = q < rp.ksteps ? rp.ks_parity[q] : 0, p.ks_erel[q] = q < rp.ksteps ? rp.ks_erel[q] : 0;
     p.act = a.act, p.alpha = a.alpha;
-    static const int rw_ablate = getenv("SNNB_UMMA_ABLATE") ? atoi(getenv("SNNB_UMMA_ABLATE")) : 0;
-    p.ablate                   = rw_ablate;
     p.feed_hi = in->feed_hi, p.feed_lo = in->feed_lo, p.feed_h = in->feed_h, p.feed_w = in->feed_w, p.feed_py = in->feed_py;
     p.feed_seg_bytes = feed ? (uint32_t) (254 + 2 * fp.nch) * 8u : 0u;
     const int terms = conv_terms(ctx, a);
     p.lo_off      = (uint32_t) p.parities * RW_ARR_BYTES;
     p.row_bytes   = (terms == 1 ? 1u : 2u) * p.lo_off;
     // feed mode: ceil(kh / 4) groups of filter rows, as even as possible (7 -> 4 + 3, 3 -> 3, 9 -> 3 + 3 + 3)
-    static const int one_row = getenv("SNNB_FEED_ONE_ROW") != nullptr;
-    p.rows_per_stage = (feed && !one_row) ? (a.k + (a.k + 3) / 4 - 1) / ((a.k + 3) / 4) : 1;
+    p.rows_per_stage = feed ? (a.k + (a.k + 3) / 4 - 1) / ((a.k + 3) / 4) : 1;
     p.stage_bytes    = (uint32_t) p.rows_per_stage * p.row_bytes;
     p.feed_prows  = feed ? (a.k + fp.rows_per_panel - 1) / fp.rows_per_panel : 0;
-    p.b_bytes     = (uint32_t) round_up((terms == 3 ? 2 : 1) * (feed ? p.feed_prows : a.k * p.panels) * p.n_blk * 128, 1024);
-    // a second staging buffer when the ring keeps >= 2 stages beside it (one slab per tile: n_blk <= 64 always holds here)
-    static const int one_stg = getenv("SNNB_ROWWIN_ONE_STAGING") != nullptr;
-    const int ring_room      = RW_SMEM_BYTES - 1024 - RW_BAR_BYTES - (int) p.b_bytes;
-    p.stg_bufs    = (!one_stg && (ring_room - 2 * UM_STG_BYTES) / (int) p.stage_bytes >= 2) ? 2 : 1;
-    p.stages      = std::min(RW_MAX_STAGES, (ring_room - p.stg_bufs * UM_STG_BYTES) / (int) p.stage_bytes);
+    const int vrows = feed ? p.feed_prows : a.k * p.panels; // 128-byte weight rows per output channel
+    p.b_bytes     = (uint32_t) round_up((terms == 3 ? 2 : 1) * vrows * p.n_blk * 128, 1024);
+    const int ring_room = RW_SMEM_BYTES - 1024 - RW_BAR_BYTES - (int) p.b_bytes - UM_STG_BYTES;
+    p.stages      = std::min(RW_MAX_STAGES, ring_room / (int) p.stage_bytes);
     SNNB_REQUIRE(p.stages >= 2, "launch_conv2d_rowwin: weight panels of %u bytes leave no room for the activation ring", p.b_bytes);
 
     // A: per plane and column parity a 4-D view (8 ch | de-interleaved pixel index | row | image) of the NHWC plane
@@ -1759,36 +1083,26 @@ static int launch_conv2d_rowwin(snnb_context* ctx, const ConvArgs& a, EncodeTile
             SNNB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(A, rowwin) failed: %d", (int) r);
         }
     {
-        const cuuint64_t dims[2]    = {64, (cuuint64_t) (feed ? (a.k + fp.rows_per_panel - 1) / fp.rows_per_panel : a.k * p.panels) * a.w->ocr}; // [ky][panel][OCr] rows of 64 K columns
-        const cuuint64_t strides[1] = {128};
-        const cuuint32_t box[2]     = {64, (cuuint32_t) p.n_blk};
-        const cuuint32_t estr[2]    = {1, 1};
+        // [weight row v][OCr][64 K columns]; a box of n_blk channel rows reads zeros past OCr
+        const cuuint64_t dims[3]    = {64, (cuuint64_t) a.w->ocr, (cuuint64_t) vrows};
+        const cuuint64_t strides[2] = {128, (cuuint64_t) a.w->ocr * 128};
+        const cuuint32_t box[3]     = {64, (cuuint32_t) p.n_blk, 1};
+        const cuuint32_t estr[3]    = {1, 1, 1};
         void* planes[2] = {(void*) (feed ? a.w->w_feed_hi : a.w->w_row_hi), (void*) (feed ? a.w->w_feed_lo : a.w->w_row_lo)}; // 2-term: the hi plane alone = fp16_rn(w)
         for (int i = 0; i < 2; ++i) {
-            CUresult r = encode(&tmB[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, planes[i], dims, strides, box, estr,
+            CUresult r = encode(&tmB[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, planes[i], dims, strides, box, estr,
                                 CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
             SNNB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(B, rowwin) failed: %d", (int) r);
         }
     }
     CUtensorMap tmO[2];
     if (encode_nhwc_box_maps(encode, out, p.n_blk, UM_BLOCK_M, 1, 1, p.n_blk == 64, tmO)) return 2;
-    if (!(ctx->func_attr_mask & ATTR_ROWWIN)) {
-        for (int t = 1; t <= 3; ++t)
-            for (int f = 0; f <= 4; ++f) SNNB_CUDA_OK(cudaFuncSetAttribute(rowwin_kernel_of(t, f), cudaFuncAttributeMaxDynamicSharedMemorySize, RW_SMEM_BYTES));
-        ctx->func_attr_mask |= ATTR_ROWWIN;
-    }
+    const int fks = feed ? fp.ksteps : 0;
+    auto* kern    = rowwin_kernel_of(terms, fks, p.n_blk);
+    if (ensure_smem_attr(ctx, (const void*) kern, ATTR_ROWWIN0 + ((terms - 1) * 5 + fks) * 2 + (p.n_blk == 64 ? 1 : 0), RW_SMEM_BYTES)) return 1;
     const int total_tiles = p.N * p.OH * p.tiles_x;
     const int grid        = std::min(total_tiles, ctx->sm_count);
-    p.trace = nullptr;
-    if (trace_enabled() && trace_begin(ctx, &p.trace)) return 1;
-    auto* kern = rowwin_kernel_of(terms, feed ? fp.ksteps : 0);
     const cudaError_t le = launch_k_pdl(kern, dim3(grid), dim3(RW_THREADS), RW_SMEM_BYTES, ctx->stream, tmA[0], tmA[1], tmA[2], tmA[3], tmB[0], tmB[1], tmO[0], tmO[1], p);
-    if (p.trace) {
-        char hdr[256];
-        snprintf(hdr, sizeof hdr, "rowwin%s k%d s%d IC%d OC%d out %dx%dx%d n_blk %d tiles %d grid %d kh %d ksteps %d terms %d", feed ? "<feed>" : "", a.k, a.stride, a.in->c,
-                 a.out->c, a.out->n, a.out->h, a.out->w, p.n_blk, total_tiles, grid, p.kh, p.ksteps, terms);
-        if (trace_end(ctx, p.trace, hdr)) return 1;
-    }
     cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
     if (e != cudaSuccess) {
         set_error("conv_rowwin_kernel launch failed: %s", cudaGetErrorString(e));
@@ -1806,8 +1120,6 @@ int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
     const snnb_tensor* in = a.in;
     snnb_tensor* out      = a.out;
     UmmaParams p;
-    p.out_hi = out->hi, p.out_lo = out->lo;
-    p.res_hi = a.residual ? a.residual->hi : nullptr, p.res_lo = a.residual ? a.residual->lo : nullptr;
     p.has_res = a.residual != nullptr;
     p.bias    = a.w->bias;
     p.N = out->n, p.OH = out->h, p.OW = out->w, p.OC = out->c, p.OCp = out->cp;
@@ -1819,38 +1131,11 @@ int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
     p.cblocks = (in->c + UM_BLOCK_K - 1) / UM_BLOCK_K;
     const int terms = conv_terms(ctx, a);
     p.has_lo        = out->lo != nullptr;
-    p.b_stages = 0, p.b_stage_bytes = 0;
-    OcPlan op       = plan_oc_ksplit(out->c, tp.tiles_x * tp.tiles_y * tp.tiles_n, p.rows_used, tp.tw, a.k * a.k * p.cblocks, ctx->sm_count, terms, false, a.stream_k);
-    // halo mode (3x3, stride 1): 8 x 16-pixel tiles whose nine taps share one halo load; taken when the cost model prefers it
-    // (fewer bytes per K block against the MMA rows lost where 8 / 16 do not divide the feature map)
-    static const bool no_halo = getenv("SNNB_NO_HALO") != nullptr;
-    bool halo                 = false;
-    if (!no_halo && a.k == 3 && a.stride == 1 && a.pad_x <= 1 && a.pad_y <= 1) {
-        const int hx = (out->w + HL_TW - 1) / HL_TW, hy = (out->h + HL_TH - 1) / HL_TH;
-        const OcPlan hp = plan_oc_ksplit(out->c, hx * hy * out->n, UM_BLOCK_M, HL_TW, 9 * p.cblocks, ctx->sm_count, terms, true);
-        if (hp.n_blk > 0 && hp.cost < op.cost) {
-            halo = true, op = hp;
-            p.b_stage_bytes = (terms == 3 ? 2 : 1) * op.n_blk * 128 <= UM_B_BYTES ? UM_B_BYTES : 2 * UM_B_BYTES; // 16 KB when a stage fits, else 32 KB
-            p.b_stages      = HL_B_RING_BYTES / p.b_stage_bytes;
-            p.tw = HL_TW, p.th = HL_TH, p.tn = 1, p.rows_used = UM_BLOCK_M;
-            p.tiles_x = hx, p.tiles_y = hy, p.tiles_n = out->n;
-        }
-    }
+    const OcPlan op = plan_oc_ksplit(out->c, tp.tiles_x * tp.tiles_y * tp.tiles_n, p.rows_used, a.k * a.k * p.cblocks, ctx->sm_count, terms, a.stream_k);
     SNNB_REQUIRE(op.n_blk > 0, "launch_conv2d_umma: no output-channel plan");
     p.n_blk = op.n_blk, p.tiles_oc = op.tiles_oc, p.ksplit = op.ksplit, p.kb_per_split = op.kb_per_split;
-    p.sk = halo ? 0 : op.sk, p.sk_dp = op.sk_dp, p.sk_ctas = op.sk_ctas, p.sk_units = op.sk_units;
+    p.sk = op.sk, p.sk_dp = op.sk_dp, p.sk_ctas = op.sk_ctas, p.sk_units = op.sk_units;
     p.partials = nullptr, p.counters = nullptr;
-    if (!ctx->sched_counter) { // created by the first (eager) launch; graph capture replays use the same word
-        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-        SNNB_CUDA_OK(cudaStreamIsCapturing(ctx->stream, &cap));
-        SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone, "launch_conv2d_umma: the scheduler counter must be allocated by an eager pass before graph capture");
-        void* pnew = nullptr;
-        SNNB_CUDA_OK(cudaMalloc(&pnew, 256));
-        SNNB_CUDA_OK(cudaMemset(pnew, 0, 256));
-        ctx->scratch_blocks.push_back(pnew);
-        ctx->sched_counter = static_cast<int*>(pnew);
-    }
-    p.sched_counter = ctx->sched_counter;
     if (p.ksplit > 1 || p.sk) {
         // partial-tile slots: split-K [tile][split]; stream-K [tile past sk_dp][4 pieces]
         const size_t tiles = p.sk ? (size_t) p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_oc - p.sk_dp : (size_t) p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_oc;
@@ -1864,15 +1149,13 @@ int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
     }
     p.ICp     = round_up(in->c, 8);
     p.act = a.act, p.alpha = a.alpha;
-    static const int ablate = getenv("SNNB_UMMA_ABLATE") ? atoi(getenv("SNNB_UMMA_ABLATE")) : 0;
-    p.ablate                = ablate;
     SNNB_REQUIRE(a.w->kp == a.k * a.k * p.ICp, "launch_conv2d_umma: packed weights do not match (kp %d vs %d)", a.w->kp, a.k * a.k * p.ICp);
 
     CUtensorMap tmA[2], tmB[2];
     {
         const cuuint64_t dims[4]    = {(cuuint64_t) in->c, (cuuint64_t) in->w, (cuuint64_t) in->h, (cuuint64_t) in->n};
         const cuuint64_t strides[3] = {(cuuint64_t) in->cp * 2, (cuuint64_t) in->w * in->cp * 2, (cuuint64_t) in->h * in->w * in->cp * 2};
-        const cuuint32_t box[4]     = {(cuuint32_t) UM_BLOCK_K, (cuuint32_t) (halo ? HL_W : p.tw * a.stride), (cuuint32_t) (halo ? HL_H : p.th * a.stride), (cuuint32_t) p.tn};
+        const cuuint32_t box[4]     = {(cuuint32_t) UM_BLOCK_K, (cuuint32_t) (p.tw * a.stride), (cuuint32_t) (p.th * a.stride), (cuuint32_t) p.tn};
         const cuuint32_t estr[4]    = {1, (cuuint32_t) a.stride, (cuuint32_t) a.stride, 1};
         __half* planes[2]    = {in->hi, in->lo ? in->lo : in->hi}; // fp16 storage mode: the lo map is never issued
         for (int i = 0; i < 2; ++i) {
@@ -1894,7 +1177,7 @@ int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
             SNNB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(B) failed: %d (kp %d ocr %d n_blk %d)", (int) r, a.w->kp, a.w->ocr, p.n_blk);
         }
     }
-    // epilogue maps: full 64-channel slabs (swizzled) and the tail slab (n_blk % 64 channels, dense)
+    // epilogue maps: full 64-channel slabs (swizzled) and the narrow slab of a 32-channel tile (dense)
     CUtensorMap tmO64[2], tmOT[2], tmR64[2], tmRT[2];
     {
         const int wT = p.n_blk % 64;
@@ -1904,48 +1187,13 @@ int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
         if (encode_nhwc_box_maps(encode, res, p.n_blk >= 64 ? 64 : wT, p.tw, p.th, p.tn, p.n_blk >= 64, tmR64)) return 2;
         if (encode_nhwc_box_maps(encode, res, wT ? wT : 64, p.tw, p.th, p.tn, wT == 0, tmRT)) return 2;
     }
-    if (!(ctx->func_attr_mask & ATTR_UMMA)) {
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES, false, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES, false, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES, false, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES - 1, true, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES_SPLIT));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES - 1, true, 2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES_SPLIT));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES - 1, true, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES_SPLIT));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<HL_B_STAGES, false, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HL_SMEM_BYTES));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<HL_B_STAGES, false, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HL_SMEM_BYTES));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<HL_B_STAGES, false, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, HL_SMEM_BYTES));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES, false, 1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES, false, 2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES));
-        SNNB_CUDA_OK(cudaFuncSetAttribute(conv_umma_kernel<UM_STAGES, false, 3, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, UM_SMEM_BYTES));
-        ctx->func_attr_mask |= ATTR_UMMA;
-    }
+    const UmmaChoice kc = umma_choice(terms, p.n_blk, p.sk != 0);
+    if (ensure_smem_attr(ctx, (const void*) kc.kernel, kc.bit, kc.smem)) return 1;
     const int total_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_oc;
     const int grid        = p.sk ? (p.sk_dp > 0 ? ctx->sm_count : p.sk_ctas) : std::min(total_tiles * p.ksplit, ctx->sm_count);
-    // short K loop (1x1 convolutions): the layer runs at the speed of the epilogue -> two independent epilogue groups
-    static const bool no_split_epi = getenv("SNNB_NO_SPLIT_EPI") != nullptr;
-    const bool split_epi           = !halo && !no_split_epi && !p.sk && p.ksplit == 1 && p.ksize * p.ksize * p.cblocks <= 3 && total_tiles >= 2 * grid;
-    ctx->last_kernel = halo ? "conv_umma_kernel<halo>"
-                            : (split_epi ? "conv_umma_kernel<short-K>" : (p.sk ? "conv_umma_kernel<stream-K>" : (p.ksplit > 1 ? "conv_umma_kernel<split-K>" : "conv_umma_kernel")));
-    p.trace = nullptr;
-    if (trace_enabled() && trace_begin(ctx, &p.trace)) return 1;
-    auto* k_split = terms == 3 ? conv_umma_kernel<UM_STAGES - 1, true, 3, false> : (terms == 2 ? conv_umma_kernel<UM_STAGES - 1, true, 2, false> : conv_umma_kernel<UM_STAGES - 1, true, 1, false>);
-    auto* k_plain = p.sk ? (terms == 3 ? conv_umma_kernel<UM_STAGES, false, 3, false, true>
-                                       : (terms == 2 ? conv_umma_kernel<UM_STAGES, false, 2, false, true> : conv_umma_kernel<UM_STAGES, false, 1, false, true>) )
-                         : (terms == 3 ? conv_umma_kernel<UM_STAGES, false, 3, false> : (terms == 2 ? conv_umma_kernel<UM_STAGES, false, 2, false> : conv_umma_kernel<UM_STAGES, false, 1, false>) );
-    auto* k_halo  = terms == 3 ? conv_umma_kernel<HL_B_STAGES, false, 3, true> : (terms == 2 ? conv_umma_kernel<HL_B_STAGES, false, 2, true> : conv_umma_kernel<HL_B_STAGES, false, 1, true>);
-    const cudaError_t le =
-        halo      ? launch_k_pdl(k_halo, dim3(grid), dim3(UM_THREADS), HL_SMEM_BYTES, ctx->stream, tmA[0], tmA[1], tmB[0], tmB[1], tmO64[0], tmO64[1], tmOT[0], tmOT[1], tmR64[0],
-                                 tmR64[1], tmRT[0], tmRT[1], p)
-        : split_epi ? launch_k_pdl(k_split, dim3(grid), dim3(UM_THREADS), UM_SMEM_BYTES_SPLIT, ctx->stream, tmA[0], tmA[1], tmB[0], tmB[1], tmO64[0], tmO64[1], tmOT[0], tmOT[1],
-                                 tmR64[0], tmR64[1], tmRT[0], tmRT[1], p)
-                  : launch_k_pdl(k_plain, dim3(grid), dim3(UM_THREADS), UM_SMEM_BYTES, ctx->stream, tmA[0], tmA[1], tmB[0], tmB[1], tmO64[0], tmO64[1], tmOT[0], tmOT[1], tmR64[0],
-                                 tmR64[1], tmRT[0], tmRT[1], p);
-    if (p.trace) {
-        char hdr[256];
-        snprintf(hdr, sizeof hdr, "conv k%d s%d IC%d OC%d out %dx%dx%d n_blk %d tiles %d grid %d num_kb %d ksplit %d terms %d halo %d", a.k, a.stride, in->c, out->c, out->n,
-                 out->h, out->w, p.n_blk, total_tiles, grid, p.ksize * p.ksize * p.cblocks, split_epi ? -1 : (p.sk ? -2 : p.ksplit), terms, (int) halo); // ksplit -1 = split-epilogue variant, -2 = stream-K
-        if (trace_end(ctx, p.trace, hdr)) return 1;
-    }
+    ctx->last_kernel = p.sk ? "conv_umma_kernel<stream-K>" : (p.ksplit > 1 ? "conv_umma_kernel<split-K>" : "conv_umma_kernel");
+    const cudaError_t le = launch_k_pdl(kc.kernel, dim3(grid), dim3(UM_THREADS), kc.smem, ctx->stream, tmA[0], tmA[1], tmB[0], tmB[1], tmO64[0], tmO64[1], tmOT[0], tmOT[1],
+                                        tmR64[0], tmR64[1], tmRT[0], tmRT[1], p);
     cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
     if (e != cudaSuccess) {
         set_error("conv_umma_kernel launch failed: %s", cudaGetErrorString(e));
@@ -1954,7 +1202,6 @@ int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
     ctx->launches++;
     return 0;
 }
-
 
 // ---------------------------------------------------------------------------------------------------------------
 // Depthwise 3x3 (stride 1 / 2), TMA-staged + register-tiled (shadertemplate_vk_depthwise.comp:64-139).
@@ -2163,11 +1410,7 @@ template <int S> static int launch_depthwise_tma_s(snnb_context* ctx, const Conv
             SNNB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(depthwise input) failed: %d", (int) r);
         }
     }
-    const uint32_t attr_bit = S == 1 ? ATTR_DW1 : ATTR_DW2;
-    if (!(ctx->func_attr_mask & attr_bit)) {
-        SNNB_CUDA_OK(cudaFuncSetAttribute(depthwise_tma_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, T::SMEM_BYTES));
-        ctx->func_attr_mask |= attr_bit;
-    }
+    if (ensure_smem_attr(ctx, (const void*) depthwise_tma_kernel<S>, S == 1 ? ATTR_DW1 : ATTR_DW2, T::SMEM_BYTES)) return 1;
     const long long total = (long long) p.N * p.tiles_y * p.tiles_x * p.chunks;
     const int grid        = (int) std::min<long long>(total, 2 * ctx->sm_count); // two CTAs per SM (128 registers, <= 93 KB of shared memory each)
     const cudaError_t le  = launch_k_pdl(depthwise_tma_kernel<S>, dim3(grid), dim3(DW_THREADS), T::SMEM_BYTES, ctx->stream, tmI[0], tmI[1], p);

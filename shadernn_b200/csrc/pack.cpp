@@ -55,7 +55,7 @@ void pack_conv2d_host(int IC, int OC, int k, const float* w_oihw, const float* b
     std::vector<float> scale, shift;
     bn_fold(OC, bias, g, b, m, v, scale, shift);
     const int K = k * k * IC;
-    // tcgen05 operand: row = oc, column = tap*ICp + ic with ICp = round_up(IC, 8), so that every tap starts on a
+    // tensor-core operand: row = oc, column = tap*ICp + ic with ICp = round_up(IC, 8), so that every tap starts on a
     // 16-byte boundary (TMA box start) and the padding columns are zero.
     const int ICp = round_up(IC, 8);
     out.ocw     = round_up(OC, 64);
@@ -64,7 +64,7 @@ void pack_conv2d_host(int IC, int OC, int k, const float* w_oihw, const float* b
     out.w_f32.assign((size_t) K * out.ocw, 0.0f);
     out.w_hi.assign((size_t) out.ocr * out.kp, __float2half_rn(0.0f));
     out.w_lo.assign((size_t) out.ocr * out.kp, __float2half_rn(0.0f));
-    out.bias.assign(out.ocw + 320, 0.0f); // zero tail: the tcgen05 epilogue reads float4s up to tiles_oc * n_blk (n_blk <= 256)
+    out.bias.assign(out.ocw + 320, 0.0f); // zero tail past the folded bias
     for (int o = 0; o < OC; ++o) {
         out.bias[o] = shift[o];
         for (int i = 0; i < IC; ++i)

@@ -38,8 +38,8 @@ const char* get_error();
 static inline int round_up(int v, int m) { return (v + m - 1) / m * m; }
 
 // ---- programmatic dependent launch (PDL) -----------------------------------------------------------------------
-// The persistent TMA / tcgen05 kernels are launched with cudaLaunchAttributeProgrammaticStreamSerialization: their CTAs may
-// be scheduled (and run their prologue: barrier init, TMEM allocation, tensor-map prefetch) while the previous kernel is
+// The persistent TMA / tensor-core kernels are launched with cudaLaunchAttributeProgrammaticStreamSerialization: their CTAs may
+// be scheduled (and run their prologue: barrier init, tensor-map prefetch) while the previous kernel is
 // still draining. pdl_wait() blocks until the previous grid has completed and its writes are visible; NOTHING before it
 // may touch global memory that another kernel writes. pdl_trigger() lets the next grid start launching. ONLY the persistent
 // kernels (grid <= SM count, every CTA resident from the start) call it, first thing: in a multi-wave kernel the early
@@ -69,7 +69,7 @@ template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
     return launch_k_impl(false, kernel, grid, block, smem, stream, std::forward<Args>(args)...);
 }
-// programmatic dependent launch (the persistent TMA / tcgen05 kernels, which call pdl_trigger() and pdl_wait())
+// programmatic dependent launch (the persistent TMA / tensor-core kernels, which call pdl_trigger() and pdl_wait())
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
     return launch_k_impl(true, kernel, grid, block, smem, stream, std::forward<Args>(args)...);
@@ -82,12 +82,12 @@ inline cudaError_t launch_k_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block,
 // Activations: NHWC, channel pitch Cp = round_up(C, 8), stored as TWO fp16 planes ("split-fp16"):
 //     hi = fp16_rn(v),  lo = fp16_rn(v - hi)          (v = hi + lo to 2^-22 relative for |v| >= 2^-3; absolute 3e-8 below)
 // Same 4 bytes/element of HBM traffic as fp32, but each plane is a K-major fp16 operand that TMA can drop into shared
-// memory for tcgen05.mma (kind::f16) unmodified. Products accumulate in fp32 TMEM as
-//     3-term  hi*Whi + lo*Whi + hi*Wlo   (weights as fp16 pairs too: ~22 bits per operand)          SNNB_PRECISION_FP32X3
+// memory for wgmma (fp16 operands) unmodified. Products accumulate in fp32 registers as
+//     3-term  hi*Whi + hi*Wlo + lo*Whi   (weights as fp16 pairs too: ~22 bits per operand)          SNNB_PRECISION_FP32X3
 //     2-term  hi*Whi + lo*Whi            (weights rounded once to fp16: <= 2^-12 relative per weight)  SNNB_PRECISION_FP16W
 //     1-term  hi*Whi                     (half-precision storage mode: no lo planes at all)           SNNB_PRECISION_FP16->FP16
-// Round 1 stored bf16 pairs (8+8 bits); tcgen05's kind::f16 refuses a bf16 A with an fp16 B operand ("illegal instruction",
-// tools/umma_desc_probe.cu), so the pair format itself moved to fp16 to make the 2-term product possible. Range: values are
+// Both operands of one tensor-core instruction must have the same type, so the pair is fp16 rather than bf16: that is what makes
+// the 2-term product (fp16 weights) possible. Range: values are
 // saturated to +-65504 on store (cvt.rn.satfinite), the same range as the reference's own RGBA16F mode.
 // Channels [C, Cp) are kept at zero.
 struct snnb_tensor {
@@ -118,7 +118,7 @@ struct snnb_weights {
     // SIMT path: fp32 [K = k*k*IC][OCw], OCw = round_up(OC, 64); BN folded in.
     float* w_f32 = nullptr;
     int ocw = 0;
-    // tcgen05 path: fp16 hi/lo [OCr][Kp] K-major (k index = (ky*k+kx)*IC + ic), Kp = round_up(K, 8), OCr = round_up(OC, 16).
+    // tensor-core path: fp16 hi/lo [OCr][Kp] K-major (k index = (ky*k+kx)*IC + ic), Kp = round_up(K, 8), OCr = round_up(OC, 16).
     __half* w_hi = nullptr;
     __half* w_lo = nullptr;
     int kp = 0, ocr = 0;
@@ -154,10 +154,9 @@ struct snnb_context {
     size_t splitk_bytes    = 0;
     int* splitk_counters   = nullptr;
     size_t splitk_counter_n = 0;
-    int* sched_counter      = nullptr; // dynamic tile scheduler of conv_umma_kernel (self-resetting)
     // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) applies to the CURRENT device only: one bit per kernel, per context
     // (= per device), not a process-wide flag
-    uint32_t func_attr_mask = 0;
+    uint64_t func_attr_mask = 0;
     const char* last_kernel = nullptr; // name of the kernel the most recent launcher chose (snnb_model_layer_kernel, bench.py's roofline)
     int precision = SNNB_PRECISION_FP32X3; // default product form of per-operator convolution launches (snnb_context_set_precision)
     std::vector<void*> scratch_blocks;
@@ -190,7 +189,7 @@ struct ConvArgs {
     bool stream_k = false; // the planner may choose the stream-K decomposition (SNNB_ALGO_TCGEN05_STREAMK)
 };
 int launch_conv2d_simt(snnb_context* ctx, const ConvArgs& a);
-int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a); // kernels_umma.cu (tcgen05 + TMA)
+int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a); // kernels_umma.cu (wgmma + TMA)
 bool conv2d_umma_supported(const ConvArgs& a);
 int streamk_schedule(int tiles, int num_kb, int sms, int* rows, int capacity); // host evaluation of the stream-K work decomposition (tests)
 int launch_depthwise(snnb_context* ctx, const ConvArgs& a);
@@ -227,7 +226,7 @@ int launch_merge_u8(snnb_context* ctx, const snnb_tensor* t, uint8_t* dev_nhwc_u
 // ---- host-side weight folding/packing (pack.cpp) -----------------------------------------------------------
 // K ordering of the row-window convolution kernel (kernels_umma.cu): for stride s the taps of one filter row fall
 // into s column parities; within a parity consecutive taps read consecutive pixels of the de-interleaved row, so one
-// tcgen05.mma K step (16 fp16 = 2 pixels x 8 channels) covers two taps of the same parity.
+// wgmma K step (16 fp16 = 2 pixels x 8 channels) covers two taps of the same parity.
 struct RowPlan {
     int parities = 0;
     int dmin[2]  = {0, 0}; // pixel offset (in de-interleaved index) of the first tap of each parity, relative to the output index

@@ -1,14 +1,14 @@
-"""Generator of tests/golden/candy_head_golden.npz — run in the container that has /root/reference:
+"""Generator of tests/golden/candy_head_golden.npz — run where a checkout of the reference exists:
 
-    python tests/golden/make_candy_golden.py
+    python tests/golden/make_candy_golden.py <reference checkout>/modelzoo/StyleTransfer/candy-9_simplified.onnx
 
-The only real-weight model in the reference checkout is modelzoo/StyleTransfer/candy-9_simplified.onnx. It cannot travel to
-the GPU box, so this script freezes (a) the initialisers of its first two stages (reflect-pad + 9x9 conv 3->32 + InstanceNorm +
+The only real-weight model in the reference checkout is modelzoo/StyleTransfer/candy-9_simplified.onnx. At 6.7 MB it is not
+part of this repository, so this script freezes (a) the initialisers of its first two stages (reflect-pad + 9x9 conv 3->32 + InstanceNorm +
 ReLU; reflect-pad + 3x3 stride-2 conv 32->64 + InstanceNorm + ReLU: ~105 KB of fp32), (b) a 64x64 input in the model's own
 range [0, 255], and (c) what torch computes for those ONNX nodes (shadernn_b200/onnx2snn.torch_eval on the truncated graph,
 i.e. the ONNX semantics themselves, no conversion involved). tests/ rebuild the SNN model from (a) with the converter and
-hold the oracle and the CUDA engine to (c). When /root/reference is present, __graft_entry__.build() also converts the WHOLE
-model into tests/golden/_ref_models/ (git-ignored, travels to the GPU box) with a full-size golden output beside it.
+hold the oracle and the CUDA engine to (c). With SNNB_REFERENCE set to a reference checkout, __graft_entry__.build() also converts
+the WHOLE model into tests/golden/_ref_models/ (git-ignored) with a full-size golden output beside it (full_model below).
 """
 import os
 import sys
@@ -19,7 +19,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)
 sys.path.insert(0, ROOT)
 from shadernn_b200 import modelzoo, onnx2snn  # noqa: E402
 
-SRC = "/root/reference/modelzoo/StyleTransfer/candy-9_simplified.onnx"
 HEAD_NODES = 8  # Pad Conv IN Relu Pad Conv IN Relu
 
 
@@ -29,8 +28,8 @@ def truncated(g, n_nodes):
     return {"nodes": nodes, "init": {k: v for k, v in g["init"].items() if k in used}, "inputs": g["inputs"], "outputs": [(nodes[-1]["output"][0], [])]}
 
 
-def main():
-    g = onnx2snn.load_onnx(SRC)
+def main(src):
+    g = onnx2snn.load_onnx(src)
     head = truncated(g, HEAD_NODES)
     x = modelzoo.synthetic_input("candy", 1, (64, 64))
     y = onnx2snn.torch_eval(head, x)
@@ -42,15 +41,15 @@ def main():
     print(path, os.path.getsize(path), "bytes; output", y.shape, "max", float(np.abs(y).max()))
 
 
-def full_model(out_dir, hw=(224, 224)):
+def full_model(src, out_dir, hw=(224, 224)):
     """Whole-model conversion + golden output (torch on the ONNX graph) for the GPU tests; returns the JSON path."""
     os.makedirs(out_dir, exist_ok=True)
-    g = onnx2snn.load_onnx(SRC)
-    path, _ = onnx2snn.convert(SRC, out_dir, input_hw=hw)
+    g = onnx2snn.load_onnx(src)
+    path, _ = onnx2snn.convert(src, out_dir, input_hw=hw)
     x = modelzoo.synthetic_input("candy", 1, hw)
     np.savez_compressed(os.path.join(out_dir, "candy_full_golden.npz"), x=x, y=onnx2snn.torch_eval(g, x))
     return path
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

@@ -1,8 +1,8 @@
 """Generate tests/golden/ref_cpu_golden.npz from the REFERENCE ITSELF (oracle/_ref/libsnn_ref.so = the reference's
-core/src/ic2/cpulayer.h + demo/common/prng.h compiled where they lie under /root/reference).
+core/src/ic2/cpulayer.h + demo/common/prng.h compiled where they lie in a checkout of the reference).
 
-/root/reference does not exist on the GPU box, so the outputs are committed here as a small fixture and this script is
-the recipe that produced them:   make -C oracle ref && python tests/golden/make_golden.py
+The reference is not part of this repository, so the outputs are committed here as a small fixture and this script is
+the recipe that produced them:   make -C oracle ref REF=<reference checkout> && python tests/golden/make_golden.py
 """
 import ctypes as C
 import os
@@ -17,7 +17,7 @@ from oracle import oracle  # noqa: E402
 
 def main():
     r = oracle.ref()
-    assert r is not None, "build oracle/_ref first (needs /root/reference)"
+    assert r is not None, "build oracle/_ref first (needs a reference checkout)"
     out = {}
     # --- prng.h: seed 7767517 (convolutionTest.cpp:417) ---
     r.ref_srand(C.c_uint64(7767517))

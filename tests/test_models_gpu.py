@@ -305,7 +305,7 @@ REF_MODELS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", 
 
 
 @pytest.mark.skipif(not os.path.exists(os.path.join(REF_MODELS, "candy-9_simplified_layers.json")),
-                    reason="tests/golden/_ref_models/ is generated by __graft_entry__.build() where /root/reference exists (and travels with the snapshot)")
+                    reason="tests/golden/_ref_models/ is generated by __graft_entry__.build() when SNNB_REFERENCE names a reference checkout")
 @pytest.mark.parametrize("precision", ["fp32x3", "fp16w"])
 def test_real_candy_whole_model_vs_torch_and_oracle(ctx, precision):
     # the WHOLE real-weight model (converted from the reference's ONNX file by build()): final image against torch's evaluation
@@ -618,7 +618,7 @@ def test_stem_feed_mode_shapes(ctx, tmp_path, h, w, c, k, oc, padding, prepad):
 
 
 def test_repeated_loads_and_first_launches(ctx, model_dir):
-    # Regression test of a start-up race of the halo convolution (pre-issued weight stages waited for after the MMA thread had released
+    # Regression test of start-up races of the persistent convolution kernels (a first version waited for pre-issued weight stages the MMA side had released
     # them): it only showed on FIRST launches, when the producer warp was slow (cold instruction cache) - so load, run once, drop, repeat.
     path, _ = modelzoo.build("resnet18", model_dir, input_hw=(224, 224))
     x = modelzoo.synthetic_input("resnet18", 32, (224, 224))

@@ -1,4 +1,4 @@
-"""GPU parity tests for the tcgen05 + TMA implicit-GEMM convolution (kernels_umma.cu), forced with algo="tcgen05",
+"""GPU parity tests for the wgmma + TMA implicit-GEMM convolution (kernels_umma.cu), forced with algo="tcgen05" (the API name of that path),
 against the oracle — and against the CUDA-core kernel on the same inputs, which isolates the 3-term split-bf16 product.
 Shapes are the tensor-path layers of the BASELINE graphs (ResNet-18 3x3s, MobileNetV2 1x1 expand/project,
 YOLOv3-tiny 13x13 / heads) plus ragged edges: tiles that overhang the image, channel tails that are not multiples of
@@ -158,14 +158,14 @@ def test_stride2_tma_traversal_stride(ctx, k, ic, oc, h):
     (1, 13, 13, 1024, 512, 1, False, "leakyRelu"),  # long-K 1x1 (YOLO head): 16 K blocks
 ])
 def test_split_k(ctx, n, h, w, ic, oc, k, residual, act):
-    # layers with too few output tiles for 148 SMs: K is split over several CTAs, fp32 partials are reduced by the last
+    # layers with too few output tiles for 132 SMs: K is split over several CTAs, fp32 partials are reduced by the last
     # arriver in split order. Run twice: the second launch checks that the arrival counters were left at zero.
     run_case(ctx, n, h, w, ic, oc, k, act=act, residual=residual, seed=ic + h)
     run_case(ctx, n, h, w, ic, oc, k, act=act, residual=residual, seed=ic + h + 1)
 
 
 @pytest.mark.parametrize("n,h,w,ic,oc,k,s,residual", [
-    (32, 28, 28, 128, 128, 3, 1, True),   # 196 tiles on 148 SMs: one whole wave + 48 tiles cut into K-block ranges
+    (32, 28, 28, 128, 128, 3, 1, True),   # 196 tiles on 132 SMs: one whole wave + 64 tiles cut into K-block ranges
     (32, 14, 14, 256, 256, 3, 1, False),  # fewer tiles than SMs: every tile cut
     (8, 7, 7, 512, 512, 3, 1, True),      # long K, few tiles
     (5, 33, 21, 64, 96, 3, 2, False),     # ragged
