@@ -290,6 +290,14 @@ int snnb_debug_streamk_schedule(int tiles, int num_kb, int sms, int* rows, int c
  * ksteps (K = 16 steps per filter row), rows_per_panel (filter rows sharing one 128-byte weight row)}. Returns 1 if the layer can use
  * the feed mode, 0 if not. No GPU needed. */
 int snnb_debug_feed_plan(int k, int stride, int pad_x, int ic, int out[5]);
+/* Diagnostics: how a convolution would be run, decided on the host exactly as the engine and snnb_conv2d_launch decide it.
+ * query = {in_h, in_w, in_c, out_h, out_w, out_c, k, stride, pad_x, pad_y, pad_mode, residual (0/1), algo (SNNB_ALGO_*),
+ * may_prepad (0/1: a pre-padded copy of the input may be allocated), may_feed (0/1: the input is a model input that may carry the
+ * compact feed copy), row_stride, row_pad (the weights' row-window operand; row_stride 0 = none), feed_pad (the weights' feed
+ * operand; -1 = none)}. out = {path (0 refused, 1 CUDA cores, 2 implicit GEMM, 3 row window, 4 row window on the feed copy),
+ * pad_x, pad_y, pad_mode (what the kernel sees), prepad_h, prepad_w (0 = no pre-padded copy), feed_h, feed_w, feed_py, feed_px
+ * (0 = no feed copy)}. Returns 0. No GPU needed. */
+int snnb_debug_conv_plan(const int query[18], int out[10]);
 
 #ifdef __cplusplus
 }

@@ -19,6 +19,7 @@ SOURCES = [
     "kernels_simt.cu",
     "kernels_umma.cu",
     "pack.cpp",
+    "conv_plan.cpp",
     "capi.cpp",
     "engine/modelparser.cpp",
     "engine/layers.cpp",

@@ -147,6 +147,18 @@ int snnb_debug_feed_plan(int k, int stride, int pad_x, int ic, int out[5]) {
     out[0] = fp.px, out[1] = fp.d, out[2] = fp.nch, out[3] = fp.ksteps, out[4] = fp.rows_per_panel;
     return 1;
 }
+int snnb_debug_conv_plan(const int query[18], int out[10]) {
+    SNNB_REQUIRE(query && out, "snnb_debug_conv_plan: null argument");
+    ConvQuery q;
+    q.in_h = query[0], q.in_w = query[1], q.in_c = query[2], q.out_h = query[3], q.out_w = query[4], q.out_c = query[5];
+    q.k = query[6], q.stride = query[7], q.pad_x = query[8], q.pad_y = query[9], q.pad_mode = query[10];
+    q.residual = query[11] != 0, q.algo = query[12], q.may_prepad = query[13] != 0, q.may_feed = query[14] != 0;
+    q.row_stride = query[15], q.row_pad = query[16], q.feed_pad = query[17];
+    const ConvPlan p = plan_conv(q);
+    const int v[10] = {p.path, p.pad_x, p.pad_y, p.pad_mode, p.prepad_h, p.prepad_w, p.feed_h, p.feed_w, p.feed_py, p.feed_px};
+    for (int i = 0; i < 10; ++i) out[i] = v[i];
+    return 0;
+}
 int snnb_debug_streamk_schedule(int tiles, int num_kb, int sms, int* rows, int capacity) {
     SNNB_REQUIRE(rows || capacity == 0, "snnb_debug_streamk_schedule: null buffer");
     return streamk_schedule(tiles, num_kb, sms, rows, capacity);
@@ -293,15 +305,14 @@ int snnb_conv2d_launch(snnb_context* ctx, const snnb_conv_desc* d, const snnb_we
                  in->c, out->c, d->kernel, w->in_ch, w->out_ch, w->kernel);
     SNNB_REQUIRE(in->n == out->n, "snnb_conv2d_launch: batch mismatch");
     if (residual) CHECK_DIMS_EQ(residual, out, "snnb_conv2d_launch(residual)");
+    ConvQuery q;
+    q.in_h = in->h, q.in_w = in->w, q.in_c = in->c, q.out_h = out->h, q.out_w = out->w, q.out_c = out->c;
+    q.k = d->kernel, q.stride = d->stride, q.pad_x = d->pad_x, q.pad_y = d->pad_y, q.pad_mode = d->pad_mode;
+    q.residual = residual != nullptr, q.algo = d->algo;
+    q.row_stride = w->row_stride, q.row_pad = w->row_pad, q.feed_pad = w->feed_pad;
     ConvArgs a {in, residual, out, w, d->kernel, d->stride, d->pad_x, d->pad_y, d->pad_mode, d->activation, d->leaky_alpha};
     a.stream_k = d->algo == SNNB_ALGO_TCGEN05_STREAMK;
-    if (d->algo == SNNB_ALGO_TCGEN05 || d->algo == SNNB_ALGO_TCGEN05_STREAMK) {
-        SNNB_REQUIRE(conv2d_umma_supported(a), "snnb_conv2d_launch: the tensor-core path does not support this shape (IC=%d OC=%d k=%d s=%d pad_mode=%d)", in->c, out->c,
-                     d->kernel, d->stride, d->pad_mode);
-        return launch_conv2d_umma(ctx, a);
-    }
-    if (d->algo == SNNB_ALGO_AUTO && conv2d_umma_supported(a)) return launch_conv2d_umma(ctx, a);
-    return launch_conv2d_simt(ctx, a);
+    return launch_conv2d(ctx, a, plan_conv(q));
 }
 int snnb_depthwise_launch(snnb_context* ctx, const snnb_conv_desc* d, const snnb_weights* w, const snnb_tensor* in, snnb_tensor* out) {
     SNNB_REQUIRE(ctx && d && w && in && out, "snnb_depthwise_launch: null argument");
@@ -351,17 +362,9 @@ int snnb_dense_launch(snnb_context* ctx, const snnb_weights* w, int act, float a
     SNNB_REQUIRE(ctx && w && in && out && (w->kind == 3 || w->kind == 1), "snnb_dense_launch: bad argument");
     SNNB_REQUIRE(in->h * in->w * in->c == w->in_ch && out->c == w->out_ch && out->h == 1 && out->w == 1 && in->n == out->n,
                  "snnb_dense_launch: dims do not match the weights (%d -> %d)", w->in_ch, w->out_ch);
-    snnb_tensor* flat   = nullptr;
-    const snnb_tensor* x = in;
-    if (in->h * in->w != 1) {
-        if (tensor_alloc(ctx, in->n, 1, 1, w->in_ch, &flat)) return 1;
-        if (launch_flatten(ctx, in, flat)) return 1;
-        x = flat;
-    }
-    const bool softmax = act == SNNB_ACT_SOFTMAX;
-    ConvArgs a {x, nullptr, out, w, 1, 1, 0, 0, SNNB_PAD_NONE, softmax ? SNNB_ACT_NONE : act, alpha};
-    int rc = conv2d_umma_supported(a) ? launch_conv2d_umma(ctx, a) : launch_conv2d_simt(ctx, a);
-    if (!rc && softmax) rc = launch_softmax(ctx, out, out);
+    snnb_tensor* flat = nullptr;
+    if (in->h * in->w != 1 && tensor_alloc(ctx, in->n, 1, 1, w->in_ch, &flat)) return 1;
+    const int rc = launch_dense(ctx, in, flat, out, w, act, alpha, -1);
     if (flat) {
         cudaStreamSynchronize(ctx->stream);
         snnb_tensor_free(flat);

@@ -198,48 +198,21 @@ bool MixedInferenceCore::init(std::string& err) {
         }
         for (size_t k = 0; k < nin; ++k) L->inputs.push_back(outOf.at(resolve(L->prevLayers[k])));
         if (L->typeName == "Conv2D") {
-            auto* cl  = static_cast<Conv2DLayer*>(L);
-            cl->algo = options.convAlgo;
-            // weights are not packed yet: probe with a weights stub that says "tensor path available"
-            int ph = 0, pw = 0;
-            snnb_weights probe_w;
-            probe_w.w_hi = probe_w.w_lo = reinterpret_cast<__half*>(1);
-            // ... and the row-window operand a pre-padded small-channel stem will be packed with (stride, pad 0; packWeights)
-            probe_w.w_row_hi = probe_w.w_row_lo = reinterpret_cast<__half*>(1);
-            probe_w.row_stride = (int) cl->_desc.stride, probe_w.row_pad = 0;
-            std::swap(cl->weights, probe_w);
-            const bool prepad = cl->wantsPrepad(L->inputs[0], L->output, options.convAlgo, ph, pw);
-            std::swap(cl->weights, probe_w);
-            if (prepad) {
-                if (tensor_alloc(ctx, N, ph, pw, L->inputs[0]->c, &cl->prepadded, twoPlanes)) {
+            auto* cl = static_cast<Conv2DLayer*>(L);
+            static const bool noFeed = getenv("SNNB_NO_FEED") != nullptr;
+            snnb_tensor* in          = L->inputs[0];
+            cl->plan(options.convAlgo, !noFeed && resolve(L->prevLayers[0])->isInputLayer && !in->feed_hi); // the first stem reading an input gets its feed
+            const ConvPlan& p = cl->convPlan;
+            if (p.prepad_h) {
+                if (tensor_alloc(ctx, N, p.prepad_h, p.prepad_w, in->c, &cl->prepadded, twoPlanes)) {
                     err = get_error();
                     return false;
                 }
                 ownedTensors.push_back(cl->prepadded);
             }
-            // a stride-2 RGB stem fed straight by a model input: give that input tensor the compact 4-channel copy (feed mode)
-            {
-                static const bool noFeed = getenv("SNNB_NO_FEED") != nullptr;
-                GenericModelLayer* src   = resolve(L->prevLayers[0]);
-                snnb_tensor* in          = L->inputs[0];
-                const int mode           = padModeId(cl->_desc.padding.mode);
-                uint32_t offs[4];
-                cl->_desc.padding.offsets((int) cl->_desc.kernelSize, true, offs);
-                const int k = (int) cl->_desc.kernelSize, padX = (int) offs[0], padY = (int) offs[2];
-                FeedPlan fp;
-                if (!noFeed && !prepad && src->isInputLayer && !in->feed_hi && options.convAlgo != SNNB_ALGO_SIMT && !L->residual && L->output->c <= 64 &&
-                    (mode == SNNB_PAD_NONE || mode == SNNB_PAD_CONSTANT) && make_feed_plan(k, (int) cl->_desc.stride, padX, in->c, fp)) {
-                    const int tilesX = (L->output->w + 127) / 128;
-                    const int needW  = 2 * (tilesX * 128 - 1) + 2 * fp.nch;          // last pixel a tile's window segment touches + 1
-                    const int needH  = 2 * (L->output->h - 1) + k - padY + padY;      // last input row + 1, shifted by feed_py = padY
-                    const int feedW  = (std::max(in->w + fp.px, needW) + 1) & ~1;
-                    const int feedH  = std::max(in->h + padY, needH);
-                    if (tensor_alloc_feed(in, feedH, feedW, padY, fp.px)) {
-                        err = get_error();
-                        return false;
-                    }
-                    cl->feedInput = true;
-                }
+            if (p.path == CONV_ROWWIN_FEED && tensor_alloc_feed(in, p.feed_h, p.feed_w, p.feed_py, p.feed_px)) {
+                err = get_error();
+                return false;
             }
         }
         if (L->typeName == "Dense") {
@@ -311,7 +284,7 @@ bool MixedInferenceCore::init(std::string& err) {
             const bool reads = std::find(L->inputs.begin(), L->inputs.end(), t) != L->inputs.end() || L->residual == t;
             if (!reads) continue;
             ++readers;
-            only = only && L->typeName == "Conv2D" && static_cast<Conv2DLayer*>(L)->feedInput && L->inputs.size() >= 1 && L->inputs[0] == t && L->residual != t &&
+            only = only && L->typeName == "Conv2D" && static_cast<Conv2DLayer*>(L)->convPlan.path == CONV_ROWWIN_FEED && L->inputs.size() >= 1 && L->inputs[0] == t && L->residual != t &&
                    std::count(L->inputs.begin(), L->inputs.end(), t) == 1;
         }
         for (auto* o : outputLayers) only = only && o->output != t; // a model that returns its input
@@ -427,7 +400,7 @@ bool MixedInferenceCore::init(std::string& err) {
 
 int MixedInferenceCore::enqueueForward(bool) {
     ExecOptions eo;
-    eo.convAlgo = options.convAlgo, eo.precision = options.precision;
+    eo.precision = options.precision;
     // SNNB_SYNC_LAYERS: debugging aid - wait for every layer and name the one whose kernel faulted (eager passes only)
     static const bool syncLayers = getenv("SNNB_SYNC_LAYERS") != nullptr;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -661,7 +634,7 @@ int MixedInferenceCore::timeLayers(std::vector<float>& ms) {
     std::vector<cudaEvent_t> ev(graph.sorted.size() + 1);
     for (auto& e : ev) SNNB_CUDA_OK(cudaEventCreate(&e));
     ExecOptions eo;
-    eo.convAlgo = options.convAlgo, eo.precision = options.precision;
+    eo.precision = options.precision;
     SNNB_CUDA_OK(cudaEventRecord(ev[0], ctx->stream));
     layerKernels.assign(layers.size(), std::string());
     for (size_t i = 0; i < graph.sorted.size(); ++i) {

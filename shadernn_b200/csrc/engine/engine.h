@@ -168,14 +168,15 @@ struct Conv2DDesc : GenericConvDesc {
 class Conv2DLayer : public GenericModelLayer {
 public:
     Conv2DDesc _desc;
-    int algo = SNNB_ALGO_AUTO;
+    // How this layer runs (made once at load by plan(); packWeights and run follow it)
+    snnb::ConvQuery query;
+    snnb::ConvPlan convPlan;
     // Replicate / reflect padding on the tensor path: the TMA unit can only zero-fill, so the engine materialises the
-    // padded input once (pad kernel, vk_pad.comp semantics) and runs the tensor-core kernel over it with zero padding.
+    // padded input (pad kernel, vk_pad.comp semantics) and runs the tensor-core kernel over it with zero padding.
     snnb_tensor* prepadded = nullptr;
-    // Stride-2 stem with <= 4 input channels reading a model input: the input tensor carries a compact 4-channel copy
-    // (snnb_tensor::feed_hi) and the weights get the matching K order (FeedPlan, kernels_umma.cu conv_rowwin_kernel feed mode).
-    bool feedInput = false;
-    bool wantsPrepad(const snnb_tensor* in, const snnb_tensor* out, int convAlgo, int& ph, int& pw) const;
+    // Plans the layer once its input, output and residual tensors are known. mayFeed: the input is a model input that may carry
+    // the compact 4-channel feed copy (snnb_tensor::feed_hi).
+    void plan(int convAlgo, bool mayFeed);
     Transform getOutputScaleDimAdjustment() const override; // conv2d.cpp:102-113
     void getOutputDims(uint32_t& w, uint32_t& h, uint32_t& d) const override;
     void packWeights(snnb::PackedHost& p) override;
@@ -311,7 +312,6 @@ struct ShaderGenOptions { // layeroption.h:27-48, trimmed to what a CUDA backend
     int precision              = SNNB_PRECISION_FP32X3; // layeroption.h:43 preferrHalfPrecision <-> SNNB_PRECISION_FP16
 };
 struct ExecOptions {
-    int convAlgo  = SNNB_ALGO_AUTO;
     int precision = SNNB_PRECISION_FP32X3;
 };
 

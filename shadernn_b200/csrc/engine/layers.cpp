@@ -66,65 +66,45 @@ static const float* bnv(const std::map<std::string, std::vector<float>>& bn, con
     auto it = bn.find(key);
     return (it == bn.end() || it->second.empty()) ? nullptr : it->second.data();
 }
+void Conv2DLayer::plan(int convAlgo, bool mayFeed) {
+    uint32_t offs[4];
+    _desc.padding.offsets((int) _desc.kernelSize, true, offs);
+    const int k = (int) _desc.kernelSize;
+    query = ConvQuery();
+    query.in_h = inputs[0]->h, query.in_w = inputs[0]->w, query.in_c = inputs[0]->c;
+    query.out_h = output->h, query.out_w = output->w, query.out_c = output->c;
+    query.k = k, query.stride = (int) _desc.stride;
+    // uPadx <- offsets[0] (top), uPady <- offsets[2] (left): conv2dVulkan.cpp:183-184 (SURVEY Q5). The 1x1 shader has no padding.
+    query.pad_x = k == 1 ? 0 : (int) offs[0];
+    query.pad_y = k == 1 ? 0 : (int) offs[2];
+    query.pad_mode = padModeId(_desc.padding.mode);
+    query.residual = residual != nullptr;
+    query.algo = convAlgo == SNNB_ALGO_TCGEN05_STREAMK ? SNNB_ALGO_AUTO : convAlgo; // the engine never requests the stream-K decomposition
+    query.may_prepad = true, query.may_feed = mayFeed;
+    // packWeights packs by this plan: the row-window operand for the pad the kernel sees (0 on the pre-padded copy of a replicate /
+    // reflect convolution), the feed operand for pad_x when the plan reads the feed
+    const bool zeroPad = query.pad_mode == SNNB_PAD_NONE || query.pad_mode == SNNB_PAD_CONSTANT;
+    query.row_stride = query.stride, query.row_pad = zeroPad ? query.pad_x : 0, query.feed_pad = query.pad_x;
+    convPlan = plan_conv(query);
+}
 void Conv2DLayer::packWeights(PackedHost& p) {
     const auto& bn = _desc.batchNormalization;
     const bool use = _desc.useBatchNormalization;
     pack_conv2d_host((int) numInputPlanes, (int) numOutputPlanes, (int) _desc.kernelSize, _desc.weights.data(), _desc.biases.empty() ? nullptr : _desc.biases.data(),
                      use ? bnv(bn, "gamma") : nullptr, use ? bnv(bn, "beta") : nullptr, use ? bnv(bn, "movingMean") : nullptr,
                      use ? bnv(bn, "movingVariance") : nullptr, p);
-    {
-        uint32_t offs[4];
-        _desc.padding.offsets((int) _desc.kernelSize, true, offs);
-        const int mode = padModeId(_desc.padding.mode);
-        // reflect / replicate convolutions run on a pre-padded copy of the input with pad 0 (wantsPrepad)
-        if (mode == SNNB_PAD_NONE || mode == SNNB_PAD_CONSTANT) {
-            pack_rowwin_host(p, (int) _desc.stride, _desc.kernelSize == 1 ? 0 : (int) offs[0]);
-            if (feedInput) pack_feed_host(p, (int) _desc.stride, _desc.kernelSize == 1 ? 0 : (int) offs[0]);
-        } else {
-            pack_rowwin_host(p, (int) _desc.stride, 0);
-        }
-    }
+    pack_rowwin_host(p, query.row_stride, query.row_pad);
+    if (convPlan.path == CONV_ROWWIN_FEED) pack_feed_host(p, query.stride, query.feed_pad);
     std::vector<float>().swap(_desc.weights); // host copy no longer needed
-}
-bool Conv2DLayer::wantsPrepad(const snnb_tensor* in, const snnb_tensor* out, int convAlgo, int& ph, int& pw) const {
-    const int mode = padModeId(_desc.padding.mode);
-    if (!(mode == SNNB_PAD_REPLICATE || mode == SNNB_PAD_REFLECT) || _desc.kernelSize <= 1 || convAlgo == SNNB_ALGO_SIMT) return false;
-    ConvArgs probe {in, nullptr, const_cast<snnb_tensor*>(out), &weights, (int) _desc.kernelSize, (int) _desc.stride, 0, 0, SNNB_PAD_CONSTANT, 0, 0.0f};
-    if (!conv2d_umma_supported(probe)) return false;
-    // the window of the last output pixel ends at (O-1)*s + k - 1 in padded coordinates
-    ph = (out->h - 1) * (int) _desc.stride + (int) _desc.kernelSize;
-    pw = (out->w - 1) * (int) _desc.stride + (int) _desc.kernelSize;
-    return true;
 }
 
 int Conv2DLayer::run(snnb_context* ctx, const ExecOptions& opt) {
-    uint32_t offs[4];
-    _desc.padding.offsets((int) _desc.kernelSize, true, offs);
-    if (prepadded) {
-        // padded[y][x] = in[reflect/replicate(y - pad_y)][..(x - pad_x)] with the conv's own (pad_x, pad_y) = (T, L) mapping
-        if (launch_pad(ctx, inputs[0], prepadded, (int) offs[0], (int) offs[2], padModeId(_desc.padding.mode))) return 1;
-        ConvArgs a {prepadded, residual, output, &weights, (int) _desc.kernelSize, (int) _desc.stride, 0, 0, SNNB_PAD_CONSTANT,
-                    fusedAct >= 0 ? fusedAct : _desc.activation.id, fusedAct >= 0 ? fusedAlpha : _desc.activation.alpha};
-        a.precision = opt.precision;
-        return launch_conv2d_umma(ctx, a);
-    }
-    ConvArgs a;
-    a.in = inputs[0], a.residual = residual, a.out = output, a.w = &weights;
-    a.k = (int) _desc.kernelSize, a.stride = (int) _desc.stride;
-    // uPadx <- offsets[0] (top), uPady <- offsets[2] (left): conv2dVulkan.cpp:183-184 (SURVEY Q5). The 1x1 shader has no padding.
-    a.pad_x = _desc.kernelSize == 1 ? 0 : (int) offs[0];
-    a.pad_y = _desc.kernelSize == 1 ? 0 : (int) offs[2];
-    a.pad_mode = padModeId(_desc.padding.mode);
-    a.act      = fusedAct >= 0 ? fusedAct : _desc.activation.id;
-    a.alpha    = fusedAct >= 0 ? fusedAlpha : _desc.activation.alpha;
+    // padded[y][x] = in[reflect/replicate(y - pad_y)][..(x - pad_x)] with the conv's own (pad_x, pad_y) = (T, L) mapping
+    if (prepadded && launch_pad(ctx, inputs[0], prepadded, query.pad_x, query.pad_y, query.pad_mode)) return 1;
+    ConvArgs a {prepadded ? prepadded : inputs[0], residual, output, &weights, query.k, query.stride, convPlan.pad_x, convPlan.pad_y, convPlan.pad_mode,
+                fusedAct >= 0 ? fusedAct : _desc.activation.id, fusedAct >= 0 ? fusedAlpha : _desc.activation.alpha};
     a.precision = opt.precision;
-    const int want = algo != SNNB_ALGO_AUTO ? algo : opt.convAlgo;
-    if (want != SNNB_ALGO_SIMT && conv2d_umma_supported(a)) return launch_conv2d_umma(ctx, a);
-    if (want == SNNB_ALGO_TCGEN05) {
-        set_error("%s: tensor-core path requested but unsupported for this shape", name.c_str());
-        return 2;
-    }
-    return launch_conv2d_simt(ctx, a);
+    return launch_conv2d(ctx, a, convPlan);
 }
 
 // ---- Depthwise -------------------------------------------------------------------------------------------
@@ -210,18 +190,7 @@ int DenseLayer::run(snnb_context* ctx, const ExecOptions& opt) {
     if (gapSource && gapSource->output && gap_dense_supported(gapSource->output, output, &weights))
         return launch_gap_dense(ctx, gapSource->output, output, &weights, activation.id == SNNB_ACT_SOFTMAX ? SNNB_ACT_NONE : activation.id, activation.alpha,
                                 activation.id == SNNB_ACT_SOFTMAX);
-    const snnb_tensor* x = inputs[0];
-    if (x->h * x->w != 1) { // CPU Flatten order = HWC (cpulayer.h:94-115)
-        if (launch_flatten(ctx, x, flat)) return 1;
-        x = flat;
-    }
-    const bool softmax = activation.id == SNNB_ACT_SOFTMAX;
-    ConvArgs a {x, nullptr, output, &weights, 1, 1, 0, 0, SNNB_PAD_NONE, softmax ? SNNB_ACT_NONE : activation.id, activation.alpha};
-    a.precision = opt.precision;
-    // SiLU on the CPU Dense path is a by-value no-op in the reference (cpulayer.h:245-252); we apply the real SiLU (SURVEY Q10).
-    if (conv2d_umma_supported(a) ? launch_conv2d_umma(ctx, a) : launch_conv2d_simt(ctx, a)) return 1;
-    if (softmax) return launch_softmax(ctx, output, output);
-    return 0;
+    return launch_dense(ctx, inputs[0], flat, output, &weights, activation.id, activation.alpha, opt.precision);
 }
 void FlattenLayer::getOutputDims(uint32_t& w, uint32_t& h, uint32_t& d) const {
     w = h = 1;

@@ -135,16 +135,6 @@ struct TV { // kernel-side tensor view
 static TV view(const snnb_tensor* t) { return TV {t->hi, t->lo, t->n, t->h, t->w, t->c, t->cp}; }
 static FeedV feed_view(const snnb_tensor* t) { return FeedV {t->feed_hi, t->feed_lo, t->feed_h, t->feed_w, t->feed_py, t->feed_px, t->feed_only ? 1 : 0}; }
 
-#define SNNB_LAUNCH_CHECK(ctx)                                                                          \
-    do {                                                                                                \
-        cudaError_t _e = cudaGetLastError();                                                            \
-        if (_e != cudaSuccess) {                                                                        \
-            set_error("%s:%d: kernel launch failed: %s", __FILE__, __LINE__, cudaGetErrorString(_e));   \
-            return 1;                                                                                   \
-        }                                                                                               \
-        (ctx)->launches++;                                                                              \
-    } while (0)
-
 // ------------------------------------------------------------------------------------------------------------
 // Conv2D, fp32 CUDA-core implicit GEMM (shadertemplate_vk_conv2d.comp:148-347; 1x1: vk_conv2d_1x1.comp:68-211).
 //   M = N*OH*OW pixels, Ngemm = OC, K = k*k*IC with k index = (ky*k + kx)*IC + ic.
@@ -297,9 +287,7 @@ int launch_conv2d_simt(snnb_context* ctx, const ConvArgs& a) {
     p.K  = a.k * a.k * a.in->c;
     const long long M = (long long) a.out->n * a.out->h * a.out->w;
     dim3 grid((unsigned) ((M + CV_BM - 1) / CV_BM), (unsigned) ((a.out->cp + CV_BN - 1) / CV_BN));
-    launch_k(conv2d_simt_kernel, dim3(grid), dim3(128), 0, ctx->stream, p);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(conv2d_simt_kernel, dim3(grid), dim3(128), 0, ctx->stream, p), "conv2d_simt_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -436,16 +424,11 @@ int launch_depthwise(snnb_context* ctx, const ConvArgs& a) {
         const int strips      = (a.out->w + TX - 1) / TX;
         const long long total = (long long) a.out->n * a.out->h * strips * CG;
         const unsigned blocks = (unsigned) ((total + 127) / 128);
-        if (a.stride == 1)
-            launch_k(depthwise_kernel<3, 1, TX>, dim3(blocks), dim3(128), 0, ctx->stream, p);
-        else
-            launch_k(depthwise_kernel<3, 2, TX>, dim3(blocks), dim3(128), 0, ctx->stream, p);
-    } else {
-        const long long total = (long long) a.out->n * a.out->h * a.out->w * CG;
-        launch_k(depthwise_generic_kernel, dim3((unsigned) ((total + 127) / 128)), dim3(128), 0, ctx->stream, p);
+        if (a.stride == 1) return launch_done(ctx, launch_k(depthwise_kernel<3, 1, TX>, dim3(blocks), dim3(128), 0, ctx->stream, p), "depthwise_kernel");
+        return launch_done(ctx, launch_k(depthwise_kernel<3, 2, TX>, dim3(blocks), dim3(128), 0, ctx->stream, p), "depthwise_kernel");
     }
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    const long long total = (long long) a.out->n * a.out->h * a.out->w * CG;
+    return launch_done(ctx, launch_k(depthwise_generic_kernel, dim3((unsigned) ((total + 127) / 128)), dim3(128), 0, ctx->stream, p), "depthwise_generic_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -677,10 +660,8 @@ int launch_gap_dense(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out,
     const int parts   = gap_dense_parts(in, out);
     SNNB_REQUIRE(parts > 0, "launch_gap_dense: the head does not fit in shared memory");
     const size_t smem = (size_t) (parts * in->cp + (GD_THREADS / 32 + 1) * out->cp) * sizeof(float);
-    launch_k(gap_dense_kernel, dim3((unsigned) in->n), dim3(GD_THREADS), smem, ctx->stream, view(in), view(out), (const float*) w->w_f32, w->ocw, (const float*) w->bias, act, alpha,
-             softmax ? 1 : 0, parts);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(gap_dense_kernel, dim3((unsigned) in->n), dim3(GD_THREADS), smem, ctx->stream, view(in), view(out), (const float*) w->w_f32, w->ocw, (const float*) w->bias, act, alpha,
+             softmax ? 1 : 0, parts), "gap_dense_kernel");
 }
 
 int launch_pool(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, int k, int stride, bool avg) {
@@ -688,16 +669,15 @@ int launch_pool(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, int 
     TV vi = view(in), vo = view(out);
     if (avg && out->h == 1 && out->w == 1 && k >= in->h && k >= in->w && in->h * in->w >= 16) {
         const long long warps = (long long) in->n * (out->cp >> 3);
-        launch_k(global_avgpool_kernel, dim3((unsigned) ((warps * 32 + 255) / 256)), dim3(256), 0, ctx->stream, vi, vo);
-    } else {
-        const long long total = (long long) out->n * out->h * out->w * (out->cp >> 3);
-        const dim3 grid((unsigned) ((total + 255) / 256));
-        if (k == 2) launch_k(pool_kernel<2>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
-        else if (k == 3) launch_k(pool_kernel<3>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
-        else launch_k(pool_kernel<0>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
+        return launch_done(ctx, launch_k(global_avgpool_kernel, dim3((unsigned) ((warps * 32 + 255) / 256)), dim3(256), 0, ctx->stream, vi, vo), "global_avgpool_kernel");
     }
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    const long long total = (long long) out->n * out->h * out->w * (out->cp >> 3);
+    const dim3 grid((unsigned) ((total + 255) / 256));
+    cudaError_t e;
+    if (k == 2) e = launch_k(pool_kernel<2>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
+    else if (k == 3) e = launch_k(pool_kernel<3>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
+    else e = launch_k(pool_kernel<0>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
+    return launch_done(ctx, e, "pool_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -748,19 +728,13 @@ static unsigned vec_blocks(const snnb_tensor* t, int threads) {
 
 int launch_add(snnb_context* ctx, const snnb_tensor* a, const snnb_tensor* b, snnb_tensor* out, int act, float alpha) {
     ctx->last_kernel = "add_kernel";
-    launch_k(add_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(a), view(b), view(out), act, alpha);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(add_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(a), view(b), view(out), act, alpha), "add_kernel");
 }
 int launch_batchnorm(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, const snnb_weights* w, int act, float alpha) {
-    launch_k(chanwise_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), w->var /* = BN scale, see pack.cpp */, w->mean, w->beta, 0, act, alpha);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(chanwise_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), w->var /* = BN scale, see pack.cpp */, w->mean, w->beta, 0, act, alpha), "chanwise_kernel");
 }
 int launch_activation(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, int act, float alpha) {
-    launch_k(chanwise_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), nullptr, nullptr, nullptr, 1, act, alpha);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(chanwise_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), nullptr, nullptr, nullptr, 1, act, alpha), "chanwise_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -786,9 +760,7 @@ __global__ void __launch_bounds__(128) softmax_kernel(TV in, TV out) {
 }
 int launch_softmax(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out) {
     const long long px = (long long) in->pixels();
-    launch_k(softmax_kernel, dim3((unsigned) ((px * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), view(out));
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(softmax_kernel, dim3((unsigned) ((px * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), view(out)), "softmax_kernel");
 }
 
 __global__ void __launch_bounds__(128) argmax_kernel(TV in, int* __restrict__ idx) {
@@ -835,14 +807,10 @@ __global__ void __launch_bounds__(128) result_small_kernel(TV in, float* __restr
 }
 int launch_result_small(snnb_context* ctx, const snnb_tensor* in, float* values, int* idx) {
     SNNB_REQUIRE(in->h == 1 && in->w == 1, "launch_result_small: a 1x1 tensor is expected");
-    launch_k(result_small_kernel, dim3((unsigned) (((long long) in->n * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), values, idx);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(result_small_kernel, dim3((unsigned) (((long long) in->n * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), values, idx), "result_small_kernel");
 }
 int launch_argmax(snnb_context* ctx, const snnb_tensor* in, int* dev_idx) {
-    launch_k(argmax_kernel, dim3((unsigned) (((long long) in->n * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), dev_idx);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(argmax_kernel, dim3((unsigned) (((long long) in->n * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), dev_idx), "argmax_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -882,9 +850,7 @@ __global__ void yolo_candidates_kernel(TV h0, TV h1, float thresh, int maxc, int
 int launch_yolo_candidates(snnb_context* ctx, const snnb_tensor* h0, const snnb_tensor* h1, float thresh, int maxc, int* counts, float* cand) {
     SNNB_CUDA_OK(cudaMemsetAsync(counts, 0, sizeof(int), ctx->stream));
     const long long total = (long long) h0->n * ((long long) h0->h * h0->w + (long long) h1->h * h1->w) * 3;
-    launch_k(yolo_candidates_kernel, dim3((unsigned) ((total + 255) / 256)), dim3(256), 0, ctx->stream, view(h0), view(h1), thresh, maxc, counts, cand);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(yolo_candidates_kernel, dim3((unsigned) ((total + 255) / 256)), dim3(256), 0, ctx->stream, view(h0), view(h1), thresh, maxc, counts, cand), "yolo_candidates_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -906,9 +872,7 @@ __global__ void flatten_kernel(TV in, TV out) {
 }
 int launch_flatten(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out) {
     const size_t total = (size_t) out->n * out->cp;
-    launch_k(flatten_kernel, dim3((unsigned) ((total + 255) / 256)), dim3(256), 0, ctx->stream, view(in), view(out));
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(flatten_kernel, dim3((unsigned) ((total + 255) / 256)), dim3(256), 0, ctx->stream, view(in), view(out)), "flatten_kernel");
 }
 
 // Concatenate along channels (vk_concat.comp:39-52).
@@ -928,9 +892,7 @@ __global__ void concat_kernel(TV a, TV b, TV out) {
 }
 int launch_concat(snnb_context* ctx, const snnb_tensor* a, const snnb_tensor* b, snnb_tensor* out) {
     const size_t total = out->pixels() * out->cp;
-    launch_k(concat_kernel, dim3((unsigned) ((total + 255) / 256)), dim3(256), 0, ctx->stream, view(a), view(b), view(out));
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(concat_kernel, dim3((unsigned) ((total + 255) / 256)), dim3(256), 0, ctx->stream, view(a), view(b), view(out)), "concat_kernel");
 }
 
 // UpSampling2D (vk_upsampling2d_nearest.comp:43-64; vk_upsampling2d_bilinear.comp:43-86), 8-channel vectors.
@@ -976,9 +938,7 @@ __global__ void upsample_kernel(TV in, TV out, float inv, int bilinear) {
 }
 int launch_upsample(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, float scale, bool bilinear) {
     ctx->last_kernel = "upsample_kernel";
-    launch_k(upsample_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), 1.0f / scale, bilinear ? 1 : 0);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(upsample_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), 1.0f / scale, bilinear ? 1 : 0), "upsample_kernel");
 }
 
 // Pad (vk_pad.comp:42-70): constant(0) / replicate / reflect.
@@ -1003,9 +963,7 @@ __global__ void pad_kernel(TV in, TV out, int pad_x, int pad_y, int mode) {
 }
 int launch_pad(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, int pad_x, int pad_y, int mode) {
     ctx->last_kernel = "pad_kernel";
-    launch_k(pad_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), pad_x, pad_y, mode);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(pad_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), pad_x, pad_y, mode), "pad_kernel");
 }
 
 // InstanceNorm (+act) (vk_instancenorm.comp:53-175): per (n, c) mean and biased variance over H*W, eps 1e-5.
@@ -1098,13 +1056,9 @@ int launch_instancenorm(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* o
     chunks     = std::max(1, std::min(chunks, (HW + 2047) / 2048)); // at least ~2 k pixels per CTA
     const int chunk_px = (HW + chunks - 1) / chunks;
     chunks             = (HW + chunk_px - 1) / chunk_px;
-    launch_k(instnorm_partial_kernel, dim3((unsigned) groups, (unsigned) chunks), dim3(256), 0, ctx->stream, view(in), partial, chunks, chunk_px);
-    SNNB_LAUNCH_CHECK(ctx);
-    launch_k(instnorm_finalize_kernel, dim3((unsigned) ((in->n * in->cp + 127) / 128)), dim3(128), 0, ctx->stream, view(in), (const float*) partial, stats, chunks);
-    SNNB_LAUNCH_CHECK(ctx);
-    launch_k(instnorm_apply_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), stats, w->gamma, w->beta, act, alpha);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    if (launch_done(ctx, launch_k(instnorm_partial_kernel, dim3((unsigned) groups, (unsigned) chunks), dim3(256), 0, ctx->stream, view(in), partial, chunks, chunk_px), "instnorm_partial_kernel")) return 1;
+    if (launch_done(ctx, launch_k(instnorm_finalize_kernel, dim3((unsigned) ((in->n * in->cp + 127) / 128)), dim3(128), 0, ctx->stream, view(in), (const float*) partial, stats, chunks), "instnorm_finalize_kernel")) return 1;
+    return launch_done(ctx, launch_k(instnorm_apply_kernel, dim3(vec_blocks(out, 256)), dim3(256), 0, ctx->stream, view(in), view(out), stats, w->gamma, w->beta, act, alpha), "instnorm_apply_kernel");
 }
 
 // Subpixel: depth_to_space(r) + tanh (vk_subpixel.comp:43-70; component = x%r + r*(y%r), fs_subpixel.glsl:41).
@@ -1127,9 +1081,7 @@ __global__ void subpixel_kernel(TV in, TV out, int r) {
 }
 int launch_subpixel(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, int r) {
     const long long total = (long long) out->pixels();
-    launch_k(subpixel_kernel, dim3((unsigned) ((total + 255) / 256)), dim3(256), 0, ctx->stream, view(in), view(out), r);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(subpixel_kernel, dim3((unsigned) ((total + 255) / 256)), dim3(256), 0, ctx->stream, view(in), view(out), r), "subpixel_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1184,16 +1136,12 @@ __global__ void merge_kernel(TV t, float* __restrict__ dst, FeedV f) {
         if (c + j < t.C) dst[px * t.C + c + j] = v[j];
 }
 int launch_split_f32(snnb_context* ctx, const float* dev_nhwc, snnb_tensor* t) {
-    launch_k(split_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, dev_nhwc, view(t), feed_view(t));
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(split_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, dev_nhwc, view(t), feed_view(t)), "split_kernel");
 }
 int launch_split_u8(snnb_context* ctx, const uint8_t* dev_nhwc_u8, snnb_tensor* t, const float mean[4], const float norm[4]) {
     U8Norm q;
     for (int i = 0; i < 4; ++i) q.mean[i] = mean[i], q.norm[i] = norm[i];
-    launch_k(split_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, dev_nhwc_u8, view(t), q, feed_view(t));
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(split_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, dev_nhwc_u8, view(t), q, feed_view(t)), "split_u8_kernel");
 }
 // u8 image of ANOTHER size -> resize (linear or nearest) -> (x - mean[c]) * norm[c] -> split-fp16: ImageTexture::resize
 // (core/inc/snn/imageTexture.h:137) = shadertemplate_vk_resize.comp:42-61: the output texel centre (x + 0.5) / outW is sampled from
@@ -1238,9 +1186,7 @@ __global__ void resize_u8_kernel(const uint8_t* __restrict__ src, int sh, int sw
 int launch_resize_u8(snnb_context* ctx, const uint8_t* dev_nhwc_u8, int src_h, int src_w, snnb_tensor* t, const float mean[4], const float norm[4], bool linear) {
     U8Norm q;
     for (int i = 0; i < 4; ++i) q.mean[i] = mean[i], q.norm[i] = norm[i];
-    launch_k(resize_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, dev_nhwc_u8, src_h, src_w, view(t), q, linear ? 1 : 0, feed_view(t));
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(resize_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, dev_nhwc_u8, src_h, src_w, view(t), q, linear ? 1 : 0, feed_view(t)), "resize_u8_kernel");
 }
 // tensor -> 8-bit image, dense NHWC: clamp(round(v * scale + offset), 0, 255) (the image-to-image models' outputs: style transfer,
 // super-resolution); a quarter of the fp32 bytes cross PCIe on the way back
@@ -1259,14 +1205,10 @@ __global__ void merge_u8_kernel(TV t, uint8_t* __restrict__ dst, float scale, fl
         if (c + j < t.C) dst[px * t.C + c + j] = (uint8_t) fminf(fmaxf(rintf(v[j] * scale + offset), 0.0f), 255.0f);
 }
 int launch_merge_u8(snnb_context* ctx, const snnb_tensor* t, uint8_t* dev_nhwc_u8, float scale, float offset) {
-    launch_k(merge_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, view(t), dev_nhwc_u8, scale, offset);
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(merge_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, view(t), dev_nhwc_u8, scale, offset), "merge_u8_kernel");
 }
 int launch_merge_f32(snnb_context* ctx, const snnb_tensor* t, float* dev_nhwc) {
-    launch_k(merge_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, view(t), dev_nhwc, feed_view(t));
-    SNNB_LAUNCH_CHECK(ctx);
-    return 0;
+    return launch_done(ctx, launch_k(merge_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, view(t), dev_nhwc, feed_view(t)), "merge_kernel");
 }
 
 } // namespace snnb

@@ -6,7 +6,8 @@
 //   D[M = 128 output pixels, N = n_blk <= 128 output channels] += A[M, K] * B[N, K]^T,   K = (tap, 64-channel block)
 //
 // fp32-faithful arithmetic out of fp16 tensor cores: activations and weights are stored as hi + lo fp16 pairs
-// (snnb_internal.h); every K step accumulates into the same fp32 accumulator, template parameter TERMS:
+// (snnb_internal.h); the product terms of one K block (one ring stage) accumulate into a fresh fp32 accumulator, which is then
+// added to the tile's fp32 sum (acc_promote). Template parameter TERMS:
 //   3:  A_hi*B_hi + A_hi*B_lo + A_lo*B_hi  (the dropped A_lo*B_lo term is ~2^-24 relative): ~22 mantissa bits per operand.
 //   2:  (A_hi + A_lo) * B_hi: the weights rounded ONCE to fp16 (<= 2^-12 relative per weight, per-layer error vs the oracle
 //       ~1e-4 of the tensor's range - inside the 1e-3 budget).
@@ -35,15 +36,13 @@
 
 namespace snnb {
 
-constexpr int UM_BLOCK_M     = 128;
+// UM_BLOCK_M, UM_STG_BYTES, UM_SMEM_LIMIT and the RW_* limits the planner reads are in snnb_internal.h
 constexpr int UM_BLOCK_K     = 64;  // fp16 elements: 128 bytes = one SWIZZLE_128B row
 constexpr int UM_MAX_N       = 128; // widest output-channel tile: 64 fp32 accumulator registers per consumer thread
 constexpr int UM_A_BYTES     = UM_BLOCK_M * 128;
 constexpr int UM_CONSUMERS   = 2;                          // consumer warpgroups, 64 tile rows each
 constexpr int UM_THREADS     = 128 * (1 + UM_CONSUMERS);   // warpgroup 0 = producer
 constexpr int UM_EPI_THREADS = 128 * UM_CONSUMERS;
-constexpr int UM_STG_BYTES   = 2 * UM_BLOCK_M * 128;       // epilogue staging: one 64-channel slab, hi + lo planes (32 KB)
-constexpr int UM_SMEM_LIMIT  = 227 * 1024;                 // opt-in shared memory per block on sm_90
 constexpr int UM_BAR_BYTES   = 256;
 
 // Shared-memory carve-up of conv_umma_kernel<TERMS, NB>: [ring: STAGES x (A_hi, A_lo, B_hi, B_lo)] [staging] [barriers]. A stage
@@ -570,12 +569,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_consta
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int RW_MAX_STAGES    = 16;                           // ring depth is chosen per launch: whatever shared memory is left, see RowWinParams::stages
 constexpr int RW_THREADS       = UM_THREADS;
-constexpr int RW_MAX_N         = 64;
-constexpr int RW_BOXW          = 144;                          // 128 tile pixels + up to 8 of window overhang, padded
-constexpr int RW_ARR_BYTES     = RW_BOXW * 16;                 // one (plane, parity) pixel row segment
 constexpr int RW_SMEM_BYTES    = UM_SMEM_LIMIT;                // everything: resident weight panels | epilogue staging | A ring | barriers
-constexpr int RW_BAR_BYTES     = 512;
-constexpr int RW_B_MAX_BYTES   = RW_SMEM_BYTES - 1024 - RW_BAR_BYTES - UM_STG_BYTES - 4 * 4 * RW_ARR_BYTES; // weights must leave room for >= 4 stages
 
 struct RowWinParams {
     const float* bias;
@@ -952,32 +946,6 @@ static int conv_terms(const snnb_context* ctx, const ConvArgs& a) {
     return prec == SNNB_PRECISION_FP16W ? 2 : (prec == SNNB_PRECISION_FP16 ? 1 : 3);
 }
 
-static int rowwin_nblk(int oc) { return oc <= 32 ? 32 : 64; }
-
-static bool feed_usable(const ConvArgs& a, FeedPlan& fp);
-static bool rowwin_supported(const ConvArgs& a) {
-    // small-C stems: IC <= 8 (one 16-byte vector per pixel), stride 1 or 2, <= 8 K steps per filter row, weights packed
-    // for exactly this (stride, pad_x), whole panel set resident in smem - in the layout the launch will use (feed mode: one panel)
-    RowPlan rp;
-    if (!(a.in->cp == 8 && a.w && a.w->w_row_hi && a.w->w_row_lo && a.w->row_stride == a.stride && a.w->row_pad == a.pad_x && a.out->c <= RW_MAX_N &&
-          a.residual == nullptr && make_row_plan(a.k, a.stride, a.pad_x, rp) && 128 + rp.span <= RW_BOXW))
-        return false;
-    FeedPlan fp;
-    const int wrows = feed_usable(a, fp) ? (a.k + fp.rows_per_panel - 1) / fp.rows_per_panel : a.k * ((rp.ksteps + 3) / 4); // 128-byte weight rows per channel
-    return wrows * 2 * rowwin_nblk(a.out->c) * 128 <= RW_B_MAX_BYTES;
-}
-
-bool conv2d_umma_supported(const ConvArgs& a) {
-    if (!a.w || !a.w->w_hi || !a.w->w_lo) return false;
-    if (!(a.pad_mode == SNNB_PAD_NONE || a.pad_mode == SNNB_PAD_CONSTANT)) return false; // replicate / reflect: SIMT gather
-    if (rowwin_supported(a)) return true;
-    if (!(a.stride == 1 || a.stride == 2)) return false; // stride 2 = TMA traversal stride (elementStrides) on W and H
-    if (a.in->c < 16) return false; // wider small-C cases the row-GEMM variant cannot take: K would be >75% zero padding
-    if (a.k < 1 || a.k > 11) return false;
-    if (a.pad_x > 127 || a.pad_y > 127) return false;
-    return true;
-}
-
 // Bits of snnb_context::func_attr_mask (cudaFuncSetAttribute applies per device): one per kernel instantiation
 enum { ATTR_UMMA0 = 0, ATTR_ROWWIN0 = 18, ATTR_DW1 = 48, ATTR_DW2 = 49 };
 static int ensure_smem_attr(snnb_context* ctx, const void* kernel, int bit, int bytes) {
@@ -1019,24 +987,21 @@ static RowWinKernel rowwin_kernel_of(int terms, int fks, int nb) {
     return terms == 3 ? rowwin_kernel_t<3>(fks, nb) : (terms == 2 ? rowwin_kernel_t<2>(fks, nb) : rowwin_kernel_t<1>(fks, nb));
 }
 
-// FEED mode: the input tensor carries the compact 4-channel copy this layer's weights were packed for, and it is large enough
-static bool feed_usable(const ConvArgs& a, FeedPlan& fp) {
-    const snnb_tensor* in = a.in;
-    if (!in->feed_hi || !a.w->w_feed_hi || !a.w->w_feed_lo || a.w->feed_pad != a.pad_x) return false;
-    if (!make_feed_plan(a.k, a.stride, a.pad_x, in->c, fp) || fp.px != in->feed_px || in->feed_py != a.pad_y) return false;
-    const int tiles_x = (a.out->w + UM_BLOCK_M - 1) / UM_BLOCK_M;
-    return in->feed_w >= 2 * (tiles_x * UM_BLOCK_M - 1) + 2 * fp.nch && in->feed_h >= 2 * (a.out->h - 1) + a.k &&
-           (254 + 2 * fp.nch) * 8 <= RW_ARR_BYTES;
-}
-
-static int launch_conv2d_rowwin(snnb_context* ctx, const ConvArgs& a, EncodeTiledFn encode) {
+int launch_conv2d_rowwin(snnb_context* ctx, const ConvArgs& a, const ConvPlan& plan) {
+    EncodeTiledFn encode = get_encode(ctx);
+    SNNB_REQUIRE(encode, "launch_conv2d_rowwin: cuTensorMapEncodeTiled is unavailable in this driver");
     const snnb_tensor* in = a.in;
     snnb_tensor* out      = a.out;
-    RowPlan rp;
-    SNNB_REQUIRE(make_row_plan(a.k, a.stride, a.pad_x, rp), "launch_conv2d_rowwin: no row plan");
-    FeedPlan fp;
-    const bool feed = feed_usable(a, fp);
+    const bool feed       = plan.path == CONV_ROWWIN_FEED;
+    SNNB_REQUIRE(plan.path == CONV_ROWWIN || feed, "launch_conv2d_rowwin: the plan is not a row-window launch");
+    SNNB_REQUIRE(a.w->w_row_hi && a.w->w_row_lo && a.w->row_stride == a.stride && a.w->row_pad == a.pad_x,
+                 "launch_conv2d_rowwin: the weights carry no row-window operand for stride %d, pad %d", a.stride, a.pad_x);
     SNNB_REQUIRE(feed || !in->feed_only, "launch_conv2d_rowwin: the input tensor only exists as a stem feed, which this launch cannot read");
+    SNNB_REQUIRE(!feed || (a.w->w_feed_hi && a.w->w_feed_lo && a.w->feed_pad == a.pad_x), "launch_conv2d_rowwin: the weights carry no feed operand for pad %d", a.pad_x);
+    SNNB_REQUIRE(!feed || (in->feed_hi && in->feed_h == plan.feed_h && in->feed_w == plan.feed_w && in->feed_py == plan.feed_py && in->feed_px == plan.feed_px),
+                 "launch_conv2d_rowwin: the input tensor does not carry the planned feed copy");
+    RowPlan rp          = plan.rp;
+    const FeedPlan& fp  = plan.fp;
     if (feed) { // one dense segment per plane, K steps at consecutive 32-byte offsets
         rp.parities = 1, rp.ksteps = fp.ksteps;
         for (int q = 0; q < fp.ksteps; ++q) rp.ks_parity[q] = 0, rp.ks_erel[q] = 2 * q;
@@ -1102,20 +1067,12 @@ static int launch_conv2d_rowwin(snnb_context* ctx, const ConvArgs& a, EncodeTile
     if (ensure_smem_attr(ctx, (const void*) kern, ATTR_ROWWIN0 + ((terms - 1) * 5 + fks) * 2 + (p.n_blk == 64 ? 1 : 0), RW_SMEM_BYTES)) return 1;
     const int total_tiles = p.N * p.OH * p.tiles_x;
     const int grid        = std::min(total_tiles, ctx->sm_count);
-    const cudaError_t le = launch_k_pdl(kern, dim3(grid), dim3(RW_THREADS), RW_SMEM_BYTES, ctx->stream, tmA[0], tmA[1], tmA[2], tmA[3], tmB[0], tmB[1], tmO[0], tmO[1], p);
-    cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
-    if (e != cudaSuccess) {
-        set_error("conv_rowwin_kernel launch failed: %s", cudaGetErrorString(e));
-        return 1;
-    }
-    ctx->launches++;
-    return 0;
+    return launch_done(ctx, launch_k_pdl(kern, dim3(grid), dim3(RW_THREADS), RW_SMEM_BYTES, ctx->stream, tmA[0], tmA[1], tmA[2], tmA[3], tmB[0], tmB[1], tmO[0], tmO[1], p), "conv_rowwin_kernel");
 }
 
 int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
     EncodeTiledFn encode = get_encode(ctx);
     SNNB_REQUIRE(encode, "launch_conv2d_umma: cuTensorMapEncodeTiled is unavailable in this driver");
-    if (rowwin_supported(a)) return launch_conv2d_rowwin(ctx, a, encode);
     SNNB_REQUIRE(!a.in->feed_only, "launch_conv2d_umma: the input tensor only exists as a stem feed, which this launch cannot read");
     const snnb_tensor* in = a.in;
     snnb_tensor* out      = a.out;
@@ -1192,15 +1149,8 @@ int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
     const int total_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_oc;
     const int grid        = p.sk ? (p.sk_dp > 0 ? ctx->sm_count : p.sk_ctas) : std::min(total_tiles * p.ksplit, ctx->sm_count);
     ctx->last_kernel = p.sk ? "conv_umma_kernel<stream-K>" : (p.ksplit > 1 ? "conv_umma_kernel<split-K>" : "conv_umma_kernel");
-    const cudaError_t le = launch_k_pdl(kc.kernel, dim3(grid), dim3(UM_THREADS), kc.smem, ctx->stream, tmA[0], tmA[1], tmB[0], tmB[1], tmO64[0], tmO64[1], tmOT[0], tmOT[1],
-                                        tmR64[0], tmR64[1], tmRT[0], tmRT[1], p);
-    cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
-    if (e != cudaSuccess) {
-        set_error("conv_umma_kernel launch failed: %s", cudaGetErrorString(e));
-        return 1;
-    }
-    ctx->launches++;
-    return 0;
+    return launch_done(ctx, launch_k_pdl(kc.kernel, dim3(grid), dim3(UM_THREADS), kc.smem, ctx->stream, tmA[0], tmA[1], tmB[0], tmB[1], tmO64[0], tmO64[1], tmOT[0], tmOT[1],
+                            tmR64[0], tmR64[1], tmRT[0], tmRT[1], p), "conv_umma_kernel");
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1413,14 +1363,7 @@ template <int S> static int launch_depthwise_tma_s(snnb_context* ctx, const Conv
     if (ensure_smem_attr(ctx, (const void*) depthwise_tma_kernel<S>, S == 1 ? ATTR_DW1 : ATTR_DW2, T::SMEM_BYTES)) return 1;
     const long long total = (long long) p.N * p.tiles_y * p.tiles_x * p.chunks;
     const int grid        = (int) std::min<long long>(total, 2 * ctx->sm_count); // two CTAs per SM (128 registers, <= 93 KB of shared memory each)
-    const cudaError_t le  = launch_k_pdl(depthwise_tma_kernel<S>, dim3(grid), dim3(DW_THREADS), T::SMEM_BYTES, ctx->stream, tmI[0], tmI[1], p);
-    cudaError_t e = le != cudaSuccess ? le : cudaGetLastError();
-    if (e != cudaSuccess) {
-        set_error("depthwise_tma_kernel launch failed: %s", cudaGetErrorString(e));
-        return 1;
-    }
-    ctx->launches++;
-    return 0;
+    return launch_done(ctx, launch_k_pdl(depthwise_tma_kernel<S>, dim3(grid), dim3(DW_THREADS), T::SMEM_BYTES, ctx->stream, tmI[0], tmI[1], p), "depthwise_tma_kernel");
 }
 
 int launch_depthwise_tma(snnb_context* ctx, const ConvArgs& a) {

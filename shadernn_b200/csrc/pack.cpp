@@ -83,7 +83,7 @@ void pack_conv2d_host(int IC, int OC, int k, const float* w_oihw, const float* b
 
 void pack_rowwin_host(PackedHost& p, int stride, int pad_x) {
     RowPlan rp;
-    if (p.kind != 1 || p.in_ch > 8 || p.out_ch > 64 || !make_row_plan(p.kernel, stride, pad_x, rp)) return;
+    if (p.kind != 1 || !rowwin_packable(p.in_ch, p.out_ch, p.kernel, stride, pad_x, rp)) return;
     const int k = p.kernel, IC = p.in_ch, OC = p.out_ch;
     p.row_stride = stride, p.row_pad = pad_x;
     const int panels = (rp.ksteps + 3) / 4; // 64 K columns (4 K steps) per panel: [ky][panel][OCr][64]
@@ -107,7 +107,7 @@ void pack_rowwin_host(PackedHost& p, int stride, int pad_x) {
 
 void pack_feed_host(PackedHost& p, int stride, int pad_x) {
     FeedPlan fp;
-    if (p.kind != 1 || p.out_ch > 64 || p.w_row_hi.empty() || !make_feed_plan(p.kernel, stride, pad_x, p.in_ch, fp)) return;
+    if (p.kind != 1 || !feed_packable(p.in_ch, p.out_ch, p.kernel, stride, pad_x, fp)) return;
     const int k = p.kernel, IC = p.in_ch, OC = p.out_ch;
     p.feed_pad = pad_x;
     const int rpp = fp.rows_per_panel, prows = (k + rpp - 1) / rpp, sub = 64 / rpp; // filter rows per 128-byte weight row, K columns each

@@ -177,6 +177,18 @@ namespace snnb {
 
 int ensure_stage(snnb_context* ctx, size_t bytes);
 
+// Every kernel launch ends here: `launched` is the launch call's result. A failed launch (that result, else cudaGetLastError)
+// is reported under the kernel's name; a successful one is counted in ctx->launches.
+static inline int launch_done(snnb_context* ctx, cudaError_t launched, const char* kernel) {
+    const cudaError_t e = launched != cudaSuccess ? launched : cudaGetLastError();
+    if (e != cudaSuccess) {
+        set_error("%s launch failed: %s", kernel, cudaGetErrorString(e));
+        return 1;
+    }
+    ctx->launches++;
+    return 0;
+}
+
 // ---- kernel launchers (kernels_simt.cu) -------------------------------------------------------------------
 struct ConvArgs {
     const snnb_tensor* in;
@@ -188,9 +200,10 @@ struct ConvArgs {
     int precision = -1; // SNNB_PRECISION_* of this launch; -1 = the context's default
     bool stream_k = false; // the planner may choose the stream-K decomposition (SNNB_ALGO_TCGEN05_STREAMK)
 };
+struct ConvPlan;
 int launch_conv2d_simt(snnb_context* ctx, const ConvArgs& a);
-int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a); // kernels_umma.cu (wgmma + TMA)
-bool conv2d_umma_supported(const ConvArgs& a);
+int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a);                         // kernels_umma.cu: implicit GEMM (wgmma + TMA)
+int launch_conv2d_rowwin(snnb_context* ctx, const ConvArgs& a, const ConvPlan& plan); // kernels_umma.cu: small-channel row window / stem feed
 int streamk_schedule(int tiles, int num_kb, int sms, int* rows, int capacity); // host evaluation of the stream-K work decomposition (tests)
 int launch_depthwise(snnb_context* ctx, const ConvArgs& a);
 bool depthwise_tma_supported(const ConvArgs& a);          // 3x3 stride 1/2: TMA-staged, register-tiled (kernels_umma.cu)
@@ -282,6 +295,49 @@ static inline bool make_feed_plan(int k, int stride, int pad_x, int ic, FeedPlan
     fp.rows_per_panel = fp.ksteps == 1 ? 4 : (fp.ksteps == 2 ? 2 : 1);
     return fp.ksteps <= 4;
 }
+
+// ---- geometry of the tensor-core convolution kernels (kernels_umma.cu), read by the planner too ----------------
+constexpr int UM_BLOCK_M    = 128;                    // output pixels per tile
+constexpr int UM_STG_BYTES  = 2 * UM_BLOCK_M * 128;   // epilogue staging: one 64-channel slab, hi + lo planes (32 KB)
+constexpr int UM_SMEM_LIMIT = 227 * 1024;             // opt-in shared memory per block on sm_90
+constexpr int RW_MAX_N      = 64;                     // widest output-channel tile of the row-window kernel
+constexpr int RW_BOXW       = 144;                    // 128 tile pixels + up to 8 of window overhang, padded
+constexpr int RW_ARR_BYTES  = RW_BOXW * 16;           // one (plane, parity) pixel row segment
+constexpr int RW_BAR_BYTES  = 512;
+constexpr int RW_B_MAX_BYTES = UM_SMEM_LIMIT - 1024 - RW_BAR_BYTES - UM_STG_BYTES - 4 * 4 * RW_ARR_BYTES; // weights must leave room for >= 4 stages
+static inline int rowwin_nblk(int oc) { return oc <= 32 ? 32 : 64; }
+
+// ---- convolution planning (conv_plan.cpp) ------------------------------------------------------------------------
+// The one place that decides which kernel runs a convolution, whether it reads a pre-padded copy of its input and whether
+// a model input gets the compact feed copy. The engine plans every layer once at load; a single C-ABI launch plans itself.
+enum ConvPath { CONV_REFUSED = 0, CONV_SIMT, CONV_IGEMM, CONV_ROWWIN, CONV_ROWWIN_FEED };
+struct ConvQuery {
+    int in_h = 0, in_w = 0, in_c = 0, out_h = 0, out_w = 0, out_c = 0;
+    int k = 1, stride = 1, pad_x = 0, pad_y = 0, pad_mode = SNNB_PAD_NONE;
+    bool residual   = false;
+    int algo        = SNNB_ALGO_AUTO; // SNNB_ALGO_*: SIMT, AUTO, or the tensor path forced (TCGEN05*)
+    bool may_prepad = false;          // a pre-padded copy of the input may be allocated
+    bool may_feed   = false;          // the input is a model input that may carry the compact feed copy
+    // What the weights carry: the row-window operand packed for (row_stride, row_pad) (row_stride 0: none) and the feed operand
+    // packed for x padding feed_pad (-1: none).
+    int row_stride = 0, row_pad = 0, feed_pad = -1;
+};
+struct ConvPlan {
+    int path = CONV_SIMT;
+    int pad_x = 0, pad_y = 0, pad_mode = SNNB_PAD_NONE; // the padding the kernel sees
+    int prepad_h = 0, prepad_w = 0;                     // > 0: the kernel reads a copy of the input padded to this size
+    int feed_h = 0, feed_w = 0, feed_py = 0, feed_px = 0; // CONV_ROWWIN_FEED: the input's feed copy (snnb_tensor::feed_hi)
+    RowPlan rp;                                         // CONV_ROWWIN*
+    FeedPlan fp;                                        // CONV_ROWWIN_FEED
+};
+// Whether pack_rowwin_host / pack_feed_host give a layer the row-window / feed operand
+bool rowwin_packable(int in_c, int out_c, int k, int stride, int pad_x, RowPlan& rp);
+bool feed_packable(int in_c, int out_c, int k, int stride, int pad_x, FeedPlan& fp);
+ConvPlan plan_conv(const ConvQuery& q);
+// Runs the planned kernel; the tensors and weights must be the ones the plan was made for (an error otherwise).
+int launch_conv2d(snnb_context* ctx, const ConvArgs& a, const ConvPlan& plan);
+// Dense: flatten into `flat` (only when `in` is not 1x1), 1x1 convolution planned with SNNB_ALGO_AUTO, then softmax if act is SNNB_ACT_SOFTMAX
+int launch_dense(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* flat, snnb_tensor* out, const snnb_weights* w, int act, float alpha, int precision);
 
 struct PackedHost {
     std::vector<float> w_f32;           // [K][OCw]
