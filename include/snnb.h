@@ -221,6 +221,42 @@ typedef struct {
 } snnb_image_io;
 int snnb_model_submit_image(snnb_model* m, const snnb_image_io* io, int* ticket);
 int snnb_model_wait(snnb_model* m, int ticket);
+/* Inputs and outputs that already live in device memory, ordered on the caller's CUDA stream: the counterpart of attaching GPU images
+ * to the model (ModelInput / ModelOutput attach(), genericModelProcessorVulkan.cpp:112-121, styleTransferProcessorGL.cpp:175-181;
+ * RunParameters::inputImages / outputImages, core/inc/snn/core.h:78-80) and run(). Nothing crosses PCIe and nothing waits on the host.
+ *
+ * A buffer is `data`: device (or managed) memory of the model's device, dense in `layout`, the batch x H x W x C of its tensor
+ * (N x C x H x W for NCHW), aligned to its element size. U8 inputs are normalised as (x - mean4[c & 3]) * norm4[c & 3], exactly as
+ * snnb_model_submit_u8; U8 outputs are clamp(round(v * scale + offset), 0, 255), exactly as snnb_image_io.output_u8; F16 outputs are
+ * the fp32 values rounded to nearest. The other fields are ignored. */
+enum { SNNB_DTYPE_F32 = 0, SNNB_DTYPE_F16 = 1, SNNB_DTYPE_U8 = 2 };
+enum { SNNB_LAYOUT_NHWC = 0, SNNB_LAYOUT_NCHW = 1 };
+typedef struct {
+    void* data;
+    int dtype, layout;        /* SNNB_DTYPE_*, SNNB_LAYOUT_* */
+    float mean4[4], norm4[4]; /* U8 inputs only */
+    float scale, offset;      /* U8 outputs only */
+} snnb_device_buffer;
+/* - inputs: num_inputs must equal snnb_model_num_inputs(); inputs[i] feeds InputLayer i in "inputIndex" order (so a model with several
+ *   inputs can be fed here, while run() / submit() feed input 0 only).
+ * - outputs: outputs[j] receives model output j, for j < num_outputs <= snnb_model_num_outputs(); an entry with data == NULL is skipped,
+ *   and num_outputs may be 0 (classes only).
+ * - classes_1based_dev: NULL, or device int32[batch] that receives arg-max + 1 per image (core.cpp:228-233). An error for a model that
+ *   is not a classifier.
+ * - stream: a cudaStream_t of the model's device, or NULL for the context's stream. To order against a default stream, pass
+ *   cudaStreamLegacy or cudaStreamPerThread, not NULL. The call returns without waiting for the GPU: work enqueued on `stream` before
+ *   the call happens before the inputs are read, and work enqueued on `stream` after it sees the outputs. The model's work itself runs
+ *   on the context's stream, behind two events per model (the caller's stream -> the context's stream -> the caller's stream), so calls
+ *   from different streams, and calls mixed with run() / submit(), are serialised on the model's tensors. A stream that is being
+ *   captured is refused: capturing this call into the caller's CUDA graph is not supported.
+ * - The batch is the loaded batch. A model whose output 0 is a YOLO layer is refused: its detections come through the host paths
+ *   (run() / submit() + snnb_model_get_boxes).
+ * Every argument is checked on the host before anything is enqueued: null pointers, unknown dtype or layout, the input count, buffers
+ * that cudaPointerGetAttributes does not report as device or managed memory of the context's device, and misaligned buffers are errors
+ * (snnb_last_error()) with no work enqueued. A buffer's size cannot be checked: it must hold its tensor's elements. Cost beyond the
+ * forward pass: one kernel launch per input, one per output and one for the classes. */
+int snnb_model_run_device(snnb_model* m, const snnb_device_buffer* inputs, int num_inputs, const snnb_device_buffer* outputs, int num_outputs,
+                          int* classes_1based_dev, void* stream);
 /* Device-resident variant: inputs already uploaded with snnb_model_set_input(); forward only, asynchronous. */
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input_nhwc);
 int snnb_model_forward(snnb_model* m);

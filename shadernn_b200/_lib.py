@@ -61,6 +61,23 @@ class ImageIO(C.Structure):
     ]
 
 
+DTYPE_F32, DTYPE_F16, DTYPE_U8 = 0, 1, 2
+LAYOUT_NHWC, LAYOUT_NCHW = 0, 1
+
+
+class DeviceBuffer(C.Structure):
+    """snnb_device_buffer"""
+    _fields_ = [
+        ("data", C.c_void_p),
+        ("dtype", C.c_int),
+        ("layout", C.c_int),
+        ("mean4", C.c_float * 4),
+        ("norm4", C.c_float * 4),
+        ("scale", C.c_float),
+        ("offset", C.c_float),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/snnb.h declares
 SIGNATURES = {
     "snnb_version": (C.c_int, []),
@@ -122,6 +139,7 @@ SIGNATURES = {
     "snnb_model_submit_u8": (C.c_int, [vp, vp, vp, vp, vp, C.c_size_t, vp, c_int_p]),
     "snnb_model_submit_image": (C.c_int, [vp, C.POINTER(ImageIO), c_int_p]),
     "snnb_model_wait": (C.c_int, [vp, C.c_int]),
+    "snnb_model_run_device": (C.c_int, [vp, C.POINTER(DeviceBuffer), C.c_int, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),

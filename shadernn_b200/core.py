@@ -348,6 +348,10 @@ class MixedInferenceCore:
         return self._dims(lib().snnb_model_output_dims, idx)
 
     @property
+    def num_inputs(self):
+        return lib().snnb_model_num_inputs(self.h)
+
+    @property
     def num_outputs(self):
         return lib().snnb_model_num_outputs(self.h)
 
@@ -419,6 +423,50 @@ class MixedInferenceCore:
 
     def wait(self, ticket):
         check(lib().snnb_model_wait(self.h, int(ticket)), "snnb_model_wait")
+
+    def run_torch(self, inputs, layout="nhwc", mean4=None, norm4=None, out_dtype=None, out_layout="nhwc", out_scale=1.0, out_offset=0.0,
+                  want_classes=False):
+        """snnb_model_run_device with torch CUDA tensors, ordered on the current torch stream and never synchronising.
+
+        inputs: a CUDA tensor (float32, float16 or uint8), or a list with one per model input, each batch x H x W x C ("nhwc") or
+        batch x C x H x W ("nchw"); uint8 inputs are normalised as (x - mean4[c & 3]) * norm4[c & 3] (default mean 0, norm 1).
+        Outputs are allocated here as out_dtype (float32 by default, float16 or uint8: clamp(round(v * out_scale + out_offset), 0, 255))
+        in out_layout. Returns output 0 for a one-output model, else the list of outputs; with want_classes, (outputs, the 1-based
+        classes as a device int32 tensor)."""
+        import torch
+        dtypes = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.uint8: _lib.DTYPE_U8}
+        layouts = {"nhwc": _lib.LAYOUT_NHWC, "nchw": _lib.LAYOUT_NCHW}
+        out_dtype = torch.float32 if out_dtype is None else out_dtype
+        if out_dtype not in dtypes or layout not in layouts or out_layout not in layouts:
+            raise ValueError("run_torch: dtype %s / layouts %r, %r: expected float32, float16 or uint8 and 'nhwc' or 'nchw'" % (out_dtype, layout, out_layout))
+
+        def shape_in(shape, lay):
+            n, h, w, c = shape
+            return (n, h, w, c) if lay == "nhwc" else (n, c, h, w)
+
+        xs = [inputs] if isinstance(inputs, torch.Tensor) else list(inputs)
+        keep = [x.contiguous() for x in xs]  # alive until the call has enqueued its reads; the stream fence orders any reuse after them
+        ins = (_lib.DeviceBuffer * max(1, len(keep)))()
+        for i, x in enumerate(keep):
+            if x.dtype not in dtypes:
+                raise ValueError("run_torch: input %d has dtype %s; float32, float16 or uint8 is supported" % (i, x.dtype))
+            if i < self.num_inputs and tuple(x.shape) != shape_in(self.input_shape(i), layout):
+                raise ValueError("run_torch: input %d has shape %s, the model takes %s (%s)" % (i, tuple(x.shape), shape_in(self.input_shape(i), layout), layout))
+            ins[i].data, ins[i].dtype, ins[i].layout = x.data_ptr(), dtypes[x.dtype], layouts[layout]
+            ins[i].mean4 = (C.c_float * 4)(*[float(v) for v in (mean4 if mean4 is not None else [0.0] * 4)])
+            ins[i].norm4 = (C.c_float * 4)(*[float(v) for v in (norm4 if norm4 is not None else [1.0] * 4)])
+        device = torch.device("cuda", self.ctx.device)
+        outs = [torch.empty(shape_in(self.output_shape(j), out_layout), dtype=out_dtype, device=device) for j in range(self.num_outputs)]
+        obufs = (_lib.DeviceBuffer * max(1, len(outs)))()
+        for j, o in enumerate(outs):
+            obufs[j].data, obufs[j].dtype, obufs[j].layout = o.data_ptr(), dtypes[out_dtype], layouts[out_layout]
+            obufs[j].scale, obufs[j].offset = float(out_scale), float(out_offset)
+        classes = torch.empty(self.batch, dtype=torch.int32, device=device) if want_classes else None
+        # torch's default stream is the legacy NULL stream, which the library reads as "the context's stream": name it cudaStreamLegacy (1)
+        stream = torch.cuda.current_stream(device).cuda_stream or 1
+        check(lib().snnb_model_run_device(self.h, ins, len(keep), obufs, len(outs), classes.data_ptr() if want_classes else None, stream), "snnb_model_run_device")
+        result = outs[0] if len(outs) == 1 else outs
+        return (result, classes) if want_classes else result
 
     def set_input(self, images, idx=0):
         images = _f32(images)

@@ -40,6 +40,8 @@ MixedInferenceCore::~MixedInferenceCore() {
         if (sl.resultReady) cudaEventDestroy(sl.resultReady);
     }
     if (copyStream) cudaStreamDestroy(copyStream);
+    if (callerReady) cudaEventDestroy(callerReady);
+    if (deviceDone) cudaEventDestroy(deviceDone);
 }
 
 std::unique_ptr<MixedInferenceCore> MixedInferenceCore::create(snnb_context* ctx, const std::string& modelFileName, const ShaderGenOptions& options,
@@ -611,6 +613,88 @@ int MixedInferenceCore::wait(int ticket) {
         const int rc = yolo->finishDecode(sl.yoloHost, sl.yoloDev, boxes);
         SNNB_REQUIRE(rc >= 0, "wait: corrupt detection candidate list");
         return rc;
+    }
+    return 0;
+}
+
+// ---- device-resident inputs and outputs on the caller's stream (snnb_model_run_device) -------------------------------------
+static const char* memoryTypeName(cudaMemoryType t) {
+    switch (t) {
+    case cudaMemoryTypeUnregistered: return "unregistered host memory";
+    case cudaMemoryTypeHost: return "pinned host memory";
+    case cudaMemoryTypeDevice: return "device memory";
+    case cudaMemoryTypeManaged: return "managed memory";
+    }
+    return "unknown memory";
+}
+// A pointer the kernels may dereference: device or managed memory of `device`, aligned to its `elem`-byte elements.
+static int checkDevicePointer(const void* p, size_t elem, int device, const char* what, int idx) {
+    SNNB_REQUIRE(p, "snnb_model_run_device: %s %d: null data pointer", what, idx);
+    cudaPointerAttributes a {};
+    const cudaError_t e = cudaPointerGetAttributes(&a, p);
+    if (e != cudaSuccess) cudaGetLastError(); // not sticky: leave no error behind for the next call
+    SNNB_REQUIRE(e == cudaSuccess, "snnb_model_run_device: %s %d: cudaPointerGetAttributes(%p) failed: %s", what, idx, p, cudaGetErrorString(e));
+    SNNB_REQUIRE((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device,
+                 "snnb_model_run_device: %s %d: %p is %s of device %d; device or managed memory of device %d is required", what, idx, p, memoryTypeName(a.type), a.device,
+                 device);
+    SNNB_REQUIRE(reinterpret_cast<uintptr_t>(p) % elem == 0, "snnb_model_run_device: %s %d: %p is not aligned to its %zu-byte elements", what, idx, p, elem);
+    return 0;
+}
+static int checkDeviceBuffer(const snnb_device_buffer& b, int device, const char* what, int idx) {
+    SNNB_REQUIRE(b.dtype == SNNB_DTYPE_F32 || b.dtype == SNNB_DTYPE_F16 || b.dtype == SNNB_DTYPE_U8, "snnb_model_run_device: %s %d: unknown dtype %d", what, idx, b.dtype);
+    SNNB_REQUIRE(b.layout == SNNB_LAYOUT_NHWC || b.layout == SNNB_LAYOUT_NCHW, "snnb_model_run_device: %s %d: unknown layout %d", what, idx, b.layout);
+    const size_t elem = b.dtype == SNNB_DTYPE_F32 ? 4 : (b.dtype == SNNB_DTYPE_F16 ? 2 : 1);
+    return checkDevicePointer(b.data, elem, device, what, idx);
+}
+
+int MixedInferenceCore::runDevice(const snnb_device_buffer* inputs, int numInputs, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev,
+                                  cudaStream_t stream) {
+    // everything is validated before the first enqueue: a refused call leaves no work behind
+    SNNB_REQUIRE(inputs, "snnb_model_run_device: null inputs");
+    SNNB_REQUIRE(numInputs == (int) inputLayers.size(), "snnb_model_run_device: %d inputs given, the model has %d", numInputs, (int) inputLayers.size());
+    SNNB_REQUIRE(numOutputs >= 0 && numOutputs <= (int) outputLayers.size(), "snnb_model_run_device: %d outputs requested, the model has %d", numOutputs,
+                 (int) outputLayers.size());
+    SNNB_REQUIRE(outputs || numOutputs == 0, "snnb_model_run_device: null outputs");
+    SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO",
+                 "snnb_model_run_device: output 0 is a YOLO detection list, which has no device form; use snnb_model_run or snnb_model_submit / snnb_model_wait "
+                 "and read the boxes with snnb_model_get_boxes");
+    const int device = ctx->device;
+    for (int i = 0; i < numInputs; ++i)
+        if (int rc = checkDeviceBuffer(inputs[i], device, "input", i)) return rc;
+    for (int j = 0; j < numOutputs; ++j) {
+        if (!outputs[j].data) continue;
+        SNNB_REQUIRE(outputLayers[j]->output, "snnb_model_run_device: output %d (%s) has no device tensor", j, outputLayers[j]->name.c_str());
+        if (int rc = checkDeviceBuffer(outputs[j], device, "output", j)) return rc;
+    }
+    if (classes1Dev) {
+        SNNB_REQUIRE(isClassifier, "snnb_model_run_device: classes requested, but the model is not a classifier (output 0 is not 1 x 1 x C with C > 1)");
+        if (int rc = checkDevicePointer(classes1Dev, sizeof(int), device, "classes", 0)) return rc;
+    }
+    if (stream) {
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        const cudaError_t e = cudaStreamIsCapturing(stream, &cap);
+        if (e != cudaSuccess) cudaGetLastError();
+        SNNB_REQUIRE(e == cudaSuccess, "snnb_model_run_device: stream %p: %s", (void*) stream, cudaGetErrorString(e));
+        SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone, "snnb_model_run_device: stream %p is being captured; capture into the caller's CUDA graph is not supported",
+                     (void*) stream);
+    }
+    if (!callerReady) SNNB_CUDA_OK(cudaEventCreateWithFlags(&callerReady, cudaEventDisableTiming));
+    if (!deviceDone) SNNB_CUDA_OK(cudaEventCreateWithFlags(&deviceDone, cudaEventDisableTiming));
+
+    const bool fence = stream && stream != ctx->stream;
+    if (fence) { // a stream of another device fails here, before anything is launched
+        SNNB_CUDA_OK(cudaEventRecord(callerReady, stream));
+        SNNB_CUDA_OK(cudaStreamWaitEvent(ctx->stream, callerReady, 0));
+    }
+    for (int i = 0; i < numInputs; ++i)
+        if (launch_device_input(ctx, inputs[i], inputLayers[i]->output)) return 1;
+    if (forward()) return 1;
+    for (int j = 0; j < numOutputs; ++j)
+        if (outputs[j].data && launch_device_output(ctx, outputLayers[j]->output, outputs[j])) return 1;
+    if (classes1Dev && launch_argmax(ctx, outputLayers[0]->output, classes1Dev, 1)) return 1; // core.cpp:228-233: argmax + 1
+    if (fence) {
+        SNNB_CUDA_OK(cudaEventRecord(deviceDone, ctx->stream));
+        SNNB_CUDA_OK(cudaStreamWaitEvent(stream, deviceDone, 0));
     }
     return 0;
 }

@@ -349,6 +349,8 @@ public:
                    const snnb_image_io* io = nullptr);
     int submitImage(const snnb_image_io& io, int* ticket);
     int wait(int ticket);
+    // snnb_model_run_device: device buffers in and out, fenced against the caller's stream (NULL: the context's); asynchronous
+    int runDevice(const snnb_device_buffer* inputs, int numInputs, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
     int layerOutput(int layerId, float* host, size_t capacityFloats);
     int timeLayers(std::vector<float>& ms);
     int dumpOutputs(const std::string& dir);
@@ -403,6 +405,8 @@ private:
     cudaStream_t copyStream = nullptr;
     int nextTicket = 0;
     int ensureStreaming();
+    // runDevice's fences: the caller's stream -> the context's stream (callerReady), and back (deviceDone); created on first use
+    cudaEvent_t callerReady = nullptr, deviceDone = nullptr;
 };
 
 } // namespace snn

@@ -123,6 +123,12 @@ int snnb_model_wait(snnb_model* m, int ticket) {
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->wait(ticket);
 }
+int snnb_model_run_device(snnb_model* m, const snnb_device_buffer* inputs, int num_inputs, const snnb_device_buffer* outputs, int num_outputs,
+                          int* classes_1based_dev, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_run_device: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->runDevice(inputs, num_inputs, outputs, num_outputs, classes_1based_dev, static_cast<cudaStream_t>(stream));
+}
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input) {
     SNNB_REQUIRE(m, "snnb_model_set_input: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));

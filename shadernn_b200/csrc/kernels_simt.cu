@@ -739,7 +739,8 @@ int launch_activation(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out
 
 // ------------------------------------------------------------------------------------------------------------
 // Softmax over channels, per pixel (cpulayer.h:175-191: max-subtracted, fp32). One warp per pixel.
-// Argmax over channels per image -> 0-based index of the FIRST maximum (core.cpp:228-233 adds 1 at the API).
+// Argmax over channels per image -> index of the FIRST maximum plus base_index (0 where the host adds 1 at the API,
+// core.cpp:228-233; 1 where the 1-based classes stay in device memory).
 // ------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) softmax_kernel(TV in, TV out) {
     pdl_wait();
@@ -763,7 +764,7 @@ int launch_softmax(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out) {
     return launch_done(ctx, launch_k(softmax_kernel, dim3((unsigned) ((px * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), view(out)), "softmax_kernel");
 }
 
-__global__ void __launch_bounds__(128) argmax_kernel(TV in, int* __restrict__ idx) {
+__global__ void __launch_bounds__(128) argmax_kernel(TV in, int* __restrict__ idx, int base_index) {
     pdl_wait();
     const int n    = (int) (((long long) blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const int lane = threadIdx.x & 31;
@@ -780,7 +781,7 @@ __global__ void __launch_bounds__(128) argmax_kernel(TV in, int* __restrict__ id
         int oi   = __shfl_xor_sync(0xffffffffu, bi, o);
         if (ob > best || (ob == best && oi < bi)) best = ob, bi = oi;
     }
-    if (lane == 0) idx[n] = bi;
+    if (lane == 0) idx[n] = bi + base_index;
 }
 // Classifier result in one launch: fp32 values of a 1x1xC tensor and/or the arg-max per image, written wherever the pointers point -
 // the streaming path hands in MAPPED PINNED HOST memory, so a small result needs no device->host copy commands at all.
@@ -809,8 +810,9 @@ int launch_result_small(snnb_context* ctx, const snnb_tensor* in, float* values,
     SNNB_REQUIRE(in->h == 1 && in->w == 1, "launch_result_small: a 1x1 tensor is expected");
     return launch_done(ctx, launch_k(result_small_kernel, dim3((unsigned) (((long long) in->n * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), values, idx), "result_small_kernel");
 }
-int launch_argmax(snnb_context* ctx, const snnb_tensor* in, int* dev_idx) {
-    return launch_done(ctx, launch_k(argmax_kernel, dim3((unsigned) (((long long) in->n * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), dev_idx), "argmax_kernel");
+int launch_argmax(snnb_context* ctx, const snnb_tensor* in, int* dev_idx, int base_index) {
+    return launch_done(ctx, launch_k(argmax_kernel, dim3((unsigned) (((long long) in->n * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), dev_idx, base_index),
+                       "argmax_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1209,6 +1211,138 @@ int launch_merge_u8(snnb_context* ctx, const snnb_tensor* t, uint8_t* dev_nhwc_u
 }
 int launch_merge_f32(snnb_context* ctx, const snnb_tensor* t, float* dev_nhwc) {
     return launch_done(ctx, launch_k(merge_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, view(t), dev_nhwc, feed_view(t)), "merge_kernel");
+}
+
+// Caller-owned device buffers (snnb_model_run_device): F32 / F16 / U8, dense NHWC or NCHW. One thread per (pixel, 8-channel group) as
+// in split_kernel / merge_kernel, and the same values and stores. In NCHW the pixel is the fastest-moving index, so consecutive threads
+// read (write) consecutive pixels of one channel plane; their 16-byte tensor-side vectors are Cp * 2 bytes apart.
+struct EdgeIndex {
+    size_t px;   // linear (n, y, x) pixel
+    int c;       // first channel of the group
+    size_t base; // buffer element of channel 0 of this pixel
+    size_t step; // buffer elements from one channel to the next
+};
+__device__ __forceinline__ EdgeIndex edge_index(size_t gid, const TV& t, int nchw) {
+    const int CG    = t.Cp >> 3;
+    const size_t HW = (size_t) t.H * t.W;
+    EdgeIndex e;
+    if (nchw) {
+        const size_t hw = gid % HW, q = gid / HW;
+        const size_t n  = q / CG;
+        e.c    = (int) (q % CG) * 8;
+        e.px   = n * HW + hw;
+        e.base = n * t.C * HW + hw;
+        e.step = HW;
+    } else {
+        e.px   = gid / CG;
+        e.c    = (int) (gid % CG) * 8;
+        e.base = e.px * t.C;
+        e.step = 1;
+    }
+    return e;
+}
+__device__ __forceinline__ float edge_in(const float* p, int, const U8Norm&) { return __ldg(p); }
+__device__ __forceinline__ float edge_in(const __half* p, int, const U8Norm&) { return __half2float(__ldg(p)); }
+__device__ __forceinline__ float edge_in(const uint8_t* p, int c, const U8Norm& q) { return ((float) __ldg(p) - q.mean[c & 3]) * q.norm[c & 3]; } // = split_u8_kernel
+__device__ __forceinline__ void edge_out(float* p, float v, float, float) { *p = v; }
+__device__ __forceinline__ void edge_out(__half* p, float v, float, float) { *p = __float2half_rn(v); }
+__device__ __forceinline__ void edge_out(uint8_t* p, float v, float scale, float offset) { *p = (uint8_t) fminf(fmaxf(rintf(v * scale + offset), 0.0f), 255.0f); } // = merge_u8_kernel
+
+template <typename T>
+__global__ void device_input_kernel(const T* __restrict__ src, int nchw, TV t, U8Norm q, FeedV f) {
+    pdl_wait();
+    const size_t total = (size_t) t.N * t.H * t.W * (t.Cp >> 3);
+    const size_t gid   = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= total) return;
+    const EdgeIndex e = edge_index(gid, t, nchw);
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = (e.c + j < t.C) ? edge_in(src + e.base + (size_t) (e.c + j) * e.step, e.c + j, q) : 0.0f;
+    if (!f.only) store8(t.hi, t.lo, e.px * t.Cp + e.c, v);
+    if (f.hi) store_feed(f, e.px, t.H, t.W, v);
+}
+// NCHW input with more than 8 channels: a tile of 32 pixels x 64 channels passes through shared memory, so that the reads of a channel
+// plane AND the 16-byte tensor-side stores are contiguous across neighbouring threads. In device_input_kernel those stores are Cp * 2
+// bytes apart and fill sectors partially: at 64 channels it ran 3.3x slower than the NHWC input (H100 80GB HBM3, 400 W power limit,
+// tools/device_io_bench.py).
+// (The NCHW output reads such strided vectors, which cost it far less: it stays direct.) A tensor with a feed copy has <= 4 channels.
+template <typename T>
+__global__ void __launch_bounds__(256) device_input_nchw_tiled_kernel(const T* __restrict__ src, TV t, U8Norm q) {
+    pdl_wait();
+    __shared__ float s[64][33];
+    const int HW = t.H * t.W, hw0 = blockIdx.x * 32, c0 = blockIdx.y * 64, n = blockIdx.z;
+    const T* img = src + (size_t) n * t.C * HW;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const int ch = ty + 8 * k, c = c0 + ch, hw = hw0 + tx;
+        s[ch][tx] = (c < t.C && hw < HW) ? edge_in(img + (size_t) c * HW + hw, c, q) : 0.0f;
+    }
+    __syncthreads();
+    const int g = threadIdx.x & 7, p = threadIdx.x >> 3; // 8 consecutive threads: the 8 channel groups of one pixel
+    const int hw = hw0 + p, c = c0 + g * 8;
+    if (hw >= HW || c >= t.Cp) return;
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = s[g * 8 + j][p];
+    store8(t.hi, t.lo, ((size_t) n * HW + hw) * t.Cp + c, v);
+}
+// A model output is never feed_only (MixedInferenceCore::init), so the regular planes are always the source.
+template <typename T>
+__global__ void device_output_kernel(TV t, T* __restrict__ dst, int nchw, float scale, float offset) {
+    pdl_wait();
+    const size_t total = (size_t) t.N * t.H * t.W * (t.Cp >> 3);
+    const size_t gid   = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= total) return;
+    const EdgeIndex e = edge_index(gid, t, nchw);
+    float v[8];
+    load8(t.hi, t.lo, e.px * t.Cp + e.c, v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+        if (e.c + j < t.C) edge_out(dst + e.base + (size_t) (e.c + j) * e.step, v[j], scale, offset);
+}
+int launch_device_input(snnb_context* ctx, const snnb_device_buffer& b, snnb_tensor* t) {
+    U8Norm q;
+    for (int i = 0; i < 4; ++i) q.mean[i] = b.mean4[i], q.norm[i] = b.norm4[i];
+    const int nchw = b.layout == SNNB_LAYOUT_NCHW ? 1 : 0;
+    if (nchw && t->c > 8 && !t->feed_hi) {
+        const dim3 tiles((unsigned) ((t->h * t->w + 31) / 32), (unsigned) ((t->c + 63) / 64), (unsigned) t->n);
+        switch (b.dtype) {
+        case SNNB_DTYPE_F32:
+            return launch_done(ctx, launch_k(device_input_nchw_tiled_kernel<float>, tiles, dim3(256), 0, ctx->stream, (const float*) b.data, view(t), q),
+                               "device_input_nchw_tiled_kernel<f32>");
+        case SNNB_DTYPE_F16:
+            return launch_done(ctx, launch_k(device_input_nchw_tiled_kernel<__half>, tiles, dim3(256), 0, ctx->stream, (const __half*) b.data, view(t), q),
+                               "device_input_nchw_tiled_kernel<f16>");
+        case SNNB_DTYPE_U8:
+            return launch_done(ctx, launch_k(device_input_nchw_tiled_kernel<uint8_t>, tiles, dim3(256), 0, ctx->stream, (const uint8_t*) b.data, view(t), q),
+                               "device_input_nchw_tiled_kernel<u8>");
+        }
+    }
+    const dim3 grid(vec_blocks(t, 256)), block(256);
+    switch (b.dtype) {
+    case SNNB_DTYPE_F32:
+        return launch_done(ctx, launch_k(device_input_kernel<float>, grid, block, 0, ctx->stream, (const float*) b.data, nchw, view(t), q, feed_view(t)), "device_input_kernel<f32>");
+    case SNNB_DTYPE_F16:
+        return launch_done(ctx, launch_k(device_input_kernel<__half>, grid, block, 0, ctx->stream, (const __half*) b.data, nchw, view(t), q, feed_view(t)), "device_input_kernel<f16>");
+    case SNNB_DTYPE_U8:
+        return launch_done(ctx, launch_k(device_input_kernel<uint8_t>, grid, block, 0, ctx->stream, (const uint8_t*) b.data, nchw, view(t), q, feed_view(t)), "device_input_kernel<u8>");
+    }
+    SNNB_REQUIRE(false, "launch_device_input: unknown dtype %d", b.dtype);
+}
+int launch_device_output(snnb_context* ctx, const snnb_tensor* t, const snnb_device_buffer& b) {
+    SNNB_REQUIRE(!t->feed_only, "launch_device_output: the tensor has no regular planes");
+    const int nchw = b.layout == SNNB_LAYOUT_NCHW ? 1 : 0;
+    const dim3 grid(vec_blocks(t, 256)), block(256);
+    switch (b.dtype) {
+    case SNNB_DTYPE_F32:
+        return launch_done(ctx, launch_k(device_output_kernel<float>, grid, block, 0, ctx->stream, view(t), (float*) b.data, nchw, b.scale, b.offset), "device_output_kernel<f32>");
+    case SNNB_DTYPE_F16:
+        return launch_done(ctx, launch_k(device_output_kernel<__half>, grid, block, 0, ctx->stream, view(t), (__half*) b.data, nchw, b.scale, b.offset), "device_output_kernel<f16>");
+    case SNNB_DTYPE_U8:
+        return launch_done(ctx, launch_k(device_output_kernel<uint8_t>, grid, block, 0, ctx->stream, view(t), (uint8_t*) b.data, nchw, b.scale, b.offset), "device_output_kernel<u8>");
+    }
+    SNNB_REQUIRE(false, "launch_device_output: unknown dtype %d", b.dtype);
 }
 
 } // namespace snnb

@@ -216,7 +216,7 @@ int launch_add(snnb_context* ctx, const snnb_tensor* a, const snnb_tensor* b, sn
 int launch_batchnorm(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, const snnb_weights* w, int act, float alpha);
 int launch_activation(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, int act, float alpha);
 int launch_softmax(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out);
-int launch_argmax(snnb_context* ctx, const snnb_tensor* in, int* dev_idx);
+int launch_argmax(snnb_context* ctx, const snnb_tensor* in, int* dev_idx, int base_index = 0); // dev_idx[n] = arg-max of image n + base_index
 // YOLO decode, device part: cells whose score can pass `thresh` -> ONE candidate list [maxc][8] = {image, scan index, d0..d5}; counts[0] = its length
 int launch_yolo_candidates(snnb_context* ctx, const snnb_tensor* h0, const snnb_tensor* h1, float thresh, int maxc, int* counts, float* cand);
 int launch_flatten(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out);
@@ -235,6 +235,11 @@ int launch_result_small(snnb_context* ctx, const snnb_tensor* t, float* values, 
 // u8 NHWC image of size src_h x src_w -> resized (linear / nearest, vk_resize.comp) + normalised -> t
 int launch_resize_u8(snnb_context* ctx, const uint8_t* dev_nhwc_u8, int src_h, int src_w, snnb_tensor* t, const float mean[4], const float norm[4], bool linear);
 int launch_merge_u8(snnb_context* ctx, const snnb_tensor* t, uint8_t* dev_nhwc_u8, float scale, float offset); // clamp(round(v*scale+offset), 0, 255)
+// Caller-owned device buffers (snnb_model_run_device): dense F32 / F16 / U8 (SNNB_DTYPE_*) in NHWC or NCHW (SNNB_LAYOUT_*).
+// Input: the values split_kernel / split_u8_kernel would write (U8 normalised with b.mean4 / b.norm4), feed copy included.
+// Output: hi + lo as F32, __float2half_rn of it as F16, clamp(round(v * b.scale + b.offset), 0, 255) as U8. Never reads a feed copy.
+int launch_device_input(snnb_context* ctx, const snnb_device_buffer& b, snnb_tensor* t);
+int launch_device_output(snnb_context* ctx, const snnb_tensor* t, const snnb_device_buffer& b);
 
 // ---- host-side weight folding/packing (pack.cpp) -----------------------------------------------------------
 // K ordering of the row-window convolution kernel (kernels_umma.cu): for stride s the taps of one filter row fall

@@ -1,0 +1,221 @@
+"""Device-resident inputs and outputs (snnb_model_run_device through MixedInferenceCore.run_torch) against the host paths, on one GPU.
+
+    python tools/device_io_bench.py --out DIR [--seconds 2] [--rounds 3]
+
+Writes DIR/device_io_bench.json and prints it. Three parts, all in one process:
+
+  throughput   ResNet-18 224x224 batch 32 fed with uint8 NCHW images already on the GPU (what a GPU JPEG decoder returns), device
+               classes and logits out, against snnb_model_submit_u8 / snnb_model_wait from pinned host uint8 NHWC images; and Candy 720x720
+               batch 8, uint8 NCHW in and uint8 NCHW out, against snnb_model_submit_image / wait with pinned host uint8 in and out. The two
+               paths alternate, `rounds` times, each for at least `seconds` after warm-up; frames/s = images over host time ending in a
+               device synchronise.
+  conversions  each conversion kernel's device time, from torch.profiler (CUDA activity) over 50 calls per configuration in a run of its
+               own, and bytes read + written (from shapes) over that time against the H100 SXM's 3.35 TB/s of HBM3: the kernels do no
+               arithmetic to speak of, so HBM bandwidth is their bound. A 64-channel tensor compares NCHW with NHWC, the case where the
+               tensor-side accesses of NCHW threads are strided.
+  card         name, power limit and maximum SM clock, read by nvidia-smi in the same run.
+"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import tempfile
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+HBM_BYTES_PER_S = 3.35e12  # H100 SXM data sheet
+
+
+def card():
+    q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True)
+    name, power, clock = [s.strip() for s in q.stdout.strip().split(",")] if q.returncode == 0 else ("?", "?", "?")
+    return {"name": name, "power_limit": power, "sm_clock_max": clock}
+
+
+def timed(fn, seconds, batch, sync):
+    """Call fn() until `seconds` have passed; frames/s over the host time of the calls plus the final synchronise."""
+    n, t0 = 0, time.perf_counter()
+    while True:
+        fn()
+        n += 1
+        if n % 8 == 0 and time.perf_counter() - t0 >= seconds:
+            break
+    sync()
+    dt = time.perf_counter() - t0
+    return {"frames_per_s": n * batch / dt, "calls": n, "seconds": dt}
+
+
+class HostPipeline:
+    """Double-buffered snnb_model_submit_u8 / submit_image + wait from pinned host buffers (bench.py's e2e loop)."""
+
+    def __init__(self, torch, m, images_u8_nhwc, mean4, norm4, image_out):
+        from shadernn_b200._lib import ImageIO
+        self.m, self.image_out, self.mean4, self.norm4 = m, image_out, mean4, norm4
+        self.ins = [torch.from_numpy(images_u8_nhwc).pin_memory() for _ in range(2)]
+        n_out = int(np.prod(m.output_shape(0)))
+        self.outs = [torch.empty(n_out, dtype=torch.uint8 if image_out else torch.float32).pin_memory() for _ in range(2)]
+        self.cls = [torch.zeros(m.batch, dtype=torch.int32).pin_memory() for _ in range(2)]
+        self.io = []
+        for i in range(2):
+            io = ImageIO()
+            _, h, w, _ = images_u8_nhwc.shape
+            io.input_u8, io.src_height, io.src_width, io.linear_filter = self.ins[i].data_ptr(), h, w, 1
+            io.mean4, io.norm4 = (C.c_float * 4)(*mean4), (C.c_float * 4)(*norm4)
+            io.output_u8, io.output_capacity, io.out_scale, io.out_offset = self.outs[i].data_ptr(), n_out, 1.0, 0.0
+            self.io.append(io)
+        self.pending, self.i = None, 0
+
+    def step(self):
+        from shadernn_b200._lib import check, lib
+        k = self.i & 1
+        if self.image_out:
+            t = C.c_int()
+            check(lib().snnb_model_submit_image(self.m.h, C.byref(self.io[k]), C.byref(t)), "snnb_model_submit_image")
+            t = t.value
+        else:
+            t = self.m.submit_u8_raw(self.ins[k].data_ptr(), self.mean4, self.norm4, self.outs[k].data_ptr(), self.outs[k].numel(), self.cls[k].data_ptr())
+        if self.pending is not None:
+            self.m.wait(self.pending)
+        self.pending, self.i = t, self.i + 1
+
+    def drain(self):
+        if self.pending is not None:
+            self.m.wait(self.pending)
+            self.pending = None
+
+
+def throughput(torch, ctx, core, modelzoo, d, args):
+    res = {}
+    cases = [("resnet18", (224, 224), 32, ([127.5] * 4, [1.0 / 127.5] * 4), False), ("candy", (720, 720), 8, ([0.0] * 4, [1.0] * 4), True)]
+    for name, hw, batch, (mean4, norm4), image_out in cases:
+        path, _ = modelzoo.build(name, os.path.join(d, name), input_hw=hw)
+        m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+        img = np.random.default_rng(1).integers(0, 256, (batch, hw[0], hw[1], 3), dtype=np.uint8)
+        dev_in = torch.from_numpy(img.transpose(0, 3, 1, 2).copy()).cuda()
+        if image_out:
+            dev = lambda: m.run_torch(dev_in, layout="nchw", mean4=mean4, norm4=norm4, out_dtype=torch.uint8, out_layout="nchw")  # noqa: E731
+        else:
+            dev = lambda: m.run_torch(dev_in, layout="nchw", mean4=mean4, norm4=norm4, want_classes=True)  # noqa: E731
+        hp = HostPipeline(torch, m, img, mean4, norm4, image_out)
+        for _ in range(5):
+            dev()
+            hp.step()
+        hp.drain()
+        torch.cuda.synchronize()
+        rounds = []
+        for _ in range(args.rounds):
+            r_dev = timed(dev, args.seconds, batch, torch.cuda.synchronize)
+            r_host = timed(hp.step, args.seconds, batch, hp.drain)
+            rounds.append({"device": r_dev, "host": r_host})
+        med = lambda k: float(np.median([r[k]["frames_per_s"] for r in rounds]))  # noqa: E731
+        res[name] = {
+            "shape": "%dx%d batch %d" % (hw[0], hw[1], batch),
+            "device_path": "run_torch: uint8 NCHW CUDA tensor in, " + ("uint8 NCHW CUDA tensor out" if image_out else "fp32 logits + int32 classes as CUDA tensors out"),
+            "host_path": ("snnb_model_submit_image/wait: pinned uint8 NHWC in, pinned uint8 NHWC out" if image_out else
+                          "snnb_model_submit_u8/wait: pinned uint8 NHWC in, pinned fp32 logits + classes out"),
+            "device_frames_per_s_median": med("device"),
+            "host_frames_per_s_median": med("host"),
+            "device_over_host": med("device") / med("host"),
+            "rounds": rounds,
+        }
+        m.close()
+    return res
+
+
+def kernel_times_us(torch, fn, calls):
+    """Average device time (us) per launch of the input and the output conversion kernel fn() launches (device_input*_kernel,
+    device_output_kernel)."""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(5):
+        fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            fn()
+        torch.cuda.synchronize()
+    out = {}
+    for e in prof.key_averages():
+        if "snnb::device_input" in e.key or "snnb::device_output" in e.key:
+            total = getattr(e, "device_time_total", None)
+            total = e.cuda_time_total if total is None else total
+            kind = "input" if "snnb::device_input" in e.key else "output"
+            out[kind] = {"kernel": e.key, "launches": e.count, "us_per_launch": total / e.count}
+    return out
+
+
+def conversions(torch, ctx, core, modelzoo, d, calls=50):
+    res = []
+    # (label, model, hw, batch, input dtype, input layout, output dtype, output layout, bytes read + written per pixel by the input kernel
+    # and by the output kernel). The tensor side is split-fp16: 2 planes x 2 bytes x Cp (= C rounded up to 8) per pixel; ResNet-18's input
+    # is read by its stem alone, so only the 4-channel feed copy is written (2 planes x 2 bytes x 4).
+    b = modelzoo.Builder()
+    b.batchnorm(b.input(112, 112, 64))
+    wide = modelzoo.write_model(b.layers, os.path.join(d, "bn64.json"))
+    cases = [
+        ("resnet18 u8 nchw in (feed copy only)", "resnet18", (224, 224), 32, torch.uint8, "nchw", None, None, 3 * 1 + 16, None),
+        ("candy u8 nchw in / u8 nchw out", "candy", (720, 720), 8, torch.uint8, "nchw", torch.uint8, "nchw", 3 * 1 + 32, 32 + 3 * 1),
+        ("candy f32 nhwc in / f32 nhwc out", "candy", (720, 720), 8, torch.float32, "nhwc", torch.float32, "nhwc", 3 * 4 + 32, 32 + 3 * 4),
+        ("64 channels f32 nhwc in / out", wide, (112, 112), 32, torch.float32, "nhwc", torch.float32, "nhwc", 64 * 4 + 64 * 4, 64 * 4 + 64 * 4),
+        ("64 channels f32 nchw in / out", wide, (112, 112), 32, torch.float32, "nchw", torch.float32, "nchw", 64 * 4 + 64 * 4, 64 * 4 + 64 * 4),
+        ("64 channels f16 nchw in / out", wide, (112, 112), 32, torch.float16, "nchw", torch.float16, "nchw", 64 * 2 + 64 * 4, 64 * 4 + 64 * 2),
+    ]
+    paths = {}
+    for label, name, hw, batch, din, lin, dout, lout, in_bpp, out_bpp in cases:
+        if name.endswith(".json"):
+            path = name
+        else:
+            if (name, hw) not in paths:
+                paths[(name, hw)], _ = modelzoo.build(name, os.path.join(d, "%s_%d" % (name, hw[0])), input_hw=hw)
+            path = paths[(name, hw)]
+        m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+        n, h, w, c = m.input_shape(0)
+        shape = (n, h, w, c) if lin == "nhwc" else (n, c, h, w)
+        x = (torch.randint(0, 256, shape, dtype=torch.uint8) if din == torch.uint8 else torch.rand(shape).to(din)).cuda()
+        kw = {"layout": lin}
+        if dout is not None:
+            kw.update(out_dtype=dout, out_layout=lout)
+        times = kernel_times_us(torch, lambda: m.run_torch(x, **kw), calls)
+        px = n * h * w
+        for kind, bpp in (("input", in_bpp), ("output", out_bpp)):
+            if bpp is None or kind not in times:
+                continue
+            t = times[kind]
+            nbytes = px * bpp
+            t.update({"case": label, "bytes": nbytes, "bytes_per_s": nbytes / (t["us_per_launch"] * 1e-6)})
+            t["share_of_hbm_peak"] = t["bytes_per_s"] / HBM_BYTES_PER_S
+            t["bound"] = "HBM bandwidth (3.35 TB/s, H100 SXM data sheet)"
+            res.append(t)
+        m.close()
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--out", required=True)
+    ap.add_argument("--seconds", type=float, default=2.0)
+    ap.add_argument("--rounds", type=int, default=3)
+    args = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("device_io_bench: no CUDA device; this measurement needs the GPU")
+    from shadernn_b200 import core, modelzoo
+    os.makedirs(args.out, exist_ok=True)
+    d = tempfile.mkdtemp(prefix="snnb_devio_")
+    ctx = core.GpuContext(0)
+    result = {"card": card(), "torch_device_name": torch.cuda.get_device_name(0)}
+    result["throughput"] = throughput(torch, ctx, core, modelzoo, d, args)
+    result["conversions"] = conversions(torch, ctx, core, modelzoo, d)
+    text = json.dumps(result, indent=1)
+    with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
+        f.write(text)
+    print(text)
+
+
+if __name__ == "__main__":
+    main()
