@@ -249,14 +249,24 @@ typedef struct {
  *   on the context's stream, behind two events per model (the caller's stream -> the context's stream -> the caller's stream), so calls
  *   from different streams, and calls mixed with run() / submit(), are serialised on the model's tensors. A stream that is being
  *   captured is refused: capturing this call into the caller's CUDA graph is not supported.
- * - The batch is the loaded batch. A model whose output 0 is a YOLO layer is refused: its detections come through the host paths
- *   (run() / submit() + snnb_model_get_boxes).
+ * - The batch is the loaded batch. A model whose output 0 is a YOLO layer is refused: its detections come through
+ *   snnb_model_detect_device below, or the host paths (run() / submit() + snnb_model_get_boxes).
  * Every argument is checked on the host before anything is enqueued: null pointers, unknown dtype or layout, the input count, buffers
  * that cudaPointerGetAttributes does not report as device or managed memory of the context's device, and misaligned buffers are errors
  * (snnb_last_error()) with no work enqueued. A buffer's size cannot be checked: it must hold its tensor's elements. Cost beyond the
  * forward pass: one kernel launch per input, one per output and one for the classes. */
 int snnb_model_run_device(snnb_model* m, const snnb_device_buffer* inputs, int num_inputs, const snnb_device_buffer* outputs, int num_outputs,
                           int* classes_1based_dev, void* stream);
+/* Detectors on device-resident inputs: the forward pass, then YOLO decode + score sort + NMS (yololayer.cpp:56-226) on the device.
+ * inputs: exactly as snnb_model_run_device. rows_dev: float32 [batch][max_rows][6] {class, score, x, y, w, h}, rows past an image's
+ * count are zero; counts_dev: int32 [batch], min(kept boxes, max_rows, 100) per image, as snnb_model_get_boxes counts them.
+ * 1 <= max_rows <= 100. Same stream contract, fences and host-side argument checks as snnb_model_run_device; refused for a model
+ * without a YOLO output. Does not touch the host detections that snnb_model_get_boxes returns.
+ * The rows are those of the host paths, in the same order, with one difference in arithmetic: the device uses the correctly rounded
+ * exponential, (float) exp((double) x), where the host calls the C library's expf, so a score or coordinate can differ in its last
+ * bit or two. Cost beyond the forward pass: one kernel launch per input, one memset and three decode kernels. */
+int snnb_model_detect_device(snnb_model* m, const snnb_device_buffer* inputs, int num_inputs, float* rows_dev, int max_rows,
+                             int* counts_dev, void* stream);
 /* Device-resident variant: inputs already uploaded with snnb_model_set_input(); forward only, asynchronous. */
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input_nhwc);
 int snnb_model_forward(snnb_model* m);

@@ -140,6 +140,7 @@ SIGNATURES = {
     "snnb_model_submit_image": (C.c_int, [vp, C.POINTER(ImageIO), c_int_p]),
     "snnb_model_wait": (C.c_int, [vp, C.c_int]),
     "snnb_model_run_device": (C.c_int, [vp, C.POINTER(DeviceBuffer), C.c_int, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
+    "snnb_model_detect_device": (C.c_int, [vp, C.POINTER(DeviceBuffer), C.c_int, vp, C.c_int, vp, vp]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),

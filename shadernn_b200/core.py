@@ -424,6 +424,44 @@ class MixedInferenceCore:
     def wait(self, ticket):
         check(lib().snnb_model_wait(self.h, int(ticket)), "snnb_model_wait")
 
+    _TORCH_LAYOUTS = {"nhwc": _lib.LAYOUT_NHWC, "nchw": _lib.LAYOUT_NCHW}
+
+    @staticmethod
+    def _torch_dtypes():
+        import torch
+        return {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.uint8: _lib.DTYPE_U8}
+
+    @staticmethod
+    def _nhwc_as(shape, layout):
+        n, h, w, c = shape
+        return (n, h, w, c) if layout == "nhwc" else (n, c, h, w)
+
+    def _device_inputs(self, who, inputs, layout, mean4, norm4):
+        """The snnb_device_buffer array for run_torch / detect_torch: returns (the contiguous tensors, which must stay alive until the
+        call has enqueued its reads, the buffers)."""
+        import torch
+        dtypes = self._torch_dtypes()
+        if layout not in self._TORCH_LAYOUTS:
+            raise ValueError("%s: layout %r: expected 'nhwc' or 'nchw'" % (who, layout))
+        xs = [inputs] if isinstance(inputs, torch.Tensor) else list(inputs)
+        keep = [x.contiguous() for x in xs]  # the stream fence orders any reuse of the memory after the reads
+        ins = (_lib.DeviceBuffer * max(1, len(keep)))()
+        for i, x in enumerate(keep):
+            if x.dtype not in dtypes:
+                raise ValueError("%s: input %d has dtype %s; float32, float16 or uint8 is supported" % (who, i, x.dtype))
+            want = self._nhwc_as(self.input_shape(i), layout) if i < self.num_inputs else None
+            if want is not None and tuple(x.shape) != want:
+                raise ValueError("%s: input %d has shape %s, the model takes %s (%s)" % (who, i, tuple(x.shape), want, layout))
+            ins[i].data, ins[i].dtype, ins[i].layout = x.data_ptr(), dtypes[x.dtype], self._TORCH_LAYOUTS[layout]
+            ins[i].mean4 = (C.c_float * 4)(*[float(v) for v in (mean4 if mean4 is not None else [0.0] * 4)])
+            ins[i].norm4 = (C.c_float * 4)(*[float(v) for v in (norm4 if norm4 is not None else [1.0] * 4)])
+        return keep, ins
+
+    def _torch_stream(self):
+        import torch
+        # torch's default stream is the legacy NULL stream, which the library reads as "the context's stream": name it cudaStreamLegacy (1)
+        return torch.cuda.current_stream(torch.device("cuda", self.ctx.device)).cuda_stream or 1
+
     def run_torch(self, inputs, layout="nhwc", mean4=None, norm4=None, out_dtype=None, out_layout="nhwc", out_scale=1.0, out_offset=0.0,
                   want_classes=False):
         """snnb_model_run_device with torch CUDA tensors, ordered on the current torch stream and never synchronising.
@@ -434,39 +472,37 @@ class MixedInferenceCore:
         in out_layout. Returns output 0 for a one-output model, else the list of outputs; with want_classes, (outputs, the 1-based
         classes as a device int32 tensor)."""
         import torch
-        dtypes = {torch.float32: _lib.DTYPE_F32, torch.float16: _lib.DTYPE_F16, torch.uint8: _lib.DTYPE_U8}
-        layouts = {"nhwc": _lib.LAYOUT_NHWC, "nchw": _lib.LAYOUT_NCHW}
+        dtypes, layouts = self._torch_dtypes(), self._TORCH_LAYOUTS
         out_dtype = torch.float32 if out_dtype is None else out_dtype
         if out_dtype not in dtypes or layout not in layouts or out_layout not in layouts:
             raise ValueError("run_torch: dtype %s / layouts %r, %r: expected float32, float16 or uint8 and 'nhwc' or 'nchw'" % (out_dtype, layout, out_layout))
-
-        def shape_in(shape, lay):
-            n, h, w, c = shape
-            return (n, h, w, c) if lay == "nhwc" else (n, c, h, w)
-
-        xs = [inputs] if isinstance(inputs, torch.Tensor) else list(inputs)
-        keep = [x.contiguous() for x in xs]  # alive until the call has enqueued its reads; the stream fence orders any reuse after them
-        ins = (_lib.DeviceBuffer * max(1, len(keep)))()
-        for i, x in enumerate(keep):
-            if x.dtype not in dtypes:
-                raise ValueError("run_torch: input %d has dtype %s; float32, float16 or uint8 is supported" % (i, x.dtype))
-            if i < self.num_inputs and tuple(x.shape) != shape_in(self.input_shape(i), layout):
-                raise ValueError("run_torch: input %d has shape %s, the model takes %s (%s)" % (i, tuple(x.shape), shape_in(self.input_shape(i), layout), layout))
-            ins[i].data, ins[i].dtype, ins[i].layout = x.data_ptr(), dtypes[x.dtype], layouts[layout]
-            ins[i].mean4 = (C.c_float * 4)(*[float(v) for v in (mean4 if mean4 is not None else [0.0] * 4)])
-            ins[i].norm4 = (C.c_float * 4)(*[float(v) for v in (norm4 if norm4 is not None else [1.0] * 4)])
+        keep, ins = self._device_inputs("run_torch", inputs, layout, mean4, norm4)
         device = torch.device("cuda", self.ctx.device)
-        outs = [torch.empty(shape_in(self.output_shape(j), out_layout), dtype=out_dtype, device=device) for j in range(self.num_outputs)]
+        outs = [torch.empty(self._nhwc_as(self.output_shape(j), out_layout), dtype=out_dtype, device=device) for j in range(self.num_outputs)]
         obufs = (_lib.DeviceBuffer * max(1, len(outs)))()
         for j, o in enumerate(outs):
             obufs[j].data, obufs[j].dtype, obufs[j].layout = o.data_ptr(), dtypes[out_dtype], layouts[out_layout]
             obufs[j].scale, obufs[j].offset = float(out_scale), float(out_offset)
         classes = torch.empty(self.batch, dtype=torch.int32, device=device) if want_classes else None
-        # torch's default stream is the legacy NULL stream, which the library reads as "the context's stream": name it cudaStreamLegacy (1)
-        stream = torch.cuda.current_stream(device).cuda_stream or 1
-        check(lib().snnb_model_run_device(self.h, ins, len(keep), obufs, len(outs), classes.data_ptr() if want_classes else None, stream), "snnb_model_run_device")
+        check(lib().snnb_model_run_device(self.h, ins, len(keep), obufs, len(outs), classes.data_ptr() if want_classes else None, self._torch_stream()),
+              "snnb_model_run_device")
         result = outs[0] if len(outs) == 1 else outs
         return (result, classes) if want_classes else result
+
+    def detect_torch(self, inputs, layout="nhwc", mean4=None, norm4=None, max_rows=100):
+        """snnb_model_detect_device with torch CUDA tensors: the forward pass and the YOLO decode, score sort and NMS on the device,
+        ordered on the current torch stream and never synchronising. Inputs as in run_torch.
+
+        Returns (rows, counts): rows a CUDA float32 tensor batch x max_rows x 6 of {class, score, x, y, w, h}, zero past each image's
+        count; counts a CUDA int32 tensor [batch] with min(kept boxes, max_rows, 100), the rows boxes(n) returns after run()."""
+        import torch
+        keep, ins = self._device_inputs("detect_torch", inputs, layout, mean4, norm4)
+        device = torch.device("cuda", self.ctx.device)
+        rows = torch.empty((self.batch, max(int(max_rows), 0), 6), dtype=torch.float32, device=device)
+        counts = torch.empty(self.batch, dtype=torch.int32, device=device)
+        check(lib().snnb_model_detect_device(self.h, ins, len(keep), rows.data_ptr() or None, int(max_rows), counts.data_ptr(), self._torch_stream()),
+              "snnb_model_detect_device")
+        return rows, counts
 
     def set_input(self, images, idx=0):
         images = _f32(images)

@@ -41,6 +41,7 @@ MixedInferenceCore::~MixedInferenceCore() {
     }
     if (copyStream) cudaStreamDestroy(copyStream);
     if (callerReady) cudaEventDestroy(callerReady);
+    if (detectScratch) cudaFree(detectScratch);
     if (deviceDone) cudaEventDestroy(deviceDone);
 }
 
@@ -628,75 +629,107 @@ static const char* memoryTypeName(cudaMemoryType t) {
     return "unknown memory";
 }
 // A pointer the kernels may dereference: device or managed memory of `device`, aligned to its `elem`-byte elements.
-static int checkDevicePointer(const void* p, size_t elem, int device, const char* what, int idx) {
-    SNNB_REQUIRE(p, "snnb_model_run_device: %s %d: null data pointer", what, idx);
+static int checkDevicePointer(const char* api, const void* p, size_t elem, int device, const char* what, int idx) {
+    SNNB_REQUIRE(p, "%s: %s %d: null data pointer", api, what, idx);
     cudaPointerAttributes a {};
     const cudaError_t e = cudaPointerGetAttributes(&a, p);
     if (e != cudaSuccess) cudaGetLastError(); // not sticky: leave no error behind for the next call
-    SNNB_REQUIRE(e == cudaSuccess, "snnb_model_run_device: %s %d: cudaPointerGetAttributes(%p) failed: %s", what, idx, p, cudaGetErrorString(e));
+    SNNB_REQUIRE(e == cudaSuccess, "%s: %s %d: cudaPointerGetAttributes(%p) failed: %s", api, what, idx, p, cudaGetErrorString(e));
     SNNB_REQUIRE((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device,
-                 "snnb_model_run_device: %s %d: %p is %s of device %d; device or managed memory of device %d is required", what, idx, p, memoryTypeName(a.type), a.device,
+                 "%s: %s %d: %p is %s of device %d; device or managed memory of device %d is required", api, what, idx, p, memoryTypeName(a.type), a.device,
                  device);
-    SNNB_REQUIRE(reinterpret_cast<uintptr_t>(p) % elem == 0, "snnb_model_run_device: %s %d: %p is not aligned to its %zu-byte elements", what, idx, p, elem);
+    SNNB_REQUIRE(reinterpret_cast<uintptr_t>(p) % elem == 0, "%s: %s %d: %p is not aligned to its %zu-byte elements", api, what, idx, p, elem);
     return 0;
 }
-static int checkDeviceBuffer(const snnb_device_buffer& b, int device, const char* what, int idx) {
-    SNNB_REQUIRE(b.dtype == SNNB_DTYPE_F32 || b.dtype == SNNB_DTYPE_F16 || b.dtype == SNNB_DTYPE_U8, "snnb_model_run_device: %s %d: unknown dtype %d", what, idx, b.dtype);
-    SNNB_REQUIRE(b.layout == SNNB_LAYOUT_NHWC || b.layout == SNNB_LAYOUT_NCHW, "snnb_model_run_device: %s %d: unknown layout %d", what, idx, b.layout);
+static int checkDeviceBuffer(const char* api, const snnb_device_buffer& b, int device, const char* what, int idx) {
+    SNNB_REQUIRE(b.dtype == SNNB_DTYPE_F32 || b.dtype == SNNB_DTYPE_F16 || b.dtype == SNNB_DTYPE_U8, "%s: %s %d: unknown dtype %d", api, what, idx, b.dtype);
+    SNNB_REQUIRE(b.layout == SNNB_LAYOUT_NHWC || b.layout == SNNB_LAYOUT_NCHW, "%s: %s %d: unknown layout %d", api, what, idx, b.layout);
     const size_t elem = b.dtype == SNNB_DTYPE_F32 ? 4 : (b.dtype == SNNB_DTYPE_F16 ? 2 : 1);
-    return checkDevicePointer(b.data, elem, device, what, idx);
+    return checkDevicePointer(api, b.data, elem, device, what, idx);
 }
 
-int MixedInferenceCore::runDevice(const snnb_device_buffer* inputs, int numInputs, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev,
-                                  cudaStream_t stream) {
-    // everything is validated before the first enqueue: a refused call leaves no work behind
-    SNNB_REQUIRE(inputs, "snnb_model_run_device: null inputs");
-    SNNB_REQUIRE(numInputs == (int) inputLayers.size(), "snnb_model_run_device: %d inputs given, the model has %d", numInputs, (int) inputLayers.size());
-    SNNB_REQUIRE(numOutputs >= 0 && numOutputs <= (int) outputLayers.size(), "snnb_model_run_device: %d outputs requested, the model has %d", numOutputs,
-                 (int) outputLayers.size());
-    SNNB_REQUIRE(outputs || numOutputs == 0, "snnb_model_run_device: null outputs");
-    SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO",
-                 "snnb_model_run_device: output 0 is a YOLO detection list, which has no device form; use snnb_model_run or snnb_model_submit / snnb_model_wait "
-                 "and read the boxes with snnb_model_get_boxes");
-    const int device = ctx->device;
+int MixedInferenceCore::checkDeviceInputs(const char* api, const snnb_device_buffer* inputs, int numInputs, cudaStream_t stream) {
+    SNNB_REQUIRE(inputs, "%s: null inputs", api);
+    SNNB_REQUIRE(numInputs == (int) inputLayers.size(), "%s: %d inputs given, the model has %d", api, numInputs, (int) inputLayers.size());
     for (int i = 0; i < numInputs; ++i)
-        if (int rc = checkDeviceBuffer(inputs[i], device, "input", i)) return rc;
-    for (int j = 0; j < numOutputs; ++j) {
-        if (!outputs[j].data) continue;
-        SNNB_REQUIRE(outputLayers[j]->output, "snnb_model_run_device: output %d (%s) has no device tensor", j, outputLayers[j]->name.c_str());
-        if (int rc = checkDeviceBuffer(outputs[j], device, "output", j)) return rc;
-    }
-    if (classes1Dev) {
-        SNNB_REQUIRE(isClassifier, "snnb_model_run_device: classes requested, but the model is not a classifier (output 0 is not 1 x 1 x C with C > 1)");
-        if (int rc = checkDevicePointer(classes1Dev, sizeof(int), device, "classes", 0)) return rc;
-    }
+        if (int rc = checkDeviceBuffer(api, inputs[i], ctx->device, "input", i)) return rc;
     if (stream) {
         cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
         const cudaError_t e = cudaStreamIsCapturing(stream, &cap);
         if (e != cudaSuccess) cudaGetLastError();
-        SNNB_REQUIRE(e == cudaSuccess, "snnb_model_run_device: stream %p: %s", (void*) stream, cudaGetErrorString(e));
-        SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone, "snnb_model_run_device: stream %p is being captured; capture into the caller's CUDA graph is not supported",
-                     (void*) stream);
+        SNNB_REQUIRE(e == cudaSuccess, "%s: stream %p: %s", api, (void*) stream, cudaGetErrorString(e));
+        SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone, "%s: stream %p is being captured; capture into the caller's CUDA graph is not supported", api, (void*) stream);
     }
+    return 0;
+}
+
+// The caller's stream -> the context's stream, the input conversions and the forward pass. Called after every check has passed.
+int MixedInferenceCore::enqueueDeviceForward(const snnb_device_buffer* inputs, int numInputs, cudaStream_t stream) {
     if (!callerReady) SNNB_CUDA_OK(cudaEventCreateWithFlags(&callerReady, cudaEventDisableTiming));
     if (!deviceDone) SNNB_CUDA_OK(cudaEventCreateWithFlags(&deviceDone, cudaEventDisableTiming));
-
-    const bool fence = stream && stream != ctx->stream;
-    if (fence) { // a stream of another device fails here, before anything is launched
+    if (stream && stream != ctx->stream) { // a stream of another device fails here, before anything is launched
         SNNB_CUDA_OK(cudaEventRecord(callerReady, stream));
         SNNB_CUDA_OK(cudaStreamWaitEvent(ctx->stream, callerReady, 0));
     }
     for (int i = 0; i < numInputs; ++i)
         if (launch_device_input(ctx, inputs[i], inputLayers[i]->output)) return 1;
-    if (forward()) return 1;
-    for (int j = 0; j < numOutputs; ++j)
-        if (outputs[j].data && launch_device_output(ctx, outputLayers[j]->output, outputs[j])) return 1;
-    if (classes1Dev && launch_argmax(ctx, outputLayers[0]->output, classes1Dev, 1)) return 1; // core.cpp:228-233: argmax + 1
-    if (fence) {
+    return forward();
+}
+
+// The context's stream -> the caller's: work enqueued on `stream` from now on sees everything enqueued above.
+int MixedInferenceCore::fenceToCaller(cudaStream_t stream) {
+    if (stream && stream != ctx->stream) {
         SNNB_CUDA_OK(cudaEventRecord(deviceDone, ctx->stream));
         SNNB_CUDA_OK(cudaStreamWaitEvent(stream, deviceDone, 0));
     }
     return 0;
+}
+
+int MixedInferenceCore::runDevice(const snnb_device_buffer* inputs, int numInputs, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev,
+                                  cudaStream_t stream) {
+    // everything is validated before the first enqueue: a refused call leaves no work behind
+    static const char* api = "snnb_model_run_device";
+    SNNB_REQUIRE(numOutputs >= 0 && numOutputs <= (int) outputLayers.size(), "snnb_model_run_device: %d outputs requested, the model has %d", numOutputs,
+                 (int) outputLayers.size());
+    SNNB_REQUIRE(outputs || numOutputs == 0, "snnb_model_run_device: null outputs");
+    SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO",
+                 "snnb_model_run_device: output 0 is a YOLO detection list; use snnb_model_detect_device for device detections, or snnb_model_run or "
+                 "snnb_model_submit / snnb_model_wait and read the boxes with snnb_model_get_boxes");
+    if (int rc = checkDeviceInputs(api, inputs, numInputs, stream)) return rc;
+    const int device = ctx->device;
+    for (int j = 0; j < numOutputs; ++j) {
+        if (!outputs[j].data) continue;
+        SNNB_REQUIRE(outputLayers[j]->output, "snnb_model_run_device: output %d (%s) has no device tensor", j, outputLayers[j]->name.c_str());
+        if (int rc = checkDeviceBuffer(api, outputs[j], device, "output", j)) return rc;
+    }
+    if (classes1Dev) {
+        SNNB_REQUIRE(isClassifier, "snnb_model_run_device: classes requested, but the model is not a classifier (output 0 is not 1 x 1 x C with C > 1)");
+        if (int rc = checkDevicePointer(api, classes1Dev, sizeof(int), device, "classes", 0)) return rc;
+    }
+
+    if (enqueueDeviceForward(inputs, numInputs, stream)) return 1;
+    for (int j = 0; j < numOutputs; ++j)
+        if (outputs[j].data && launch_device_output(ctx, outputLayers[j]->output, outputs[j])) return 1;
+    if (classes1Dev && launch_argmax(ctx, outputLayers[0]->output, classes1Dev, 1)) return 1; // core.cpp:228-233: argmax + 1
+    return fenceToCaller(stream);
+}
+
+// Detections in device memory: the forward pass, then the whole YOLO decode (threshold, stable score sort, NMS) in three kernels.
+// Reads the heads only: the host detection lists (`boxes`) and the candidate buffers of run() / submit() are not touched.
+int MixedInferenceCore::detectDevice(const snnb_device_buffer* inputs, int numInputs, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
+    static const char* api = "snnb_model_detect_device";
+    SNNB_REQUIRE(yolo, "snnb_model_detect_device: the model has no YOLO output; use snnb_model_run_device");
+    SNNB_REQUIRE(maxRows >= 1 && maxRows <= 100, "snnb_model_detect_device: max_rows %d is outside 1..100", maxRows);
+    if (int rc = checkDeviceInputs(api, inputs, numInputs, stream)) return rc;
+    if (int rc = checkDevicePointer(api, rowsDev, sizeof(float), ctx->device, "rows", 0)) return rc;
+    if (int rc = checkDevicePointer(api, countsDev, sizeof(int), ctx->device, "counts", 0)) return rc;
+    SNNB_REQUIRE(yolo->inputs.size() == 2 && yolo->inputs[0]->c >= 18 && yolo->inputs[1]->c >= 18, "snnb_model_detect_device: %s: YOLO expects two heads of >= 18 channels",
+                 yolo->name.c_str());
+    if (!detectScratch) SNNB_CUDA_OK(cudaMalloc(&detectScratch, yolo_detect_scratch_bytes(yolo->inputs[0], yolo->inputs[1])));
+
+    if (enqueueDeviceForward(inputs, numInputs, stream)) return 1;
+    if (launch_yolo_detect(ctx, yolo->inputs[0], yolo->inputs[1], detectScratch, maxRows, rowsDev, countsDev)) return 1;
+    return fenceToCaller(stream);
 }
 
 int MixedInferenceCore::layerOutput(int layerId, float* host, size_t capacityFloats) {

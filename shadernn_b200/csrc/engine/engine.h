@@ -351,6 +351,8 @@ public:
     int wait(int ticket);
     // snnb_model_run_device: device buffers in and out, fenced against the caller's stream (NULL: the context's); asynchronous
     int runDevice(const snnb_device_buffer* inputs, int numInputs, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
+    // snnb_model_detect_device: runDevice's inputs and fences, then YOLO decode + score sort + NMS on the device into rows / counts
+    int detectDevice(const snnb_device_buffer* inputs, int numInputs, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
     int layerOutput(int layerId, float* host, size_t capacityFloats);
     int timeLayers(std::vector<float>& ms);
     int dumpOutputs(const std::string& dir);
@@ -407,6 +409,12 @@ private:
     int ensureStreaming();
     // runDevice's fences: the caller's stream -> the context's stream (callerReady), and back (deviceDone); created on first use
     cudaEvent_t callerReady = nullptr, deviceDone = nullptr;
+    // shared by runDevice and detectDevice: the host-side checks of the inputs and the stream (nothing enqueued), then the fenced
+    // input conversions + forward pass, and the fence back to the caller's stream
+    int checkDeviceInputs(const char* api, const snnb_device_buffer* inputs, int numInputs, cudaStream_t stream);
+    int enqueueDeviceForward(const snnb_device_buffer* inputs, int numInputs, cudaStream_t stream);
+    int fenceToCaller(cudaStream_t stream);
+    void* detectScratch = nullptr; // detectDevice's per-image keys (yolo_detect_scratch_bytes), allocated on first use
 };
 
 } // namespace snn

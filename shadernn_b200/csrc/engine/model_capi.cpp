@@ -129,6 +129,11 @@ int snnb_model_run_device(snnb_model* m, const snnb_device_buffer* inputs, int n
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->runDevice(inputs, num_inputs, outputs, num_outputs, classes_1based_dev, static_cast<cudaStream_t>(stream));
 }
+int snnb_model_detect_device(snnb_model* m, const snnb_device_buffer* inputs, int num_inputs, float* rows_dev, int max_rows, int* counts_dev, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_detect_device: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->detectDevice(inputs, num_inputs, rows_dev, max_rows, counts_dev, static_cast<cudaStream_t>(stream));
+}
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input) {
     SNNB_REQUIRE(m, "snnb_model_set_input: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));

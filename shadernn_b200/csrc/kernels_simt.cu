@@ -856,6 +856,202 @@ int launch_yolo_candidates(snnb_context* ctx, const snnb_tensor* h0, const snnb_
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// YOLO decode, all on the device (snnb_model_detect_device): exact threshold, stable score sort, greedy NMS per image. The host
+// counterpart is YOLOLayer::decode + nms (layers.cpp: decodeCell, iou, nms; yololayer.cpp:56-164). Arithmetic contract:
+//   - exp is the correctly rounded float exponential, (float) exp((double) x). The host's std::exp (glibc expf) is not correctly
+//     rounded for every input, so a score or box can differ from the host's by the ulp or so that one exp differs.
+//   - every + - * / is an IEEE-rounded intrinsic, so nvcc cannot contract a product and a sum into an FMA; the host build has no
+//     FMA either. Each operation is the host's, in the host's order.
+// Three kernels, one list per image: yolo_select_kernel evaluates every cell and appends a 64-bit key for each one that passes;
+// yolo_rank_kernel sorts the keys by rank; yolo_nms_kernel decodes the boxes in that order and suppresses greedily.
+// ------------------------------------------------------------------------------------------------------------
+namespace yolo_dev { // layers.cpp: kGridScale, kAnchors, kMasks, GC, NFIX, ONUM, kConfThresh, kIouThresh (yololayer.cpp:31-38, 182-183)
+__constant__ int kGridScale[2] = {32, 16};
+__constant__ float kAnchors[12] = {10, 14, 23, 27, 37, 58, 81, 82, 135, 169, 344, 319};
+__constant__ float kMasks[6]    = {3, 4, 5, 1, 2, 3};
+constexpr int GC = 3, NFIX = 5, ONUM = 6;
+constexpr float kConfThresh = 0.35f, kIouThresh = 0.45f;
+constexpr int NMS_THREADS = 128; // candidates resolved per step of yolo_nms_kernel: a 128-bit suppression mask (two words) each
+constexpr int MAX_ROWS    = 100; // snnb_model_get_boxes returns at most 100 rows per image
+}
+
+struct YoloBox {
+    int cls;
+    float score, x, y, w, h;
+};
+__device__ __forceinline__ float exp_cr(float x) { return (float) exp((double) x); }
+
+// decodeCell (layers.cpp) for the cell at `scan` of image n: scan = (head, gy, gx, gc) in the order the host's loops visit the cells.
+// Returns false below the confidence threshold; otherwise out.score is set, and the rest of the box when `box` is set.
+__device__ bool yolo_decode_cell(const TV& h0, const TV& h1, int n, int scan, bool box, YoloBox& out) {
+    using namespace yolo_dev;
+    const int cells0 = h0.H * h0.W * GC;
+    const int yi     = scan >= cells0 ? 1 : 0;
+    const TV& t      = yi ? h1 : h0;
+    const int s = yi ? scan - cells0 : scan, gc = s % GC, cell = s / GC;
+    const int gw = t.W, gh = t.H, gx = cell % gw, gy = cell / gw;
+    const size_t base = ((size_t) n * gh * gw + cell) * t.Cp + gc * ONUM;
+    float d[ONUM];
+#pragma unroll
+    for (int i = 0; i < ONUM; ++i) d[i] = load1(t.hi, t.lo, base + i);
+    int cls        = 0;
+    float maxLogit = -3.402823466e+38f;
+#pragma unroll
+    for (int i = NFIX; i < ONUM; ++i)
+        if (d[i] > maxLogit) maxLogit = d[i], cls = i - NFIX;
+    // prob = 1.f / ((1.f + exp(-d[4]) * (1.f + exp(-maxLogit))))
+    const float prob = __fdiv_rn(1.f, __fadd_rn(1.f, __fmul_rn(exp_cr(-d[4]), __fadd_rn(1.f, exp_cr(-maxLogit)))));
+    if (!(prob > kConfThresh)) return false;
+    out.score = prob;
+    if (!box) return true;
+    const int ai   = (int) kMasks[gc + yi * GC];
+    const float bw = kAnchors[ai * 2], bh = kAnchors[ai * 2 + 1];
+    const int netW = kGridScale[yi] * gw, netH = kGridScale[yi] * gh;
+    // cx = (gx + 1.0f / (1.0f + exp(-d[0]))) / gw, cy likewise; w_ = exp(d[2]) * bw / netW, h_ likewise
+    const float cx = __fdiv_rn(__fadd_rn((float) gx, __fdiv_rn(1.0f, __fadd_rn(1.0f, exp_cr(-d[0])))), (float) gw);
+    const float cy = __fdiv_rn(__fadd_rn((float) gy, __fdiv_rn(1.0f, __fadd_rn(1.0f, exp_cr(-d[1])))), (float) gh);
+    const float w_ = __fdiv_rn(__fmul_rn(exp_cr(d[2]), bw), (float) netW), h_ = __fdiv_rn(__fmul_rn(exp_cr(d[3]), bh), (float) netH);
+    out = YoloBox {cls, prob, __fsub_rn(cx, __fdiv_rn(w_, 2.f)), __fsub_rn(cy, __fdiv_rn(h_, 2.f)), w_, h_};
+    return true;
+}
+// iou (layers.cpp), with std::max(a, b) = a < b ? b : a and std::min(a, b) = b < a ? b : a
+__device__ __forceinline__ float yolo_iou(const YoloBox& a, const YoloBox& b) {
+    const float ix0 = a.x < b.x ? b.x : a.x, iy0 = a.y < b.y ? b.y : a.y;
+    const float ax1 = __fadd_rn(a.x, a.w), bx1 = __fadd_rn(b.x, b.w), ay1 = __fadd_rn(a.y, a.h), by1 = __fadd_rn(b.y, b.h);
+    const float ix1 = bx1 < ax1 ? bx1 : ax1, iy1 = by1 < ay1 ? by1 : ay1;
+    if (ix1 < ix0 || iy1 < iy0) return 0;
+    const float inter = __fmul_rn(__fsub_rn(ix1, ix0), __fsub_rn(iy1, iy0));
+    return __fdiv_rn(inter, __fsub_rn(__fadd_rn(__fmul_rn(a.w, a.h), __fmul_rn(b.w, b.h)), inter));
+}
+// Sort key: std::stable_sort by descending score over the scan-ordered list == descending (score, -scan). Scores are > 0.35, so
+// their bits order like unsigned integers; every key is distinct.
+__device__ __forceinline__ unsigned long long yolo_key(float score, int scan) {
+    return ((unsigned long long) __float_as_uint(score) << 32) | (unsigned long long) (0xffffffffu - (unsigned) scan);
+}
+__device__ __forceinline__ int yolo_key_scan(unsigned long long k) { return (int) (0xffffffffu - (unsigned) (k & 0xffffffffu)); }
+
+// One thread per (cell, anchor) of image blockIdx.y: cells that pass append their key to the image's list (arbitrary order).
+__global__ void __launch_bounds__(256) yolo_select_kernel(TV h0, TV h1, int cap, int* __restrict__ counts, unsigned long long* __restrict__ keys) {
+    pdl_wait();
+    const int n = blockIdx.y, scan = blockIdx.x * blockDim.x + threadIdx.x;
+    if (scan >= cap) return;
+    YoloBox b;
+    if (yolo_decode_cell(h0, h1, n, scan, false, b)) keys[(size_t) n * cap + atomicAdd(&counts[n], 1)] = yolo_key(b.score, scan);
+}
+
+// Rank sort of image blockIdx.y's keys: the rank of a key is the number of larger keys, so sorted[rank] is the descending order.
+// Quadratic in the image's candidate count, spread over the grid; blocks past the count exit at once.
+__global__ void __launch_bounds__(256) yolo_rank_kernel(int cap, const int* __restrict__ counts, const unsigned long long* __restrict__ keys,
+                                                         unsigned long long* __restrict__ sorted) {
+    pdl_wait();
+    __shared__ unsigned long long tile[256];
+    const int n = blockIdx.y, count = counts[n];
+    if ((int) (blockIdx.x * blockDim.x) >= count) return;
+    const unsigned long long* k = keys + (size_t) n * cap;
+    const int i                 = blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned long long mine = i < count ? k[i] : 0ull;
+    int rank = 0;
+    for (int t0 = 0; t0 < count; t0 += 256) {
+        __syncthreads();
+        if (t0 + (int) threadIdx.x < count) tile[threadIdx.x] = k[t0 + threadIdx.x];
+        __syncthreads();
+        const int m = min(256, count - t0);
+        for (int j = 0; j < m; ++j) rank += tile[j] > mine ? 1 : 0;
+    }
+    if (i < count) sorted[(size_t) n * cap + rank] = mine;
+}
+
+// Greedy NMS of image blockIdx.x over its sorted list (nms, layers.cpp): a box is kept unless a kept box before it of the same class
+// overlaps it with IoU > 0.45, which is what the host's loop computes. The list is walked NMS_THREADS candidates at a time: each thread
+// decodes one, tests it against the boxes kept so far and records which earlier candidates of the step would suppress it; thread 0 then
+// resolves the step in order. The walk stops at max_rows kept boxes: later boxes cannot change earlier ones.
+// rows[n][max_rows][6] = {class, score, x, y, w, h}, zero past the count; out_counts[n] = the number of rows.
+__global__ void __launch_bounds__(yolo_dev::NMS_THREADS) yolo_nms_kernel(TV h0, TV h1, int cap, const int* __restrict__ counts,
+                                                                        const unsigned long long* __restrict__ sorted, int max_rows,
+                                                                        float* __restrict__ rows, int* __restrict__ out_counts) {
+    using namespace yolo_dev;
+    pdl_wait();
+    __shared__ YoloBox kept[MAX_ROWS];
+    __shared__ YoloBox step[NMS_THREADS];
+    __shared__ unsigned long long mask[NMS_THREADS][2];
+    __shared__ int live[NMS_THREADS];
+    __shared__ int nkept;
+    const int n = blockIdx.x, tid = threadIdx.x, count = counts[n];
+    const unsigned long long* s = sorted + (size_t) n * cap;
+    if (tid == 0) nkept = 0;
+    __syncthreads();
+    for (int c0 = 0; c0 < count && nkept < max_rows; c0 += NMS_THREADS) {
+        const int i = c0 + tid;
+        YoloBox b {};
+        bool alive = i < count;
+        if (alive) alive = yolo_decode_cell(h0, h1, n, yolo_key_scan(s[i]), true, b);
+        step[tid] = b;
+        const int k0 = nkept;
+        for (int k = 0; k < k0 && alive; ++k)
+            if (kept[k].cls == b.cls && yolo_iou(kept[k], b) > kIouThresh) alive = false;
+        live[tid] = alive ? 1 : 0;
+        __syncthreads();
+        unsigned long long m0 = 0, m1 = 0; // bit j: live candidate j of this step (j < tid) suppresses this one
+        if (alive)
+            for (int j = 0; j < tid; ++j)
+                if (live[j] && step[j].cls == b.cls && yolo_iou(step[j], b) > kIouThresh) {
+                    if (j < 64) m0 |= 1ull << j;
+                    else m1 |= 1ull << (j - 64);
+                }
+        mask[tid][0] = m0, mask[tid][1] = m1;
+        __syncthreads();
+        if (tid == 0) {
+            unsigned long long k0m = 0, k1m = 0; // the candidates of this step kept so far
+            int nk = nkept;
+            for (int j = 0; j < NMS_THREADS && nk < max_rows; ++j) {
+                if (!live[j] || (mask[j][0] & k0m) || (mask[j][1] & k1m)) continue;
+                if (j < 64) k0m |= 1ull << j;
+                else k1m |= 1ull << (j - 64);
+                kept[nk++] = step[j];
+            }
+            nkept = nk;
+        }
+        __syncthreads();
+    }
+    const int nk = nkept;
+    float* r = rows + (size_t) n * max_rows * 6;
+    for (int e = tid; e < max_rows * 6; e += NMS_THREADS) {
+        const int k = e / 6, f = e % 6;
+        float v = 0.0f;
+        if (k < nk) {
+            const YoloBox& b = kept[k];
+            v = f == 0 ? (float) b.cls : f == 1 ? b.score : f == 2 ? b.x : f == 3 ? b.y : f == 4 ? b.w : b.h;
+        }
+        r[e] = v;
+    }
+    if (tid == 0) out_counts[n] = nk;
+}
+
+// scratch: the candidate count of every image (rounded up to 256 bytes), then the keys and the sorted keys, [N][cells per image] each
+static size_t yolo_counts_bytes(int N) { return ((size_t) N * sizeof(int) + 255) & ~(size_t) 255; }
+static long long yolo_cells(const snnb_tensor* h0, const snnb_tensor* h1) { return ((long long) h0->h * h0->w + (long long) h1->h * h1->w) * yolo_dev::GC; }
+size_t yolo_detect_scratch_bytes(const snnb_tensor* h0, const snnb_tensor* h1) {
+    return yolo_counts_bytes(h0->n) + (size_t) h0->n * (size_t) yolo_cells(h0, h1) * 2 * sizeof(unsigned long long);
+}
+int launch_yolo_detect(snnb_context* ctx, const snnb_tensor* h0, const snnb_tensor* h1, void* scratch, int max_rows, float* rows, int* out_counts) {
+    SNNB_REQUIRE(h0->n == h1->n && h0->c >= yolo_dev::GC * yolo_dev::ONUM && h1->c >= yolo_dev::GC * yolo_dev::ONUM, "launch_yolo_detect: two heads of >= 18 channels");
+    SNNB_REQUIRE(max_rows >= 1 && max_rows <= yolo_dev::MAX_ROWS, "launch_yolo_detect: max_rows %d is outside 1..%d", max_rows, yolo_dev::MAX_ROWS);
+    const long long capl = yolo_cells(h0, h1);
+    SNNB_REQUIRE(capl < 0x7fffffffLL, "launch_yolo_detect: %lld cells per image", capl);
+    const int cap = (int) capl, N = h0->n;
+    int* counts  = static_cast<int*>(scratch);
+    auto* keys   = reinterpret_cast<unsigned long long*>(static_cast<char*>(scratch) + yolo_counts_bytes(N));
+    auto* sorted = keys + (size_t) N * cap;
+    SNNB_CUDA_OK(cudaMemsetAsync(counts, 0, sizeof(int) * N, ctx->stream));
+    const dim3 grid((unsigned) ((cap + 255) / 256), (unsigned) N);
+    if (launch_done(ctx, launch_k(yolo_select_kernel, grid, dim3(256), 0, ctx->stream, view(h0), view(h1), cap, counts, keys), "yolo_select_kernel")) return 1;
+    if (launch_done(ctx, launch_k(yolo_rank_kernel, grid, dim3(256), 0, ctx->stream, cap, (const int*) counts, (const unsigned long long*) keys, sorted), "yolo_rank_kernel")) return 1;
+    return launch_done(ctx, launch_k(yolo_nms_kernel, dim3((unsigned) N), dim3(yolo_dev::NMS_THREADS), 0, ctx->stream, view(h0), view(h1), cap, (const int*) counts,
+                                     (const unsigned long long*) sorted, max_rows, rows, out_counts),
+                       "yolo_nms_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // Layout ops (scalar-per-element kernels: rarely on the hot path).
 // ------------------------------------------------------------------------------------------------------------
 // Flatten, HWC order (cpulayer.h:94-115): out[n, (y*W + x)*C + c] = in[n,y,x,c]

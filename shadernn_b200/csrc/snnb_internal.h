@@ -219,6 +219,11 @@ int launch_softmax(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out);
 int launch_argmax(snnb_context* ctx, const snnb_tensor* in, int* dev_idx, int base_index = 0); // dev_idx[n] = arg-max of image n + base_index
 // YOLO decode, device part: cells whose score can pass `thresh` -> ONE candidate list [maxc][8] = {image, scan index, d0..d5}; counts[0] = its length
 int launch_yolo_candidates(snnb_context* ctx, const snnb_tensor* h0, const snnb_tensor* h1, float thresh, int maxc, int* counts, float* cand);
+// YOLO decode all on the device (snnb_model_detect_device): exact score threshold, stable score sort and greedy NMS per image into
+// rows[N][max_rows][6] (zero past the count) and out_counts[N]. One memset and three kernels; `scratch` holds
+// yolo_detect_scratch_bytes(h0, h1) bytes.
+size_t yolo_detect_scratch_bytes(const snnb_tensor* h0, const snnb_tensor* h1);
+int launch_yolo_detect(snnb_context* ctx, const snnb_tensor* h0, const snnb_tensor* h1, void* scratch, int max_rows, float* rows, int* out_counts);
 int launch_flatten(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out);
 int launch_concat(snnb_context* ctx, const snnb_tensor* a, const snnb_tensor* b, snnb_tensor* out);
 int launch_upsample(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, float scale, bool bilinear);

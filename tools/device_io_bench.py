@@ -13,6 +13,10 @@ Writes DIR/device_io_bench.json and prints it. Three parts, all in one process:
                own, and bytes read + written (from shapes) over that time against the H100 SXM's 3.35 TB/s of HBM3: the kernels do no
                arithmetic to speak of, so HBM bandwidth is their bound. A 64-channel tensor compares NCHW with NHWC, the case where the
                tensor-side accesses of NCHW threads are strided.
+  detector     YOLOv3-tiny 416x416 batch 16: uint8 NCHW CUDA frames into detect_torch (decode, score sort and NMS on the device, boxes
+               in device memory) against snnb_model_submit_u8 / wait + snnb_model_get_boxes for every image from pinned host memory,
+               alternating as above; and the device time of the decode kernels (yolo_select / yolo_rank / yolo_nms) next to the forward
+               pass's kernels, from torch.profiler over 50 calls, on the synthetic heads and on all-pass heads (every cell passes).
   card         name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -195,11 +199,96 @@ def conversions(torch, ctx, core, modelzoo, d, calls=50):
     return res
 
 
+def detector_kernel_times_us(torch, fn, calls):
+    """Device time per call (us) of the decode kernels, the forward pass's kernels and the input conversion that fn() launches."""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(5):
+        fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            fn()
+        torch.cuda.synchronize()
+    out = {"decode": {}, "forward_us": 0.0, "input_us": 0.0}
+    for e in prof.key_averages():
+        total = getattr(e, "device_time_total", None)
+        total = e.cuda_time_total if total is None else total
+        if "snnb::" not in e.key or total <= 0:
+            continue
+        if "snnb::yolo_" in e.key:
+            out["decode"][e.key.split("(")[0].replace("void ", "")] = {"launches": e.count, "us_per_call": total / calls}
+        elif "snnb::device_input" in e.key:
+            out["input_us"] += total / calls
+        else:
+            out["forward_us"] += total / calls
+    out["decode_us"] = sum(v["us_per_call"] for v in out["decode"].values())
+    return out
+
+
+def detector(torch, ctx, core, modelzoo, d, args):
+    from shadernn_b200._lib import check, lib
+    hw, batch = (416, 416), 16
+    mean4, norm4 = [127.5] * 4, [1.0 / 127.5] * 4  # the model takes [-1, 1]
+    path, layers = modelzoo.build("yolov3tiny", os.path.join(d, "yolov3tiny"), input_hw=hw)
+    m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+    # BASELINE's synthetic input as 8-bit frames: few cells pass the threshold (uniform noise frames would give 100 boxes per image)
+    img = np.clip(np.rint((modelzoo.synthetic_input("yolov3tiny", batch, hw) + 1.0) * 127.5), 0, 255).astype(np.uint8)
+    dev_in = torch.from_numpy(img.transpose(0, 3, 1, 2).copy()).cuda()
+    dev = lambda: m.detect_torch(dev_in, layout="nchw", mean4=mean4, norm4=norm4)  # noqa: E731
+    hp = HostPipeline(torch, m, img, mean4, norm4, False)
+    rows, cnt = np.empty((100, 6), np.float32), C.c_int()
+
+    def host_step():  # the boxes of the previous submission are ready after its wait(): read every image's list
+        waited = hp.pending is not None
+        hp.step()
+        if waited:
+            for n in range(batch):
+                check(lib().snnb_model_get_boxes(m.h, n, rows.ctypes.data_as(C.POINTER(C.c_float)), 100, C.byref(cnt)), "snnb_model_get_boxes")
+
+    for _ in range(5):
+        dev()
+        host_step()
+    hp.drain()
+    torch.cuda.synchronize()
+    rounds = []
+    for _ in range(args.rounds):
+        r_dev = timed(dev, args.seconds, batch, torch.cuda.synchronize)
+        r_host = timed(host_step, args.seconds, batch, hp.drain)
+        rounds.append({"device": r_dev, "host": r_host})
+    med = lambda k: float(np.median([r[k]["frames_per_s"] for r in rounds]))  # noqa: E731
+    res = {
+        "shape": "%dx%d batch %d" % (hw[0], hw[1], batch),
+        "device_path": "detect_torch: uint8 NCHW CUDA tensor in, rows [16, 100, 6] + counts [16] as CUDA tensors out",
+        "host_path": "snnb_model_submit_u8/wait: pinned uint8 NHWC in, decode finished on the host, snnb_model_get_boxes for every image",
+        "device_frames_per_s_median": med("device"),
+        "host_frames_per_s_median": med("host"),
+        "device_over_host": med("device") / med("host"),
+        "rounds": rounds,
+    }
+    counts = m.detect_torch(dev_in, layout="nchw", mean4=mean4, norm4=norm4)[1]
+    res["synthetic_heads"] = detector_kernel_times_us(torch, dev, 50)
+    res["synthetic_heads"]["boxes_per_image"] = counts.cpu().tolist()
+    m.close()
+    # all-pass heads: objectness and class bias +8 for every anchor, so all 2535 cells of every image pass and NMS runs deep
+    for head in [l for l in layers if l["type"] == "Conv2D" and l["outputPlanes"] == 18]:
+        head["_w"]["bias"][:] = 0
+        head["_w"]["bias"][[4, 5, 10, 11, 16, 17]] = 8.0
+    allpass = modelzoo.write_model(layers, os.path.join(d, "yolov3tiny_allpass.json"), split=True)
+    m = core.MixedInferenceCore(ctx, allpass, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+    dev = lambda: m.detect_torch(dev_in, layout="nchw", mean4=mean4, norm4=norm4)  # noqa: E731
+    counts = m.detect_torch(dev_in, layout="nchw", mean4=mean4, norm4=norm4)[1]
+    res["all_pass_heads"] = detector_kernel_times_us(torch, dev, 50)
+    res["all_pass_heads"]["boxes_per_image"] = counts.cpu().tolist()
+    m.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
     ap.add_argument("--seconds", type=float, default=2.0)
     ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--parts", default="throughput,conversions,detector", help="comma-separated subset of throughput, conversions, detector")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -209,8 +298,13 @@ def main():
     d = tempfile.mkdtemp(prefix="snnb_devio_")
     ctx = core.GpuContext(0)
     result = {"card": card(), "torch_device_name": torch.cuda.get_device_name(0)}
-    result["throughput"] = throughput(torch, ctx, core, modelzoo, d, args)
-    result["conversions"] = conversions(torch, ctx, core, modelzoo, d)
+    parts = args.parts.split(",")
+    if "throughput" in parts:
+        result["throughput"] = throughput(torch, ctx, core, modelzoo, d, args)
+    if "conversions" in parts:
+        result["conversions"] = conversions(torch, ctx, core, modelzoo, d)
+    if "detector" in parts:
+        result["detector"] = detector(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
