@@ -267,6 +267,34 @@ int snnb_model_run_device(snnb_model* m, const snnb_device_buffer* inputs, int n
  * bit or two. Cost beyond the forward pass: one kernel launch per input, one memset and three decode kernels. */
 int snnb_model_detect_device(snnb_model* m, const snnb_device_buffer* inputs, int num_inputs, float* rows_dev, int max_rows,
                              int* counts_dev, void* stream);
+/* Device-resident 8-bit video frames of any size (NVDEC's NV12, nvJPEG's I420, a camera's NV21, an RGBA image) into input 0 of a
+ * model with exactly one input of 1 to 4 channels: the reference's camera path NativeFrameProvider::copyImageData = nv12ToRgba8 /
+ * nv21ToRgba8 / i420ToRgba8 (core/src/image.cpp:1076-1136, libyuv's 6-bit fixed-point YuvPixel, BT.601 limited range) ->
+ * ImageTexture::resize -> convertToRGBA32FAndNormalize, fused into ONE kernel that writes the model input. Model channel c is RGBA
+ * component c. Per output pixel: the source taps of ImageTexture::resize (snnb_image_io; when the frame has the model's size, the
+ * pixel itself), each converted to RGBA8 exactly as libyuv does, pixel (x, y) using chroma sample (x / 2, y / 2); then the same
+ * interpolation and normalisation as snnb_model_submit_image. The model input is therefore bit-identical to snnb_model_submit_image
+ * fed libyuv's RGBA8 image (its first C components). */
+enum { SNNB_FRAME_NV12 = 0, SNNB_FRAME_NV21 = 1, SNNB_FRAME_I420 = 2, SNNB_FRAME_RGBA8 = 3 };
+enum { SNNB_YUV_BT601 = 0 /* libyuv kYuvI601Constants: the reference's nv12ToRgba8 */, SNNB_YUV_BT709 = 1 /* kYuvH709Constants */ };
+typedef struct {
+    int format, matrix;          /* SNNB_FRAME_*, SNNB_YUV_* (matrix ignored for RGBA8) */
+    int width, height;           /* frame size, any >= 1 (odd allowed: chroma is ceil(w/2) x ceil(h/2), as libyuv) */
+    const uint8_t* plane[3];     /* NV12/NV21: Y, UV|VU; I420: Y, U, V; RGBA8: RGBA. Device memory of the model's device */
+    int pitch[3];                /* bytes per row, >= the row's bytes */
+    long long image_stride[3];   /* bytes from image n to image n+1 of the batch, per plane */
+    int linear_filter;           /* as snnb_image_io */
+    float mean4[4], norm4[4];    /* (x - mean4[c]) * norm4[c] on the RGBA component c */
+} snnb_frames;
+/* snnb_model_run_device / snnb_model_detect_device with `frames` (the loaded batch of them) in place of the input buffers: outputs,
+ * classes, rows, counts, the stream contract and the fences are exactly theirs; run_frames refuses YOLO models, detect_frames requires
+ * them. Checked on the host before anything is enqueued: format and matrix, width and height >= 1, each pitch >= its row's bytes, each
+ * plane device or managed memory of the context's device, a model with one input of <= 4 channels, a stream that is not capturing.
+ * A plane's size cannot be checked: it must hold the batch. Cost beyond the forward pass: one kernel launch for the input (1920x1080
+ * NV12 to YOLOv3-tiny 416x416 x 16: 50 us, to ResNet-18 224x224 x 32: 30 us; NVIDIA H100 80GB HBM3, 700 W power limit). */
+int snnb_model_run_frames(snnb_model* m, const snnb_frames* frames, const snnb_device_buffer* outputs, int num_outputs, int* classes_1based_dev,
+                          void* stream);
+int snnb_model_detect_frames(snnb_model* m, const snnb_frames* frames, float* rows_dev, int max_rows, int* counts_dev, void* stream);
 /* Device-resident variant: inputs already uploaded with snnb_model_set_input(); forward only, asynchronous. */
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input_nhwc);
 int snnb_model_forward(snnb_model* m);

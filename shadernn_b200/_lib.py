@@ -78,6 +78,26 @@ class DeviceBuffer(C.Structure):
     ]
 
 
+FRAME_NV12, FRAME_NV21, FRAME_I420, FRAME_RGBA8 = 0, 1, 2, 3
+YUV_BT601, YUV_BT709 = 0, 1
+
+
+class Frames(C.Structure):
+    """snnb_frames"""
+    _fields_ = [
+        ("format", C.c_int),
+        ("matrix", C.c_int),
+        ("width", C.c_int),
+        ("height", C.c_int),
+        ("plane", C.c_void_p * 3),
+        ("pitch", C.c_int * 3),
+        ("image_stride", C.c_longlong * 3),
+        ("linear_filter", C.c_int),
+        ("mean4", C.c_float * 4),
+        ("norm4", C.c_float * 4),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/snnb.h declares
 SIGNATURES = {
     "snnb_version": (C.c_int, []),
@@ -141,6 +161,8 @@ SIGNATURES = {
     "snnb_model_wait": (C.c_int, [vp, C.c_int]),
     "snnb_model_run_device": (C.c_int, [vp, C.POINTER(DeviceBuffer), C.c_int, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
     "snnb_model_detect_device": (C.c_int, [vp, C.POINTER(DeviceBuffer), C.c_int, vp, C.c_int, vp, vp]),
+    "snnb_model_run_frames": (C.c_int, [vp, C.POINTER(Frames), C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
+    "snnb_model_detect_frames": (C.c_int, [vp, C.POINTER(Frames), vp, C.c_int, vp, vp]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),

@@ -471,12 +471,23 @@ class MixedInferenceCore:
         Outputs are allocated here as out_dtype (float32 by default, float16 or uint8: clamp(round(v * out_scale + out_offset), 0, 255))
         in out_layout. Returns output 0 for a one-output model, else the list of outputs; with want_classes, (outputs, the 1-based
         classes as a device int32 tensor)."""
+        if layout not in self._TORCH_LAYOUTS:
+            raise ValueError("run_torch: layout %r: expected 'nhwc' or 'nchw'" % (layout,))
+        outs, obufs, classes = self._device_outputs("run_torch", out_dtype, out_layout, out_scale, out_offset, want_classes)
+        keep, ins = self._device_inputs("run_torch", inputs, layout, mean4, norm4)
+        check(lib().snnb_model_run_device(self.h, ins, len(keep), obufs, len(outs), classes.data_ptr() if want_classes else None, self._torch_stream()),
+              "snnb_model_run_device")
+        result = outs[0] if len(outs) == 1 else outs
+        return (result, classes) if want_classes else result
+
+    def _device_outputs(self, who, out_dtype, out_layout, out_scale, out_offset, want_classes):
+        """run_torch / run_frames: every model output allocated with torch as out_dtype in out_layout, their snnb_device_buffer array,
+        and the classes tensor (or None)."""
         import torch
         dtypes, layouts = self._torch_dtypes(), self._TORCH_LAYOUTS
         out_dtype = torch.float32 if out_dtype is None else out_dtype
-        if out_dtype not in dtypes or layout not in layouts or out_layout not in layouts:
-            raise ValueError("run_torch: dtype %s / layouts %r, %r: expected float32, float16 or uint8 and 'nhwc' or 'nchw'" % (out_dtype, layout, out_layout))
-        keep, ins = self._device_inputs("run_torch", inputs, layout, mean4, norm4)
+        if out_dtype not in dtypes or out_layout not in layouts:
+            raise ValueError("%s: output dtype %s / layout %r: expected float32, float16 or uint8 and 'nhwc' or 'nchw'" % (who, out_dtype, out_layout))
         device = torch.device("cuda", self.ctx.device)
         outs = [torch.empty(self._nhwc_as(self.output_shape(j), out_layout), dtype=out_dtype, device=device) for j in range(self.num_outputs)]
         obufs = (_lib.DeviceBuffer * max(1, len(outs)))()
@@ -484,10 +495,7 @@ class MixedInferenceCore:
             obufs[j].data, obufs[j].dtype, obufs[j].layout = o.data_ptr(), dtypes[out_dtype], layouts[out_layout]
             obufs[j].scale, obufs[j].offset = float(out_scale), float(out_offset)
         classes = torch.empty(self.batch, dtype=torch.int32, device=device) if want_classes else None
-        check(lib().snnb_model_run_device(self.h, ins, len(keep), obufs, len(outs), classes.data_ptr() if want_classes else None, self._torch_stream()),
-              "snnb_model_run_device")
-        result = outs[0] if len(outs) == 1 else outs
-        return (result, classes) if want_classes else result
+        return outs, obufs, classes
 
     def detect_torch(self, inputs, layout="nhwc", mean4=None, norm4=None, max_rows=100):
         """snnb_model_detect_device with torch CUDA tensors: the forward pass and the YOLO decode, score sort and NMS on the device,
@@ -502,6 +510,69 @@ class MixedInferenceCore:
         counts = torch.empty(self.batch, dtype=torch.int32, device=device)
         check(lib().snnb_model_detect_device(self.h, ins, len(keep), rows.data_ptr() or None, int(max_rows), counts.data_ptr(), self._torch_stream()),
               "snnb_model_detect_device")
+        return rows, counts
+
+    _FRAME_FORMATS = {"nv12": _lib.FRAME_NV12, "nv21": _lib.FRAME_NV21, "i420": _lib.FRAME_I420, "rgba8": _lib.FRAME_RGBA8}
+    _YUV_MATRICES = {"bt601": _lib.YUV_BT601, "bt709": _lib.YUV_BT709}
+
+    def _frames(self, who, frames, format, matrix, linear, mean4, norm4):
+        """The snnb_frames descriptor of a uint8 CUDA tensor: NV12 / NV21 / I420 as [N, H * 3 // 2, W] (the packed 4:2:0 layout, H and W
+        even; NV12 / NV21 rows may be pitched, I420 rows must be dense), RGBA8 as [N, H, W, 4] (rows may be pitched)."""
+        import torch
+        if format not in self._FRAME_FORMATS or matrix not in self._YUV_MATRICES:
+            raise ValueError("%s: format %r / matrix %r: expected one of %s and one of %s" % (who, format, matrix, sorted(self._FRAME_FORMATS),
+                                                                                               sorted(self._YUV_MATRICES)))
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+            raise ValueError("%s: frames must be a uint8 CUDA tensor" % who)
+        f = _lib.Frames()
+        f.format, f.matrix, f.linear_filter = self._FRAME_FORMATS[format], self._YUV_MATRICES[matrix], int(bool(linear))
+        f.mean4 = (C.c_float * 4)(*[float(v) for v in (mean4 if mean4 is not None else [0.0] * 4)])
+        f.norm4 = (C.c_float * 4)(*[float(v) for v in (norm4 if norm4 is not None else [1.0] * 4)])
+        shape, st, base = tuple(frames.shape), frames.stride(), frames.data_ptr()
+        if format == "rgba8":
+            if len(shape) != 4 or shape[3] != 4 or st[3] != 1 or st[2] != 4:
+                raise ValueError("%s: rgba8 frames are [N, H, W, 4] with dense pixels; got shape %s, strides %s" % (who, shape, st))
+            n, f.height, f.width = shape[0], shape[1], shape[2]
+            f.plane[0], f.pitch[0], f.image_stride[0] = base, st[1], st[0]
+        else:
+            if len(shape) != 3 or shape[1] % 3 or shape[1] < 3 or shape[2] % 2 or st[2] != 1:
+                raise ValueError("%s: %s frames are [N, H * 3 // 2, W] with H and W even and dense rows; got shape %s, strides %s" % (who, format, shape, st))
+            n, f.height, f.width = shape[0], shape[1] // 3 * 2, shape[2]
+            pitch = st[1]
+            if format == "i420" and pitch != f.width:
+                raise ValueError("%s: i420 frames must have dense rows (row stride %d, width %d)" % (who, pitch, f.width))
+            f.plane[0], f.pitch[0] = base, pitch
+            f.plane[1], f.pitch[1] = base + f.height * pitch, pitch if format != "i420" else f.width // 2
+            if format == "i420":
+                f.plane[2], f.pitch[2] = base + f.height * pitch + (f.height // 2) * (f.width // 2), f.width // 2
+            for p in range(3):
+                f.image_stride[p] = st[0]
+        if n != self.batch:
+            raise ValueError("%s: %d frames given, the model's batch is %d" % (who, n, self.batch))
+        return f
+
+    def run_frames(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_dtype=None, out_layout="nhwc", out_scale=1.0,
+                   out_offset=0.0, want_classes=False):
+        """snnb_model_run_frames: a batch of 8-bit video frames of any size on the GPU (NV12, NV21, I420 or RGBA8, see _frames) converted
+        to RGBA8 exactly as libyuv does, resized to the model input (linear or nearest, as run_image), normalised as
+        (x - mean4[c]) * norm4[c] (default mean 0, norm 1) and run, ordered on the current torch stream and never synchronising.
+        Model channel c is RGBA component c. Outputs and classes as run_torch."""
+        outs, obufs, classes = self._device_outputs("run_frames", out_dtype, out_layout, out_scale, out_offset, want_classes)
+        f = self._frames("run_frames", frames, format, matrix, linear, mean4, norm4)
+        check(lib().snnb_model_run_frames(self.h, C.byref(f), obufs, len(outs), classes.data_ptr() if want_classes else None, self._torch_stream()),
+              "snnb_model_run_frames")
+        result = outs[0] if len(outs) == 1 else outs
+        return (result, classes) if want_classes else result
+
+    def detect_frames(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, max_rows=100):
+        """snnb_model_detect_frames: run_frames' input, detect_torch's forward pass, device decode and (rows, counts)."""
+        import torch
+        f = self._frames("detect_frames", frames, format, matrix, linear, mean4, norm4)
+        device = torch.device("cuda", self.ctx.device)
+        rows = torch.empty((self.batch, max(int(max_rows), 0), 6), dtype=torch.float32, device=device)
+        counts = torch.empty(self.batch, dtype=torch.int32, device=device)
+        check(lib().snnb_model_detect_frames(self.h, C.byref(f), rows.data_ptr() or None, int(max_rows), counts.data_ptr(), self._torch_stream()),
+              "snnb_model_detect_frames")
         return rows, counts
 
     def set_input(self, images, idx=0):

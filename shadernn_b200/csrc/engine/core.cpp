@@ -648,11 +648,39 @@ static int checkDeviceBuffer(const char* api, const snnb_device_buffer& b, int d
     return checkDevicePointer(api, b.data, elem, device, what, idx);
 }
 
-int MixedInferenceCore::checkDeviceInputs(const char* api, const snnb_device_buffer* inputs, int numInputs, cudaStream_t stream) {
-    SNNB_REQUIRE(inputs, "%s: null inputs", api);
-    SNNB_REQUIRE(numInputs == (int) inputLayers.size(), "%s: %d inputs given, the model has %d", api, numInputs, (int) inputLayers.size());
-    for (int i = 0; i < numInputs; ++i)
-        if (int rc = checkDeviceBuffer(api, inputs[i], ctx->device, "input", i)) return rc;
+// The frames' row bytes of plane p (NV12 / NV21 rows of ceil(w/2) UV pairs, I420 rows of ceil(w/2) samples), 0 for an unused plane.
+static long long frameRowBytes(const snnb_frames& f, int p) {
+    const long long cw = (f.width + 1) / 2;
+    switch (f.format) {
+    case SNNB_FRAME_NV12:
+    case SNNB_FRAME_NV21: return p == 0 ? f.width : (p == 1 ? 2 * cw : 0);
+    case SNNB_FRAME_I420: return p == 0 ? f.width : cw;
+    case SNNB_FRAME_RGBA8: return p == 0 ? 4LL * f.width : 0;
+    }
+    return 0;
+}
+
+int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, cudaStream_t stream) {
+    if (in.frames) {
+        const snnb_frames& f = *in.frames;
+        SNNB_REQUIRE(f.format >= SNNB_FRAME_NV12 && f.format <= SNNB_FRAME_RGBA8, "%s: unknown frame format %d", api, f.format);
+        SNNB_REQUIRE(f.format == SNNB_FRAME_RGBA8 || f.matrix == SNNB_YUV_BT601 || f.matrix == SNNB_YUV_BT709, "%s: unknown YUV matrix %d", api, f.matrix);
+        SNNB_REQUIRE(f.width >= 1 && f.height >= 1, "%s: frame size %d x %d; width and height must be >= 1", api, f.width, f.height);
+        SNNB_REQUIRE(inputLayers.size() == 1, "%s: the model has %d inputs; frames feed a model with exactly one", api, (int) inputLayers.size());
+        const snnb_tensor* t = inputLayers[0]->output;
+        SNNB_REQUIRE(t->c >= 1 && t->c <= 4, "%s: the model input has %d channels; frames feed 1 to 4 (RGBA components)", api, t->c);
+        for (int p = 0; p < 3; ++p) {
+            const long long row = frameRowBytes(f, p);
+            if (!row) continue;
+            SNNB_REQUIRE(f.pitch[p] >= row, "%s: plane %d: pitch %d is less than its row's %lld bytes", api, p, f.pitch[p], row);
+            if (int rc = checkDevicePointer(api, f.plane[p], 1, ctx->device, "plane", p)) return rc;
+        }
+    } else {
+        SNNB_REQUIRE(in.inputs, "%s: null inputs", api);
+        SNNB_REQUIRE(in.numInputs == (int) inputLayers.size(), "%s: %d inputs given, the model has %d", api, in.numInputs, (int) inputLayers.size());
+        for (int i = 0; i < in.numInputs; ++i)
+            if (int rc = checkDeviceBuffer(api, in.inputs[i], ctx->device, "input", i)) return rc;
+    }
     if (stream) {
         cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
         const cudaError_t e = cudaStreamIsCapturing(stream, &cap);
@@ -663,16 +691,20 @@ int MixedInferenceCore::checkDeviceInputs(const char* api, const snnb_device_buf
     return 0;
 }
 
-// The caller's stream -> the context's stream, the input conversions and the forward pass. Called after every check has passed.
-int MixedInferenceCore::enqueueDeviceForward(const snnb_device_buffer* inputs, int numInputs, cudaStream_t stream) {
+// The caller's stream -> the context's stream, the input staging and the forward pass. Called after every check has passed.
+int MixedInferenceCore::enqueueDeviceForward(const DeviceFeed& in, cudaStream_t stream) {
     if (!callerReady) SNNB_CUDA_OK(cudaEventCreateWithFlags(&callerReady, cudaEventDisableTiming));
     if (!deviceDone) SNNB_CUDA_OK(cudaEventCreateWithFlags(&deviceDone, cudaEventDisableTiming));
     if (stream && stream != ctx->stream) { // a stream of another device fails here, before anything is launched
         SNNB_CUDA_OK(cudaEventRecord(callerReady, stream));
         SNNB_CUDA_OK(cudaStreamWaitEvent(ctx->stream, callerReady, 0));
     }
-    for (int i = 0; i < numInputs; ++i)
-        if (launch_device_input(ctx, inputs[i], inputLayers[i]->output)) return 1;
+    if (in.frames) {
+        if (launch_frame_input(ctx, *in.frames, inputLayers[0]->output)) return 1;
+    } else {
+        for (int i = 0; i < in.numInputs; ++i)
+            if (launch_device_input(ctx, in.inputs[i], inputLayers[i]->output)) return 1;
+    }
     return forward();
 }
 
@@ -687,27 +719,40 @@ int MixedInferenceCore::fenceToCaller(cudaStream_t stream) {
 
 int MixedInferenceCore::runDevice(const snnb_device_buffer* inputs, int numInputs, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev,
                                   cudaStream_t stream) {
+    DeviceFeed in;
+    in.inputs = inputs, in.numInputs = numInputs;
+    return runDeviceFeed("snnb_model_run_device", in, outputs, numOutputs, classes1Dev, stream);
+}
+int MixedInferenceCore::runFrames(const snnb_frames* frames, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_run_frames: null frames");
+    DeviceFeed in;
+    in.frames = frames;
+    return runDeviceFeed("snnb_model_run_frames", in, outputs, numOutputs, classes1Dev, stream);
+}
+
+int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev,
+                                      cudaStream_t stream) {
     // everything is validated before the first enqueue: a refused call leaves no work behind
-    static const char* api = "snnb_model_run_device";
-    SNNB_REQUIRE(numOutputs >= 0 && numOutputs <= (int) outputLayers.size(), "snnb_model_run_device: %d outputs requested, the model has %d", numOutputs,
+    SNNB_REQUIRE(numOutputs >= 0 && numOutputs <= (int) outputLayers.size(), "%s: %d outputs requested, the model has %d", api, numOutputs,
                  (int) outputLayers.size());
-    SNNB_REQUIRE(outputs || numOutputs == 0, "snnb_model_run_device: null outputs");
+    SNNB_REQUIRE(outputs || numOutputs == 0, "%s: null outputs", api);
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO",
-                 "snnb_model_run_device: output 0 is a YOLO detection list; use snnb_model_detect_device for device detections, or snnb_model_run or "
-                 "snnb_model_submit / snnb_model_wait and read the boxes with snnb_model_get_boxes");
-    if (int rc = checkDeviceInputs(api, inputs, numInputs, stream)) return rc;
+                 "%s: output 0 is a YOLO detection list; use %s for device detections, or snnb_model_run or "
+                 "snnb_model_submit / snnb_model_wait and read the boxes with snnb_model_get_boxes",
+                 api, in.frames ? "snnb_model_detect_frames" : "snnb_model_detect_device");
+    if (int rc = checkDeviceFeed(api, in, stream)) return rc;
     const int device = ctx->device;
     for (int j = 0; j < numOutputs; ++j) {
         if (!outputs[j].data) continue;
-        SNNB_REQUIRE(outputLayers[j]->output, "snnb_model_run_device: output %d (%s) has no device tensor", j, outputLayers[j]->name.c_str());
+        SNNB_REQUIRE(outputLayers[j]->output, "%s: output %d (%s) has no device tensor", api, j, outputLayers[j]->name.c_str());
         if (int rc = checkDeviceBuffer(api, outputs[j], device, "output", j)) return rc;
     }
     if (classes1Dev) {
-        SNNB_REQUIRE(isClassifier, "snnb_model_run_device: classes requested, but the model is not a classifier (output 0 is not 1 x 1 x C with C > 1)");
+        SNNB_REQUIRE(isClassifier, "%s: classes requested, but the model is not a classifier (output 0 is not 1 x 1 x C with C > 1)", api);
         if (int rc = checkDevicePointer(api, classes1Dev, sizeof(int), device, "classes", 0)) return rc;
     }
 
-    if (enqueueDeviceForward(inputs, numInputs, stream)) return 1;
+    if (enqueueDeviceForward(in, stream)) return 1;
     for (int j = 0; j < numOutputs; ++j)
         if (outputs[j].data && launch_device_output(ctx, outputLayers[j]->output, outputs[j])) return 1;
     if (classes1Dev && launch_argmax(ctx, outputLayers[0]->output, classes1Dev, 1)) return 1; // core.cpp:228-233: argmax + 1
@@ -717,17 +762,28 @@ int MixedInferenceCore::runDevice(const snnb_device_buffer* inputs, int numInput
 // Detections in device memory: the forward pass, then the whole YOLO decode (threshold, stable score sort, NMS) in three kernels.
 // Reads the heads only: the host detection lists (`boxes`) and the candidate buffers of run() / submit() are not touched.
 int MixedInferenceCore::detectDevice(const snnb_device_buffer* inputs, int numInputs, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
-    static const char* api = "snnb_model_detect_device";
-    SNNB_REQUIRE(yolo, "snnb_model_detect_device: the model has no YOLO output; use snnb_model_run_device");
-    SNNB_REQUIRE(maxRows >= 1 && maxRows <= 100, "snnb_model_detect_device: max_rows %d is outside 1..100", maxRows);
-    if (int rc = checkDeviceInputs(api, inputs, numInputs, stream)) return rc;
+    DeviceFeed in;
+    in.inputs = inputs, in.numInputs = numInputs;
+    return detectDeviceFeed("snnb_model_detect_device", in, rowsDev, maxRows, countsDev, stream);
+}
+int MixedInferenceCore::detectFrames(const snnb_frames* frames, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_detect_frames: null frames");
+    DeviceFeed in;
+    in.frames = frames;
+    return detectDeviceFeed("snnb_model_detect_frames", in, rowsDev, maxRows, countsDev, stream);
+}
+
+int MixedInferenceCore::detectDeviceFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
+    SNNB_REQUIRE(yolo, "%s: the model has no YOLO output; use %s", api, in.frames ? "snnb_model_run_frames" : "snnb_model_run_device");
+    SNNB_REQUIRE(maxRows >= 1 && maxRows <= 100, "%s: max_rows %d is outside 1..100", api, maxRows);
+    if (int rc = checkDeviceFeed(api, in, stream)) return rc;
     if (int rc = checkDevicePointer(api, rowsDev, sizeof(float), ctx->device, "rows", 0)) return rc;
     if (int rc = checkDevicePointer(api, countsDev, sizeof(int), ctx->device, "counts", 0)) return rc;
-    SNNB_REQUIRE(yolo->inputs.size() == 2 && yolo->inputs[0]->c >= 18 && yolo->inputs[1]->c >= 18, "snnb_model_detect_device: %s: YOLO expects two heads of >= 18 channels",
+    SNNB_REQUIRE(yolo->inputs.size() == 2 && yolo->inputs[0]->c >= 18 && yolo->inputs[1]->c >= 18, "%s: %s: YOLO expects two heads of >= 18 channels", api,
                  yolo->name.c_str());
     if (!detectScratch) SNNB_CUDA_OK(cudaMalloc(&detectScratch, yolo_detect_scratch_bytes(yolo->inputs[0], yolo->inputs[1])));
 
-    if (enqueueDeviceForward(inputs, numInputs, stream)) return 1;
+    if (enqueueDeviceForward(in, stream)) return 1;
     if (launch_yolo_detect(ctx, yolo->inputs[0], yolo->inputs[1], detectScratch, maxRows, rowsDev, countsDev)) return 1;
     return fenceToCaller(stream);
 }

@@ -353,6 +353,9 @@ public:
     int runDevice(const snnb_device_buffer* inputs, int numInputs, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
     // snnb_model_detect_device: runDevice's inputs and fences, then YOLO decode + score sort + NMS on the device into rows / counts
     int detectDevice(const snnb_device_buffer* inputs, int numInputs, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
+    // snnb_model_run_frames / snnb_model_detect_frames: runDevice / detectDevice with device video frames as input 0
+    int runFrames(const snnb_frames* frames, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
+    int detectFrames(const snnb_frames* frames, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
     int layerOutput(int layerId, float* host, size_t capacityFloats);
     int timeLayers(std::vector<float>& ms);
     int dumpOutputs(const std::string& dir);
@@ -409,10 +412,19 @@ private:
     int ensureStreaming();
     // runDevice's fences: the caller's stream -> the context's stream (callerReady), and back (deviceDone); created on first use
     cudaEvent_t callerReady = nullptr, deviceDone = nullptr;
-    // shared by runDevice and detectDevice: the host-side checks of the inputs and the stream (nothing enqueued), then the fenced
-    // input conversions + forward pass, and the fence back to the caller's stream
-    int checkDeviceInputs(const char* api, const snnb_device_buffer* inputs, int numInputs, cudaStream_t stream);
-    int enqueueDeviceForward(const snnb_device_buffer* inputs, int numInputs, cudaStream_t stream);
+    // What a device-resident call feeds the model: one snnb_device_buffer per input, or (frames != NULL) a batch of frames into input 0.
+    // The input staging is the only step in which the buffer and frame entry points differ.
+    struct DeviceFeed {
+        const snnb_device_buffer* inputs = nullptr;
+        int numInputs = 0;
+        const snnb_frames* frames = nullptr;
+    };
+    // shared by runDevice, detectDevice, runFrames and detectFrames: the host-side checks of the feed and the stream (nothing
+    // enqueued), then the fenced input staging + forward pass, the outputs or the detections, and the fence back to the caller's stream
+    int runDeviceFeed(const char* api, const DeviceFeed& in, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
+    int detectDeviceFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
+    int checkDeviceFeed(const char* api, const DeviceFeed& in, cudaStream_t stream);
+    int enqueueDeviceForward(const DeviceFeed& in, cudaStream_t stream);
     int fenceToCaller(cudaStream_t stream);
     void* detectScratch = nullptr; // detectDevice's per-image keys (yolo_detect_scratch_bytes), allocated on first use
 };

@@ -134,6 +134,16 @@ int snnb_model_detect_device(snnb_model* m, const snnb_device_buffer* inputs, in
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->detectDevice(inputs, num_inputs, rows_dev, max_rows, counts_dev, static_cast<cudaStream_t>(stream));
 }
+int snnb_model_run_frames(snnb_model* m, const snnb_frames* frames, const snnb_device_buffer* outputs, int num_outputs, int* classes_1based_dev, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_run_frames: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->runFrames(frames, outputs, num_outputs, classes_1based_dev, static_cast<cudaStream_t>(stream));
+}
+int snnb_model_detect_frames(snnb_model* m, const snnb_frames* frames, float* rows_dev, int max_rows, int* counts_dev, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_detect_frames: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->detectFrames(frames, rows_dev, max_rows, counts_dev, static_cast<cudaStream_t>(stream));
+}
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input) {
     SNNB_REQUIRE(m, "snnb_model_set_input: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));

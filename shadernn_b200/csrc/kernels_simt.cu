@@ -1341,9 +1341,38 @@ int launch_split_u8(snnb_context* ctx, const uint8_t* dev_nhwc_u8, snnb_tensor* 
     for (int i = 0; i < 4; ++i) q.mean[i] = mean[i], q.norm[i] = norm[i];
     return launch_done(ctx, launch_k(split_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, dev_nhwc_u8, view(t), q, feed_view(t)), "split_u8_kernel");
 }
-// u8 image of ANOTHER size -> resize (linear or nearest) -> (x - mean[c]) * norm[c] -> split-fp16: ImageTexture::resize
-// (core/inc/snn/imageTexture.h:137) = shadertemplate_vk_resize.comp:42-61: the output texel centre (x + 0.5) / outW is sampled from
-// the source texture with the sampler's filter (texel centres at (i + 0.5) / inW, clamp to edge), then normalised.
+// ImageTexture::resize (core/inc/snn/imageTexture.h:137) = shadertemplate_vk_resize.comp:42-61: the output texel centre (x + 0.5) / outW
+// is sampled from the source texture with the sampler's filter (texel centres at (i + 0.5) / inW, clamp to edge). The taps of output
+// pixel (ox, oy) of a W x H image from a sw x sh source, and the bilinear blend: shared by resize_u8_kernel and frame_input_kernel, so
+// that a frame is resampled exactly as an 8-bit image is. Nearest: x0 == x1, y0 == y1, and blend() is not used.
+struct ResizeTaps {
+    int x0, x1, y0, y1;
+    float ax, ay;
+    __device__ __forceinline__ float blend(float p00, float p01, float p10, float p11) const {
+        const float top = p00 + ax * (p01 - p00), bot = p10 + ax * (p11 - p10);
+        return top + ay * (bot - top);
+    }
+};
+// The source position of output pixel (ox, oy), then its taps.
+__device__ __forceinline__ float2 resize_pos(int ox, int oy, int W, int H, int sw, int sh) {
+    return make_float2(((float) ox + 0.5f) / (float) W * (float) sw, ((float) oy + 0.5f) / (float) H * (float) sh);
+}
+__device__ __forceinline__ ResizeTaps resize_taps(float2 pos, int sw, int sh, int linear) {
+    const float fx = pos.x, fy = pos.y;
+    ResizeTaps r;
+    if (linear) {
+        const float sx = fx - 0.5f, sy = fy - 0.5f;
+        const float x0f = floorf(sx), y0f = floorf(sy);
+        r.ax = sx - x0f, r.ay = sy - y0f;
+        r.x0 = min(max((int) x0f, 0), sw - 1), r.x1 = min(max((int) x0f + 1, 0), sw - 1);
+        r.y0 = min(max((int) y0f, 0), sh - 1), r.y1 = min(max((int) y0f + 1, 0), sh - 1);
+    } else {
+        r.x0 = r.x1 = min((int) fx, sw - 1), r.y0 = r.y1 = min((int) fy, sh - 1);
+        r.ax = r.ay = 0.0f;
+    }
+    return r;
+}
+// u8 image of ANOTHER size -> resize (linear or nearest, resize_taps) -> (x - mean[c]) * norm[c] -> split-fp16.
 __global__ void resize_u8_kernel(const uint8_t* __restrict__ src, int sh, int sw, TV t, U8Norm q, int linear, FeedV f) {
     pdl_wait();
     const size_t total = (size_t) t.N * t.H * t.W * (t.Cp >> 3);
@@ -1353,30 +1382,25 @@ __global__ void resize_u8_kernel(const uint8_t* __restrict__ src, int sh, int sw
     const size_t px = gid / CG;
     const int c     = (int) (gid % CG) * 8;
     const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
-    const float fx = ((float) ox + 0.5f) / (float) t.W * (float) sw, fy = ((float) oy + 0.5f) / (float) t.H * (float) sh;
+    const float2 pos = resize_pos(ox, oy, t.W, t.H, sw, sh);
     const uint8_t* img = src + (size_t) n * sh * sw * t.C;
     float v[8];
     if (linear) {
-        const float sx = fx - 0.5f, sy = fy - 0.5f;
-        const float x0f = floorf(sx), y0f = floorf(sy);
-        const float ax = sx - x0f, ay = sy - y0f;
-        const int x0 = min(max((int) x0f, 0), sw - 1), x1 = min(max((int) x0f + 1, 0), sw - 1);
-        const int y0 = min(max((int) y0f, 0), sh - 1), y1 = min(max((int) y0f + 1, 0), sh - 1);
+        const ResizeTaps r = resize_taps(pos, sw, sh, 1);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            float r = 0.0f;
+            float o = 0.0f;
             if (c + j < t.C) {
-                const float p00 = (float) __ldg(img + ((size_t) y0 * sw + x0) * t.C + c + j), p01 = (float) __ldg(img + ((size_t) y0 * sw + x1) * t.C + c + j);
-                const float p10 = (float) __ldg(img + ((size_t) y1 * sw + x0) * t.C + c + j), p11 = (float) __ldg(img + ((size_t) y1 * sw + x1) * t.C + c + j);
-                const float top = p00 + ax * (p01 - p00), bot = p10 + ax * (p11 - p10);
-                r               = ((top + ay * (bot - top)) - q.mean[(c + j) & 3]) * q.norm[(c + j) & 3];
+                const float p00 = (float) __ldg(img + ((size_t) r.y0 * sw + r.x0) * t.C + c + j), p01 = (float) __ldg(img + ((size_t) r.y0 * sw + r.x1) * t.C + c + j);
+                const float p10 = (float) __ldg(img + ((size_t) r.y1 * sw + r.x0) * t.C + c + j), p11 = (float) __ldg(img + ((size_t) r.y1 * sw + r.x1) * t.C + c + j);
+                o               = (r.blend(p00, p01, p10, p11) - q.mean[(c + j) & 3]) * q.norm[(c + j) & 3];
             }
-            v[j] = r;
+            v[j] = o;
         }
     } else {
-        const int x0 = min((int) fx, sw - 1), y0 = min((int) fy, sh - 1);
+        const ResizeTaps r = resize_taps(pos, sw, sh, 0);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = (c + j < t.C) ? ((float) __ldg(img + ((size_t) y0 * sw + x0) * t.C + c + j) - q.mean[(c + j) & 3]) * q.norm[(c + j) & 3] : 0.0f;
+        for (int j = 0; j < 8; ++j) v[j] = (c + j < t.C) ? ((float) __ldg(img + ((size_t) r.y0 * sw + r.x0) * t.C + c + j) - q.mean[(c + j) & 3]) * q.norm[(c + j) & 3] : 0.0f;
     }
     if (!f.only) store8(t.hi, t.lo, gid * 8, v);
     if (f.hi) store_feed(f, px, t.H, t.W, v);
@@ -1539,6 +1563,98 @@ int launch_device_output(snnb_context* ctx, const snnb_tensor* t, const snnb_dev
         return launch_done(ctx, launch_k(device_output_kernel<uint8_t>, grid, block, 0, ctx->stream, view(t), (uint8_t*) b.data, nchw, b.scale, b.offset), "device_output_kernel<u8>");
     }
     SNNB_REQUIRE(false, "launch_device_output: unknown dtype %d", b.dtype);
+}
+
+// Device video frames (snnb_model_run_frames) -> the model input: ImageTexture::resize's taps (resize_taps), each tap converted to
+// RGBA8 with libyuv's integer YuvPixel (row_common.cc:1444-1484, the portable C rows), then resize_u8_kernel's blend, normalisation and
+// stores. The constants are libyuv's YuvConstants written for U and V in their own roles; libyuv's NV12ToABGR reaches the same sums
+// through the swapped kYvu* tables.
+struct FrameV {
+    const uint8_t* plane[3];
+    int pitch[3];
+    long long stride[3];
+    int w, h;
+    int yg, ub, ug, vg, vr, bb, bg, br;
+};
+// RGBA8 of source pixel (x, y) of image n; pixel (x, y) takes chroma sample (x / 2, y / 2) (NV12ToARGBRow_C, row_common.cc:1945-1967)
+template <int FMT>
+__device__ __forceinline__ void frame_texel(const FrameV& s, int n, int x, int y, float rgba[4]) {
+    if (FMT == SNNB_FRAME_RGBA8) {
+        const uint8_t* p = s.plane[0] + n * s.stride[0] + (size_t) y * s.pitch[0] + (size_t) x * 4;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) rgba[c] = (float) __ldg(p + c);
+        return;
+    }
+    const int Y = __ldg(s.plane[0] + n * s.stride[0] + (size_t) y * s.pitch[0] + x);
+    int U, V;
+    if (FMT == SNNB_FRAME_I420) {
+        U = __ldg(s.plane[1] + n * s.stride[1] + (size_t) (y >> 1) * s.pitch[1] + (x >> 1));
+        V = __ldg(s.plane[2] + n * s.stride[2] + (size_t) (y >> 1) * s.pitch[2] + (x >> 1));
+    } else {
+        const uint8_t* uv = s.plane[1] + n * s.stride[1] + (size_t) (y >> 1) * s.pitch[1] + (size_t) (x >> 1) * 2;
+        U = __ldg(uv + (FMT == SNNB_FRAME_NV21 ? 1 : 0));
+        V = __ldg(uv + (FMT == SNNB_FRAME_NV21 ? 0 : 1));
+    }
+    const int y1 = (int) ((uint32_t) (Y * 0x0101 * s.yg) >> 16);
+    rgba[0] = (float) min(max((-(V * s.vr) + y1 + s.br) >> 6, 0), 255);
+    rgba[1] = (float) min(max((-(U * s.ug + V * s.vg) + y1 + s.bg) >> 6, 0), 255);
+    rgba[2] = (float) min(max((-(U * s.ub) + y1 + s.bb) >> 6, 0), 255);
+    rgba[3] = 255.0f;
+}
+// One thread per output pixel (C <= 4: one 8-channel group). A frame of the model's size is sampled directly, as submitImpl does.
+template <int FMT>
+__global__ void __launch_bounds__(256) frame_input_kernel(FrameV s, TV t, U8Norm q, int linear, FeedV f) {
+    pdl_wait();
+    const size_t total = (size_t) t.N * t.H * t.W;
+    const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (px >= total) return;
+    const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
+    const bool direct = s.w == t.W && s.h == t.H;
+    ResizeTaps r;
+    if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
+    else r = resize_taps(resize_pos(ox, oy, t.W, t.H, s.w, s.h), s.w, s.h, linear);
+    float p00[4];
+    frame_texel<FMT>(s, n, r.x0, r.y0, p00);
+    float v[8];
+    if (linear && !direct) {
+        float p01[4], p10[4], p11[4];
+        frame_texel<FMT>(s, n, r.x1, r.y0, p01);
+        frame_texel<FMT>(s, n, r.x0, r.y1, p10);
+        frame_texel<FMT>(s, n, r.x1, r.y1, p11);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = (j < t.C) ? (r.blend(p00[j & 3], p01[j & 3], p10[j & 3], p11[j & 3]) - q.mean[j & 3]) * q.norm[j & 3] : 0.0f;
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = (j < t.C) ? (p00[j & 3] - q.mean[j & 3]) * q.norm[j & 3] : 0.0f;
+    }
+    if (!f.only) store8(t.hi, t.lo, px * 8, v);
+    if (f.hi) store_feed(f, px, t.H, t.W, v);
+}
+int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t) {
+    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
+    // libyuv row_common.cc:1115-1358: YG, YGB, UB, UG, VG, VR of BT.601 (kYuvI601Constants) and BT.709 (kYuvH709Constants)
+    static const int M[2][6] = {{18997, -1160, -128, 25, 52, -102}, {18997, -1160, -128, 14, 34, -115}};
+    const int* m = M[fr.matrix == SNNB_YUV_BT709 ? 1 : 0];
+    FrameV s;
+    for (int i = 0; i < 3; ++i) s.plane[i] = fr.plane[i], s.pitch[i] = fr.pitch[i], s.stride[i] = fr.image_stride[i];
+    s.w = fr.width, s.h = fr.height;
+    s.yg = m[0], s.ub = m[2], s.ug = m[3], s.vg = m[4], s.vr = m[5];
+    s.bb = m[2] * 128 + m[1], s.bg = m[3] * 128 + m[4] * 128 + m[1], s.br = m[5] * 128 + m[1];
+    U8Norm q;
+    for (int i = 0; i < 4; ++i) q.mean[i] = fr.mean4[i], q.norm[i] = fr.norm4[i];
+    const int linear = fr.linear_filter ? 1 : 0;
+    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
+    switch (fr.format) {
+    case SNNB_FRAME_NV12:
+        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<nv12>");
+    case SNNB_FRAME_NV21:
+        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<nv21>");
+    case SNNB_FRAME_I420:
+        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<i420>");
+    case SNNB_FRAME_RGBA8:
+        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<rgba8>");
+    }
+    SNNB_REQUIRE(false, "launch_frame_input: unknown format %d", fr.format);
 }
 
 } // namespace snnb

@@ -245,6 +245,8 @@ int launch_merge_u8(snnb_context* ctx, const snnb_tensor* t, uint8_t* dev_nhwc_u
 // Output: hi + lo as F32, __float2half_rn of it as F16, clamp(round(v * b.scale + b.offset), 0, 255) as U8. Never reads a feed copy.
 int launch_device_input(snnb_context* ctx, const snnb_device_buffer& b, snnb_tensor* t);
 int launch_device_output(snnb_context* ctx, const snnb_tensor* t, const snnb_device_buffer& b);
+// Device frames (snnb_model_run_frames, checked by the caller) -> libyuv RGBA8 per tap -> resized + normalised -> t (C <= 4)
+int launch_frame_input(snnb_context* ctx, const snnb_frames& f, snnb_tensor* t);
 
 // ---- host-side weight folding/packing (pack.cpp) -----------------------------------------------------------
 // K ordering of the row-window convolution kernel (kernels_umma.cu): for stride s the taps of one filter row fall

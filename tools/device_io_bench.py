@@ -2,7 +2,7 @@
 
     python tools/device_io_bench.py --out DIR [--seconds 2] [--rounds 3]
 
-Writes DIR/device_io_bench.json and prints it. Three parts, all in one process:
+Writes DIR/device_io_bench.json and prints it. Four parts, all in one process:
 
   throughput   ResNet-18 224x224 batch 32 fed with uint8 NCHW images already on the GPU (what a GPU JPEG decoder returns), device
                classes and logits out, against snnb_model_submit_u8 / snnb_model_wait from pinned host uint8 NHWC images; and Candy 720x720
@@ -17,6 +17,13 @@ Writes DIR/device_io_bench.json and prints it. Three parts, all in one process:
                in device memory) against snnb_model_submit_u8 / wait + snnb_model_get_boxes for every image from pinned host memory,
                alternating as above; and the device time of the decode kernels (yolo_select / yolo_rank / yolo_nms) next to the forward
                pass's kernels, from torch.profiler over 50 calls, on the synthetic heads and on all-pass heads (every cell passes).
+  frames       YOLOv3-tiny 416x416 batch 16 and ResNet-18 224x224 batch 32 fed with 1920x1080 NV12 frames on the GPU (what NVDEC
+               returns): detect_frames / run_frames (colour conversion, resize and normalisation in frame_input_kernel) against what a
+               user does without them, a torch NV12 -> RGB conversion (BT.601 limited range, float) + F.interpolate (bilinear) + the
+               normalisation, then detect_torch / run_torch with the float32 NCHW tensor; alternating as above. And frame_input_kernel's
+               device time per batch from torch.profiler over 50 calls, with bytes/s from what it must move: the model-input planes it
+               writes, plus the source bytes under its taps (4 per output pixel, each a Y byte and a UV pair, capped by the planes'
+               sizes), or plus the whole frame as the upper bound.
   card         name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -283,12 +290,97 @@ def detector(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def torch_nv12_to_model(torch, frames, hw, mean4, norm4):
+    """The path without run_frames: NV12 [N, H * 3 // 2, W] uint8 -> float RGB (BT.601 limited range) -> bilinear resize -> normalised
+    float32 NCHW."""
+    import torch.nn.functional as F
+    n, rows, w = frames.shape
+    h = rows // 3 * 2
+    y = frames[:, :h].float() - 16.0
+    uv = frames[:, h:].reshape(n, h // 2, w // 2, 2).float() - 128.0
+    u = uv[..., 0].repeat_interleave(2, 1).repeat_interleave(2, 2)
+    v = uv[..., 1].repeat_interleave(2, 1).repeat_interleave(2, 2)
+    c = 1.164 * y
+    rgb = torch.stack([c + 1.596 * v, c - 0.391 * u - 0.813 * v, c + 2.018 * u], 1).clamp_(0.0, 255.0)
+    x = F.interpolate(rgb, size=hw, mode="bilinear", align_corners=False)
+    mean = torch.tensor(mean4[:3], device=x.device).view(1, 3, 1, 1)
+    norm = torch.tensor(norm4[:3], device=x.device).view(1, 3, 1, 1)
+    return ((x - mean) * norm).contiguous()
+
+
+def frame_kernel_us(torch, fn, calls):
+    """Device time per call (us) of frame_input_kernel, from torch.profiler."""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(5):
+        fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            fn()
+        torch.cuda.synchronize()
+    for e in prof.key_averages():
+        if "snnb::frame_input_kernel" in e.key:
+            total = getattr(e, "device_time_total", None)
+            total = e.cuda_time_total if total is None else total
+            return {"kernel": e.key, "launches": e.count, "us_per_batch": total / calls}
+    raise RuntimeError("frame_input_kernel did not appear in the profile")
+
+
+def frames(torch, ctx, core, modelzoo, d, args):
+    H, W = 1080, 1920
+    res = []
+    # (model, hw, batch, mean, norm, bytes written per model pixel: ResNet-18's input is read by its stem alone, so only the 4-channel
+    # feed copy is written (2 planes x 2 bytes x 4); YOLOv3-tiny's stem reads the regular planes (2 planes x 2 bytes x 8 channels))
+    cases = [("yolov3tiny", (416, 416), 16, [127.5] * 4, [1.0 / 127.5] * 4, 32), ("resnet18", (224, 224), 32, [127.5] * 4, [1.0 / 127.5] * 4, 16)]
+    for name, hw, batch, mean4, norm4, out_bpp in cases:
+        path, _ = modelzoo.build(name, os.path.join(d, "frames_%s" % name), input_hw=hw)
+        m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+        g = torch.Generator().manual_seed(7)
+        nv12 = torch.randint(16, 236, (batch, H * 3 // 2, W), dtype=torch.uint8, generator=g).cuda()
+        if name == "yolov3tiny":
+            fused = lambda: m.detect_frames(nv12, mean4=mean4, norm4=norm4)  # noqa: E731
+            unfused = lambda: m.detect_torch(torch_nv12_to_model(torch, nv12, hw, mean4, norm4), layout="nchw")  # noqa: E731
+        else:
+            fused = lambda: m.run_frames(nv12, mean4=mean4, norm4=norm4, want_classes=True)  # noqa: E731
+            unfused = lambda: m.run_torch(torch_nv12_to_model(torch, nv12, hw, mean4, norm4), layout="nchw", want_classes=True)  # noqa: E731
+        for _ in range(5):
+            fused()
+            unfused()
+        torch.cuda.synchronize()
+        rounds = []
+        for _ in range(args.rounds):
+            rounds.append({"frames": timed(fused, args.seconds, batch, torch.cuda.synchronize), "torch": timed(unfused, args.seconds, batch, torch.cuda.synchronize)})
+        med = lambda k: float(np.median([r[k]["frames_per_s"] for r in rounds]))  # noqa: E731
+        kt = frame_kernel_us(torch, fused, 50)
+        px = batch * hw[0] * hw[1]
+        written = px * out_bpp
+        sampled = batch * (min(4 * hw[0] * hw[1], H * W) + 2 * min(4 * hw[0] * hw[1], (H // 2) * (W // 2)))
+        whole = batch * H * W * 3 // 2
+        sec = kt["us_per_batch"] * 1e-6
+        kt.update({"bytes_written": written, "bytes_sampled": sampled, "bytes_whole_frames": whole,
+                   "bytes_per_s_sampled": (written + sampled) / sec, "bytes_per_s_whole_frames": (written + whole) / sec})
+        kt["share_of_hbm_peak_sampled"] = kt["bytes_per_s_sampled"] / HBM_BYTES_PER_S
+        kt["share_of_hbm_peak_whole_frames"] = kt["bytes_per_s_whole_frames"] / HBM_BYTES_PER_S
+        res.append({
+            "case": "%s %dx%d batch %d from %dx%d NV12" % (name, hw[0], hw[1], batch, W, H),
+            "frames_path": "detect_frames" if name == "yolov3tiny" else "run_frames (+ device classes)",
+            "torch_path": "torch NV12 -> RGB + F.interpolate + normalise, then %s with float32 NCHW" % ("detect_torch" if name == "yolov3tiny" else "run_torch"),
+            "frames_frames_per_s_median": med("frames"),
+            "torch_frames_per_s_median": med("torch"),
+            "frames_over_torch": med("frames") / med("torch"),
+            "rounds": rounds,
+            "frame_input_kernel": kt,
+        })
+        m.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
     ap.add_argument("--seconds", type=float, default=2.0)
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--parts", default="throughput,conversions,detector", help="comma-separated subset of throughput, conversions, detector")
+    ap.add_argument("--parts", default="throughput,conversions,detector,frames", help="comma-separated subset of throughput, conversions, detector, frames")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -305,6 +397,8 @@ def main():
         result["conversions"] = conversions(torch, ctx, core, modelzoo, d)
     if "detector" in parts:
         result["detector"] = detector(torch, ctx, core, modelzoo, d, args)
+    if "frames" in parts:
+        result["frames"] = frames(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
