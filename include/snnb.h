@@ -295,6 +295,38 @@ typedef struct {
 int snnb_model_run_frames(snnb_model* m, const snnb_frames* frames, const snnb_device_buffer* outputs, int num_outputs, int* classes_1based_dev,
                           void* stream);
 int snnb_model_detect_frames(snnb_model* m, const snnb_frames* frames, float* rows_dev, int max_rows, int* counts_dev, void* stream);
+/* Image-to-image models (style transfer, super-resolution) from device frames to device frames: snnb_model_run_frames' input, the
+ * forward pass, then output 0 written as the loaded batch of 8-bit frames of any size, for an encoder (NV12) or a display (RGBA8). It
+ * replaces a U8 output followed by a resize, an RGB -> YUV conversion and a pack in the caller's own code. The reference's path is
+ * the same: the output goes to an RGBA8 texture, ImageTexture::resize, then rgba8ToNv12 / rgba8ToNv21 / rgba8ToI420
+ * (core/src/image.cpp:1051-1100 = libyuv ABGRToNV12 / ABGRToNV21 / ABGRToI420). Every output byte, for image n of output 0
+ * (H_o x W_o x C, C = 1, 3 or 4):
+ *   1. M, an RGBA8 image of the model's size: each component clamp(rint(v * scale + offset), 0, 255), exactly the U8 output of
+ *      snnb_model_run_device. C = 4: RGBA; C = 3: RGB, A = 255; C = 1: R = G = B = that value, A = 255 (a luminance or a mask).
+ *   2. F = ImageTexture::resize of M to width x height (the taps of snnb_image_io; F = M at equal sizes). Linear: top = p00 + ax * (p01
+ *      - p00), bot = p10 + ax * (p11 - p10), v = top + ay * (bot - top) in IEEE float32 with every operation rounded on its own, then
+ *      rint(v).
+ *   3. RGBA8: F. NV12 / NV21 / I420: libyuv's ABGRToNV12 / ABGRToNV21 / ABGRToI420 of F with its portable C rows: BT.601 limited range,
+ *      Y = (66 R + 129 G + 25 B + 0x1080) >> 8; each chroma sample averages its 2 x 2 block as (a + b + c + d) >> 2 (an odd last column
+ *      (a + b) >> 1 over its two rows, an odd last row paired with itself), U = (112 B - 74 G - 38 R + 0x8080) >> 8, V = (112 R - 94 G -
+ *      18 B + 0x8080) >> 8. An encoder fed these frames must signal BT.601 limited range.
+ * Bytes of a plane outside its rows (pitch padding, gaps between planes and images) are not written. `out` may alias `frames` (an
+ * in-place filter of a decoder surface): the output is written after the forward pass, in stream order. */
+typedef struct {
+    int format;                 /* SNNB_FRAME_*; the YUV formats are BT.601 limited range */
+    int width, height;          /* any >= 1 (odd allowed: chroma is ceil(w/2) x ceil(h/2), as libyuv) */
+    uint8_t* plane[3];          /* NV12/NV21: Y, UV|VU; I420: Y, U, V; RGBA8: RGBA. Device memory of the model's device */
+    int pitch[3];               /* bytes per row, >= the row's bytes */
+    long long image_stride[3];  /* bytes from image n to image n+1, per plane */
+    int linear_filter;          /* resize filter, as snnb_image_io */
+    float scale, offset;        /* model output -> 8 bits, exactly as the U8 output of snnb_model_run_device */
+} snnb_frames_out;
+/* frames: exactly as snnb_model_run_frames, with the same checks. Also checked on the host before anything is enqueued: out's format,
+ * width and height >= 1, each used pitch >= its row's bytes, each used plane device or managed memory of the context's device, and an
+ * output 0 of 1, 3 or 4 channels that is not a YOLO layer. Stream contract and fences: those of snnb_model_run_device. Cost beyond the
+ * forward pass: one kernel launch for the input and one for the output (Candy 720x720 x 8 to 1920x1080 NV12: 263 us; NVIDIA H100 80GB
+ * HBM3, 400 W power limit). */
+int snnb_model_transform_frames(snnb_model* m, const snnb_frames* frames, const snnb_frames_out* out, void* stream);
 /* Device-resident variant: inputs already uploaded with snnb_model_set_input(); forward only, asynchronous. */
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input_nhwc);
 int snnb_model_forward(snnb_model* m);

@@ -98,6 +98,21 @@ class Frames(C.Structure):
     ]
 
 
+class FramesOut(C.Structure):
+    """snnb_frames_out"""
+    _fields_ = [
+        ("format", C.c_int),
+        ("width", C.c_int),
+        ("height", C.c_int),
+        ("plane", C.c_void_p * 3),
+        ("pitch", C.c_int * 3),
+        ("image_stride", C.c_longlong * 3),
+        ("linear_filter", C.c_int),
+        ("scale", C.c_float),
+        ("offset", C.c_float),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/snnb.h declares
 SIGNATURES = {
     "snnb_version": (C.c_int, []),
@@ -163,6 +178,7 @@ SIGNATURES = {
     "snnb_model_detect_device": (C.c_int, [vp, C.POINTER(DeviceBuffer), C.c_int, vp, C.c_int, vp, vp]),
     "snnb_model_run_frames": (C.c_int, [vp, C.POINTER(Frames), C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
     "snnb_model_detect_frames": (C.c_int, [vp, C.POINTER(Frames), vp, C.c_int, vp, vp]),
+    "snnb_model_transform_frames": (C.c_int, [vp, C.POINTER(Frames), C.POINTER(FramesOut), vp]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),

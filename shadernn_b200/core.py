@@ -522,34 +522,42 @@ class MixedInferenceCore:
         if format not in self._FRAME_FORMATS or matrix not in self._YUV_MATRICES:
             raise ValueError("%s: format %r / matrix %r: expected one of %s and one of %s" % (who, format, matrix, sorted(self._FRAME_FORMATS),
                                                                                                sorted(self._YUV_MATRICES)))
-        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
-            raise ValueError("%s: frames must be a uint8 CUDA tensor" % who)
         f = _lib.Frames()
         f.format, f.matrix, f.linear_filter = self._FRAME_FORMATS[format], self._YUV_MATRICES[matrix], int(bool(linear))
         f.mean4 = (C.c_float * 4)(*[float(v) for v in (mean4 if mean4 is not None else [0.0] * 4)])
         f.norm4 = (C.c_float * 4)(*[float(v) for v in (norm4 if norm4 is not None else [1.0] * 4)])
+        n = self._frame_planes(who, "frames", frames, format, f)
+        if n != self.batch:
+            raise ValueError("%s: %d frames given, the model's batch is %d" % (who, n, self.batch))
+        return f
+
+    @staticmethod
+    def _frame_planes(who, what, frames, format, f):
+        """The size, planes, pitches and image strides of an snnb_frames / snnb_frames_out `f` from a uint8 CUDA tensor in the layouts
+        of _frames; returns the number of frames."""
+        import torch
+        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+            raise ValueError("%s: %s must be a uint8 CUDA tensor" % (who, what))
         shape, st, base = tuple(frames.shape), frames.stride(), frames.data_ptr()
         if format == "rgba8":
             if len(shape) != 4 or shape[3] != 4 or st[3] != 1 or st[2] != 4:
-                raise ValueError("%s: rgba8 frames are [N, H, W, 4] with dense pixels; got shape %s, strides %s" % (who, shape, st))
+                raise ValueError("%s: rgba8 %s are [N, H, W, 4] with dense pixels; got shape %s, strides %s" % (who, what, shape, st))
             n, f.height, f.width = shape[0], shape[1], shape[2]
             f.plane[0], f.pitch[0], f.image_stride[0] = base, st[1], st[0]
         else:
             if len(shape) != 3 or shape[1] % 3 or shape[1] < 3 or shape[2] % 2 or st[2] != 1:
-                raise ValueError("%s: %s frames are [N, H * 3 // 2, W] with H and W even and dense rows; got shape %s, strides %s" % (who, format, shape, st))
+                raise ValueError("%s: %s %s are [N, H * 3 // 2, W] with H and W even and dense rows; got shape %s, strides %s" % (who, format, what, shape, st))
             n, f.height, f.width = shape[0], shape[1] // 3 * 2, shape[2]
             pitch = st[1]
             if format == "i420" and pitch != f.width:
-                raise ValueError("%s: i420 frames must have dense rows (row stride %d, width %d)" % (who, pitch, f.width))
+                raise ValueError("%s: i420 %s must have dense rows (row stride %d, width %d)" % (who, what, pitch, f.width))
             f.plane[0], f.pitch[0] = base, pitch
             f.plane[1], f.pitch[1] = base + f.height * pitch, pitch if format != "i420" else f.width // 2
             if format == "i420":
                 f.plane[2], f.pitch[2] = base + f.height * pitch + (f.height // 2) * (f.width // 2), f.width // 2
             for p in range(3):
                 f.image_stride[p] = st[0]
-        if n != self.batch:
-            raise ValueError("%s: %d frames given, the model's batch is %d" % (who, n, self.batch))
-        return f
+        return n
 
     def run_frames(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_dtype=None, out_layout="nhwc", out_scale=1.0,
                    out_offset=0.0, want_classes=False):
@@ -574,6 +582,34 @@ class MixedInferenceCore:
         check(lib().snnb_model_detect_frames(self.h, C.byref(f), rows.data_ptr() or None, int(max_rows), counts.data_ptr(), self._torch_stream()),
               "snnb_model_detect_frames")
         return rows, counts
+
+    def transform_frames(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_format=None, out_hw=None,
+                         out_linear=True, out_scale=1.0, out_offset=0.0, out=None):
+        """snnb_model_transform_frames: run_frames' input and forward pass, then output 0 (1, 3 or 4 channels) written as 8-bit frames:
+        clamp(round(v * out_scale + out_offset), 0, 255) as RGBA8 (1 channel: grey; 3: alpha 255), resized to out_hw (linear or
+        nearest, as run_image) and converted as libyuv's ABGRToNV12 / ABGRToNV21 / ABGRToI420 (BT.601 limited range). Ordered on the
+        current torch stream and never synchronising.
+
+        out_format defaults to `format` and out_hw to the input frames' size. Returns `out`, a uint8 CUDA tensor in _frames' layouts
+        ([N, H * 3 // 2, W] for the YUV formats, [N, H, W, 4] for RGBA8), allocated here unless given; it may be `frames` itself."""
+        import torch
+        out_format = format if out_format is None else out_format
+        if out_format not in self._FRAME_FORMATS:
+            raise ValueError("transform_frames: out_format %r: expected one of %s" % (out_format, sorted(self._FRAME_FORMATS)))
+        f = self._frames("transform_frames", frames, format, matrix, linear, mean4, norm4)
+        oh, ow = (f.height, f.width) if out_hw is None else (int(out_hw[0]), int(out_hw[1]))
+        if out is None:
+            if out_format != "rgba8" and (oh % 2 or ow % 2):
+                raise ValueError("transform_frames: %s frames of %d x %d: the packed layout needs H and W even" % (out_format, oh, ow))
+            shape = (self.batch, oh, ow, 4) if out_format == "rgba8" else (self.batch, oh * 3 // 2, ow)
+            out = torch.empty(shape, dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+        o = _lib.FramesOut()
+        o.format, o.linear_filter, o.scale, o.offset = self._FRAME_FORMATS[out_format], int(bool(out_linear)), float(out_scale), float(out_offset)
+        n = self._frame_planes("transform_frames", "out frames", out, out_format, o)
+        if n != self.batch or (out_hw is not None and (o.height, o.width) != (oh, ow)):
+            raise ValueError("transform_frames: out holds %d frames of %d x %d; expected %d of %d x %d" % (n, o.height, o.width, self.batch, oh, ow))
+        check(lib().snnb_model_transform_frames(self.h, C.byref(f), C.byref(o), self._torch_stream()), "snnb_model_transform_frames")
+        return out
 
     def set_input(self, images, idx=0):
         images = _f32(images)

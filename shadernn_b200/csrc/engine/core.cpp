@@ -648,14 +648,15 @@ static int checkDeviceBuffer(const char* api, const snnb_device_buffer& b, int d
     return checkDevicePointer(api, b.data, elem, device, what, idx);
 }
 
-// The frames' row bytes of plane p (NV12 / NV21 rows of ceil(w/2) UV pairs, I420 rows of ceil(w/2) samples), 0 for an unused plane.
-static long long frameRowBytes(const snnb_frames& f, int p) {
-    const long long cw = (f.width + 1) / 2;
-    switch (f.format) {
+// The row bytes of plane p of `width`-pixel frames (NV12 / NV21 rows of ceil(w/2) UV pairs, I420 rows of ceil(w/2) samples), 0 for an
+// unused plane.
+static long long frameRowBytes(int format, int width, int p) {
+    const long long cw = (width + 1) / 2;
+    switch (format) {
     case SNNB_FRAME_NV12:
-    case SNNB_FRAME_NV21: return p == 0 ? f.width : (p == 1 ? 2 * cw : 0);
-    case SNNB_FRAME_I420: return p == 0 ? f.width : cw;
-    case SNNB_FRAME_RGBA8: return p == 0 ? 4LL * f.width : 0;
+    case SNNB_FRAME_NV21: return p == 0 ? width : (p == 1 ? 2 * cw : 0);
+    case SNNB_FRAME_I420: return p == 0 ? width : cw;
+    case SNNB_FRAME_RGBA8: return p == 0 ? 4LL * width : 0;
     }
     return 0;
 }
@@ -670,7 +671,7 @@ int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, c
         const snnb_tensor* t = inputLayers[0]->output;
         SNNB_REQUIRE(t->c >= 1 && t->c <= 4, "%s: the model input has %d channels; frames feed 1 to 4 (RGBA components)", api, t->c);
         for (int p = 0; p < 3; ++p) {
-            const long long row = frameRowBytes(f, p);
+            const long long row = frameRowBytes(f.format, f.width, p);
             if (!row) continue;
             SNNB_REQUIRE(f.pitch[p] >= row, "%s: plane %d: pitch %d is less than its row's %lld bytes", api, p, f.pitch[p], row);
             if (int rc = checkDevicePointer(api, f.plane[p], 1, ctx->device, "plane", p)) return rc;
@@ -785,6 +786,34 @@ int MixedInferenceCore::detectDeviceFeed(const char* api, const DeviceFeed& in, 
 
     if (enqueueDeviceForward(in, stream)) return 1;
     if (launch_yolo_detect(ctx, yolo->inputs[0], yolo->inputs[1], detectScratch, maxRows, rowsDev, countsDev)) return 1;
+    return fenceToCaller(stream);
+}
+
+// Frames in, frames out: runFrames' input staging and forward pass, then output 0 quantised, resized and colour-converted into `out` in
+// one kernel. The output kernel runs after the forward pass on the context's stream, so `out` may alias the input frames.
+int MixedInferenceCore::transformFrames(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream) {
+    static const char* api = "snnb_model_transform_frames";
+    SNNB_REQUIRE(frames, "snnb_model_transform_frames: null frames");
+    SNNB_REQUIRE(out, "snnb_model_transform_frames: null out");
+    DeviceFeed in;
+    in.frames = frames;
+    if (int rc = checkDeviceFeed(api, in, stream)) return rc;
+    const snnb_frames_out& o = *out;
+    SNNB_REQUIRE(o.format >= SNNB_FRAME_NV12 && o.format <= SNNB_FRAME_RGBA8, "%s: unknown out frame format %d", api, o.format);
+    SNNB_REQUIRE(o.width >= 1 && o.height >= 1, "%s: out frame size %d x %d; width and height must be >= 1", api, o.width, o.height);
+    for (int p = 0; p < 3; ++p) {
+        const long long row = frameRowBytes(o.format, o.width, p);
+        if (!row) continue;
+        SNNB_REQUIRE(o.pitch[p] >= row, "%s: out plane %d: pitch %d is less than its row's %lld bytes", api, p, o.pitch[p], row);
+        if (int rc = checkDevicePointer(api, o.plane[p], 1, ctx->device, "out plane", p)) return rc;
+    }
+    SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; frames are written from an image output", api);
+    const snnb_tensor* t = outputLayers[0]->output;
+    SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
+    SNNB_REQUIRE(t->c == 1 || t->c == 3 || t->c == 4, "%s: output 0 has %d channels; frames are written from 1 (grey), 3 (RGB) or 4 (RGBA)", api, t->c);
+
+    if (enqueueDeviceForward(in, stream)) return 1;
+    if (launch_frame_output(ctx, t, o)) return 1;
     return fenceToCaller(stream);
 }
 

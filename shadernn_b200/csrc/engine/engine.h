@@ -356,6 +356,8 @@ public:
     // snnb_model_run_frames / snnb_model_detect_frames: runDevice / detectDevice with device video frames as input 0
     int runFrames(const snnb_frames* frames, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
     int detectFrames(const snnb_frames* frames, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
+    // snnb_model_transform_frames: runFrames' input and fences, then output 0 written as device video frames
+    int transformFrames(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream);
     int layerOutput(int layerId, float* host, size_t capacityFloats);
     int timeLayers(std::vector<float>& ms);
     int dumpOutputs(const std::string& dir);

@@ -144,6 +144,11 @@ int snnb_model_detect_frames(snnb_model* m, const snnb_frames* frames, float* ro
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->detectFrames(frames, rows_dev, max_rows, counts_dev, static_cast<cudaStream_t>(stream));
 }
+int snnb_model_transform_frames(snnb_model* m, const snnb_frames* frames, const snnb_frames_out* out, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_transform_frames: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->transformFrames(frames, out, static_cast<cudaStream_t>(stream));
+}
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input) {
     SNNB_REQUIRE(m, "snnb_model_set_input: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));

@@ -1410,6 +1410,9 @@ int launch_resize_u8(snnb_context* ctx, const uint8_t* dev_nhwc_u8, int src_h, i
     for (int i = 0; i < 4; ++i) q.mean[i] = mean[i], q.norm[i] = norm[i];
     return launch_done(ctx, launch_k(resize_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, dev_nhwc_u8, src_h, src_w, view(t), q, linear ? 1 : 0, feed_view(t)), "resize_u8_kernel");
 }
+// A model output value as 8 bits: clamp(round(v * scale + offset), 0, 255). Every U8 output (merge_u8_kernel, device_output_kernel<u8>,
+// frame_output_kernel) quantises here, so that they cannot drift apart.
+__device__ __forceinline__ float quant_u8(float v, float scale, float offset) { return fminf(fmaxf(rintf(v * scale + offset), 0.0f), 255.0f); }
 // tensor -> 8-bit image, dense NHWC: clamp(round(v * scale + offset), 0, 255) (the image-to-image models' outputs: style transfer,
 // super-resolution); a quarter of the fp32 bytes cross PCIe on the way back
 __global__ void merge_u8_kernel(TV t, uint8_t* __restrict__ dst, float scale, float offset) {
@@ -1424,7 +1427,7 @@ __global__ void merge_u8_kernel(TV t, uint8_t* __restrict__ dst, float scale, fl
     load8(t.hi, t.lo, gid * 8, v);
 #pragma unroll
     for (int j = 0; j < 8; ++j)
-        if (c + j < t.C) dst[px * t.C + c + j] = (uint8_t) fminf(fmaxf(rintf(v[j] * scale + offset), 0.0f), 255.0f);
+        if (c + j < t.C) dst[px * t.C + c + j] = (uint8_t) quant_u8(v[j], scale, offset);
 }
 int launch_merge_u8(snnb_context* ctx, const snnb_tensor* t, uint8_t* dev_nhwc_u8, float scale, float offset) {
     return launch_done(ctx, launch_k(merge_u8_kernel, dim3(vec_blocks(t, 256)), dim3(256), 0, ctx->stream, view(t), dev_nhwc_u8, scale, offset), "merge_u8_kernel");
@@ -1466,7 +1469,7 @@ __device__ __forceinline__ float edge_in(const __half* p, int, const U8Norm&) { 
 __device__ __forceinline__ float edge_in(const uint8_t* p, int c, const U8Norm& q) { return ((float) __ldg(p) - q.mean[c & 3]) * q.norm[c & 3]; } // = split_u8_kernel
 __device__ __forceinline__ void edge_out(float* p, float v, float, float) { *p = v; }
 __device__ __forceinline__ void edge_out(__half* p, float v, float, float) { *p = __float2half_rn(v); }
-__device__ __forceinline__ void edge_out(uint8_t* p, float v, float scale, float offset) { *p = (uint8_t) fminf(fmaxf(rintf(v * scale + offset), 0.0f), 255.0f); } // = merge_u8_kernel
+__device__ __forceinline__ void edge_out(uint8_t* p, float v, float scale, float offset) { *p = (uint8_t) quant_u8(v, scale, offset); }
 
 template <typename T>
 __global__ void device_input_kernel(const T* __restrict__ src, int nchw, TV t, U8Norm q, FeedV f) {
@@ -1655,6 +1658,147 @@ int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t)
         return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<rgba8>");
     }
     SNNB_REQUIRE(false, "launch_frame_input: unknown format %d", fr.format);
+}
+
+// Model output 0 -> device video frames (snnb_model_transform_frames), the reverse of frame_input_kernel. Each frame pixel is
+// ImageTexture::resize (resize_taps) of M, the model-size RGBA8 image whose texels are quant_u8 of the output's channels; then libyuv's
+// ABGRToNV12 / ABGRToNV21 / ABGRToI420 with its portable C rows (row_common.cc:423-473: RGBToY, RGBToU, RGBToV and MAKEROWY's 2 x 2
+// chroma average).
+struct FrameOutV {
+    uint8_t* plane[3];
+    int pitch[3];
+    long long stride[3];
+    int w, h;
+    float scale, offset;
+};
+// ResizeTaps::blend with every + - * rounded on its own: nothing is contracted into an FMA, so numpy float32 restates it exactly.
+__device__ __forceinline__ float blend_rn(const ResizeTaps& r, float p00, float p01, float p10, float p11) {
+    const float top = __fadd_rn(p00, __fmul_rn(r.ax, __fsub_rn(p01, p00)));
+    const float bot = __fadd_rn(p10, __fmul_rn(r.ax, __fsub_rn(p11, p10)));
+    return __fadd_rn(top, __fmul_rn(r.ay, __fsub_rn(bot, top)));
+}
+// Texel (x, y) of image n of M: C = 4 RGBA, C = 3 RGB + alpha 255, C = 1 grey (R = G = B) + alpha 255
+__device__ __forceinline__ void out_texel(const TV& t, int n, int x, int y, float scale, float offset, float rgba[4]) {
+    float v[8];
+    load8(t.hi, t.lo, (((size_t) n * t.H + y) * t.W + x) * t.Cp, v);
+    if (t.C == 1) {
+        rgba[0] = rgba[1] = rgba[2] = quant_u8(v[0], scale, offset);
+    } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) rgba[c] = quant_u8(v[c], scale, offset);
+    }
+    rgba[3] = t.C == 4 ? quant_u8(v[3], scale, offset) : 255.0f;
+}
+// Pixel (x, y) of image n of the frame-size RGBA8 image F. A frame of the output's size takes M as it is.
+__device__ __forceinline__ void frame_out_pixel(const TV& t, const FrameOutV& o, int n, int x, int y, int linear, int rgba[4]) {
+    const bool direct = o.w == t.W && o.h == t.H;
+    ResizeTaps r;
+    if (direct) r.x0 = r.x1 = x, r.y0 = r.y1 = y, r.ax = r.ay = 0.0f;
+    else r = resize_taps(resize_pos(x, y, o.w, o.h, t.W, t.H), t.W, t.H, linear);
+    float p00[4];
+    out_texel(t, n, r.x0, r.y0, o.scale, o.offset, p00);
+    if (linear && !direct) {
+        float p01[4], p10[4], p11[4];
+        out_texel(t, n, r.x1, r.y0, o.scale, o.offset, p01);
+        out_texel(t, n, r.x0, r.y1, o.scale, o.offset, p10);
+        out_texel(t, n, r.x1, r.y1, o.scale, o.offset, p11);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) rgba[c] = (int) rintf(blend_rn(r, p00[c], p01[c], p10[c], p11[c]));
+    } else {
+#pragma unroll
+        for (int c = 0; c < 4; ++c) rgba[c] = (int) p00[c];
+    }
+}
+// Two bytes at p, in one store where p is 2-byte aligned
+__device__ __forceinline__ void store_2u8(uint8_t* p, int a, int b) {
+    if ((reinterpret_cast<uintptr_t>(p) & 1) == 0) *reinterpret_cast<uint16_t*>(p) = (uint16_t) (a | (b << 8));
+    else p[0] = (uint8_t) a, p[1] = (uint8_t) b;
+}
+// One thread per 2 x 2 block of frame pixels, i.e. per chroma sample: its 4 pixels of F, then 4 Y bytes and the chroma sample (or
+// 4 RGBA8 pixels). Pixels past an odd width or height are not written.
+template <int FMT>
+__global__ void __launch_bounds__(256) frame_output_kernel(TV t, FrameOutV o, int linear) {
+    pdl_wait();
+    const int cw = (o.w + 1) >> 1, ch = (o.h + 1) >> 1;
+    const size_t total = (size_t) t.N * ch * cw;
+    const size_t gid   = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= total) return;
+    const int bx = (int) (gid % cw), by = (int) ((gid / cw) % ch), n = (int) (gid / ((size_t) cw * ch));
+    const int x = 2 * bx, y = 2 * by;
+    const bool has_x1 = x + 1 < o.w, has_y1 = y + 1 < o.h;
+    int p[2][2][4];
+    frame_out_pixel(t, o, n, x, y, linear, p[0][0]);
+    if (has_x1) frame_out_pixel(t, o, n, x + 1, y, linear, p[0][1]);
+    if (has_y1) frame_out_pixel(t, o, n, x, y + 1, linear, p[1][0]);
+    if (has_x1 && has_y1) frame_out_pixel(t, o, n, x + 1, y + 1, linear, p[1][1]);
+    if (FMT == SNNB_FRAME_RGBA8) {
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy)
+#pragma unroll
+            for (int dx = 0; dx < 2; ++dx) {
+                if ((dx && !has_x1) || (dy && !has_y1)) continue;
+                const int* q = p[dy][dx];
+                uint8_t* d = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + (size_t) (x + dx) * 4;
+                if ((reinterpret_cast<uintptr_t>(d) & 3) == 0) *reinterpret_cast<uint32_t*>(d) = (uint32_t) (q[0] | (q[1] << 8) | (q[2] << 16) | (q[3] << 24));
+                else d[0] = (uint8_t) q[0], d[1] = (uint8_t) q[1], d[2] = (uint8_t) q[2], d[3] = (uint8_t) q[3];
+            }
+        return;
+    }
+#pragma unroll
+    for (int dy = 0; dy < 2; ++dy) {
+        if (dy && !has_y1) break;
+        uint8_t* d = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + x;
+        const int* a = p[dy][0];
+        const int ya = (66 * a[0] + 129 * a[1] + 25 * a[2] + 0x1080) >> 8;
+        if (has_x1) {
+            const int* b = p[dy][1];
+            store_2u8(d, ya, (66 * b[0] + 129 * b[1] + 25 * b[2] + 0x1080) >> 8);
+        } else {
+            d[0] = (uint8_t) ya;
+        }
+    }
+    // libyuv pairs an odd last row with itself (ABGRToUVRow with stride 0) and averages an odd last column over its two rows
+    int avg[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int a = p[0][0][c], cc = has_y1 ? p[1][0][c] : a;
+        if (has_x1) {
+            const int b = p[0][1][c], dd = has_y1 ? p[1][1][c] : b;
+            avg[c] = (a + b + cc + dd) >> 2;
+        } else {
+            avg[c] = (a + cc) >> 1;
+        }
+    }
+    const int U = (112 * avg[2] - 74 * avg[1] - 38 * avg[0] + 0x8080) >> 8, V = (112 * avg[0] - 94 * avg[1] - 18 * avg[2] + 0x8080) >> 8;
+    if (FMT == SNNB_FRAME_I420) {
+        o.plane[1][n * o.stride[1] + (size_t) by * o.pitch[1] + bx] = (uint8_t) U;
+        o.plane[2][n * o.stride[2] + (size_t) by * o.pitch[2] + bx] = (uint8_t) V;
+    } else {
+        uint8_t* d = o.plane[1] + n * o.stride[1] + (size_t) by * o.pitch[1] + (size_t) bx * 2;
+        if (FMT == SNNB_FRAME_NV12) store_2u8(d, U, V);
+        else store_2u8(d, V, U);
+    }
+}
+int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames_out& fr) {
+    SNNB_REQUIRE((t->c == 1 || t->c == 3 || t->c == 4) && t->cp == 8 && !t->feed_only, "launch_frame_output: the output tensor has %d channels; frames are written from 1, 3 or 4",
+                 t->c);
+    FrameOutV o;
+    for (int i = 0; i < 3; ++i) o.plane[i] = fr.plane[i], o.pitch[i] = fr.pitch[i], o.stride[i] = fr.image_stride[i];
+    o.w = fr.width, o.h = fr.height, o.scale = fr.scale, o.offset = fr.offset;
+    const int linear = fr.linear_filter ? 1 : 0;
+    const size_t blocks = (size_t) t->n * ((fr.height + 1) / 2) * ((fr.width + 1) / 2);
+    const dim3 grid((unsigned) ((blocks + 255) / 256)), block(256);
+    switch (fr.format) {
+    case SNNB_FRAME_NV12:
+        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<nv12>");
+    case SNNB_FRAME_NV21:
+        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<nv21>");
+    case SNNB_FRAME_I420:
+        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<i420>");
+    case SNNB_FRAME_RGBA8:
+        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<rgba8>");
+    }
+    SNNB_REQUIRE(false, "launch_frame_output: unknown format %d", fr.format);
 }
 
 } // namespace snnb

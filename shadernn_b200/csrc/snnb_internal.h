@@ -247,6 +247,8 @@ int launch_device_input(snnb_context* ctx, const snnb_device_buffer& b, snnb_ten
 int launch_device_output(snnb_context* ctx, const snnb_tensor* t, const snnb_device_buffer& b);
 // Device frames (snnb_model_run_frames, checked by the caller) -> libyuv RGBA8 per tap -> resized + normalised -> t (C <= 4)
 int launch_frame_input(snnb_context* ctx, const snnb_frames& f, snnb_tensor* t);
+// t (C = 1, 3 or 4) -> 8 bits as launch_device_output's U8 -> RGBA8 -> resized -> libyuv ABGRTo* -> device frames (checked by the caller)
+int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames_out& f);
 
 // ---- host-side weight folding/packing (pack.cpp) -----------------------------------------------------------
 // K ordering of the row-window convolution kernel (kernels_umma.cu): for stride s the taps of one filter row fall

@@ -24,6 +24,11 @@ Writes DIR/device_io_bench.json and prints it. Four parts, all in one process:
                device time per batch from torch.profiler over 50 calls, with bytes/s from what it must move: the model-input planes it
                writes, plus the source bytes under its taps (4 per output pixel, each a Y byte and a UV pair, capped by the planes'
                sizes), or plus the whole frame as the upper bound.
+  transform    (opt-in) Candy 720x720 batch 8 from 1920x1080 NV12 frames to 1920x1080 NV12 frames: transform_frames (output 0 resized
+               and converted to NV12 in frame_output_kernel) against what a user does without it, run_frames(out_dtype=uint8) then
+               F.interpolate (bilinear), a torch RGB -> NV12 conversion (BT.601 limited range) and packing; alternating as above. And
+               frame_output_kernel's device time per batch from torch.profiler over 50 calls, with bytes/s from the frame planes it writes
+               plus the model-output planes it reads under its taps.
   card         name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -308,8 +313,8 @@ def torch_nv12_to_model(torch, frames, hw, mean4, norm4):
     return ((x - mean) * norm).contiguous()
 
 
-def frame_kernel_us(torch, fn, calls):
-    """Device time per call (us) of frame_input_kernel, from torch.profiler."""
+def frame_kernel_us(torch, fn, calls, kernel="frame_input_kernel"):
+    """Device time per call (us) of `kernel` (frame_input_kernel or frame_output_kernel), from torch.profiler."""
     from torch.profiler import ProfilerActivity, profile
     for _ in range(5):
         fn()
@@ -319,11 +324,11 @@ def frame_kernel_us(torch, fn, calls):
             fn()
         torch.cuda.synchronize()
     for e in prof.key_averages():
-        if "snnb::frame_input_kernel" in e.key:
+        if "snnb::" + kernel in e.key:
             total = getattr(e, "device_time_total", None)
             total = e.cuda_time_total if total is None else total
             return {"kernel": e.key, "launches": e.count, "us_per_batch": total / calls}
-    raise RuntimeError("frame_input_kernel did not appear in the profile")
+    raise RuntimeError("%s did not appear in the profile" % kernel)
 
 
 def frames(torch, ctx, core, modelzoo, d, args):
@@ -375,12 +380,67 @@ def frames(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def torch_rgb_to_nv12(torch, rgb_u8_nhwc, hw):
+    """The path without transform_frames: uint8 RGB [N, h, w, 3] -> float -> F.interpolate (bilinear) to hw -> BT.601 limited-range Y, U,
+    V (float) -> chroma averaged over 2 x 2 -> rounded and packed as NV12 [N, H * 3 // 2, W] uint8."""
+    import torch.nn.functional as F
+    x = F.interpolate(rgb_u8_nhwc.permute(0, 3, 1, 2).float(), size=hw, mode="bilinear", align_corners=False)
+    r, g, b = x[:, 0], x[:, 1], x[:, 2]
+    y = 0.257 * r + 0.504 * g + 0.098 * b + 16.0
+    c = F.avg_pool2d(x, 2)
+    u = -0.148 * c[:, 0] - 0.291 * c[:, 1] + 0.439 * c[:, 2] + 128.0
+    v = 0.439 * c[:, 0] - 0.368 * c[:, 1] - 0.071 * c[:, 2] + 128.0
+    uv = torch.stack([u, v], -1).reshape(x.shape[0], hw[0] // 2, hw[1])
+    return torch.cat([y, uv], 1).round_().clamp_(0.0, 255.0).to(torch.uint8)
+
+
+def transform(torch, ctx, core, modelzoo, d, args):
+    H, W = 1080, 1920
+    hw, batch = (720, 720), 8
+    path, _ = modelzoo.build("candy", os.path.join(d, "transform_candy"), input_hw=hw)
+    m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+    g = torch.Generator().manual_seed(7)
+    nv12 = torch.randint(16, 236, (batch, H * 3 // 2, W), dtype=torch.uint8, generator=g).cuda()
+    out = torch.empty_like(nv12)
+    fused = lambda: m.transform_frames(nv12, out=out)  # noqa: E731
+    unfused = lambda: torch_rgb_to_nv12(torch, m.run_frames(nv12, out_dtype=torch.uint8), (H, W))  # noqa: E731
+    for _ in range(5):
+        fused()
+        unfused()
+    torch.cuda.synchronize()
+    rounds = []
+    for _ in range(args.rounds):
+        rounds.append({"transform": timed(fused, args.seconds, batch, torch.cuda.synchronize), "torch": timed(unfused, args.seconds, batch, torch.cuda.synchronize)})
+    med = lambda k: float(np.median([r[k]["frames_per_s"] for r in rounds]))  # noqa: E731
+    kt = frame_kernel_us(torch, fused, 50, "frame_output_kernel")
+    # written: the Y plane and the interleaved UV plane; read: Candy's 3-channel output as split-fp16 (2 planes x 8 channels x 2 bytes per
+    # pixel). Every output texel lies under some frame pixel's taps at this 1.5x upscale, so the whole tensor is read.
+    written = batch * (H * W + H * W // 2)
+    read = batch * hw[0] * hw[1] * 2 * 8 * 2
+    sec = kt["us_per_batch"] * 1e-6
+    kt.update({"bytes_written": written, "bytes_read": read, "bytes_per_s": (written + read) / sec})
+    kt["share_of_hbm_peak"] = kt["bytes_per_s"] / HBM_BYTES_PER_S
+    res = {
+        "case": "candy %dx%d batch %d from %dx%d NV12 to %dx%d NV12" % (hw[0], hw[1], batch, W, H, W, H),
+        "transform_path": "transform_frames (frame_input_kernel, forward pass, frame_output_kernel)",
+        "torch_path": "run_frames(out_dtype=uint8), then F.interpolate + torch RGB -> NV12 (BT.601 limited range) + packing",
+        "transform_frames_per_s_median": med("transform"),
+        "torch_frames_per_s_median": med("torch"),
+        "transform_over_torch": med("transform") / med("torch"),
+        "rounds": rounds,
+        "frame_output_kernel": kt,
+    }
+    m.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
     ap.add_argument("--seconds", type=float, default=2.0)
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--parts", default="throughput,conversions,detector,frames", help="comma-separated subset of throughput, conversions, detector, frames")
+    ap.add_argument("--parts", default="throughput,conversions,detector,frames",
+                    help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -399,6 +459,8 @@ def main():
         result["detector"] = detector(torch, ctx, core, modelzoo, d, args)
     if "frames" in parts:
         result["frames"] = frames(torch, ctx, core, modelzoo, d, args)
+    if "transform" in parts:
+        result["transform"] = transform(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
