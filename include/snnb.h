@@ -327,6 +327,48 @@ typedef struct {
  * forward pass: one kernel launch for the input and one for the output (Candy 720x720 x 8 to 1920x1080 NV12: 263 us; NVIDIA H100 80GB
  * HBM3, 400 W power limit). */
 int snnb_model_transform_frames(snnb_model* m, const snnb_frames* frames, const snnb_frames_out* out, void* stream);
+/* Regions of device frames as the batch: the second stage of a detection pipeline (classify, describe or embed what a detector found)
+ * without a host round trip. A region is a pixel rectangle [x, x + width) x [y, y + height) of frame `frame` of the frames given; `row`
+ * is carried for the caller (the detection row it came from, or anything) and ignored by the engine. */
+typedef struct {
+    int frame, row, x, y, width, height;
+} snnb_roi;
+/* The model's loaded batch B is the number of region slots. rois_dev: device memory holding snnb_roi[B]. count_dev: NULL (all B slots
+ * are used) or a device int; slots i < clamp(*count_dev, 0, B) are used. frames: an snnb_frames exactly as snnb_model_run_frames takes
+ * it, holding num_frames >= 1 frames (independent of B). A used slot is valid when 0 <= frame < num_frames, width, height >= 1,
+ * 0 <= x, x + width <= frames.width, 0 <= y and y + height <= frames.height; the regions live on the device, so this cannot be checked
+ * on the host.
+ * Slot i, when valid, gets exactly the model input snnb_model_run_frames computes for an RGBA8 frame S_i: S_i is the rectangle cut out of
+ * libyuv's RGBA8 image of the whole frame (chroma sited in frame coordinates: pixel (x, y) takes chroma sample (x / 2, y / 2)), then
+ * resized as run_frames resizes a frame, with taps clamped to the edges of the region; a region of the model's size is sampled directly.
+ * Slots past the count and invalid slots get an all-zero input, and every byte of their outputs and their class is zero (classes are
+ * 1-based: 0 = no region). The forward pass runs on the whole batch.
+ * Outputs, classes, the stream contract and the fences are those of snnb_model_run_frames; YOLO models are refused (no detection on
+ * regions). Checked on the host before anything is enqueued: everything run_frames checks, num_frames >= 1, rois_dev (and count_dev
+ * unless NULL) device or managed memory of the context's device, aligned to 4 bytes. Cost beyond run_frames: one kernel launch per
+ * output buffer and one for the classes, which clear the slots that hold no region. */
+int snnb_model_run_rois(snnb_model* m, const snnb_frames* frames, int num_frames, const snnb_roi* rois_dev, const int* count_dev,
+                        const snnb_device_buffer* outputs, int num_outputs, int* classes_1based_dev, void* stream);
+typedef struct {
+    float min_score; /* rows with score >= min_score are kept */
+    int class_id;    /* -1 = any class, else rows of this class only */
+    float expand;    /* >= 0: the fraction of w (h) added on each side */
+} snnb_roi_select;
+/* snnb_model_detect_frames / snnb_model_detect_device rows (rows_dev float32 [num_frames][max_rows][6] {class, score, x, y, w, h},
+ * normalised, x, y the top-left corner) and counts (counts_dev int32 [num_frames]) -> regions of frame_width x frame_height frames, for
+ * snnb_model_run_rois. One kernel on `stream` (NULL: the context's stream); never synchronises. Rows r < min(counts[n], max_rows) of
+ * frame n are visited frame by frame, rows in order (descending score). A row is kept when score >= min_score, class_id is -1 or the
+ * row's class, and its rectangle is non-empty. The rectangle, in float32 with every operation rounded on its own (no FMA):
+ *   ex = expand * w, ey = expand * h
+ *   fx0 = (x - ex) * W, fx1 = ((x + w) + ex) * W, fy0 = (y - ey) * H, fy1 = ((y + h) + ey) * H      (W, H = frame_width, frame_height)
+ *   a NaN among them drops the row; else each is clamped to [0, W] (resp. [0, H]), x0 = floor(fx0), x1 = ceil(fx1), y0 = floor(fy0),
+ *   y1 = ceil(fy1), and the region is {n, r, x0, y0, x1 - x0, y1 - y0}.
+ * The mapping is direct because run_frames / detect_frames stretch the whole frame to the model input (no letterbox). The first
+ * `capacity` kept rows are written to rois_dev (snnb_roi[capacity]), entries past them are zeroed, and *count_dev = min(kept, capacity).
+ * Checked on the host before anything is enqueued: non-null device or managed pointers of the context's device aligned to 4 bytes,
+ * num_frames >= 1, 1 <= max_rows <= 100, frame size >= 1, capacity >= 1, expand finite and >= 0, a stream that is not capturing. */
+int snnb_rois_from_detections(snnb_context* ctx, const float* rows_dev, const int* counts_dev, int num_frames, int max_rows, int frame_width,
+                              int frame_height, const snnb_roi_select* sel, snnb_roi* rois_dev, int capacity, int* count_dev, void* stream);
 /* Device-resident variant: inputs already uploaded with snnb_model_set_input(); forward only, asynchronous. */
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input_nhwc);
 int snnb_model_forward(snnb_model* m);

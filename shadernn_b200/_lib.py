@@ -113,6 +113,27 @@ class FramesOut(C.Structure):
     ]
 
 
+class Roi(C.Structure):
+    """snnb_roi"""
+    _fields_ = [
+        ("frame", C.c_int),
+        ("row", C.c_int),
+        ("x", C.c_int),
+        ("y", C.c_int),
+        ("width", C.c_int),
+        ("height", C.c_int),
+    ]
+
+
+class RoiSelect(C.Structure):
+    """snnb_roi_select"""
+    _fields_ = [
+        ("min_score", C.c_float),
+        ("class_id", C.c_int),
+        ("expand", C.c_float),
+    ]
+
+
 # name -> (restype, argtypes): every symbol include/snnb.h declares
 SIGNATURES = {
     "snnb_version": (C.c_int, []),
@@ -179,6 +200,8 @@ SIGNATURES = {
     "snnb_model_run_frames": (C.c_int, [vp, C.POINTER(Frames), C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
     "snnb_model_detect_frames": (C.c_int, [vp, C.POINTER(Frames), vp, C.c_int, vp, vp]),
     "snnb_model_transform_frames": (C.c_int, [vp, C.POINTER(Frames), C.POINTER(FramesOut), vp]),
+    "snnb_model_run_rois": (C.c_int, [vp, C.POINTER(Frames), C.c_int, vp, vp, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
+    "snnb_rois_from_detections": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(RoiSelect), vp, C.c_int, vp, vp]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),

@@ -51,6 +51,28 @@ class GpuContext:
     def launches(self):
         return int(lib().snnb_launch_count(self.h))
 
+    def rois_from_detections(self, rows, counts, frame_hw, capacity, min_score=0.0, class_id=-1, expand=0.0):
+        """snnb_rois_from_detections: detect_frames / detect_torch rows (float32 CUDA [N, max_rows, 6]) and counts (int32 CUDA [N]) ->
+        regions of frame_hw = (H, W) frames for MixedInferenceCore.run_rois, on the device, ordered on the current torch stream and
+        never synchronising. Rows with score >= min_score and of class class_id (-1: any) are kept, each box grown by `expand` times its
+        width (height) on each side and clipped to the frame, in frame order then row order. Returns (rois, count): an int32 CUDA tensor
+        [capacity, 6] of {frame, row, x, y, width, height}, zero past the count, and an int32 CUDA tensor [1] with min(kept, capacity)."""
+        import torch
+        if not (isinstance(rows, torch.Tensor) and rows.is_cuda and rows.dtype == torch.float32 and rows.dim() == 3 and rows.shape[2] == 6):
+            raise ValueError("rois_from_detections: rows must be a float32 CUDA tensor [N, max_rows, 6]")
+        if not (isinstance(counts, torch.Tensor) and counts.is_cuda and counts.dtype == torch.int32 and tuple(counts.shape) == (rows.shape[0],)):
+            raise ValueError("rois_from_detections: counts must be an int32 CUDA tensor [N] for rows of %d frames" % rows.shape[0])
+        device = torch.device("cuda", self.device)
+        rows, counts = rows.contiguous(), counts.contiguous()
+        rois = torch.empty((max(int(capacity), 0), 6), dtype=torch.int32, device=device)
+        count = torch.empty(1, dtype=torch.int32, device=device)
+        sel = _lib.RoiSelect(float(min_score), int(class_id), float(expand))
+        stream = torch.cuda.current_stream(device).cuda_stream or 1  # the legacy default stream is cudaStreamLegacy (1), not NULL
+        check(lib().snnb_rois_from_detections(self.h, rows.data_ptr() or None, counts.data_ptr() or None, rows.shape[0], rows.shape[1], int(frame_hw[1]),
+                                              int(frame_hw[0]), C.byref(sel), rois.data_ptr() or None, int(capacity), count.data_ptr(), stream),
+              "snnb_rois_from_detections")
+        return rois, count
+
     def close(self):
         if self.h:
             lib().snnb_context_destroy(self.h)
@@ -517,8 +539,14 @@ class MixedInferenceCore:
 
     def _frames(self, who, frames, format, matrix, linear, mean4, norm4):
         """The snnb_frames descriptor of a uint8 CUDA tensor: NV12 / NV21 / I420 as [N, H * 3 // 2, W] (the packed 4:2:0 layout, H and W
-        even; NV12 / NV21 rows may be pitched, I420 rows must be dense), RGBA8 as [N, H, W, 4] (rows may be pitched)."""
-        import torch
+        even; NV12 / NV21 rows may be pitched, I420 rows must be dense), RGBA8 as [N, H, W, 4] (rows may be pitched). N is the batch."""
+        f, n = self._frames_any(who, frames, format, matrix, linear, mean4, norm4)
+        if n != self.batch:
+            raise ValueError("%s: %d frames given, the model's batch is %d" % (who, n, self.batch))
+        return f
+
+    def _frames_any(self, who, frames, format, matrix, linear, mean4, norm4):
+        """_frames for any number of frames: returns (the descriptor, the number of frames)."""
         if format not in self._FRAME_FORMATS or matrix not in self._YUV_MATRICES:
             raise ValueError("%s: format %r / matrix %r: expected one of %s and one of %s" % (who, format, matrix, sorted(self._FRAME_FORMATS),
                                                                                                sorted(self._YUV_MATRICES)))
@@ -526,10 +554,7 @@ class MixedInferenceCore:
         f.format, f.matrix, f.linear_filter = self._FRAME_FORMATS[format], self._YUV_MATRICES[matrix], int(bool(linear))
         f.mean4 = (C.c_float * 4)(*[float(v) for v in (mean4 if mean4 is not None else [0.0] * 4)])
         f.norm4 = (C.c_float * 4)(*[float(v) for v in (norm4 if norm4 is not None else [1.0] * 4)])
-        n = self._frame_planes(who, "frames", frames, format, f)
-        if n != self.batch:
-            raise ValueError("%s: %d frames given, the model's batch is %d" % (who, n, self.batch))
-        return f
+        return f, self._frame_planes(who, "frames", frames, format, f)
 
     @staticmethod
     def _frame_planes(who, what, frames, format, f):
@@ -569,6 +594,27 @@ class MixedInferenceCore:
         f = self._frames("run_frames", frames, format, matrix, linear, mean4, norm4)
         check(lib().snnb_model_run_frames(self.h, C.byref(f), obufs, len(outs), classes.data_ptr() if want_classes else None, self._torch_stream()),
               "snnb_model_run_frames")
+        result = outs[0] if len(outs) == 1 else outs
+        return (result, classes) if want_classes else result
+
+    def run_rois(self, frames, rois, count=None, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_dtype=None, out_layout="nhwc",
+                 out_scale=1.0, out_offset=0.0, want_classes=False):
+        """snnb_model_run_rois: regions of device frames as the batch. frames: any number of frames in _frames' layouts. rois: an int32
+        CUDA tensor [batch, 6] of {frame, row, x, y, width, height} (rois_from_detections makes one); count: None (every slot is used)
+        or an int32 CUDA tensor of one element (slots i < clamp(count, 0, batch) are used). Each used slot whose region lies inside an
+        existing frame gets exactly what run_frames computes for that region cut out as an RGBA8 frame of its own; every other slot
+        comes out all zero, class 0. Outputs, classes and the stream contract as run_frames."""
+        import torch
+        if not (isinstance(rois, torch.Tensor) and rois.is_cuda and rois.dtype == torch.int32 and tuple(rois.shape) == (self.batch, 6)):
+            raise ValueError("run_rois: rois must be an int32 CUDA tensor [%d, 6] (the model's batch)" % self.batch)
+        if count is not None and not (isinstance(count, torch.Tensor) and count.is_cuda and count.dtype == torch.int32 and count.numel() == 1):
+            raise ValueError("run_rois: count must be None or an int32 CUDA tensor of one element")
+        outs, obufs, classes = self._device_outputs("run_rois", out_dtype, out_layout, out_scale, out_offset, want_classes)
+        f, n = self._frames_any("run_rois", frames, format, matrix, linear, mean4, norm4)
+        rois = rois.contiguous()
+        check(lib().snnb_model_run_rois(self.h, C.byref(f), n, rois.data_ptr(), count.data_ptr() if count is not None else None, obufs, len(outs),
+                                        classes.data_ptr() if want_classes else None, self._torch_stream()),
+              "snnb_model_run_rois")
         result = outs[0] if len(outs) == 1 else outs
         return (result, classes) if want_classes else result
 

@@ -1,6 +1,7 @@
 // MixedInferenceCore: init (tensor plan, weight arena, fusion, CUDA-graph capture) and run.
 // Counterpart of core/src/ic2/core.cpp:294-410 (init) and :97-245 (run).
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <unordered_map>
 #include <unordered_set>
@@ -661,6 +662,18 @@ static long long frameRowBytes(int format, int width, int p) {
     return 0;
 }
 
+// A caller's stream that work may be ordered on: NULL (the context's), or a stream that is not being captured.
+static int checkCallerStream(const char* api, cudaStream_t stream) {
+    if (stream) {
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        const cudaError_t e = cudaStreamIsCapturing(stream, &cap);
+        if (e != cudaSuccess) cudaGetLastError();
+        SNNB_REQUIRE(e == cudaSuccess, "%s: stream %p: %s", api, (void*) stream, cudaGetErrorString(e));
+        SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone, "%s: stream %p is being captured; capture into the caller's CUDA graph is not supported", api, (void*) stream);
+    }
+    return 0;
+}
+
 int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, cudaStream_t stream) {
     if (in.frames) {
         const snnb_frames& f = *in.frames;
@@ -676,20 +689,20 @@ int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, c
             SNNB_REQUIRE(f.pitch[p] >= row, "%s: plane %d: pitch %d is less than its row's %lld bytes", api, p, f.pitch[p], row);
             if (int rc = checkDevicePointer(api, f.plane[p], 1, ctx->device, "plane", p)) return rc;
         }
+        if (in.rois) {
+            SNNB_REQUIRE(in.numFrames >= 1, "%s: num_frames %d; at least one frame is required", api, in.numFrames);
+            SNNB_REQUIRE(options.batch <= 65535, "%s: batch %u; regions fill at most 65535 slots", api, options.batch);
+            if (int rc = checkDevicePointer(api, in.rois, sizeof(int), ctx->device, "rois", 0)) return rc;
+            if (in.roiCount)
+                if (int rc = checkDevicePointer(api, in.roiCount, sizeof(int), ctx->device, "count", 0)) return rc;
+        }
     } else {
         SNNB_REQUIRE(in.inputs, "%s: null inputs", api);
         SNNB_REQUIRE(in.numInputs == (int) inputLayers.size(), "%s: %d inputs given, the model has %d", api, in.numInputs, (int) inputLayers.size());
         for (int i = 0; i < in.numInputs; ++i)
             if (int rc = checkDeviceBuffer(api, in.inputs[i], ctx->device, "input", i)) return rc;
     }
-    if (stream) {
-        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-        const cudaError_t e = cudaStreamIsCapturing(stream, &cap);
-        if (e != cudaSuccess) cudaGetLastError();
-        SNNB_REQUIRE(e == cudaSuccess, "%s: stream %p: %s", api, (void*) stream, cudaGetErrorString(e));
-        SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone, "%s: stream %p is being captured; capture into the caller's CUDA graph is not supported", api, (void*) stream);
-    }
-    return 0;
+    return checkCallerStream(api, stream);
 }
 
 // The caller's stream -> the context's stream, the input staging and the forward pass. Called after every check has passed.
@@ -700,7 +713,9 @@ int MixedInferenceCore::enqueueDeviceForward(const DeviceFeed& in, cudaStream_t 
         SNNB_CUDA_OK(cudaEventRecord(callerReady, stream));
         SNNB_CUDA_OK(cudaStreamWaitEvent(ctx->stream, callerReady, 0));
     }
-    if (in.frames) {
+    if (in.rois) {
+        if (launch_frame_roi_input(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, inputLayers[0]->output)) return 1;
+    } else if (in.frames) {
         if (launch_frame_input(ctx, *in.frames, inputLayers[0]->output)) return 1;
     } else {
         for (int i = 0; i < in.numInputs; ++i)
@@ -730,6 +745,14 @@ int MixedInferenceCore::runFrames(const snnb_frames* frames, const snnb_device_b
     in.frames = frames;
     return runDeviceFeed("snnb_model_run_frames", in, outputs, numOutputs, classes1Dev, stream);
 }
+int MixedInferenceCore::runRois(const snnb_frames* frames, int numFrames, const snnb_roi* roisDev, const int* countDev, const snnb_device_buffer* outputs,
+                                int numOutputs, int* classes1Dev, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_run_rois: null frames");
+    SNNB_REQUIRE(roisDev, "snnb_model_run_rois: null rois");
+    DeviceFeed in;
+    in.frames = frames, in.rois = roisDev, in.roiCount = countDev, in.numFrames = numFrames;
+    return runDeviceFeed("snnb_model_run_rois", in, outputs, numOutputs, classes1Dev, stream);
+}
 
 int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev,
                                       cudaStream_t stream) {
@@ -737,6 +760,7 @@ int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, con
     SNNB_REQUIRE(numOutputs >= 0 && numOutputs <= (int) outputLayers.size(), "%s: %d outputs requested, the model has %d", api, numOutputs,
                  (int) outputLayers.size());
     SNNB_REQUIRE(outputs || numOutputs == 0, "%s: null outputs", api);
+    SNNB_REQUIRE(!(in.rois && outputLayers[0]->typeName == "YOLO"), "%s: output 0 is a YOLO detection list; detection on regions is not supported", api);
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO",
                  "%s: output 0 is a YOLO detection list; use %s for device detections, or snnb_model_run or "
                  "snnb_model_submit / snnb_model_wait and read the boxes with snnb_model_get_boxes",
@@ -757,6 +781,16 @@ int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, con
     for (int j = 0; j < numOutputs; ++j)
         if (outputs[j].data && launch_device_output(ctx, outputLayers[j]->output, outputs[j])) return 1;
     if (classes1Dev && launch_argmax(ctx, outputLayers[0]->output, classes1Dev, 1)) return 1; // core.cpp:228-233: argmax + 1
+    if (in.rois) { // the slots without a valid region: every output byte and the class zero
+        const int B = (int) options.batch;
+        for (int j = 0; j < numOutputs; ++j) {
+            if (!outputs[j].data) continue;
+            const snnb_tensor* t = outputLayers[j]->output;
+            const long long elem = outputs[j].dtype == SNNB_DTYPE_F32 ? 4 : (outputs[j].dtype == SNNB_DTYPE_F16 ? 2 : 1);
+            if (launch_roi_clear(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, B, outputs[j].data, (long long) t->h * t->w * t->c * elem)) return 1;
+        }
+        if (classes1Dev && launch_roi_clear(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, B, classes1Dev, (long long) sizeof(int))) return 1;
+    }
     return fenceToCaller(stream);
 }
 
@@ -871,3 +905,22 @@ int MixedInferenceCore::dumpOutputs(const std::string& dir) {
 }
 
 } // namespace snn
+
+// snnb_rois_from_detections: a context-level call with no model state, so its one kernel runs on the caller's stream itself.
+int snnb::rois_from_detections(snnb_context* ctx, const float* rows, const int* counts, int numFrames, int maxRows, int fw, int fh, const snnb_roi_select* sel,
+                               snnb_roi* rois, int capacity, int* count, cudaStream_t stream) {
+    static const char* api = "snnb_rois_from_detections";
+    SNNB_REQUIRE(sel, "%s: null sel", api);
+    SNNB_REQUIRE(numFrames >= 1, "%s: num_frames %d; at least one frame is required", api, numFrames);
+    SNNB_REQUIRE(maxRows >= 1 && maxRows <= 100, "%s: max_rows %d is outside 1..100", api, maxRows);
+    SNNB_REQUIRE((long long) numFrames * maxRows <= 0x7fffffffLL, "%s: %d frames of %d rows", api, numFrames, maxRows);
+    SNNB_REQUIRE(fw >= 1 && fh >= 1, "%s: frame size %d x %d; width and height must be >= 1", api, fw, fh);
+    SNNB_REQUIRE(capacity >= 1, "%s: capacity %d; at least one region is required", api, capacity);
+    SNNB_REQUIRE(std::isfinite(sel->expand) && sel->expand >= 0.0f, "%s: expand %g; a finite value >= 0 is required", api, (double) sel->expand);
+    if (int rc = snn::checkDevicePointer(api, rows, sizeof(float), ctx->device, "rows", 0)) return rc;
+    if (int rc = snn::checkDevicePointer(api, counts, sizeof(int), ctx->device, "counts", 0)) return rc;
+    if (int rc = snn::checkDevicePointer(api, rois, sizeof(int), ctx->device, "rois", 0)) return rc;
+    if (int rc = snn::checkDevicePointer(api, count, sizeof(int), ctx->device, "count", 0)) return rc;
+    if (int rc = snn::checkCallerStream(api, stream)) return rc;
+    return launch_rois_from_detections(ctx, stream ? stream : ctx->stream, rows, counts, numFrames, maxRows, fw, fh, *sel, rois, capacity, count);
+}

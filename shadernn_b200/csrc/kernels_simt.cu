@@ -1604,6 +1604,30 @@ __device__ __forceinline__ void frame_texel(const FrameV& s, int n, int x, int y
     rgba[2] = (float) min(max((-(U * s.ub) + y1 + s.bb) >> 6, 0), 255);
     rgba[3] = 255.0f;
 }
+// The model input of one pixel (C <= 4: one 8-channel group) from its taps `r` in image n of the frames: each tap as libyuv's RGBA8,
+// then resize_u8_kernel's blend (linear, unless the source is sampled directly) and normalisation. Shared by frame_input_kernel and
+// frame_roi_input_kernel.
+template <int FMT>
+__device__ __forceinline__ void frame_pixel(const FrameV& s, int n, const ResizeTaps& r, int linear, bool direct, const TV& t, const U8Norm& q, float v[8]) {
+    float p00[4];
+    frame_texel<FMT>(s, n, r.x0, r.y0, p00);
+    if (linear && !direct) {
+        float p01[4], p10[4], p11[4];
+        frame_texel<FMT>(s, n, r.x1, r.y0, p01);
+        frame_texel<FMT>(s, n, r.x0, r.y1, p10);
+        frame_texel<FMT>(s, n, r.x1, r.y1, p11);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = (j < t.C) ? (r.blend(p00[j & 3], p01[j & 3], p10[j & 3], p11[j & 3]) - q.mean[j & 3]) * q.norm[j & 3] : 0.0f;
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = (j < t.C) ? (p00[j & 3] - q.mean[j & 3]) * q.norm[j & 3] : 0.0f;
+    }
+}
+// The stores of model-input pixel px: the regular planes (unless feed_only) and the stem feed copy
+__device__ __forceinline__ void store_input_pixel(const TV& t, const FeedV& f, size_t px, const float v[8]) {
+    if (!f.only) store8(t.hi, t.lo, px * 8, v);
+    if (f.hi) store_feed(f, px, t.H, t.W, v);
+}
 // One thread per output pixel (C <= 4: one 8-channel group). A frame of the model's size is sampled directly, as submitImpl does.
 template <int FMT>
 __global__ void __launch_bounds__(256) frame_input_kernel(FrameV s, TV t, U8Norm q, int linear, FeedV f) {
@@ -1616,25 +1640,12 @@ __global__ void __launch_bounds__(256) frame_input_kernel(FrameV s, TV t, U8Norm
     ResizeTaps r;
     if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
     else r = resize_taps(resize_pos(ox, oy, t.W, t.H, s.w, s.h), s.w, s.h, linear);
-    float p00[4];
-    frame_texel<FMT>(s, n, r.x0, r.y0, p00);
     float v[8];
-    if (linear && !direct) {
-        float p01[4], p10[4], p11[4];
-        frame_texel<FMT>(s, n, r.x1, r.y0, p01);
-        frame_texel<FMT>(s, n, r.x0, r.y1, p10);
-        frame_texel<FMT>(s, n, r.x1, r.y1, p11);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = (j < t.C) ? (r.blend(p00[j & 3], p01[j & 3], p10[j & 3], p11[j & 3]) - q.mean[j & 3]) * q.norm[j & 3] : 0.0f;
-    } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = (j < t.C) ? (p00[j & 3] - q.mean[j & 3]) * q.norm[j & 3] : 0.0f;
-    }
-    if (!f.only) store8(t.hi, t.lo, px * 8, v);
-    if (f.hi) store_feed(f, px, t.H, t.W, v);
+    frame_pixel<FMT>(s, n, r, linear, direct, t, q, v);
+    store_input_pixel(t, f, px, v);
 }
-int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t) {
-    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
+// The kernel-side view of an snnb_frames: planes, size and libyuv's constants of its matrix; and its mean / norm
+static FrameV frame_view(const snnb_frames& fr) {
     // libyuv row_common.cc:1115-1358: YG, YGB, UB, UG, VG, VR of BT.601 (kYuvI601Constants) and BT.709 (kYuvH709Constants)
     static const int M[2][6] = {{18997, -1160, -128, 25, 52, -102}, {18997, -1160, -128, 14, 34, -115}};
     const int* m = M[fr.matrix == SNNB_YUV_BT709 ? 1 : 0];
@@ -1643,8 +1654,17 @@ int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t)
     s.w = fr.width, s.h = fr.height;
     s.yg = m[0], s.ub = m[2], s.ug = m[3], s.vg = m[4], s.vr = m[5];
     s.bb = m[2] * 128 + m[1], s.bg = m[3] * 128 + m[4] * 128 + m[1], s.br = m[5] * 128 + m[1];
+    return s;
+}
+static U8Norm frame_norm(const snnb_frames& fr) {
     U8Norm q;
     for (int i = 0; i < 4; ++i) q.mean[i] = fr.mean4[i], q.norm[i] = fr.norm4[i];
+    return q;
+}
+int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t) {
+    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
+    const FrameV s = frame_view(fr);
+    const U8Norm q = frame_norm(fr);
     const int linear = fr.linear_filter ? 1 : 0;
     const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
     switch (fr.format) {
@@ -1658,6 +1678,153 @@ int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t)
         return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<rgba8>");
     }
     SNNB_REQUIRE(false, "launch_frame_input: unknown format %d", fr.format);
+}
+
+// Regions of device frames (snnb_model_run_rois): batch slot n is region rois[n] of frame rois[n].frame. A used slot (n < the count)
+// is valid when its region lies inside a frame that exists; roi_slot is the one test of that, so the input kernel and the clear kernel
+// cannot disagree on which slots they serve.
+struct RoiV {
+    const snnb_roi* rois; // [N]
+    const int* count;     // nullptr: every slot is used
+    int num_frames;
+};
+__device__ __forceinline__ bool roi_slot(const RoiV& g, int slot, int N, int fw, int fh, snnb_roi& r) {
+    const int* p = reinterpret_cast<const int*>(g.rois + slot);
+    r.frame = __ldg(p), r.row = __ldg(p + 1), r.x = __ldg(p + 2), r.y = __ldg(p + 3), r.width = __ldg(p + 4), r.height = __ldg(p + 5);
+    const int used = g.count ? min(max(__ldg(g.count), 0), N) : N;
+    return slot < used && r.frame >= 0 && r.frame < g.num_frames && r.width >= 1 && r.height >= 1 && r.x >= 0 && r.y >= 0 && r.x <= fw - r.width &&
+           r.y <= fh - r.height;
+}
+// One thread per model-input pixel, as frame_input_kernel: the taps of ImageTexture::resize from a region-sized source, clamped to the
+// region, then offset to the region's origin in the frame (so chroma is sited in frame coordinates). A region of the model's size is
+// sampled directly. Invalid and unused slots get an all-zero input.
+template <int FMT>
+__global__ void __launch_bounds__(256) frame_roi_input_kernel(FrameV s, RoiV g, TV t, U8Norm q, int linear, FeedV f) {
+    pdl_wait();
+    const size_t total = (size_t) t.N * t.H * t.W;
+    const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (px >= total) return;
+    const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
+    snnb_roi roi;
+    float v[8];
+    if (roi_slot(g, n, t.N, s.w, s.h, roi)) {
+        const bool direct = roi.width == t.W && roi.height == t.H;
+        ResizeTaps r;
+        if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
+        else r = resize_taps(resize_pos(ox, oy, t.W, t.H, roi.width, roi.height), roi.width, roi.height, linear);
+        r.x0 += roi.x, r.x1 += roi.x, r.y0 += roi.y, r.y1 += roi.y;
+        frame_pixel<FMT>(s, roi.frame, r, linear, direct, t, q, v);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = 0.0f;
+    }
+    store_input_pixel(t, f, px, v);
+}
+int launch_frame_roi_input(snnb_context* ctx, const snnb_frames& fr, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t) {
+    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_roi_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
+    const FrameV s = frame_view(fr);
+    const U8Norm q = frame_norm(fr);
+    const RoiV g {rois, count, num_frames};
+    const int linear = fr.linear_filter ? 1 : 0;
+    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
+    switch (fr.format) {
+    case SNNB_FRAME_NV12:
+        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<nv12>");
+    case SNNB_FRAME_NV21:
+        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<nv21>");
+    case SNNB_FRAME_I420:
+        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<i420>");
+    case SNNB_FRAME_RGBA8:
+        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<rgba8>");
+    }
+    SNNB_REQUIRE(false, "launch_frame_roi_input: unknown format %d", fr.format);
+}
+// Zeroes batch slot blockIdx.y of a caller's buffer (slot_bytes per slot, slots contiguous) when roi_slot rejects it. A slot is the
+// outermost dimension in NHWC and NCHW alike. Runs after the outputs and classes are written.
+__global__ void __launch_bounds__(256) roi_clear_kernel(RoiV g, int N, int fw, int fh, uint8_t* __restrict__ dst, long long slot_bytes) {
+    pdl_wait();
+    snnb_roi roi;
+    if (roi_slot(g, (int) blockIdx.y, N, fw, fh, roi)) return;
+    uint8_t* p = dst + (long long) blockIdx.y * slot_bytes;
+    for (long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * 16; i < slot_bytes; i += (long long) gridDim.x * blockDim.x * 16) {
+        if ((reinterpret_cast<uintptr_t>(p + i) & 15) == 0 && i + 16 <= slot_bytes) {
+            *reinterpret_cast<uint4*>(p + i) = make_uint4(0u, 0u, 0u, 0u);
+        } else {
+            for (long long k = i; k < i + 16 && k < slot_bytes; ++k) p[k] = 0;
+        }
+    }
+}
+int launch_roi_clear(snnb_context* ctx, const snnb_frames& fr, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes) {
+    SNNB_REQUIRE(batch >= 1 && batch <= 65535 && slot_bytes >= 1, "launch_roi_clear: batch %d, %lld bytes per slot", batch, slot_bytes);
+    const RoiV g {rois, count, num_frames};
+    const long long chunks = (slot_bytes + 16 * 256 - 1) / (16 * 256);
+    const dim3 grid((unsigned) std::min(chunks, 1024LL), (unsigned) batch);
+    return launch_done(ctx, launch_k(roi_clear_kernel, grid, dim3(256), 0, ctx->stream, g, batch, fr.width, fr.height, static_cast<uint8_t*>(dst), slot_bytes),
+                       "roi_clear_kernel");
+}
+
+// Detection rows -> regions (snnb_rois_from_detections). The rectangle of one row, every operation IEEE-rounded on its own (no FMA
+// contraction), so that a float32 restatement reproduces it; false when the row is not kept.
+__device__ __forceinline__ bool roi_from_row(const float* __restrict__ row, float W, float H, const snnb_roi_select& sel, snnb_roi& r) {
+    const float cls = __ldg(row), score = __ldg(row + 1), x = __ldg(row + 2), y = __ldg(row + 3), w = __ldg(row + 4), h = __ldg(row + 5);
+    if (!(score >= sel.min_score) || (sel.class_id != -1 && cls != (float) sel.class_id)) return false;
+    const float ex = __fmul_rn(sel.expand, w), ey = __fmul_rn(sel.expand, h);
+    const float fx0 = __fmul_rn(__fsub_rn(x, ex), W), fx1 = __fmul_rn(__fadd_rn(__fadd_rn(x, w), ex), W);
+    const float fy0 = __fmul_rn(__fsub_rn(y, ey), H), fy1 = __fmul_rn(__fadd_rn(__fadd_rn(y, h), ey), H);
+    if (isnan(fx0) || isnan(fx1) || isnan(fy0) || isnan(fy1)) return false;
+    const int x0 = (int) floorf(fminf(fmaxf(fx0, 0.0f), W)), x1 = (int) ceilf(fminf(fmaxf(fx1, 0.0f), W));
+    const int y0 = (int) floorf(fminf(fmaxf(fy0, 0.0f), H)), y1 = (int) ceilf(fminf(fmaxf(fy1, 0.0f), H));
+    if (x1 <= x0 || y1 <= y0) return false;
+    r.x = x0, r.y = y0, r.width = x1 - x0, r.height = y1 - y0;
+    return true;
+}
+// One CTA visits rows (n, k), k < min(counts[n], max_rows), in order (frame, then row), a chunk of ROI_THREADS at a time: keep flags,
+// a block prefix sum over them, and the kept rows scattered to their rank while it is below `capacity`. Then the tail is zeroed.
+constexpr int ROI_THREADS = 1024;
+__global__ void __launch_bounds__(ROI_THREADS) rois_from_detections_kernel(const float* __restrict__ rows, const int* __restrict__ counts, int num_frames,
+                                                                         int max_rows, int fw, int fh, snnb_roi_select sel, snnb_roi* __restrict__ out,
+                                                                         int capacity, int* __restrict__ count_out) {
+    pdl_wait();
+    __shared__ int warp_incl[ROI_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = ROI_THREADS / 32;
+    const int total = num_frames * max_rows;
+    int kept = 0; // rows kept before the current chunk (uniform over the CTA)
+    for (int c0 = 0; c0 < total; c0 += ROI_THREADS) {
+        const int i = c0 + threadIdx.x;
+        snnb_roi r;
+        bool keep = false;
+        if (i < total) {
+            const int n = i / max_rows, k = i - n * max_rows;
+            if (k < min(__ldg(counts + n), max_rows)) keep = roi_from_row(rows + (size_t) i * 6, (float) fw, (float) fh, sel, r);
+            r.frame = n, r.row = k;
+        }
+        const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) warp_incl[warp] = __popc(ballot);
+        __syncthreads();
+        if (warp == 0) {
+            int v = warp_incl[lane];
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int u = __shfl_up_sync(0xffffffffu, v, d);
+                if (lane >= d) v += u;
+            }
+            warp_incl[lane] = v;
+        }
+        __syncthreads();
+        const int rank = kept + (warp ? warp_incl[warp - 1] : 0) + __popc(ballot & ((1u << lane) - 1u));
+        if (keep && rank < capacity) out[rank] = r;
+        kept += warp_incl[warps - 1];
+        __syncthreads(); // warp_incl is rewritten by the next chunk
+    }
+    const int written = min(kept, capacity);
+    for (int i = written + threadIdx.x; i < capacity; i += ROI_THREADS) out[i] = snnb_roi {0, 0, 0, 0, 0, 0};
+    if (threadIdx.x == 0) *count_out = written;
+}
+int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh,
+                                const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count) {
+    return launch_done(ctx, launch_k(rois_from_detections_kernel, dim3(1), dim3(ROI_THREADS), 0, stream, rows, counts, num_frames, max_rows, fw, fh, sel, rois,
+                                     capacity, count),
+                       "rois_from_detections_kernel");
 }
 
 // Model output 0 -> device video frames (snnb_model_transform_frames), the reverse of frame_input_kernel. Each frame pixel is

@@ -249,6 +249,17 @@ int launch_device_output(snnb_context* ctx, const snnb_tensor* t, const snnb_dev
 int launch_frame_input(snnb_context* ctx, const snnb_frames& f, snnb_tensor* t);
 // t (C = 1, 3 or 4) -> 8 bits as launch_device_output's U8 -> RGBA8 -> resized -> libyuv ABGRTo* -> device frames (checked by the caller)
 int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames_out& f);
+// Regions of device frames (snnb_model_run_rois, checked by the caller) -> t (C <= 4): slot n is rois[n] sampled as launch_frame_input
+// samples a frame of the region's size; invalid slots and slots past *count (count NULL: all used) are zero
+int launch_frame_roi_input(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t);
+// Zeroes each of `batch` contiguous slots of slot_bytes bytes at dst whose region launch_frame_roi_input did not serve
+int launch_roi_clear(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes);
+// Detection rows -> regions (snnb_rois_from_detections, checked by the caller), one CTA on `stream`
+int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh,
+                                const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count);
+// The host-side checks of snnb_rois_from_detections, then its launch (engine/core.cpp, beside the device-feed checks)
+int rois_from_detections(snnb_context* ctx, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh, const snnb_roi_select* sel,
+                         snnb_roi* rois, int capacity, int* count, cudaStream_t stream);
 
 // ---- host-side weight folding/packing (pack.cpp) -----------------------------------------------------------
 // K ordering of the row-window convolution kernel (kernels_umma.cu): for stride s the taps of one filter row fall

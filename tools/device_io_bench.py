@@ -29,6 +29,14 @@ Writes DIR/device_io_bench.json and prints it. Four parts, all in one process:
                F.interpolate (bilinear), a torch RGB -> NV12 conversion (BT.601 limited range) and packing; alternating as above. And
                frame_output_kernel's device time per batch from torch.profiler over 50 calls, with bytes/s from the frame planes it writes
                plus the model-output planes it reads under its taps.
+  rois         (opt-in) The second stage of a detection pipeline on 1920x1080 NV12 frames. (a) The full chain: YOLOv3-tiny 416x416
+               batch 16 with all-pass heads (every cell passes, so each frame has 100 rows and the second stage always gets its 64
+               regions) detect_frames -> rois_from_detections -> ResNet-18 112x112 batch 64 run_rois, against what a user does without
+               them: rows and counts to the host, a torch NV12 -> RGB conversion, a crop + F.interpolate (bilinear) per box, stack,
+               normalise, then run_torch; frames/s are detector frames, alternating as above. (b) The input kernel alone on a fixed grid
+               of caller-made regions (2 x 2 cells of 960x540 in each of the 16 frames: 64 regions): frame_roi_input_kernel's device
+               time per batch from torch.profiler over 50 calls, with bytes/s from the model-input planes it writes plus the source bytes
+               under its taps (4 per model pixel, each a Y byte and a UV pair, capped by the region's size).
   card         name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -295,10 +303,8 @@ def detector(torch, ctx, core, modelzoo, d, args):
     return res
 
 
-def torch_nv12_to_model(torch, frames, hw, mean4, norm4):
-    """The path without run_frames: NV12 [N, H * 3 // 2, W] uint8 -> float RGB (BT.601 limited range) -> bilinear resize -> normalised
-    float32 NCHW."""
-    import torch.nn.functional as F
+def torch_nv12_to_rgb(torch, frames):
+    """NV12 [N, H * 3 // 2, W] uint8 -> float RGB [N, 3, H, W] (BT.601 limited range)."""
     n, rows, w = frames.shape
     h = rows // 3 * 2
     y = frames[:, :h].float() - 16.0
@@ -306,7 +312,14 @@ def torch_nv12_to_model(torch, frames, hw, mean4, norm4):
     u = uv[..., 0].repeat_interleave(2, 1).repeat_interleave(2, 2)
     v = uv[..., 1].repeat_interleave(2, 1).repeat_interleave(2, 2)
     c = 1.164 * y
-    rgb = torch.stack([c + 1.596 * v, c - 0.391 * u - 0.813 * v, c + 2.018 * u], 1).clamp_(0.0, 255.0)
+    return torch.stack([c + 1.596 * v, c - 0.391 * u - 0.813 * v, c + 2.018 * u], 1).clamp_(0.0, 255.0)
+
+
+def torch_nv12_to_model(torch, frames, hw, mean4, norm4):
+    """The path without run_frames: NV12 [N, H * 3 // 2, W] uint8 -> float RGB (BT.601 limited range) -> bilinear resize -> normalised
+    float32 NCHW."""
+    import torch.nn.functional as F
+    rgb = torch_nv12_to_rgb(torch, frames)
     x = F.interpolate(rgb, size=hw, mode="bilinear", align_corners=False)
     mean = torch.tensor(mean4[:3], device=x.device).view(1, 3, 1, 1)
     norm = torch.tensor(norm4[:3], device=x.device).view(1, 3, 1, 1)
@@ -314,7 +327,7 @@ def torch_nv12_to_model(torch, frames, hw, mean4, norm4):
 
 
 def frame_kernel_us(torch, fn, calls, kernel="frame_input_kernel"):
-    """Device time per call (us) of `kernel` (frame_input_kernel or frame_output_kernel), from torch.profiler."""
+    """Device time per call (us) of `kernel` (frame_input_kernel, frame_output_kernel, frame_roi_input_kernel, ...), from torch.profiler."""
     from torch.profiler import ProfilerActivity, profile
     for _ in range(5):
         fn()
@@ -434,13 +447,98 @@ def transform(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def host_regions(rows, counts, H, W, capacity):
+    """What a user computes on the host without rois_from_detections: the pixel rectangles of the first `capacity` rows (frame by frame,
+    row order), each clipped to the frame; empty ones skipped."""
+    out = []
+    for n in range(rows.shape[0]):
+        r = rows[n, :max(0, min(int(counts[n]), rows.shape[1]))]
+        x0, x1 = np.floor(np.clip(r[:, 2] * W, 0, W)), np.ceil(np.clip((r[:, 2] + r[:, 4]) * W, 0, W))
+        y0, y1 = np.floor(np.clip(r[:, 3] * H, 0, H)), np.ceil(np.clip((r[:, 3] + r[:, 5]) * H, 0, H))
+        for i in np.nonzero((x1 > x0) & (y1 > y0))[0]:
+            out.append((n, int(x0[i]), int(y0[i]), int(x1[i]), int(y1[i])))
+    return out[:capacity]
+
+
+def rois(torch, ctx, core, modelzoo, d, args):
+    import torch.nn.functional as F
+    H, W = 1080, 1920
+    dhw, dbatch, chw, cbatch = (416, 416), 16, (112, 112), 64
+    dmean, dnorm = [127.5] * 4, [1.0 / 127.5] * 4
+    mean4, norm4 = [127.5] * 4, [1.0 / 127.5] * 4
+    path, layers = modelzoo.build("yolov3tiny", os.path.join(d, "rois_yolov3tiny"), input_hw=dhw)
+    for head in [l for l in layers if l["type"] == "Conv2D" and l["outputPlanes"] == 18]:  # all-pass heads (see `detector`)
+        head["_w"]["bias"][:] = 0
+        head["_w"]["bias"][[4, 5, 10, 11, 16, 17]] = 8.0
+    det = core.MixedInferenceCore(ctx, modelzoo.write_model(layers, os.path.join(d, "rois_allpass.json"), split=True), batch=dbatch, input_hw=dhw,
+                                  fuse=True, use_cuda_graph=True)
+    cpath, _ = modelzoo.build("resnet18", os.path.join(d, "rois_resnet18"), input_hw=chw)
+    cls = core.MixedInferenceCore(ctx, cpath, batch=cbatch, input_hw=chw, fuse=True, use_cuda_graph=True)
+    g = torch.Generator().manual_seed(7)
+    nv12 = torch.randint(16, 236, (dbatch, H * 3 // 2, W), dtype=torch.uint8, generator=g).cuda()
+    mean_t = torch.tensor(mean4[:3], device="cuda").view(1, 3, 1, 1)
+    norm_t = torch.tensor(norm4[:3], device="cuda").view(1, 3, 1, 1)
+
+    def chain():
+        r, c = det.detect_frames(nv12, mean4=dmean, norm4=dnorm)
+        regions, count = ctx.rois_from_detections(r, c, (H, W), cbatch)
+        return cls.run_rois(nv12, regions, count, mean4=mean4, norm4=norm4, want_classes=True)
+
+    def today():
+        r, c = det.detect_frames(nv12, mean4=dmean, norm4=dnorm)
+        regions = host_regions(r.cpu().numpy(), c.cpu().numpy(), H, W, cbatch)  # synchronises
+        rgb = torch_nv12_to_rgb(torch, nv12)
+        crops = [F.interpolate(rgb[n:n + 1, :, y0:y1, x0:x1], size=chw, mode="bilinear", align_corners=False) for n, x0, y0, x1, y1 in regions]
+        crops += [torch.zeros((cbatch - len(crops), 3) + chw, device="cuda")] if len(crops) < cbatch else []
+        x = ((torch.cat(crops) - mean_t) * norm_t).contiguous()
+        return cls.run_torch(x, layout="nchw", want_classes=True)
+
+    for _ in range(5):
+        chain()
+        today()
+    torch.cuda.synchronize()
+    kept = int(ctx.rois_from_detections(*det.detect_frames(nv12, mean4=dmean, norm4=dnorm), (H, W), cbatch)[1].item())
+    rounds = []
+    for _ in range(args.rounds):
+        rounds.append({"chain": timed(chain, args.seconds, dbatch, torch.cuda.synchronize), "today": timed(today, args.seconds, dbatch, torch.cuda.synchronize)})
+    med = lambda k: float(np.median([r[k]["frames_per_s"] for r in rounds]))  # noqa: E731
+    res = {"chain": {
+        "case": "(a) yolov3tiny all-pass heads %dx%d batch %d from %dx%d NV12 -> %d regions -> resnet18 %dx%d batch %d" % (dhw[0], dhw[1], dbatch, W, H,
+                                                                                                                       kept, chw[0], chw[1], cbatch),
+        "chain_path": "detect_frames -> rois_from_detections -> run_rois (+ device classes); no host synchronisation",
+        "today_path": "detect_frames, rows + counts to the host, torch NV12 -> RGB, per-box crop + F.interpolate, stack + normalise, run_torch",
+        "regions_per_batch": kept,
+        "chain_frames_per_s_median": med("chain"),
+        "today_frames_per_s_median": med("today"),
+        "chain_over_today": med("chain") / med("today"),
+        "rounds": rounds,
+        "kernels": {k: frame_kernel_us(torch, chain, 50, k) for k in ("rois_from_detections_kernel", "frame_roi_input_kernel", "roi_clear_kernel")},
+    }}
+    # (b) caller-made regions: a 2 x 2 grid of 960 x 540 cells in each frame
+    rw, rh = W // 2, H // 2
+    grid = [(i % dbatch, i, (i // dbatch) % 2 * rw, (i // dbatch) // 2 * rh, rw, rh) for i in range(cbatch)]
+    grid_t = torch.tensor(grid, dtype=torch.int32, device="cuda")
+    kt = frame_kernel_us(torch, lambda: cls.run_rois(nv12, grid_t, mean4=mean4, norm4=norm4), 50, "frame_roi_input_kernel")
+    px = chw[0] * chw[1]
+    written = cbatch * px * 16  # ResNet-18's stem reads the 4-channel feed copy only: 2 planes x 2 bytes x 4 per pixel
+    sampled = cbatch * (min(4 * px, rw * rh) + 2 * min(4 * px, (rw // 2) * (rh // 2)))
+    sec = kt["us_per_batch"] * 1e-6
+    kt.update({"case": "(b) %d caller-made %dx%d regions of %dx%d NV12 frames -> resnet18 %dx%d batch %d" % (cbatch, rw, rh, W, H, chw[0], chw[1], cbatch),
+               "bytes_written": written, "bytes_sampled": sampled, "bytes_per_s": (written + sampled) / sec})
+    kt["share_of_hbm_peak"] = kt["bytes_per_s"] / HBM_BYTES_PER_S
+    res["input_kernel"] = kt
+    det.close()
+    cls.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
     ap.add_argument("--seconds", type=float, default=2.0)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
-                    help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in)")
+                    help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -461,6 +559,8 @@ def main():
         result["frames"] = frames(torch, ctx, core, modelzoo, d, args)
     if "transform" in parts:
         result["transform"] = transform(torch, ctx, core, modelzoo, d, args)
+    if "rois" in parts:
+        result["rois"] = rois(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
