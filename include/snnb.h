@@ -327,6 +327,28 @@ typedef struct {
  * forward pass: one kernel launch for the input and one for the output (Candy 720x720 x 8 to 1920x1080 NV12: 263 us; NVIDIA H100 80GB
  * HBM3, 400 W power limit). */
 int snnb_model_transform_frames(snnb_model* m, const snnb_frames* frames, const snnb_frames_out* out, void* stream);
+/* Luma models (ESPCN-style super-resolution; a denoiser, deblocker or sharpener of Y) from device frames to device frames: the Y plane
+ * feeds a model whose one input has 1 channel, output 0 (1 channel) becomes the Y plane of `out`, and the source chroma is resized
+ * beside it, so the colour of the video is kept. It replaces a copy of the Y plane, a U8 run, a chroma resize and a pack in the
+ * caller's own code. No colour conversion happens. Every byte, for image n of the loaded batch:
+ *   1. Model input: (Y' - mean4[0]) * norm4[0], Y' = ImageTexture::resize of the Y plane to the model's size with frames.linear_filter
+ *      (the taps of snnb_image_io; the byte itself at equal sizes). Bit-identical to snnb_model_submit_image fed the Y planes as an
+ *      N x H x W x 1 8-bit image. frames.matrix is checked as snnb_model_run_frames checks it and not used.
+ *   2. Y plane: M = clamp(rint(v * scale + offset), 0, 255) of output 0 (exactly the U8 output of snnb_model_run_device), then
+ *      ImageTexture::resize of M to out.width x out.height with out.linear_filter, blended and rounded as step 2 of
+ *      snnb_model_transform_frames (Y = M at equal sizes). This is the byte snnb_model_transform_frames writes as R for that output.
+ *   3. Chroma: U and V each ImageTexture::resize of the source's U and V plane, plane to plane, from ceil(W/2) x ceil(H/2) to
+ *      ceil(width/2) x ceil(height/2), with out.linear_filter and the same taps, blend and rint as step 2 (a copy at equal chroma sizes).
+ *      Resizing the planes on their own, as libyuv's I420Scale does, keeps each sample sited at the centre of its 2 x 2 block.
+ * frames.format and out.format are NV12, NV21 or I420 and may differ; RGBA8 is refused on either side. Bytes of a plane outside its rows
+ * (pitch padding, gaps between planes and images) are not written. Aliasing: the Y plane is written after the forward pass, but the
+ * output kernel reads the source chroma while it writes. So `out` may be `frames` itself (same format, size, planes, pitches and image
+ * strides: an in-place luma filter); otherwise no out plane may overlap a source chroma plane. Checked on the host before anything is
+ * enqueued: everything snnb_model_transform_frames checks, a model input and an output 0 of exactly 1 channel, and the overlap rule on
+ * each plane's bytes, plane + (N - 1) * image_stride + (rows - 1) * pitch + its row's bytes. Stream contract and fences: those of
+ * snnb_model_run_device. Cost beyond the forward pass: one kernel launch for the input and one for the output (ESPCN 1920x1080 x 1
+ * from 1920x1080 NV12 to 3840x2160 NV12: 24 us and 106 us; NVIDIA H100 80GB HBM3, 400 W power limit). */
+int snnb_model_transform_luma(snnb_model* m, const snnb_frames* frames, const snnb_frames_out* out, void* stream);
 /* Regions of device frames as the batch: the second stage of a detection pipeline (classify, describe or embed what a detector found)
  * without a host round trip. A region is a pixel rectangle [x, x + width) x [y, y + height) of frame `frame` of the frames given; `row`
  * is carried for the caller (the detection row it came from, or anything) and ignored by the engine. */

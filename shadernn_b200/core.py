@@ -9,6 +9,7 @@ Every call goes through libsnn_b200.so; nothing here computes.
 """
 import ctypes as C
 import sys
+import weakref
 
 import numpy as np
 
@@ -35,6 +36,7 @@ class GpuContext:
         self.h = vp()
         check(lib().snnb_context_create(int(device), C.byref(self.h)), "snnb_context_create")
         self.device = device
+        self._models = weakref.WeakSet()  # the open MixedInferenceCores on this context: destroying one uses its context
 
     def sync(self):
         check(lib().snnb_sync(self.h), "snnb_sync")
@@ -74,7 +76,11 @@ class GpuContext:
         return rois, count
 
     def close(self):
+        """Destroys the context, after closing every model still open on it (snnb_model_destroy needs the context; a model that is
+        collected later, e.g. out of a reference cycle, then has nothing left to destroy)."""
         if self.h:
+            for m in list(self._models):
+                m.close()
             lib().snnb_context_destroy(self.h)
             self.h = vp()
 
@@ -341,6 +347,7 @@ class MixedInferenceCore:
                            int(bool(fuse)), PRECISION[precision])
         self.h = vp()
         check(lib().snnb_model_load_json(ctx.h, json_path.encode(), C.byref(opt), C.byref(self.h)), "snnb_model_load_json")
+        ctx._models.add(self)
 
     @classmethod
     def create(cls, ctx, json_path, **kw):
@@ -655,6 +662,40 @@ class MixedInferenceCore:
         if n != self.batch or (out_hw is not None and (o.height, o.width) != (oh, ow)):
             raise ValueError("transform_frames: out holds %d frames of %d x %d; expected %d of %d x %d" % (n, o.height, o.width, self.batch, oh, ow))
         check(lib().snnb_model_transform_frames(self.h, C.byref(f), C.byref(o), self._torch_stream()), "snnb_model_transform_frames")
+        return out
+
+    def transform_luma(self, frames, format="nv12", linear=True, mean=0.0, norm=1.0, out_format=None, out_hw=None, out_linear=True, out_scale=1.0,
+                       out_offset=0.0, out=None):
+        """snnb_model_transform_luma, for a model with one 1-channel input and a 1-channel output 0 (ESPCN-style super-resolution, a
+        luma denoiser): the Y plane of NV12 / NV21 / I420 frames, resized to the model input (linear or nearest, as run_image) and
+        normalised as (Y - mean) * norm, feeds the model; clamp(round(v * out_scale + out_offset), 0, 255) of output 0, resized to out_hw
+        (out_linear), is written as the Y plane of `out`, and the source U and V planes are resized plane to plane beside it. No colour
+        conversion happens. Ordered on the current torch stream and never synchronising.
+
+        A model trained on Y / 255 of full-range luma takes mean=0, norm=1/255 and gives back out_scale=255. Decoder frames are usually
+        limited range, Y in [16, 235]: that model then takes mean=16, norm=1/219, and out_scale=219, out_offset=16 write its output
+        back in the decoder's range.
+
+        out_format defaults to `format` and out_hw to the input frames' size. Returns `out`, a uint8 CUDA tensor [N, H * 3 // 2, W] in
+        _frames' layouts, allocated here unless given; it may be `frames` itself (same format and size), for an in-place filter."""
+        import torch
+        out_format = format if out_format is None else out_format
+        if format not in self._FRAME_FORMATS or out_format not in self._FRAME_FORMATS:
+            raise ValueError("transform_luma: format %r / out_format %r: expected one of %s" % (format, out_format, sorted(self._FRAME_FORMATS)))
+        f = self._frames("transform_luma", frames, format, "bt601", linear, [float(mean)] * 4, [float(norm)] * 4)
+        oh, ow = (f.height, f.width) if out_hw is None else (int(out_hw[0]), int(out_hw[1]))
+        if out is None:
+            if out_format == "rgba8":
+                raise ValueError("transform_luma: out_format 'rgba8' has no Y plane; expected nv12, nv21 or i420")
+            if oh % 2 or ow % 2:
+                raise ValueError("transform_luma: %s frames of %d x %d: the packed layout needs H and W even" % (out_format, oh, ow))
+            out = torch.empty((self.batch, oh * 3 // 2, ow), dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+        o = _lib.FramesOut()
+        o.format, o.linear_filter, o.scale, o.offset = self._FRAME_FORMATS[out_format], int(bool(out_linear)), float(out_scale), float(out_offset)
+        n = self._frame_planes("transform_luma", "out frames", out, out_format, o)
+        if n != self.batch or (out_hw is not None and (o.height, o.width) != (oh, ow)):
+            raise ValueError("transform_luma: out holds %d frames of %d x %d; expected %d of %d x %d" % (n, o.height, o.width, self.batch, oh, ow))
+        check(lib().snnb_model_transform_luma(self.h, C.byref(f), C.byref(o), self._torch_stream()), "snnb_model_transform_luma")
         return out
 
     def set_input(self, images, idx=0):

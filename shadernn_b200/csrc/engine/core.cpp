@@ -683,6 +683,10 @@ int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, c
         SNNB_REQUIRE(inputLayers.size() == 1, "%s: the model has %d inputs; frames feed a model with exactly one", api, (int) inputLayers.size());
         const snnb_tensor* t = inputLayers[0]->output;
         SNNB_REQUIRE(t->c >= 1 && t->c <= 4, "%s: the model input has %d channels; frames feed 1 to 4 (RGBA components)", api, t->c);
+        if (in.luma) {
+            SNNB_REQUIRE(f.format != SNNB_FRAME_RGBA8, "%s: RGBA8 frames have no Y plane; luma input takes NV12, NV21 or I420 frames", api);
+            SNNB_REQUIRE(t->c == 1, "%s: the model input has %d channels; the Y plane feeds exactly 1", api, t->c);
+        }
         for (int p = 0; p < 3; ++p) {
             const long long row = frameRowBytes(f.format, f.width, p);
             if (!row) continue;
@@ -716,7 +720,7 @@ int MixedInferenceCore::enqueueDeviceForward(const DeviceFeed& in, cudaStream_t 
     if (in.rois) {
         if (launch_frame_roi_input(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, inputLayers[0]->output)) return 1;
     } else if (in.frames) {
-        if (launch_frame_input(ctx, *in.frames, inputLayers[0]->output)) return 1;
+        if (launch_frame_input(ctx, *in.frames, inputLayers[0]->output, in.luma)) return 1;
     } else {
         for (int i = 0; i < in.numInputs; ++i)
             if (launch_device_input(ctx, in.inputs[i], inputLayers[i]->output)) return 1;
@@ -848,6 +852,64 @@ int MixedInferenceCore::transformFrames(const snnb_frames* frames, const snnb_fr
 
     if (enqueueDeviceForward(in, stream)) return 1;
     if (launch_frame_output(ctx, t, o)) return 1;
+    return fenceToCaller(stream);
+}
+
+// The bytes plane p of `n` images spans, from its first image's first byte to its last image's last row byte; false for an unused plane
+static bool planeExtent(int format, int width, int height, const uint8_t* plane, int pitch, long long stride, int n, int p, uintptr_t& begin,
+                        uintptr_t& end) {
+    const long long row = frameRowBytes(format, width, p);
+    if (!row) return false;
+    const long long rows = p == 0 ? height : (height + 1) / 2, span = (long long) (n - 1) * stride;
+    begin = reinterpret_cast<uintptr_t>(plane) + (span < 0 ? span : 0);
+    end   = reinterpret_cast<uintptr_t>(plane) + (span > 0 ? span : 0) + (rows - 1) * pitch + row;
+    return true;
+}
+
+// Luma frames in, luma frames out: the Y plane feeds a 1-channel model, output 0 (1 channel) becomes the Y plane of `out`, and the same
+// output kernel resamples the source frames' chroma into out's chroma. The kernel reads the source chroma while it writes, so out must
+// keep clear of it unless out is the source frames themselves (each chroma sample is then read and written by one thread).
+int MixedInferenceCore::transformLuma(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream) {
+    static const char* api = "snnb_model_transform_luma";
+    SNNB_REQUIRE(frames, "snnb_model_transform_luma: null frames");
+    SNNB_REQUIRE(out, "snnb_model_transform_luma: null out");
+    DeviceFeed in;
+    in.frames = frames, in.luma = true;
+    if (int rc = checkDeviceFeed(api, in, stream)) return rc;
+    const snnb_frames& f     = *frames;
+    const snnb_frames_out& o = *out;
+    SNNB_REQUIRE(o.format >= SNNB_FRAME_NV12 && o.format <= SNNB_FRAME_RGBA8, "%s: unknown out frame format %d", api, o.format);
+    SNNB_REQUIRE(o.format != SNNB_FRAME_RGBA8, "%s: out format RGBA8 has no Y plane; luma frames are written as NV12, NV21 or I420", api);
+    SNNB_REQUIRE(o.width >= 1 && o.height >= 1, "%s: out frame size %d x %d; width and height must be >= 1", api, o.width, o.height);
+    for (int p = 0; p < 3; ++p) {
+        const long long row = frameRowBytes(o.format, o.width, p);
+        if (!row) continue;
+        SNNB_REQUIRE(o.pitch[p] >= row, "%s: out plane %d: pitch %d is less than its row's %lld bytes", api, p, o.pitch[p], row);
+        if (int rc = checkDevicePointer(api, o.plane[p], 1, ctx->device, "out plane", p)) return rc;
+    }
+    SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; frames are written from an image output", api);
+    const snnb_tensor* t = outputLayers[0]->output;
+    SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
+    SNNB_REQUIRE(t->c == 1, "%s: output 0 has %d channels; the Y plane is written from exactly 1", api, t->c);
+    bool same = o.format == f.format && o.width == f.width && o.height == f.height;
+    for (int p = 0; p < 3 && same; ++p)
+        if (frameRowBytes(f.format, f.width, p)) same = o.plane[p] == f.plane[p] && o.pitch[p] == f.pitch[p] && o.image_stride[p] == f.image_stride[p];
+    if (!same) {
+        const int n = (int) options.batch;
+        for (int p = 0; p < 3; ++p) {
+            uintptr_t ob, oe;
+            if (!planeExtent(o.format, o.width, o.height, o.plane[p], o.pitch[p], o.image_stride[p], n, p, ob, oe)) continue;
+            for (int q = 1; q < 3; ++q) {
+                uintptr_t sb, se;
+                if (!planeExtent(f.format, f.width, f.height, f.plane[q], f.pitch[q], f.image_stride[q], n, q, sb, se)) continue;
+                SNNB_REQUIRE(oe <= sb || se <= ob, "%s: out plane %d overlaps source chroma plane %d; out may alias the source chroma only as the source frames themselves",
+                             api, p, q);
+            }
+        }
+    }
+
+    if (enqueueDeviceForward(in, stream)) return 1;
+    if (launch_luma_output(ctx, t, f, o)) return 1;
     return fenceToCaller(stream);
 }
 

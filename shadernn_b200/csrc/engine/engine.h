@@ -358,6 +358,8 @@ public:
     int detectFrames(const snnb_frames* frames, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
     // snnb_model_transform_frames: runFrames' input and fences, then output 0 written as device video frames
     int transformFrames(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream);
+    // snnb_model_transform_luma: the frames' Y plane into a 1-channel model, output 0 (1 channel) out as the Y plane, chroma resampled
+    int transformLuma(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream);
     // snnb_model_run_rois: runFrames with regions of numFrames frames as the batch; slots without a valid region come out zero
     int runRois(const snnb_frames* frames, int numFrames, const snnb_roi* roisDev, const int* countDev, const snnb_device_buffer* outputs, int numOutputs,
                 int* classes1Dev, cudaStream_t stream);
@@ -418,7 +420,8 @@ private:
     // runDevice's fences: the caller's stream -> the context's stream (callerReady), and back (deviceDone); created on first use
     cudaEvent_t callerReady = nullptr, deviceDone = nullptr;
     // What a device-resident call feeds the model: one snnb_device_buffer per input, or (frames != NULL) a batch of frames into input 0,
-    // or (rois != NULL as well) regions of numFrames frames, one per batch slot, with roiCount (NULL: all slots) of them used.
+    // or (rois != NULL as well) regions of numFrames frames, one per batch slot, with roiCount (NULL: all slots) of them used, or
+    // (luma) the frames' Y plane alone into a 1-channel input.
     // The input staging (and, for regions, the clearing of the slots without one) is the only step in which these entry points differ.
     struct DeviceFeed {
         const snnb_device_buffer* inputs = nullptr;
@@ -427,6 +430,7 @@ private:
         const snnb_roi* rois = nullptr;
         const int* roiCount = nullptr;
         int numFrames = 0;
+        bool luma = false;
     };
     // shared by runDevice, detectDevice, runFrames, detectFrames and runRois: the host-side checks of the feed and the stream (nothing
     // enqueued), then the fenced input staging + forward pass, the outputs or the detections, and the fence back to the caller's stream

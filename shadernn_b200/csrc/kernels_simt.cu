@@ -1579,9 +1579,16 @@ struct FrameV {
     int w, h;
     int yg, ub, ug, vg, vr, bb, bg, br;
 };
+// Not a public format: the Y plane (plane 0) of NV12 / NV21 / I420 frames as a 1-channel 8-bit image (snnb_model_transform_luma). Every
+// component of its texel is the Y byte, so the model input is resize_u8_kernel's / split_u8_kernel's of that image.
+constexpr int FRAME_LUMA = -1;
 // RGBA8 of source pixel (x, y) of image n; pixel (x, y) takes chroma sample (x / 2, y / 2) (NV12ToARGBRow_C, row_common.cc:1945-1967)
 template <int FMT>
 __device__ __forceinline__ void frame_texel(const FrameV& s, int n, int x, int y, float rgba[4]) {
+    if (FMT == FRAME_LUMA) {
+        rgba[0] = rgba[1] = rgba[2] = rgba[3] = (float) __ldg(s.plane[0] + n * s.stride[0] + (size_t) y * s.pitch[0] + x);
+        return;
+    }
     if (FMT == SNNB_FRAME_RGBA8) {
         const uint8_t* p = s.plane[0] + n * s.stride[0] + (size_t) y * s.pitch[0] + (size_t) x * 4;
 #pragma unroll
@@ -1661,12 +1668,17 @@ static U8Norm frame_norm(const snnb_frames& fr) {
     for (int i = 0; i < 4; ++i) q.mean[i] = fr.mean4[i], q.norm[i] = fr.norm4[i];
     return q;
 }
-int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t) {
+int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t, bool luma) {
     SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
     const FrameV s = frame_view(fr);
     const U8Norm q = frame_norm(fr);
     const int linear = fr.linear_filter ? 1 : 0;
     const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
+    if (luma) {
+        SNNB_REQUIRE(t->c == 1 && fr.format != SNNB_FRAME_RGBA8, "launch_frame_input: luma input feeds 1 channel from YUV frames (%d channels, format %d)", t->c,
+                     fr.format);
+        return launch_done(ctx, launch_k(frame_input_kernel<FRAME_LUMA>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<luma>");
+    }
     switch (fr.format) {
     case SNNB_FRAME_NV12:
         return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<nv12>");
@@ -1966,6 +1978,107 @@ int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_fram
         return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<rgba8>");
     }
     SNNB_REQUIRE(false, "launch_frame_output: unknown format %d", fr.format);
+}
+
+// A 1-channel model output 0 -> the Y plane of device video frames, with the source frames' chroma resampled beside it
+// (snnb_model_transform_luma). Y is frame_out_pixel's component 0 from one value per texel; U and V are ImageTexture::resize of the
+// source chroma planes, plane to plane, with the same taps and blend_rn.
+// Texel (x, y) of image n of M for a 1-channel output: its one value, quantised
+__device__ __forceinline__ float out_luma_texel(const TV& t, int n, int x, int y, float scale, float offset) {
+    const size_t off = (((size_t) n * t.H + y) * t.W + x) * t.Cp;
+    const float v    = __half2float(__ldg(t.hi + off)) + (t.lo ? __half2float(__ldg(t.lo + off)) : 0.0f); // = load8's component 0
+    return quant_u8(v, scale, offset);
+}
+__device__ __forceinline__ int luma_out_pixel(const TV& t, const FrameOutV& o, int n, int x, int y, int linear) {
+    const bool direct = o.w == t.W && o.h == t.H;
+    ResizeTaps r;
+    if (direct) r.x0 = r.x1 = x, r.y0 = r.y1 = y, r.ax = r.ay = 0.0f;
+    else r = resize_taps(resize_pos(x, y, o.w, o.h, t.W, t.H), t.W, t.H, linear);
+    const float p00 = out_luma_texel(t, n, r.x0, r.y0, o.scale, o.offset);
+    if (!linear || direct) return (int) p00;
+    const float p01 = out_luma_texel(t, n, r.x1, r.y0, o.scale, o.offset), p10 = out_luma_texel(t, n, r.x0, r.y1, o.scale, o.offset);
+    const float p11 = out_luma_texel(t, n, r.x1, r.y1, o.scale, o.offset);
+    return (int) rintf(blend_rn(r, p00, p01, p10, p11));
+}
+// Chroma sample (x, y) of image n: U from plane 1, V from plane 2 of `s`, `step` bytes apart along a row (2 in an interleaved plane)
+__device__ __forceinline__ void chroma_texel(const FrameV& s, int step, int n, int x, int y, float& u, float& v) {
+    u = (float) __ldg(s.plane[1] + n * s.stride[1] + (size_t) y * s.pitch[1] + (size_t) x * step);
+    v = (float) __ldg(s.plane[2] + n * s.stride[2] + (size_t) y * s.pitch[2] + (size_t) x * step);
+}
+// One thread per 2 x 2 block of frame pixels, i.e. per chroma sample, as frame_output_kernel: 4 Y bytes, then the chroma sample resized
+// from the source's chroma planes. A chroma plane of the source's size is copied. Pixels past an odd width or height are not written.
+template <int FMT>
+__global__ void __launch_bounds__(256) luma_output_kernel(TV t, FrameV s, int step, FrameOutV o, int linear) {
+    pdl_wait();
+    const int cw = (o.w + 1) >> 1, ch = (o.h + 1) >> 1;
+    const size_t total = (size_t) t.N * ch * cw;
+    const size_t gid   = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= total) return;
+    const int bx = (int) (gid % cw), by = (int) ((gid / cw) % ch), n = (int) (gid / ((size_t) cw * ch));
+    const int x = 2 * bx, y = 2 * by;
+    const bool has_x1 = x + 1 < o.w, has_y1 = y + 1 < o.h;
+#pragma unroll
+    for (int dy = 0; dy < 2; ++dy) {
+        if (dy && !has_y1) break;
+        uint8_t* d   = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + x;
+        const int ya = luma_out_pixel(t, o, n, x, y + dy, linear);
+        if (has_x1) store_2u8(d, ya, luma_out_pixel(t, o, n, x + 1, y + dy, linear));
+        else d[0] = (uint8_t) ya;
+    }
+    const int scw = (s.w + 1) >> 1, sch = (s.h + 1) >> 1;
+    const bool direct = cw == scw && ch == sch;
+    ResizeTaps r;
+    if (direct) r.x0 = r.x1 = bx, r.y0 = r.y1 = by, r.ax = r.ay = 0.0f;
+    else r = resize_taps(resize_pos(bx, by, cw, ch, scw, sch), scw, sch, linear);
+    float u00, v00;
+    chroma_texel(s, step, n, r.x0, r.y0, u00, v00);
+    int U = (int) u00, V = (int) v00;
+    if (linear && !direct) {
+        float u01, v01, u10, v10, u11, v11;
+        chroma_texel(s, step, n, r.x1, r.y0, u01, v01);
+        chroma_texel(s, step, n, r.x0, r.y1, u10, v10);
+        chroma_texel(s, step, n, r.x1, r.y1, u11, v11);
+        U = (int) rintf(blend_rn(r, u00, u01, u10, u11)), V = (int) rintf(blend_rn(r, v00, v01, v10, v11));
+    }
+    if (FMT == SNNB_FRAME_I420) {
+        o.plane[1][n * o.stride[1] + (size_t) by * o.pitch[1] + bx] = (uint8_t) U;
+        o.plane[2][n * o.stride[2] + (size_t) by * o.pitch[2] + bx] = (uint8_t) V;
+    } else {
+        uint8_t* d = o.plane[1] + n * o.stride[1] + (size_t) by * o.pitch[1] + (size_t) bx * 2;
+        if (FMT == SNNB_FRAME_NV12) store_2u8(d, U, V);
+        else store_2u8(d, V, U);
+    }
+}
+int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames& src, const snnb_frames_out& fr) {
+    SNNB_REQUIRE(t->c == 1 && t->cp == 8 && !t->feed_only && src.format != SNNB_FRAME_RGBA8,
+                 "launch_luma_output: the output tensor has %d channels, source format %d; luma frames are written from 1 channel with YUV chroma", t->c, src.format);
+    // the source chroma as two planes of samples `step` bytes apart: U and V of I420, or the two bytes of an NV12 / NV21 pair
+    FrameV s {};
+    int step = 1;
+    s.w = src.width, s.h = src.height;
+    if (src.format == SNNB_FRAME_I420) {
+        for (int i = 1; i < 3; ++i) s.plane[i] = src.plane[i], s.pitch[i] = src.pitch[i], s.stride[i] = src.image_stride[i];
+    } else {
+        const int u = src.format == SNNB_FRAME_NV21 ? 1 : 0;
+        step = 2;
+        s.plane[1] = src.plane[1] + u, s.plane[2] = src.plane[1] + (1 - u);
+        s.pitch[1] = s.pitch[2] = src.pitch[1], s.stride[1] = s.stride[2] = src.image_stride[1];
+    }
+    FrameOutV o;
+    for (int i = 0; i < 3; ++i) o.plane[i] = fr.plane[i], o.pitch[i] = fr.pitch[i], o.stride[i] = fr.image_stride[i];
+    o.w = fr.width, o.h = fr.height, o.scale = fr.scale, o.offset = fr.offset;
+    const int linear = fr.linear_filter ? 1 : 0;
+    const size_t blocks = (size_t) t->n * ((fr.height + 1) / 2) * ((fr.width + 1) / 2);
+    const dim3 grid((unsigned) ((blocks + 255) / 256)), block(256);
+    switch (fr.format) {
+    case SNNB_FRAME_NV12:
+        return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<nv12>");
+    case SNNB_FRAME_NV21:
+        return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<nv21>");
+    case SNNB_FRAME_I420:
+        return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<i420>");
+    }
+    SNNB_REQUIRE(false, "launch_luma_output: out format %d; luma frames are written as NV12, NV21 or I420", fr.format);
 }
 
 } // namespace snnb

@@ -245,10 +245,14 @@ int launch_merge_u8(snnb_context* ctx, const snnb_tensor* t, uint8_t* dev_nhwc_u
 // Output: hi + lo as F32, __float2half_rn of it as F16, clamp(round(v * b.scale + b.offset), 0, 255) as U8. Never reads a feed copy.
 int launch_device_input(snnb_context* ctx, const snnb_device_buffer& b, snnb_tensor* t);
 int launch_device_output(snnb_context* ctx, const snnb_tensor* t, const snnb_device_buffer& b);
-// Device frames (snnb_model_run_frames, checked by the caller) -> libyuv RGBA8 per tap -> resized + normalised -> t (C <= 4)
-int launch_frame_input(snnb_context* ctx, const snnb_frames& f, snnb_tensor* t);
+// Device frames (snnb_model_run_frames, checked by the caller) -> libyuv RGBA8 per tap -> resized + normalised -> t (C <= 4). luma: the
+// Y plane of YUV frames as a 1-channel 8-bit image -> resized + normalised -> t (C = 1; snnb_model_transform_luma)
+int launch_frame_input(snnb_context* ctx, const snnb_frames& f, snnb_tensor* t, bool luma);
 // t (C = 1, 3 or 4) -> 8 bits as launch_device_output's U8 -> RGBA8 -> resized -> libyuv ABGRTo* -> device frames (checked by the caller)
 int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames_out& f);
+// t (C = 1) -> 8 bits -> resized -> the Y plane of NV12 / NV21 / I420 frames; their chroma resized from src's chroma planes (checked by
+// the caller, which also keeps the out planes clear of src's chroma unless out is src itself)
+int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames& src, const snnb_frames_out& f);
 // Regions of device frames (snnb_model_run_rois, checked by the caller) -> t (C <= 4): slot n is rois[n] sampled as launch_frame_input
 // samples a frame of the region's size; invalid slots and slots past *count (count NULL: all used) are zero
 int launch_frame_roi_input(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t);

@@ -37,6 +37,11 @@ Writes DIR/device_io_bench.json and prints it. Four parts, all in one process:
                of caller-made regions (2 x 2 cells of 960x540 in each of the 16 frames: 64 regions): frame_roi_input_kernel's device
                time per batch from torch.profiler over 50 calls, with bytes/s from the model-input planes it writes plus the source bytes
                under its taps (4 per model pixel, each a Y byte and a UV pair, capped by the region's size).
+  luma         (opt-in) ESPCN at 1920x1080 (the size of the reference's runESPCN input), batch 1 and 4, from 1920x1080 NV12 frames
+               to 3840x2160 NV12 frames: transform_luma (the Y plane into the model, output 0 out as the Y plane, U and V resized in
+               luma_output_kernel) against what a user does without it, the Y plane made dense, run_torch with uint8 in and out,
+               F.interpolate (bilinear) of U and V and packing; alternating as above. And the device time per batch of the input kernel
+               (frame_input_kernel<luma>) and of luma_output_kernel from torch.profiler over 50 calls, with bytes/s from what each moves.
   card         name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -447,6 +452,64 @@ def transform(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def torch_luma_today(torch, m, nv12, H, W):
+    """The path without transform_luma: the Y plane made dense, run_torch with uint8 in and out (Y / 255 in, 255 v out), U and V
+    upsampled with F.interpolate (bilinear), and the NV12 planes packed: [N, 2H * 3 // 2, 2W] uint8."""
+    import torch.nn.functional as F
+    n = nv12.shape[0]
+    y = nv12[:, :H].contiguous().unsqueeze(-1)
+    yo = m.run_torch(y, mean4=[0.0] * 4, norm4=[1.0 / 255.0] * 4, out_dtype=torch.uint8, out_scale=255.0)[..., 0]
+    uv = nv12[:, H:].reshape(n, H // 2, W // 2, 2).permute(0, 3, 1, 2).float()
+    uvo = F.interpolate(uv, size=(H, W), mode="bilinear", align_corners=False).round_().clamp_(0.0, 255.0).to(torch.uint8)
+    return torch.cat([yo, uvo.permute(0, 2, 3, 1).reshape(n, H, 2 * W)], 1)
+
+
+def luma(torch, ctx, core, modelzoo, d, args):
+    H, W = 1080, 1920
+    res = []
+    path, _ = modelzoo.build("espcn", os.path.join(d, "luma_espcn"), input_hw=(H, W))
+    for batch in (1, 4):
+        m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=(H, W), fuse=True, use_cuda_graph=True)
+        g = torch.Generator().manual_seed(7)
+        nv12 = torch.randint(16, 236, (batch, H * 3 // 2, W), dtype=torch.uint8, generator=g).cuda()
+        out = torch.empty((batch, 2 * H * 3 // 2, 2 * W), dtype=torch.uint8, device="cuda")
+        fused = lambda: m.transform_luma(nv12, norm=1.0 / 255.0, out_hw=(2 * H, 2 * W), out_scale=255.0, out=out)  # noqa: E731
+        unfused = lambda: torch_luma_today(torch, m, nv12, H, W)  # noqa: E731
+        for _ in range(5):
+            fused()
+            unfused()
+        torch.cuda.synchronize()
+        rounds = []
+        for _ in range(args.rounds):
+            rounds.append({"luma": timed(fused, args.seconds, batch, torch.cuda.synchronize), "torch": timed(unfused, args.seconds, batch, torch.cuda.synchronize)})
+        med = lambda k: float(np.median([r[k]["frames_per_s"] for r in rounds]))  # noqa: E731
+        kin = frame_kernel_us(torch, fused, 50, "frame_input_kernel")
+        kout = frame_kernel_us(torch, fused, 50, "luma_output_kernel")
+        # input: the Y plane read, the 1-channel model input written as split-fp16 (2 planes x 8 channels x 2 bytes per pixel: Cp = 8).
+        # output: that same 32 bytes per pixel of ESPCN's 1-channel output read (every 32-byte sector is touched for 2 useful bytes) plus
+        # the source chroma, and the out Y and UV planes written.
+        kin.update({"bytes_read": batch * H * W, "bytes_written": batch * H * W * 32})
+        kout.update({"bytes_read": batch * (4 * H * W * 32 + H * W // 2), "bytes_written": batch * 4 * H * W * 3 // 2})
+        for kt in (kin, kout):
+            # one launch per call: time per launch, as the profile can miss a launch at the edge of its window
+            kt["us_per_launch"] = kt["us_per_batch"] * 50 / kt["launches"]
+            kt["bytes_per_s"] = (kt["bytes_read"] + kt["bytes_written"]) / (kt["us_per_launch"] * 1e-6)
+            kt["share_of_hbm_peak"] = kt["bytes_per_s"] / HBM_BYTES_PER_S
+        res.append({
+            "case": "espcn %dx%d batch %d from %dx%d NV12 to %dx%d NV12" % (H, W, batch, W, H, 2 * W, 2 * H),
+            "luma_path": "transform_luma (frame_input_kernel<luma>, forward pass, luma_output_kernel)",
+            "torch_path": "Y plane .contiguous(), run_torch (uint8 in, uint8 out), F.interpolate (bilinear) of U and V, NV12 packing",
+            "luma_frames_per_s_median": med("luma"),
+            "torch_frames_per_s_median": med("torch"),
+            "luma_over_torch": med("luma") / med("torch"),
+            "rounds": rounds,
+            "frame_input_kernel": kin,
+            "luma_output_kernel": kout,
+        })
+        m.close()
+    return res
+
+
 def host_regions(rows, counts, H, W, capacity):
     """What a user computes on the host without rois_from_detections: the pixel rectangles of the first `capacity` rows (frame by frame,
     row order), each clipped to the frame; empty ones skipped."""
@@ -538,7 +601,7 @@ def main():
     ap.add_argument("--seconds", type=float, default=2.0)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
-                    help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in)")
+                    help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -561,6 +624,8 @@ def main():
         result["transform"] = transform(torch, ctx, core, modelzoo, d, args)
     if "rois" in parts:
         result["rois"] = rois(torch, ctx, core, modelzoo, d, args)
+    if "luma" in parts:
+        result["luma"] = luma(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
