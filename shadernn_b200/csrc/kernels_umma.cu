@@ -105,21 +105,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded wait: a broken descriptor or protocol bug must surface as a trapped kernel, never as a hung GPU.
+// Bounded wait: a broken descriptor or protocol bug must surface as a trapped kernel, never as a hung GPU (SNNB_SYNC_LAYERS=1
+// names the layer and kernel that trapped). It must not make a function call (no printf): ptxas serializes every wgmma of a kernel
+// that contains a call, each one waiting for the previous one to retire.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     const long long t0 = clock64();
-    bool reported      = false;
-    while (!mbar_try_wait(bar, parity)) {
-        const long long dt = clock64() - t0;
-        if (dt > 4000000000LL && !reported) {
-            uint32_t dyn;
-            asm volatile("mov.u32 %0, %%dynamic_smem_size;" : "=r"(dyn));
-            printf("tensor-core kernel (dynamic smem %u B): mbarrier wait timed out (block %d thread %d bar 0x%x parity %u)\n", dyn, blockIdx.x, threadIdx.x, bar, parity);
-            reported = true;
-        }
-        if (dt > 4040000000LL) __trap(); // ~20 ms after the first report: every stuck thread gets to print
-    }
+    while (!mbar_try_wait(bar, parity))
+        if (clock64() - t0 > 4000000000LL) __trap();
 }
 // One lane of a CONVERGED warp: the compiler knows a single thread is active in the guarded region, so the TMA issue is
 // one predicated instruction rather than a loop over the active lanes.
@@ -217,8 +210,8 @@ template <int NACC> __device__ __forceinline__ void acc_promote(float (&sum)[NAC
 __device__ __forceinline__ void regs_dealloc_40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
 __device__ __forceinline__ void regs_alloc_232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
-// transcendental activations only (tanh / sigmoid / SiLU): rare, kept out of line so the hot epilogue stays small
-__device__ __noinline__ float umma_act(float v, int act, float alpha) {
+// transcendental activations (tanh / sigmoid / SiLU). Inlined into the tensor-core kernels: a call would serialize their wgmmas.
+__device__ __forceinline__ float umma_act(float v, int act, float alpha) {
     switch (act) {
     case SNNB_ACT_RELU: return fmaxf(v, 0.0f);
     case SNNB_ACT_RELU6: return fminf(fmaxf(v, 0.0f), 6.0f);
@@ -229,6 +222,8 @@ __device__ __noinline__ float umma_act(float v, int act, float alpha) {
     default: return v;
     }
 }
+// out of line for the depthwise kernel, which issues no wgmma: its hot loop stays small
+__device__ __noinline__ float umma_act_call(float v, int act, float alpha) { return umma_act(v, act, alpha); }
 // split-fp16 (snnb_internal.h): packed pair conversions, round to nearest, saturated to +-65504
 __device__ __forceinline__ float2 um_h2f(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
 __device__ __forceinline__ uint32_t um_f2h(float a, float b) {
@@ -262,13 +257,12 @@ struct EpiArgs {
 };
 
 // acc: this thread's fragment of its warpgroup's 64 x NB accumulator; row0 = the tile row of its d[0] (16 w + l / 4 within the
-// warpgroup's rows), q = l % 4.
-template <int NB>
-__device__ __forceinline__ void epilogue_tile(const EpiArgs& e, const float (&acc)[NB / 2], int oc0, int c1, int c2, int c3, int row0, int q, uint32_t& res_phase) {
+// warpgroup's rows), q = l % 4. SLOW_ACT: the activation is not one of the piecewise-linear ones (umma_act).
+template <int NB, bool SLOW_ACT>
+__device__ __forceinline__ void epilogue_tile_act(const EpiArgs& e, const float (&acc)[NB / 2], int oc0, int c1, int c2, int c3, int row0, int q, uint32_t& res_phase) {
     constexpr int W      = NB < 64 ? NB : 64; // slab width in channels
     constexpr bool SW    = W == 64;            // full slab: 128-byte rows, SWIZZLE_128B
     constexpr uint32_t PITCH = SW ? 128u : (uint32_t) W * 2u;
-    const bool fast_act  = e.act == SNNB_ACT_NONE || e.act == SNNB_ACT_RELU || e.act == SNNB_ACT_RELU6 || e.act == SNNB_ACT_LEAKY_RELU;
     const float slope    = (e.act == SNNB_ACT_RELU || e.act == SNNB_ACT_RELU6) ? 0.0f : (e.act == SNNB_ACT_LEAKY_RELU ? e.alpha : 1.0f);
     const float hi_clip  = e.act == SNNB_ACT_RELU6 ? 6.0f : __int_as_float(0x7f800000);
     const uint32_t lo_off = UM_BLOCK_M * 128;
@@ -304,13 +298,12 @@ __device__ __forceinline__ void epilogue_tile(const EpiArgs& e, const float (&ac
                     v0 += rh.x + rl.x;
                     v1 += rh.y + rl.y;
                 }
-                if (e.act == SNNB_ACT_RELU) {
+                if (SLOW_ACT) {
+                    v0 = umma_act(v0, e.act, e.alpha), v1 = umma_act(v1, e.act, e.alpha);
+                } else if (e.act == SNNB_ACT_RELU) {
                     v0 = fmaxf(v0, 0.0f), v1 = fmaxf(v1, 0.0f);
-                } else if (e.act == SNNB_ACT_NONE) {
-                } else if (fast_act) {
+                } else if (e.act != SNNB_ACT_NONE) {
                     v0 = fminf(fmaxf(v0, v0 * slope), hi_clip), v1 = fminf(fmaxf(v1, v1 * slope), hi_clip);
-                } else {
-                    v0 = umma_act(v0, e.act, e.alpha), v1 = umma_act(v1, e.act, e.alpha); // out-of-line call
                 }
                 if (oc >= e.OC) v0 = 0.0f; // channels [OC, Cp) stay zero
                 if (oc + 1 >= e.OC) v1 = 0.0f;
@@ -328,6 +321,16 @@ __device__ __forceinline__ void epilogue_tile(const EpiArgs& e, const float (&ac
             bulk_commit();
         }
     }
+}
+
+// The transcendental activations get an epilogue of their own, chosen once per tile: inlined into every element of the unrolled loop
+// (the kernel makes no calls), their code would be strewn through the common epilogue's and more than double its size.
+template <int NB>
+__device__ __forceinline__ void epilogue_tile(const EpiArgs& e, const float (&acc)[NB / 2], int oc0, int c1, int c2, int c3, int row0, int q, uint32_t& res_phase) {
+    if (e.act == SNNB_ACT_NONE || e.act == SNNB_ACT_RELU || e.act == SNNB_ACT_RELU6 || e.act == SNNB_ACT_LEAKY_RELU)
+        epilogue_tile_act<NB, false>(e, acc, oc0, c1, c2, c3, row0, q, res_phase);
+    else
+        epilogue_tile_act<NB, true>(e, acc, oc0, c1, c2, c3, row0, q, res_phase);
 }
 
 // After the last tile: the issuer's bulk stores must have completed before the CTA (and its shared memory) goes away.
@@ -1298,7 +1301,7 @@ __global__ void __launch_bounds__(DW_THREADS, 2) depthwise_tma_kernel(const __gr
                         for (int j = 0; j < 8; ++j) v[j] = fminf(fmaxf(acc[t][j], acc[t][j] * slope), hi_clip);
                     } else {
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) v[j] = umma_act(acc[t][j], p.act, p.alpha);
+                        for (int j = 0; j < 8; ++j) v[j] = umma_act_call(acc[t][j], p.act, p.alpha);
                     }
 #pragma unroll
                     for (int j = 0; j < 8; ++j) v[j] = (c + j < p.C) ? v[j] : 0.0f; // channel padding stays zero
