@@ -349,6 +349,34 @@ int snnb_model_transform_frames(snnb_model* m, const snnb_frames* frames, const 
  * snnb_model_run_device. Cost beyond the forward pass: one kernel launch for the input and one for the output (ESPCN 1920x1080 x 1
  * from 1920x1080 NV12 to 3840x2160 NV12: 24 us and 106 us; NVIDIA H100 80GB HBM3, 400 W power limit). */
 int snnb_model_transform_luma(snnb_model* m, const snnb_frames* frames, const snnb_frames_out* out, void* stream);
+/* Segmentation models (U-Net, a per-pixel classifier) from device frames to an 8-bit label plane of any size: the class scores of
+ * output 0 are resampled to the plane and reduced to one byte per pixel in the same kernel, so neither the upsampled scores nor an
+ * arg-max pass ever reach memory. The input is exactly what snnb_model_run_frames feeds (luma == 0), or exactly what
+ * snnb_model_transform_luma feeds (luma == 1: the Y plane of NV12 / NV21 / I420 frames into a model input of 1 channel, for grey-input
+ * models such as the reference's U-Net). Let T be output 0 (N x h x w x C) with values v = float(hi) + float(lo) (lo absent in FP16
+ * storage): bit for bit the F32 output of snnb_model_run_device / snnb_model_run_frames. For label pixel (x, y) of image n:
+ *   1. Scores s_c: T[n, y, x, c] when the plane has the output's size; otherwise the taps of ImageTexture::resize of T to width x
+ *      height (those of snnb_image_io): nearest takes T at the tap, linear blends the four taps per channel exactly as step 2 of
+ *      snnb_model_transform_frames (every + - * rounded on its own, no FMA), on the fp32 scores rather than on 8-bit values.
+ *   2. Label: C >= 2: the smallest c whose s_c equals the maximum over the s_c that are not NaN; 0 if every s_c is NaN. C == 1:
+ *      1 if s_0 >= threshold, else 0 (NaN gives 0).
+ *   3. The label is written at plane + n * image_stride + y * pitch + x. Bytes outside the rows are not written.
+ * Checked on the host before anything is enqueued: everything snnb_model_run_frames checks (with luma, also those of
+ * snnb_model_transform_luma's input), a non-null out, width and height >= 1, pitch >= width, a plane in device or managed memory of the
+ * context's device, and an output 0 that is not a YOLO layer, has a device tensor and has at most 256 channels. A capturing stream is
+ * refused. Stream contract and fences: those of snnb_model_run_device. The labels are written after the forward pass and read only the
+ * model's tensor, so the plane may overlap the input frames. Cost beyond the forward pass: one kernel launch for the input and one
+ * for the labels (U-Net 256x256 x 8 from 1920x1080 NV12 to 1920x1080 labels: 144 us for 1 class, 591 us for 21; NVIDIA H100 80GB
+ * HBM3, 700 W power limit). */
+typedef struct {
+    int width, height;       /* label plane size, any >= 1 */
+    uint8_t* plane;          /* device memory of the model's device: one byte per pixel */
+    int pitch;               /* bytes per row, >= width */
+    long long image_stride;  /* bytes from image n to image n+1 */
+    int linear_filter;       /* resampling of the scores: 1 = linear, 0 = nearest (ImageTexture::resize's taps) */
+    float threshold;         /* 1-channel outputs only */
+} snnb_labels_out;
+int snnb_model_segment_frames(snnb_model* m, const snnb_frames* frames, int luma, const snnb_labels_out* out, void* stream);
 /* Regions of device frames as the batch: the second stage of a detection pipeline (classify, describe or embed what a detector found)
  * without a host round trip. A region is a pixel rectangle [x, x + width) x [y, y + height) of frame `frame` of the frames given; `row`
  * is carried for the caller (the detection row it came from, or anything) and ignored by the engine. */

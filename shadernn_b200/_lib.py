@@ -113,6 +113,19 @@ class FramesOut(C.Structure):
     ]
 
 
+class LabelsOut(C.Structure):
+    """snnb_labels_out"""
+    _fields_ = [
+        ("width", C.c_int),
+        ("height", C.c_int),
+        ("plane", C.c_void_p),
+        ("pitch", C.c_int),
+        ("image_stride", C.c_longlong),
+        ("linear_filter", C.c_int),
+        ("threshold", C.c_float),
+    ]
+
+
 class Roi(C.Structure):
     """snnb_roi"""
     _fields_ = [
@@ -201,6 +214,7 @@ SIGNATURES = {
     "snnb_model_detect_frames": (C.c_int, [vp, C.POINTER(Frames), vp, C.c_int, vp, vp]),
     "snnb_model_transform_frames": (C.c_int, [vp, C.POINTER(Frames), C.POINTER(FramesOut), vp]),
     "snnb_model_transform_luma": (C.c_int, [vp, C.POINTER(Frames), C.POINTER(FramesOut), vp]),
+    "snnb_model_segment_frames": (C.c_int, [vp, C.POINTER(Frames), C.c_int, C.POINTER(LabelsOut), vp]),
     "snnb_model_run_rois": (C.c_int, [vp, C.POINTER(Frames), C.c_int, vp, vp, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
     "snnb_rois_from_detections": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(RoiSelect), vp, C.c_int, vp, vp]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),

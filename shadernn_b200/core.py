@@ -698,6 +698,33 @@ class MixedInferenceCore:
         check(lib().snnb_model_transform_luma(self.h, C.byref(f), C.byref(o), self._torch_stream()), "snnb_model_transform_luma")
         return out
 
+    def segment_frames(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, luma=False, out_hw=None, out_linear=True,
+                       threshold=0.5, out=None):
+        """snnb_model_segment_frames, for segmentation models: run_frames' input and forward pass (luma=True: the Y plane into a
+        1-channel input, as transform_luma feeds it), then the class scores of output 0 resized to out_hw (out_linear: bilinear, else
+        nearest, with run_image's taps, on the fp32 scores) and reduced to one label byte per pixel: the arg-max over the channels
+        (ties to the lowest index, NaN never wins, all NaN gives 0), or for a 1-channel output 1 where the score is >= threshold.
+        Ordered on the current torch stream and never synchronising.
+
+        out_hw defaults to the input frames' size. Returns `out`, a uint8 CUDA tensor [N, H, W] with dense pixels, allocated here
+        unless given; a given `out` may have a row stride larger than W and any image stride."""
+        import torch
+        f = self._frames("segment_frames", frames, format, matrix, linear, mean4, norm4)
+        oh, ow = (f.height, f.width) if out_hw is None else (int(out_hw[0]), int(out_hw[1]))
+        if out is None:
+            out = torch.empty((self.batch, oh, ow), dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+        if not (isinstance(out, torch.Tensor) and out.dtype == torch.uint8 and out.dim() == 3 and out.stride(2) == 1):
+            raise ValueError("segment_frames: out must be a uint8 CUDA tensor [N, H, W] with dense pixels")
+        if out.shape[0] != self.batch or (out_hw is not None and tuple(out.shape[1:]) != (oh, ow)):
+            raise ValueError("segment_frames: out holds %d planes of %d x %d; expected %d of %d x %d" % (out.shape[0], out.shape[1], out.shape[2],
+                                                                                                       self.batch, oh, ow))
+        o = _lib.LabelsOut()
+        o.height, o.width, o.plane = out.shape[1], out.shape[2], out.data_ptr()
+        o.pitch, o.image_stride = out.stride(1), out.stride(0)
+        o.linear_filter, o.threshold = int(bool(out_linear)), float(threshold)
+        check(lib().snnb_model_segment_frames(self.h, C.byref(f), int(bool(luma)), C.byref(o), self._torch_stream()), "snnb_model_segment_frames")
+        return out
+
     def set_input(self, images, idx=0):
         images = _f32(images)
         check(lib().snnb_model_set_input(self.h, idx, _ptr(images)), "snnb_model_set_input")

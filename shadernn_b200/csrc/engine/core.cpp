@@ -913,6 +913,30 @@ int MixedInferenceCore::transformLuma(const snnb_frames* frames, const snnb_fram
     return fenceToCaller(stream);
 }
 
+// Frames in, labels out: runFrames' (or, with luma, transformLuma's) input staging and forward pass, then output 0's scores resampled
+// to the label plane and reduced to one byte per pixel in one kernel. The kernel reads only the model's tensor, so the plane may alias
+// the input frames.
+int MixedInferenceCore::segmentFrames(const snnb_frames* frames, bool luma, const snnb_labels_out* out, cudaStream_t stream) {
+    static const char* api = "snnb_model_segment_frames";
+    SNNB_REQUIRE(frames, "snnb_model_segment_frames: null frames");
+    SNNB_REQUIRE(out, "snnb_model_segment_frames: null out");
+    DeviceFeed in;
+    in.frames = frames, in.luma = luma;
+    if (int rc = checkDeviceFeed(api, in, stream)) return rc;
+    const snnb_labels_out& o = *out;
+    SNNB_REQUIRE(o.width >= 1 && o.height >= 1, "%s: label plane size %d x %d; width and height must be >= 1", api, o.width, o.height);
+    SNNB_REQUIRE(o.pitch >= o.width, "%s: label plane pitch %d is less than its width %d", api, o.pitch, o.width);
+    if (int rc = checkDevicePointer(api, o.plane, 1, ctx->device, "label plane", 0)) return rc;
+    SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; labels are written from per-pixel class scores", api);
+    const snnb_tensor* t = outputLayers[0]->output;
+    SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
+    SNNB_REQUIRE(t->c >= 1 && t->c <= 256, "%s: output 0 has %d channels; an 8-bit label plane is written from 1 to 256", api, t->c);
+
+    if (enqueueDeviceForward(in, stream)) return 1;
+    if (launch_segment_output(ctx, t, o)) return 1;
+    return fenceToCaller(stream);
+}
+
 int MixedInferenceCore::layerOutput(int layerId, float* host, size_t capacityFloats) {
     SNNB_REQUIRE(layerId >= 0 && layerId < (int) layers.size() && host, "layerOutput: bad argument");
     GenericModelLayer* L = layers[layerId].get();

@@ -360,6 +360,8 @@ public:
     int transformFrames(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream);
     // snnb_model_transform_luma: the frames' Y plane into a 1-channel model, output 0 (1 channel) out as the Y plane, chroma resampled
     int transformLuma(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream);
+    // snnb_model_segment_frames: runFrames' input (luma: transformLuma's), output 0's scores resampled and reduced to an 8-bit label plane
+    int segmentFrames(const snnb_frames* frames, bool luma, const snnb_labels_out* out, cudaStream_t stream);
     // snnb_model_run_rois: runFrames with regions of numFrames frames as the batch; slots without a valid region come out zero
     int runRois(const snnb_frames* frames, int numFrames, const snnb_roi* roisDev, const int* countDev, const snnb_device_buffer* outputs, int numOutputs,
                 int* classes1Dev, cudaStream_t stream);

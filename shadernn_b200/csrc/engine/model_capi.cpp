@@ -154,6 +154,11 @@ int snnb_model_transform_luma(snnb_model* m, const snnb_frames* frames, const sn
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->transformLuma(frames, out, static_cast<cudaStream_t>(stream));
 }
+int snnb_model_segment_frames(snnb_model* m, const snnb_frames* frames, int luma, const snnb_labels_out* out, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_segment_frames: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->segmentFrames(frames, luma != 0, out, static_cast<cudaStream_t>(stream));
+}
 int snnb_model_run_rois(snnb_model* m, const snnb_frames* frames, int num_frames, const snnb_roi* rois_dev, const int* count_dev,
                         const snnb_device_buffer* outputs, int num_outputs, int* classes_1based_dev, void* stream) {
     SNNB_REQUIRE(m, "snnb_model_run_rois: null model");

@@ -2081,4 +2081,86 @@ int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame
     SNNB_REQUIRE(false, "launch_luma_output: out format %d; luma frames are written as NV12, NV21 or I420", fr.format);
 }
 
+// Model output 0 -> an 8-bit label plane (snnb_model_segment_frames): the fp32 scores hi + lo resampled to the plane with
+// ImageTexture::resize's taps and blend_rn (step 2 of frame_output_kernel, on the scores rather than on quantised bytes), then one label
+// per pixel: the arg-max over the C channels, or the threshold of a 1-channel output.
+struct LabelsV {
+    uint8_t* plane;
+    int pitch;
+    long long stride;
+    int w, h;
+    float threshold;
+};
+// The label of pixel (x, y) of image n. The channel loop reads 8 channels per load8 at each tap (1, or 4 when blending) and keeps only
+// the running maximum and its index. THRESH: C == 1, no channel loop. Ties go to the lowest channel (strict >), NaN scores are never the
+// maximum, and a pixel whose scores are all NaN is labelled 0.
+template <bool THRESH>
+__device__ __forceinline__ void segment_pixel(const TV& t, const LabelsV& o, int linear, int n, int x, int y) {
+    const bool direct = o.w == t.W && o.h == t.H;
+    ResizeTaps r;
+    if (direct) r.x0 = r.x1 = x, r.y0 = r.y1 = y, r.ax = r.ay = 0.0f;
+    else r = resize_taps(resize_pos(x, y, o.w, o.h, t.W, t.H), t.W, t.H, linear);
+    const bool blend  = linear && !direct;
+    const size_t img  = (size_t) n * t.H;
+    const size_t o00 = ((img + r.y0) * t.W + r.x0) * t.Cp, o01 = ((img + r.y0) * t.W + r.x1) * t.Cp;
+    const size_t o10 = ((img + r.y1) * t.W + r.x0) * t.Cp, o11 = ((img + r.y1) * t.W + r.x1) * t.Cp;
+    int label;
+    if (THRESH) {
+        float p00[8];
+        load8(t.hi, t.lo, o00, p00);
+        float s = p00[0];
+        if (blend) {
+            float p01[8], p10[8], p11[8];
+            load8(t.hi, t.lo, o01, p01);
+            load8(t.hi, t.lo, o10, p10);
+            load8(t.hi, t.lo, o11, p11);
+            s = blend_rn(r, p00[0], p01[0], p10[0], p11[0]);
+        }
+        label = s >= o.threshold ? 1 : 0; // false for NaN
+    } else {
+        float best = -INFINITY;
+        int arg    = -1;
+#pragma unroll 1
+        for (int c = 0; c < t.C; c += 8) {
+            float s[8];
+            load8(t.hi, t.lo, o00 + c, s);
+            if (blend) {
+                float p01[8], p10[8], p11[8];
+                load8(t.hi, t.lo, o01 + c, p01);
+                load8(t.hi, t.lo, o10 + c, p10);
+                load8(t.hi, t.lo, o11 + c, p11);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) s[j] = blend_rn(r, s[j], p01[j], p10[j], p11[j]);
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                if (c + j < t.C && (s[j] > best || (arg < 0 && s[j] == s[j]))) best = s[j], arg = c + j;
+        }
+        label = arg < 0 ? 0 : arg;
+    }
+    o.plane[n * o.stride + (size_t) y * o.pitch + x] = (uint8_t) label;
+}
+// One thread per label pixel, x fastest: the pixels of a warp lie in one row and share their tap rows. A block covers SEG_THREADS
+// pixels of a row (grid x); rows and images come from grid y and z, strided past 65535, so no thread divides.
+constexpr int SEG_THREADS = 128;
+template <bool THRESH>
+__global__ void __launch_bounds__(SEG_THREADS) segment_output_kernel(TV t, LabelsV o, int linear) {
+    pdl_wait();
+    const int x = blockIdx.x * SEG_THREADS + threadIdx.x;
+    if (x >= o.w) return;
+    for (int n = blockIdx.z; n < t.N; n += gridDim.z)
+        for (int y = blockIdx.y; y < o.h; y += gridDim.y) segment_pixel<THRESH>(t, o, linear, n, x, y);
+}
+int launch_segment_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_out& lo) {
+    SNNB_REQUIRE(t->c >= 1 && t->c <= 256 && t->cp % 8 == 0 && !t->feed_only, "launch_segment_output: the output tensor has %d channels; labels are written from 1 to 256",
+                 t->c);
+    LabelsV o;
+    o.plane = lo.plane, o.pitch = lo.pitch, o.stride = lo.image_stride, o.w = lo.width, o.h = lo.height, o.threshold = lo.threshold;
+    const int linear = lo.linear_filter ? 1 : 0;
+    const dim3 grid((unsigned) ((lo.width + SEG_THREADS - 1) / SEG_THREADS), (unsigned) std::min(lo.height, 65535), (unsigned) std::min(t->n, 65535)),
+        block(SEG_THREADS);
+    if (t->c == 1) return launch_done(ctx, launch_k(segment_output_kernel<true>, grid, block, 0, ctx->stream, view(t), o, linear), "segment_output_kernel<threshold>");
+    return launch_done(ctx, launch_k(segment_output_kernel<false>, grid, block, 0, ctx->stream, view(t), o, linear), "segment_output_kernel<argmax>");
+}
+
 } // namespace snnb

@@ -253,6 +253,9 @@ int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_fram
 // t (C = 1) -> 8 bits -> resized -> the Y plane of NV12 / NV21 / I420 frames; their chroma resized from src's chroma planes (checked by
 // the caller, which also keeps the out planes clear of src's chroma unless out is src itself)
 int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames& src, const snnb_frames_out& f);
+// t (C = 1 .. 256) -> scores resized to the label plane -> one byte per pixel: arg-max over C, or s >= threshold for C = 1 (checked by
+// the caller)
+int launch_segment_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_out& out);
 // Regions of device frames (snnb_model_run_rois, checked by the caller) -> t (C <= 4): slot n is rois[n] sampled as launch_frame_input
 // samples a frame of the region's size; invalid slots and slots past *count (count NULL: all used) are zero
 int launch_frame_roi_input(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t);

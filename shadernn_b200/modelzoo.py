@@ -533,8 +533,67 @@ def espcn(input_hw=(224, 224), seed=SEED):
     return b.layers
 
 
+def calibrate_segmentation_head(layers, input_hw, images=4, logit_std=2.0):
+    """calibrate_head for the last (1x1) convolution of a segmentation model, on `images` calibration images (their own seed), with
+    every pixel a sample: the kernel is scaled so that the logits' spread over pixels and images is `logit_std`, and the bias centres
+    them. One output channel: the median pre-sigmoid value becomes 0, so the 0.5 threshold splits the pixels. Several: each class's
+    logit is centred on its mean, so the arg-max is decided by the pixel's features. Needs torch (CPU); a no-op without it."""
+    try:
+        import torch  # noqa: F401
+    except Exception:
+        return False
+    ci = max(i for i, l in enumerate(layers) if l["type"] == "Conv2D")
+    src = layers[ci]["inputId"][0]
+    x = synthetic_input("unet", images, input_hw, seed=SEED + 1000)
+    g = torch_forward(layers, x, upto=src)[src].reshape(-1, layers[ci]["inputPlanes"]).astype(np.float64)
+    w = layers[ci]["_w"]["kernel"][:, :, 0, 0].astype(np.float64)  # [K, C]
+    z = (g - g.mean(0)) @ w.T
+    w *= logit_std / max(float(z.std()), 1e-12)
+    z = g @ w.T
+    b = -np.median(z, axis=0) if w.shape[0] == 1 else -z.mean(0)
+    layers[ci]["_w"]["kernel"] = w.astype(np.float32).reshape(layers[ci]["_w"]["kernel"].shape)
+    layers[ci]["_w"]["bias"] = b.astype(np.float32)
+    return True
+
+
+def unet(input_hw=(256, 256), classes=1, seed=SEED, calibrate=True):
+    """modelzoo/U-Net/unet.param (the grey-input U-Net of demo/test_unet.sh): [3x3 conv + ReLU] x2 at 64, 128, 256 and 512 channels,
+    each followed by a 2x2 max pool, then [3x3 conv + ReLU] x2 at 1024; four decoder stages of nearest x2, a 2x2 'same' conv + ReLU at
+    half the channels, concat(that, the encoder's output of that size) and [3x3 conv + ReLU] x2; head 3x3 conv 64->2 + ReLU, 1x1 conv
+    2->1 + sigmoid. Every convolution has a bias and no BN. classes = K > 1 replaces the last two convolutions with one linear 1x1 conv
+    64->K (a multi-class variant, not a reference graph). The last convolution is calibrated (calibrate_segmentation_head)."""
+    b = Builder(seed)
+    h, w = input_hw
+    x = b.input(w, h, 1)
+
+    def double(x, oc):
+        x = b.conv(x, oc, 3, 1, "same", "relu", bias=True)
+        return b.conv(x, oc, 3, 1, "same", "relu", bias=True)
+
+    skips = []
+    for oc in (64, 128, 256, 512):
+        x = double(x, oc)
+        skips.append(x)
+        x = b.maxpool(x, 2, 2, "valid")
+    x = double(x, 1024)
+    for oc, skip in zip((512, 256, 128, 64), reversed(skips)):
+        x = b.upsample(x, 2, "nearest")
+        x = b.conv(x, oc, 2, 1, "same", "relu", bias=True)
+        x = b.concat(x, skip)
+        x = double(x, oc)
+    if classes == 1:
+        x = b.conv(x, 2, 3, 1, "same", "relu", bias=True)
+        b.conv(x, 1, 1, 1, "valid", "sigmoid", bias=True, gain=1.0)
+    else:
+        b.conv(x, classes, 1, 1, "valid", "linear", bias=True, gain=1.0)
+    if calibrate:
+        calibrate_segmentation_head(b.layers, input_hw)
+    return b.layers
+
+
 MODELS = {
     "espcn": (espcn, (224, 224), 1, (0.0, 1.0)),
+    "unet": (unet, (256, 256), 1, (0.0, 1.0)),
     "resnet18": (resnet18, (224, 224), 3, (-1.0, 1.0)),
     "mobilenetv2": (mobilenetv2, (224, 224), 3, (0.0, 1.0)),
     "yolov3tiny": (yolov3_tiny, (416, 416), 3, (-1.0, 1.0)),

@@ -42,7 +42,13 @@ Writes DIR/device_io_bench.json and prints it. Four parts, all in one process:
                luma_output_kernel) against what a user does without it, the Y plane made dense, run_torch with uint8 in and out,
                F.interpolate (bilinear) of U and V and packing; alternating as above. And the device time per batch of the input kernel
                (frame_input_kernel<luma>) and of luma_output_kernel from torch.profiler over 50 calls, with bytes/s from what each moves.
-  card         name, power limit and maximum SM clock, read by nvidia-smi in the same run.
+  segment      (opt-in) The U-Net of the model zoo at 256x256 x 1, batch 8, with 1 class (the reference's graph) and with 21, from
+               1920x1080 NV12 frames (run_frames' input, both paths) to 1920x1080 label planes: segment_frames (scores resampled and reduced
+               in segment_output_kernel) against what a user does without it, run_frames(out_dtype=float32) + F.interpolate (bilinear) +
+               the arg-max (or the 0.5 threshold) + .to(uint8); alternating as above. And segment_output_kernel's time per batch from
+               CUDA events (segment_frames calls less calls that run only the same input and forward pass) and from torch.profiler, with
+               bytes/s from the labels written plus the model-output planes read once.
+  card        name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
 import ctypes as C
@@ -510,6 +516,83 @@ def luma(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def torch_segment_today(torch, m, nv12, H, W, classes):
+    """The path without segment_frames: run_frames' fp32 scores (NCHW), F.interpolate (bilinear) to the frame, then the arg-max over
+    the channels (or the 0.5 threshold of one channel) and .to(uint8): [N, H, W] uint8."""
+    import torch.nn.functional as F
+    s = m.run_frames(nv12, mean4=[0.0] * 4, norm4=[1.0 / 255.0] * 4, out_dtype=torch.float32, out_layout="nchw")
+    s = F.interpolate(s, size=(H, W), mode="bilinear", align_corners=False)
+    return (s[:, 0] >= 0.5).to(torch.uint8) if classes == 1 else s.argmax(1).to(torch.uint8)
+
+
+def forward_only(m, f):
+    """snnb_model_run_frames with no outputs: the input kernel and the forward pass that segment_frames also runs."""
+    from shadernn_b200._lib import DeviceBuffer, check, lib
+    check(lib().snnb_model_run_frames(m.h, C.byref(f), (DeviceBuffer * 1)(), 0, None, m._torch_stream()), "snnb_model_run_frames")
+
+
+def event_us(torch, fn, calls):
+    """Device time per call (us) of `calls` back-to-back calls, between two CUDA events on the current stream."""
+    for _ in range(5):
+        fn()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    a.record()
+    for _ in range(calls):
+        fn()
+    b.record()
+    b.synchronize()
+    return a.elapsed_time(b) * 1e3 / calls
+
+
+def segment(torch, ctx, core, modelzoo, d, args):
+    H, W, hw, batch = 1080, 1920, (256, 256), 8
+    res = []
+    for classes in (1, 21):
+        path, _ = modelzoo.build("unet", os.path.join(d, "seg_unet%d" % classes), input_hw=hw, classes=classes)
+        m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+        g = torch.Generator().manual_seed(11)
+        nv12 = torch.randint(16, 236, (batch, H * 3 // 2, W), dtype=torch.uint8, generator=g).cuda()
+        out = torch.empty((batch, H, W), dtype=torch.uint8, device="cuda")
+        fused = lambda: m.segment_frames(nv12, mean4=[0.0] * 4, norm4=[1.0 / 255.0] * 4, out=out)  # noqa: E731
+        unfused = lambda: torch_segment_today(torch, m, nv12, H, W, classes)  # noqa: E731
+        for _ in range(5):
+            fused()
+            unfused()
+        torch.cuda.synchronize()
+        rounds = []
+        for _ in range(args.rounds):
+            rounds.append({"segment": timed(fused, args.seconds, batch, torch.cuda.synchronize),
+                           "torch": timed(unfused, args.seconds, batch, torch.cuda.synchronize)})
+        med = lambda k: float(np.median([r[k]["frames_per_s"] for r in rounds]))  # noqa: E731
+        # the output kernel: CUDA events around 50 segment_frames calls, less 50 calls that run the same input kernel and forward pass
+        # (run_frames with no outputs); and its device time from torch.profiler
+        f = m._frames("segment", nv12, "nv12", "bt601", True, [0.0] * 4, [1.0 / 255.0] * 4)
+        seg_us, fwd_us = event_us(torch, fused, 50), event_us(torch, lambda: forward_only(m, f), 50)
+        kt = frame_kernel_us(torch, fused, 50, "segment_output_kernel")
+        kt["us_per_launch"] = kt["us_per_batch"] * 50 / kt["launches"]
+        kt["events_us_segment_call"], kt["events_us_forward_only_call"] = seg_us, fwd_us
+        kt["events_us_difference"] = seg_us - fwd_us
+        # bytes: the label bytes written plus the model-output planes read once (hi and lo, Cp = C rounded up to 8 fp16 per pixel each)
+        cp = (classes + 7) // 8 * 8
+        kt["bytes_written"] = batch * H * W
+        kt["bytes_read"] = batch * hw[0] * hw[1] * cp * 2 * 2
+        kt["bytes_per_s"] = (kt["bytes_read"] + kt["bytes_written"]) / (kt["us_per_launch"] * 1e-6)
+        kt["share_of_hbm_peak"] = kt["bytes_per_s"] / HBM_BYTES_PER_S
+        res.append({
+            "case": "unet %dx%d x 1 -> %d classes, batch %d, from %dx%d NV12 to %dx%d labels" % (hw[0], hw[1], classes, batch, W, H, W, H),
+            "segment_path": "segment_frames (frame_input_kernel<nv12>, forward pass, segment_output_kernel)",
+            "torch_path": "run_frames(out_dtype=float32, nchw), F.interpolate (bilinear), %s, .to(uint8)" % ("s >= 0.5" if classes == 1 else "argmax(1)"),
+            "segment_frames_per_s_median": med("segment"),
+            "torch_frames_per_s_median": med("torch"),
+            "segment_over_torch": med("segment") / med("torch"),
+            "rounds": rounds,
+            "segment_output_kernel": kt,
+        })
+        m.close()
+    return res
+
+
 def host_regions(rows, counts, H, W, capacity):
     """What a user computes on the host without rois_from_detections: the pixel rectangles of the first `capacity` rows (frame by frame,
     row order), each clipped to the frame; empty ones skipped."""
@@ -601,7 +684,8 @@ def main():
     ap.add_argument("--seconds", type=float, default=2.0)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
-                    help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in)")
+                    help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in), "
+                         "segment (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -626,6 +710,8 @@ def main():
         result["rois"] = rois(torch, ctx, core, modelzoo, d, args)
     if "luma" in parts:
         result["luma"] = luma(torch, ctx, core, modelzoo, d, args)
+    if "segment" in parts:
+        result["segment"] = segment(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
