@@ -496,6 +496,11 @@ int snnb_debug_feed_plan(int k, int stride, int pad_x, int ic, int out[5]);
  * pad_x, pad_y, pad_mode (what the kernel sees), prepad_h, prepad_w (0 = no pre-padded copy), feed_h, feed_w, feed_py, feed_px
  * (0 = no feed copy)}. Returns 0. No GPU needed. */
 int snnb_debug_conv_plan(const int query[18], int out[10]);
+/* Diagnostics: the kernel instantiation of the most recent convolution launched on `ctx` (per-operator or inside a model's forward
+ * pass): out = {path (as snnb_debug_conv_plan; 0 before any convolution), terms (product form of the tensor-core kernels: 3 fp32x3,
+ * 2 fp16w, 1 fp16; 0 on the CUDA cores), n_blk (output channels per tile), ksplit (K pieces per tile, 1 = none), stream_k (0/1),
+ * fks (K steps per filter row of the row-window kernel's feed mode, 0 otherwise)}. Host-side record, no GPU work. Returns 0. */
+int snnb_debug_last_conv_variant(snnb_context* ctx, int out[6]);
 
 #ifdef __cplusplus
 }

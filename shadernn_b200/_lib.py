@@ -240,6 +240,7 @@ SIGNATURES = {
     "snnb_debug_streamk_schedule": (C.c_int, [C.c_int, C.c_int, C.c_int, c_int_p, C.c_int]),
     "snnb_debug_feed_plan": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, c_int_p]),
     "snnb_debug_conv_plan": (C.c_int, [c_int_p, c_int_p]),
+    "snnb_debug_last_conv_variant": (C.c_int, [vp, c_int_p]),
 }
 
 _lib = None

@@ -45,6 +45,14 @@ class GpuContext:
         """Default product form of per-operator convolution launches: "fp32x3" (three bf16 MMAs) or "fp16w" (fp16 weights, two)."""
         check(lib().snnb_context_set_precision(self.h, PRECISION[precision]), "snnb_context_set_precision")
 
+    def last_conv_variant(self):
+        """snnb_debug_last_conv_variant: the instantiation of the most recent convolution launch on this context, as a dict with
+        path ("simt", "igemm", "rowwin", "rowwin-feed"), terms, n_blk, ksplit, stream_k and fks."""
+        out = (C.c_int * 6)()
+        check(lib().snnb_debug_last_conv_variant(self.h, out), "snnb_debug_last_conv_variant")
+        v = list(out)
+        return {"path": ["none", "simt", "igemm", "rowwin", "rowwin-feed"][v[0]], "terms": v[1], "n_blk": v[2], "ksplit": v[3], "stream_k": v[4], "fks": v[5]}
+
     @property
     def stream(self):
         return lib().snnb_context_stream(self.h)

@@ -170,6 +170,11 @@ int snnb_debug_streamk_schedule(int tiles, int num_kb, int sms, int* rows, int c
     SNNB_REQUIRE(rows || capacity == 0, "snnb_debug_streamk_schedule: null buffer");
     return streamk_schedule(tiles, num_kb, sms, rows, capacity);
 }
+int snnb_debug_last_conv_variant(snnb_context* ctx, int out[6]) {
+    SNNB_REQUIRE(ctx && out, "snnb_debug_last_conv_variant: null argument");
+    for (int i = 0; i < 6; ++i) out[i] = ctx->last_conv[i];
+    return 0;
+}
 int snnb_tensor_planes(const snnb_tensor* t, void** hi, void** lo, int* cp) {
     SNNB_REQUIRE(t && hi && lo && cp, "snnb_tensor_planes: null argument");
     *hi = t->hi, *lo = t->lo, *cp = t->cp;

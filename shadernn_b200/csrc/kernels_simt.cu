@@ -274,6 +274,8 @@ __global__ void __launch_bounds__(128) conv2d_simt_kernel(const ConvKParams p) {
 int launch_conv2d_simt(snnb_context* ctx, const ConvArgs& a) {
     SNNB_REQUIRE(!a.in->feed_only, "launch_conv2d_simt: the input tensor only exists as a stem feed, which this kernel cannot read");
     ctx->last_kernel = "conv2d_simt_kernel";
+    const int variant[6] = {CONV_SIMT, 0, 0, 1, 0, 0}; // fp32 FMAs on the folded fp32 weights: no product form
+    std::copy(variant, variant + 6, ctx->last_conv);
     ConvKParams p;
     p.in      = view(a.in);
     p.out     = view(a.out);

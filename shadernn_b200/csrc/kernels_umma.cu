@@ -981,7 +981,6 @@ template <int TERMS, int NB> static RowWinKernel rowwin_kernel_fks(int fks) {
     case 1: return conv_rowwin_kernel<TERMS, 1, NB>;
     case 2: return conv_rowwin_kernel<TERMS, 2, NB>;
     case 3: return conv_rowwin_kernel<TERMS, 3, NB>;
-    case 4: return conv_rowwin_kernel<TERMS, 4, NB>;
     default: return conv_rowwin_kernel<TERMS, 0, NB>;
     }
 }
@@ -1067,6 +1066,8 @@ int launch_conv2d_rowwin(snnb_context* ctx, const ConvArgs& a, const ConvPlan& p
     if (encode_nhwc_box_maps(encode, out, p.n_blk, UM_BLOCK_M, 1, 1, p.n_blk == 64, tmO)) return 2;
     const int fks = feed ? fp.ksteps : 0;
     auto* kern    = rowwin_kernel_of(terms, fks, p.n_blk);
+    const int variant[6] = {plan.path, terms, p.n_blk, 1, 0, fks};
+    std::copy(variant, variant + 6, ctx->last_conv);
     if (ensure_smem_attr(ctx, (const void*) kern, ATTR_ROWWIN0 + ((terms - 1) * 5 + fks) * 2 + (p.n_blk == 64 ? 1 : 0), RW_SMEM_BYTES)) return 1;
     const int total_tiles = p.N * p.OH * p.tiles_x;
     const int grid        = std::min(total_tiles, ctx->sm_count);
@@ -1152,6 +1153,8 @@ int launch_conv2d_umma(snnb_context* ctx, const ConvArgs& a) {
     const int total_tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.tiles_oc;
     const int grid        = p.sk ? (p.sk_dp > 0 ? ctx->sm_count : p.sk_ctas) : std::min(total_tiles * p.ksplit, ctx->sm_count);
     ctx->last_kernel = p.sk ? "conv_umma_kernel<stream-K>" : (p.ksplit > 1 ? "conv_umma_kernel<split-K>" : "conv_umma_kernel");
+    const int variant[6] = {CONV_IGEMM, terms, p.n_blk, p.ksplit, p.sk ? 1 : 0, 0};
+    std::copy(variant, variant + 6, ctx->last_conv);
     return launch_done(ctx, launch_k_pdl(kc.kernel, dim3(grid), dim3(UM_THREADS), kc.smem, ctx->stream, tmA[0], tmA[1], tmB[0], tmB[1], tmO64[0], tmO64[1], tmOT[0], tmOT[1],
                             tmR64[0], tmR64[1], tmRT[0], tmRT[1], p), "conv_umma_kernel");
 }

@@ -158,6 +158,9 @@ struct snnb_context {
     // (= per device), not a process-wide flag
     uint64_t func_attr_mask = 0;
     const char* last_kernel = nullptr; // name of the kernel the most recent launcher chose (snnb_model_layer_kernel, bench.py's roofline)
+    // instantiation of the most recent convolution launch (snnb_debug_last_conv_variant): {path (ConvPath), terms, n_blk, ksplit,
+    // stream_k, fks}; zeros before the first one
+    int last_conv[6] = {0, 0, 0, 0, 0, 0};
     int precision = SNNB_PRECISION_FP32X3; // default product form of per-operator convolution launches (snnb_context_set_precision)
     std::vector<void*> scratch_blocks;
 };
@@ -325,7 +328,7 @@ static inline bool make_feed_plan(int k, int stride, int pad_x, int ic, FeedPlan
     fp.nch    = ((fp.d + k + 1) / 2 + 1) & ~1;
     fp.ksteps = fp.nch / 2;
     fp.rows_per_panel = fp.ksteps == 1 ? 4 : (fp.ksteps == 2 ? 2 : 1);
-    return fp.ksteps <= 4;
+    return fp.ksteps <= 3; // k <= 9 needs at most 3 (d + k + 1 <= 11 pixels); conv_rowwin_kernel is instantiated for FKS 1 .. 3
 }
 
 // ---- geometry of the tensor-core convolution kernels (kernels_umma.cu), read by the planner too ----------------
