@@ -275,12 +275,34 @@ int snnb_model_detect_device(snnb_model* m, const snnb_device_buffer* inputs, in
  * pixel itself), each converted to RGBA8 exactly as libyuv does, pixel (x, y) using chroma sample (x / 2, y / 2); then the same
  * interpolation and normalisation as snnb_model_submit_image. The model input is therefore bit-identical to snnb_model_submit_image
  * fed libyuv's RGBA8 image (its first C components). */
-enum { SNNB_FRAME_NV12 = 0, SNNB_FRAME_NV21 = 1, SNNB_FRAME_I420 = 2, SNNB_FRAME_RGBA8 = 3 };
-enum { SNNB_YUV_BT601 = 0 /* libyuv kYuvI601Constants: the reference's nv12ToRgba8 */, SNNB_YUV_BT709 = 1 /* kYuvH709Constants */ };
+/* 10-bit frames (SNNB_FRAME_P010: NVDEC's surfaces of HEVC Main10, AV1 and VP9 10-bit streams, NVENC's 10-bit input). Layout: NV12's,
+ * plane 0 Y and plane 1 interleaved U,V pairs (U first), with every sample a little-endian 16-bit word whose value is word >> 6 (the low
+ * 6 bits are ignored, so P016 surfaces holding 10-bit content work too). Row bytes 2 * width (Y) and 4 * ceil(width / 2) (UV); pitches
+ * and image strides must be even and planes 2-byte aligned. Model input of a P010 frame, per output pixel:
+ *   1. Each tap takes Y10, U10, V10, chroma sited as above, and libyuv's YuvPixel16 (row_common.cc:1531-1573) with the matrix's
+ *      constants computes b16, g16, r16 from Y10 and U10 >> 2, V10 >> 2 (U and V are truncated to 8 bits, as that row does).
+ *   2. R10 = clamp(r16 >> 4, 0, 1023) as StoreAR30 (row_common.cc:1713-1750), the same for G and B; the texel component is
+ *      R10 * 0.25 (exact: 8-bit units, so the same mean4 / norm4 apply), alpha 255.
+ *   3. Linear taps are blended as snnb_model_transform_frames' step 2 (every + - * rounded on its own, no FMA), then
+ *      (x - mean4[c]) * norm4[c], each rounded on its own: the model input is restatable bit for bit in float32.
+ * The Y plane of P010 frames (luma input: snnb_model_transform_luma, snnb_model_segment_frames with luma = 1) is the texel Y10 * 0.25,
+ * blended and normalised as step 3.
+ * Matrices: SNNB_YUV_BT2020 (the H.273 MatrixCoefficients code point 9, as BT.709 is 1) is kYuv2020Constants, and
+ * SNNB_YUV_BT601 | SNNB_YUV_FULL_RANGE is kYuvJPEGConstants (JPEG / JFIF full-range YUV). libyuv 1744 has no full-range BT.709 or
+ * BT.2020, so FULL_RANGE with any other matrix is refused. Every matrix applies to NV12, NV21, I420 and P010; on the 8-bit formats
+ * the model input stays bit-identical to snnb_model_submit_image fed libyuv's RGBA8 image with that matrix. Cost: 1920x1080 P010 to
+ * YOLOv3-tiny 416x416 x 16, 60 us for the input kernel against 50 us for NV12 (NVIDIA H100 80GB HBM3, 700 W power limit). */
+enum { SNNB_FRAME_NV12 = 0, SNNB_FRAME_NV21 = 1, SNNB_FRAME_I420 = 2, SNNB_FRAME_RGBA8 = 3, SNNB_FRAME_P010 = 16 };
+enum {
+    SNNB_YUV_BT601 = 0 /* libyuv kYuvI601Constants: the reference's nv12ToRgba8 */,
+    SNNB_YUV_BT709 = 1 /* kYuvH709Constants */,
+    SNNB_YUV_BT2020 = 9 /* kYuv2020Constants */,
+    SNNB_YUV_FULL_RANGE = 0x100 /* flag: SNNB_YUV_BT601 | SNNB_YUV_FULL_RANGE is kYuvJPEGConstants */
+};
 typedef struct {
     int format, matrix;          /* SNNB_FRAME_*, SNNB_YUV_* (matrix ignored for RGBA8) */
     int width, height;           /* frame size, any >= 1 (odd allowed: chroma is ceil(w/2) x ceil(h/2), as libyuv) */
-    const uint8_t* plane[3];     /* NV12/NV21: Y, UV|VU; I420: Y, U, V; RGBA8: RGBA. Device memory of the model's device */
+    const uint8_t* plane[3];     /* NV12/NV21/P010: Y, UV|VU; I420: Y, U, V; RGBA8: RGBA. Device memory of the model's device */
     int pitch[3];                /* bytes per row, >= the row's bytes */
     long long image_stride[3];   /* bytes from image n to image n+1 of the batch, per plane */
     int linear_filter;           /* as snnb_image_io */
@@ -289,7 +311,8 @@ typedef struct {
 /* snnb_model_run_device / snnb_model_detect_device with `frames` (the loaded batch of them) in place of the input buffers: outputs,
  * classes, rows, counts, the stream contract and the fences are exactly theirs; run_frames refuses YOLO models, detect_frames requires
  * them. Checked on the host before anything is enqueued: format and matrix, width and height >= 1, each pitch >= its row's bytes, each
- * plane device or managed memory of the context's device, a model with one input of <= 4 channels, a stream that is not capturing.
+ * plane device or managed memory of the context's device, a model with one input of <= 4 channels, a stream that is not capturing;
+ * for P010 also even pitches and image strides and 2-byte-aligned planes.
  * A plane's size cannot be checked: it must hold the batch. Cost beyond the forward pass: one kernel launch for the input (1920x1080
  * NV12 to YOLOv3-tiny 416x416 x 16: 50 us, to ResNet-18 224x224 x 32: 30 us; NVIDIA H100 80GB HBM3, 700 W power limit). */
 int snnb_model_run_frames(snnb_model* m, const snnb_frames* frames, const snnb_device_buffer* outputs, int num_outputs, int* classes_1based_dev,
@@ -310,13 +333,20 @@ int snnb_model_detect_frames(snnb_model* m, const snnb_frames* frames, float* ro
  *      Y = (66 R + 129 G + 25 B + 0x1080) >> 8; each chroma sample averages its 2 x 2 block as (a + b + c + d) >> 2 (an odd last column
  *      (a + b) >> 1 over its two rows, an odd last row paired with itself), U = (112 B - 74 G - 38 R + 0x8080) >> 8, V = (112 R - 94 G -
  *      18 B + 0x8080) >> 8. An encoder fed these frames must signal BT.601 limited range.
+ * P010 out (BT.601 limited range as well; no libyuv 1744 row writes 10-bit YUV, so this is the engine's own definition):
+ *   1. M10: each component clamp(rint(4 * (v * scale + offset)), 0, 1023), the product and the sum each rounded on its own; the
+ *      1-, 3- and 4-channel rules of step 1. The same scale and offset as for 8-bit output.
+ *   2. F10 = ImageTexture::resize of M10, blended and rounded as step 2.
+ *   3. Y10 = (66 R + 129 G + 25 B + 0x4080) >> 8; chroma averages the 2 x 2 block as step 3, then U10 = (112 B - 74 G - 38 R + 0x20080)
+ *      >> 8, V10 = (112 R - 94 G - 18 B + 0x20080) >> 8 (the 8-bit coefficients with offsets 64 and 512; within [64, 960] unclamped).
+ *   4. Each value is stored as the word value << 6.
  * Bytes of a plane outside its rows (pitch padding, gaps between planes and images) are not written. `out` may alias `frames` (an
  * in-place filter of a decoder surface): the output is written after the forward pass, in stream order. */
 typedef struct {
-    int format;                 /* SNNB_FRAME_*; the YUV formats are BT.601 limited range */
+    int format;                 /* SNNB_FRAME_*; the YUV formats (P010 included) are BT.601 limited range */
     int width, height;          /* any >= 1 (odd allowed: chroma is ceil(w/2) x ceil(h/2), as libyuv) */
-    uint8_t* plane[3];          /* NV12/NV21: Y, UV|VU; I420: Y, U, V; RGBA8: RGBA. Device memory of the model's device */
-    int pitch[3];               /* bytes per row, >= the row's bytes */
+    uint8_t* plane[3];          /* NV12/NV21/P010: Y, UV|VU; I420: Y, U, V; RGBA8: RGBA. Device memory of the model's device */
+    int pitch[3];               /* bytes per row, >= the row's bytes (P010: even, as the image strides, planes 2-byte aligned) */
     long long image_stride[3];  /* bytes from image n to image n+1, per plane */
     int linear_filter;          /* resize filter, as snnb_image_io */
     float scale, offset;        /* model output -> 8 bits, exactly as the U8 output of snnb_model_run_device */
@@ -340,7 +370,11 @@ int snnb_model_transform_frames(snnb_model* m, const snnb_frames* frames, const 
  *   3. Chroma: U and V each ImageTexture::resize of the source's U and V plane, plane to plane, from ceil(W/2) x ceil(H/2) to
  *      ceil(width/2) x ceil(height/2), with out.linear_filter and the same taps, blend and rint as step 2 (a copy at equal chroma sizes).
  *      Resizing the planes on their own, as libyuv's I420Scale does, keeps each sample sited at the centre of its 2 x 2 block.
- * frames.format and out.format are NV12, NV21 or I420 and may differ; RGBA8 is refused on either side. Bytes of a plane outside its rows
+ * P010 (from and to P010 only): the model input is the 10-bit Y plane as snnb_frames describes; Y10 comes from M10 as
+ * snnb_model_transform_frames' P010 steps 1-2 (1 channel); U10 and V10 are the source's resized plane to plane as step 3, and every
+ * value is stored as value << 6.
+ * frames.format and out.format are NV12, NV21, I420 or P010; the 8-bit formats may differ, but P010 pairs with P010 only (a mix of bit
+ * depths is refused). RGBA8 is refused on either side. Bytes of a plane outside its rows
  * (pitch padding, gaps between planes and images) are not written. Aliasing: the Y plane is written after the forward pass, but the
  * output kernel reads the source chroma while it writes. So `out` may be `frames` itself (same format, size, planes, pitches and image
  * strides: an in-place luma filter); otherwise no out plane may overlap a source chroma plane. Checked on the host before anything is
@@ -352,7 +386,7 @@ int snnb_model_transform_luma(snnb_model* m, const snnb_frames* frames, const sn
 /* Segmentation models (U-Net, a per-pixel classifier) from device frames to an 8-bit label plane of any size: the class scores of
  * output 0 are resampled to the plane and reduced to one byte per pixel in the same kernel, so neither the upsampled scores nor an
  * arg-max pass ever reach memory. The input is exactly what snnb_model_run_frames feeds (luma == 0), or exactly what
- * snnb_model_transform_luma feeds (luma == 1: the Y plane of NV12 / NV21 / I420 frames into a model input of 1 channel, for grey-input
+ * snnb_model_transform_luma feeds (luma == 1: the Y plane of NV12 / NV21 / I420 / P010 frames into a model input of 1 channel, for grey-input
  * models such as the reference's U-Net). Let T be output 0 (N x h x w x C) with values v = float(hi) + float(lo) (lo absent in FP16
  * storage): bit for bit the F32 output of snnb_model_run_device / snnb_model_run_frames. For label pixel (x, y) of image n:
  *   1. Scores s_c: T[n, y, x, c] when the plane has the output's size; otherwise the taps of ImageTexture::resize of T to width x

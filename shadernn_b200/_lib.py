@@ -78,8 +78,8 @@ class DeviceBuffer(C.Structure):
     ]
 
 
-FRAME_NV12, FRAME_NV21, FRAME_I420, FRAME_RGBA8 = 0, 1, 2, 3
-YUV_BT601, YUV_BT709 = 0, 1
+FRAME_NV12, FRAME_NV21, FRAME_I420, FRAME_RGBA8, FRAME_P010 = 0, 1, 2, 3, 16
+YUV_BT601, YUV_BT709, YUV_BT2020, YUV_FULL_RANGE = 0, 1, 9, 0x100
 
 
 class Frames(C.Structure):

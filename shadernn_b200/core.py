@@ -549,12 +549,14 @@ class MixedInferenceCore:
               "snnb_model_detect_device")
         return rows, counts
 
-    _FRAME_FORMATS = {"nv12": _lib.FRAME_NV12, "nv21": _lib.FRAME_NV21, "i420": _lib.FRAME_I420, "rgba8": _lib.FRAME_RGBA8}
-    _YUV_MATRICES = {"bt601": _lib.YUV_BT601, "bt709": _lib.YUV_BT709}
+    _FRAME_FORMATS = {"nv12": _lib.FRAME_NV12, "nv21": _lib.FRAME_NV21, "i420": _lib.FRAME_I420, "rgba8": _lib.FRAME_RGBA8, "p010": _lib.FRAME_P010}
+    _YUV_MATRICES = {"bt601": _lib.YUV_BT601, "bt709": _lib.YUV_BT709, "bt2020": _lib.YUV_BT2020, "jpeg": _lib.YUV_BT601 | _lib.YUV_FULL_RANGE}
 
     def _frames(self, who, frames, format, matrix, linear, mean4, norm4):
         """The snnb_frames descriptor of a uint8 CUDA tensor: NV12 / NV21 / I420 as [N, H * 3 // 2, W] (the packed 4:2:0 layout, H and W
-        even; NV12 / NV21 rows may be pitched, I420 rows must be dense), RGBA8 as [N, H, W, 4] (rows may be pitched). N is the batch."""
+        even; NV12 / NV21 rows may be pitched, I420 rows must be dense), RGBA8 as [N, H, W, 4] (rows may be pitched). P010 takes a
+        uint16 or int16 CUDA tensor in NV12's layout counted in 16-bit samples (rows may be pitched). N is the batch. matrix: "bt601",
+        "bt709", "bt2020" or "jpeg" (full-range BT.601)."""
         f, n = self._frames_any(who, frames, format, matrix, linear, mean4, norm4)
         if n != self.batch:
             raise ValueError("%s: %d frames given, the model's batch is %d" % (who, n, self.batch))
@@ -573,19 +575,24 @@ class MixedInferenceCore:
 
     @staticmethod
     def _frame_planes(who, what, frames, format, f):
-        """The size, planes, pitches and image strides of an snnb_frames / snnb_frames_out `f` from a uint8 CUDA tensor in the layouts
-        of _frames; returns the number of frames."""
+        """The size, planes, pitches and image strides (in bytes) of an snnb_frames / snnb_frames_out `f` from a CUDA tensor in the
+        layouts of _frames; returns the number of frames."""
         import torch
-        if not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
+        if format == "p010":
+            if not isinstance(frames, torch.Tensor) or frames.dtype not in (torch.uint16, torch.int16):
+                raise ValueError("%s: p010 %s must be a uint16 or int16 CUDA tensor" % (who, what))
+        elif not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8:
             raise ValueError("%s: %s must be a uint8 CUDA tensor" % (who, what))
-        shape, st, base = tuple(frames.shape), frames.stride(), frames.data_ptr()
+        shape, base = tuple(frames.shape), frames.data_ptr()
+        st = tuple(s * frames.element_size() for s in frames.stride())  # bytes; a P010 row's samples are 2 bytes apart
+        dense = frames.stride()[-1] == 1
         if format == "rgba8":
-            if len(shape) != 4 or shape[3] != 4 or st[3] != 1 or st[2] != 4:
+            if len(shape) != 4 or shape[3] != 4 or not dense or st[2] != 4:
                 raise ValueError("%s: rgba8 %s are [N, H, W, 4] with dense pixels; got shape %s, strides %s" % (who, what, shape, st))
             n, f.height, f.width = shape[0], shape[1], shape[2]
             f.plane[0], f.pitch[0], f.image_stride[0] = base, st[1], st[0]
         else:
-            if len(shape) != 3 or shape[1] % 3 or shape[1] < 3 or shape[2] % 2 or st[2] != 1:
+            if len(shape) != 3 or shape[1] % 3 or shape[1] < 3 or shape[2] % 2 or not dense:
                 raise ValueError("%s: %s %s are [N, H * 3 // 2, W] with H and W even and dense rows; got shape %s, strides %s" % (who, format, what, shape, st))
             n, f.height, f.width = shape[0], shape[1] // 3 * 2, shape[2]
             pitch = st[1]
@@ -601,8 +608,8 @@ class MixedInferenceCore:
 
     def run_frames(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_dtype=None, out_layout="nhwc", out_scale=1.0,
                    out_offset=0.0, want_classes=False):
-        """snnb_model_run_frames: a batch of 8-bit video frames of any size on the GPU (NV12, NV21, I420 or RGBA8, see _frames) converted
-        to RGBA8 exactly as libyuv does, resized to the model input (linear or nearest, as run_image), normalised as
+        """snnb_model_run_frames: a batch of video frames of any size on the GPU (NV12, NV21, I420, RGBA8 or 10-bit P010, see _frames)
+        converted to RGBA exactly as libyuv does (P010: its 10-bit rows, as R10 / 4), resized to the model input (linear or nearest, as run_image), normalised as
         (x - mean4[c]) * norm4[c] (default mean 0, norm 1) and run, ordered on the current torch stream and never synchronising.
         Model channel c is RGBA component c. Outputs and classes as run_torch."""
         outs, obufs, classes = self._device_outputs("run_frames", out_dtype, out_layout, out_scale, out_offset, want_classes)
@@ -663,7 +670,8 @@ class MixedInferenceCore:
             if out_format != "rgba8" and (oh % 2 or ow % 2):
                 raise ValueError("transform_frames: %s frames of %d x %d: the packed layout needs H and W even" % (out_format, oh, ow))
             shape = (self.batch, oh, ow, 4) if out_format == "rgba8" else (self.batch, oh * 3 // 2, ow)
-            out = torch.empty(shape, dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+            dtype = torch.uint16 if out_format == "p010" else torch.uint8
+            out = torch.empty(shape, dtype=dtype, device=torch.device("cuda", self.ctx.device))
         o = _lib.FramesOut()
         o.format, o.linear_filter, o.scale, o.offset = self._FRAME_FORMATS[out_format], int(bool(out_linear)), float(out_scale), float(out_offset)
         n = self._frame_planes("transform_frames", "out frames", out, out_format, o)
@@ -685,7 +693,9 @@ class MixedInferenceCore:
         back in the decoder's range.
 
         out_format defaults to `format` and out_hw to the input frames' size. Returns `out`, a uint8 CUDA tensor [N, H * 3 // 2, W] in
-        _frames' layouts, allocated here unless given; it may be `frames` itself (same format and size), for an in-place filter."""
+        _frames' layouts (uint16 for P010), allocated here unless given; it may be `frames` itself (same format and size), for an in-place
+        filter. P010 frames are written from P010 frames only: the Y10 / 4 texels feed the model, so the same mean, norm, out_scale and
+        out_offset apply."""
         import torch
         out_format = format if out_format is None else out_format
         if format not in self._FRAME_FORMATS or out_format not in self._FRAME_FORMATS:
@@ -697,7 +707,8 @@ class MixedInferenceCore:
                 raise ValueError("transform_luma: out_format 'rgba8' has no Y plane; expected nv12, nv21 or i420")
             if oh % 2 or ow % 2:
                 raise ValueError("transform_luma: %s frames of %d x %d: the packed layout needs H and W even" % (out_format, oh, ow))
-            out = torch.empty((self.batch, oh * 3 // 2, ow), dtype=torch.uint8, device=torch.device("cuda", self.ctx.device))
+            dtype = torch.uint16 if out_format == "p010" else torch.uint8
+            out = torch.empty((self.batch, oh * 3 // 2, ow), dtype=dtype, device=torch.device("cuda", self.ctx.device))
         o = _lib.FramesOut()
         o.format, o.linear_filter, o.scale, o.offset = self._FRAME_FORMATS[out_format], int(bool(out_linear)), float(out_scale), float(out_offset)
         n = self._frame_planes("transform_luma", "out frames", out, out_format, o)

@@ -649,8 +649,8 @@ static int checkDeviceBuffer(const char* api, const snnb_device_buffer& b, int d
     return checkDevicePointer(api, b.data, elem, device, what, idx);
 }
 
-// The row bytes of plane p of `width`-pixel frames (NV12 / NV21 rows of ceil(w/2) UV pairs, I420 rows of ceil(w/2) samples), 0 for an
-// unused plane.
+// The row bytes of plane p of `width`-pixel frames (NV12 / NV21 rows of ceil(w/2) UV pairs, I420 rows of ceil(w/2) samples, P010 the
+// NV12 rows in 16-bit samples), 0 for an unused plane.
 static long long frameRowBytes(int format, int width, int p) {
     const long long cw = (width + 1) / 2;
     switch (format) {
@@ -658,6 +658,24 @@ static long long frameRowBytes(int format, int width, int p) {
     case SNNB_FRAME_NV21: return p == 0 ? width : (p == 1 ? 2 * cw : 0);
     case SNNB_FRAME_I420: return p == 0 ? width : cw;
     case SNNB_FRAME_RGBA8: return p == 0 ? 4LL * width : 0;
+    case SNNB_FRAME_P010: return p == 0 ? 2LL * width : (p == 1 ? 4 * cw : 0);
+    }
+    return 0;
+}
+static bool knownFrameFormat(int format) { return (format >= SNNB_FRAME_NV12 && format <= SNNB_FRAME_RGBA8) || format == SNNB_FRAME_P010; }
+
+// The planes of frames in `format`: each pitch at least its row's bytes, each plane device or managed memory of `device`; P010's
+// 16-bit samples also need even pitches and image strides and 2-byte-aligned planes.
+static int checkFramePlanes(const char* api, const char* what, int format, int width, const uint8_t* const plane[3], const int pitch[3],
+                            const long long stride[3], int device) {
+    const bool p010 = format == SNNB_FRAME_P010;
+    for (int p = 0; p < 3; ++p) {
+        const long long row = frameRowBytes(format, width, p);
+        if (!row) continue;
+        SNNB_REQUIRE(pitch[p] >= row, "%s: %s %d: pitch %d is less than its row's %lld bytes", api, what, p, pitch[p], row);
+        SNNB_REQUIRE(!p010 || (pitch[p] % 2 == 0 && stride[p] % 2 == 0), "%s: %s %d: P010 pitch %d and image stride %lld must be even", api, what, p, pitch[p],
+                     stride[p]);
+        if (int rc = checkDevicePointer(api, plane[p], p010 ? 2 : 1, device, what, p)) return rc;
     }
     return 0;
 }
@@ -677,22 +695,21 @@ static int checkCallerStream(const char* api, cudaStream_t stream) {
 int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, cudaStream_t stream) {
     if (in.frames) {
         const snnb_frames& f = *in.frames;
-        SNNB_REQUIRE(f.format >= SNNB_FRAME_NV12 && f.format <= SNNB_FRAME_RGBA8, "%s: unknown frame format %d", api, f.format);
-        SNNB_REQUIRE(f.format == SNNB_FRAME_RGBA8 || f.matrix == SNNB_YUV_BT601 || f.matrix == SNNB_YUV_BT709, "%s: unknown YUV matrix %d", api, f.matrix);
+        SNNB_REQUIRE(knownFrameFormat(f.format), "%s: unknown frame format %d", api, f.format);
+        if (f.format != SNNB_FRAME_RGBA8) {
+            const int base = f.matrix & ~SNNB_YUV_FULL_RANGE;
+            SNNB_REQUIRE(base == SNNB_YUV_BT601 || base == SNNB_YUV_BT709 || base == SNNB_YUV_BT2020, "%s: unknown YUV matrix %d", api, f.matrix);
+            SNNB_REQUIRE(base == SNNB_YUV_BT601 || !(f.matrix & SNNB_YUV_FULL_RANGE), "%s: YUV matrix %d: full range is defined for BT.601 only", api, f.matrix);
+        }
         SNNB_REQUIRE(f.width >= 1 && f.height >= 1, "%s: frame size %d x %d; width and height must be >= 1", api, f.width, f.height);
         SNNB_REQUIRE(inputLayers.size() == 1, "%s: the model has %d inputs; frames feed a model with exactly one", api, (int) inputLayers.size());
         const snnb_tensor* t = inputLayers[0]->output;
         SNNB_REQUIRE(t->c >= 1 && t->c <= 4, "%s: the model input has %d channels; frames feed 1 to 4 (RGBA components)", api, t->c);
         if (in.luma) {
-            SNNB_REQUIRE(f.format != SNNB_FRAME_RGBA8, "%s: RGBA8 frames have no Y plane; luma input takes NV12, NV21 or I420 frames", api);
+            SNNB_REQUIRE(f.format != SNNB_FRAME_RGBA8, "%s: RGBA8 frames have no Y plane; luma input takes NV12, NV21, I420 or P010 frames", api);
             SNNB_REQUIRE(t->c == 1, "%s: the model input has %d channels; the Y plane feeds exactly 1", api, t->c);
         }
-        for (int p = 0; p < 3; ++p) {
-            const long long row = frameRowBytes(f.format, f.width, p);
-            if (!row) continue;
-            SNNB_REQUIRE(f.pitch[p] >= row, "%s: plane %d: pitch %d is less than its row's %lld bytes", api, p, f.pitch[p], row);
-            if (int rc = checkDevicePointer(api, f.plane[p], 1, ctx->device, "plane", p)) return rc;
-        }
+        if (int rc = checkFramePlanes(api, "plane", f.format, f.width, f.plane, f.pitch, f.image_stride, ctx->device)) return rc;
         if (in.rois) {
             SNNB_REQUIRE(in.numFrames >= 1, "%s: num_frames %d; at least one frame is required", api, in.numFrames);
             SNNB_REQUIRE(options.batch <= 65535, "%s: batch %u; regions fill at most 65535 slots", api, options.batch);
@@ -837,14 +854,9 @@ int MixedInferenceCore::transformFrames(const snnb_frames* frames, const snnb_fr
     in.frames = frames;
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
     const snnb_frames_out& o = *out;
-    SNNB_REQUIRE(o.format >= SNNB_FRAME_NV12 && o.format <= SNNB_FRAME_RGBA8, "%s: unknown out frame format %d", api, o.format);
+    SNNB_REQUIRE(knownFrameFormat(o.format), "%s: unknown out frame format %d", api, o.format);
     SNNB_REQUIRE(o.width >= 1 && o.height >= 1, "%s: out frame size %d x %d; width and height must be >= 1", api, o.width, o.height);
-    for (int p = 0; p < 3; ++p) {
-        const long long row = frameRowBytes(o.format, o.width, p);
-        if (!row) continue;
-        SNNB_REQUIRE(o.pitch[p] >= row, "%s: out plane %d: pitch %d is less than its row's %lld bytes", api, p, o.pitch[p], row);
-        if (int rc = checkDevicePointer(api, o.plane[p], 1, ctx->device, "out plane", p)) return rc;
-    }
+    if (int rc = checkFramePlanes(api, "out plane", o.format, o.width, o.plane, o.pitch, o.image_stride, ctx->device)) return rc;
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; frames are written from an image output", api);
     const snnb_tensor* t = outputLayers[0]->output;
     SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
@@ -878,15 +890,12 @@ int MixedInferenceCore::transformLuma(const snnb_frames* frames, const snnb_fram
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
     const snnb_frames& f     = *frames;
     const snnb_frames_out& o = *out;
-    SNNB_REQUIRE(o.format >= SNNB_FRAME_NV12 && o.format <= SNNB_FRAME_RGBA8, "%s: unknown out frame format %d", api, o.format);
-    SNNB_REQUIRE(o.format != SNNB_FRAME_RGBA8, "%s: out format RGBA8 has no Y plane; luma frames are written as NV12, NV21 or I420", api);
+    SNNB_REQUIRE(knownFrameFormat(o.format), "%s: unknown out frame format %d", api, o.format);
+    SNNB_REQUIRE(o.format != SNNB_FRAME_RGBA8, "%s: out format RGBA8 has no Y plane; luma frames are written as NV12, NV21, I420 or P010", api);
+    SNNB_REQUIRE((o.format == SNNB_FRAME_P010) == (f.format == SNNB_FRAME_P010),
+                 "%s: frames format %d, out format %d: the bit depths differ; P010 frames are written from P010 frames only", api, f.format, o.format);
     SNNB_REQUIRE(o.width >= 1 && o.height >= 1, "%s: out frame size %d x %d; width and height must be >= 1", api, o.width, o.height);
-    for (int p = 0; p < 3; ++p) {
-        const long long row = frameRowBytes(o.format, o.width, p);
-        if (!row) continue;
-        SNNB_REQUIRE(o.pitch[p] >= row, "%s: out plane %d: pitch %d is less than its row's %lld bytes", api, p, o.pitch[p], row);
-        if (int rc = checkDevicePointer(api, o.plane[p], 1, ctx->device, "out plane", p)) return rc;
-    }
+    if (int rc = checkFramePlanes(api, "out plane", o.format, o.width, o.plane, o.pitch, o.image_stride, ctx->device)) return rc;
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; frames are written from an image output", api);
     const snnb_tensor* t = outputLayers[0]->output;
     SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());

@@ -1355,6 +1355,12 @@ struct ResizeTaps {
         return top + ay * (bot - top);
     }
 };
+// ResizeTaps::blend with every + - * rounded on its own: nothing is contracted into an FMA, so numpy float32 restates it exactly.
+__device__ __forceinline__ float blend_rn(const ResizeTaps& r, float p00, float p01, float p10, float p11) {
+    const float top = __fadd_rn(p00, __fmul_rn(r.ax, __fsub_rn(p01, p00)));
+    const float bot = __fadd_rn(p10, __fmul_rn(r.ax, __fsub_rn(p11, p10)));
+    return __fadd_rn(top, __fmul_rn(r.ay, __fsub_rn(bot, top)));
+}
 // The source position of output pixel (ox, oy), then its taps.
 __device__ __forceinline__ float2 resize_pos(int ox, int oy, int W, int H, int sw, int sh) {
     return make_float2(((float) ox + 0.5f) / (float) W * (float) sw, ((float) oy + 0.5f) / (float) H * (float) sh);
@@ -1584,11 +1590,33 @@ struct FrameV {
 // Not a public format: the Y plane (plane 0) of NV12 / NV21 / I420 frames as a 1-channel 8-bit image (snnb_model_transform_luma). Every
 // component of its texel is the Y byte, so the model input is resize_u8_kernel's / split_u8_kernel's of that image.
 constexpr int FRAME_LUMA = -1;
-// RGBA8 of source pixel (x, y) of image n; pixel (x, y) takes chroma sample (x / 2, y / 2) (NV12ToARGBRow_C, row_common.cc:1945-1967)
+// Not a public format either: the Y plane of P010 frames, every component Y10 * 0.25 (the 10-bit sample in 8-bit units).
+constexpr int FRAME_LUMA10 = -2;
+// The 10-bit formats: their texels are exact multiples of 0.25 and are blended with blend_rn (restatable bit for bit in float32)
+__host__ __device__ constexpr bool frame_10bit(int fmt) { return fmt == SNNB_FRAME_P010 || fmt == FRAME_LUMA10; }
+// The 10-bit value of the 16-bit little-endian P010 sample at byte address p: the word's top 10 bits (P016's low 6 bits are ignored)
+__device__ __forceinline__ int p010_sample(const uint8_t* p) { return __ldg(reinterpret_cast<const uint16_t*>(p)) >> 6; }
+// RGBA8 of source pixel (x, y) of image n; pixel (x, y) takes chroma sample (x / 2, y / 2) (NV12ToARGBRow_C, row_common.cc:1945-1967).
+// P010: libyuv's YuvPixel16 (Y with 10 bits, U and V truncated to 8) and StoreAR30's Clamp10(c >> 4), as R10 * 0.25, alpha 255.
 template <int FMT>
 __device__ __forceinline__ void frame_texel(const FrameV& s, int n, int x, int y, float rgba[4]) {
     if (FMT == FRAME_LUMA) {
         rgba[0] = rgba[1] = rgba[2] = rgba[3] = (float) __ldg(s.plane[0] + n * s.stride[0] + (size_t) y * s.pitch[0] + x);
+        return;
+    }
+    if (FMT == FRAME_LUMA10) {
+        rgba[0] = rgba[1] = rgba[2] = rgba[3] = (float) p010_sample(s.plane[0] + n * s.stride[0] + (size_t) y * s.pitch[0] + (size_t) x * 2) * 0.25f;
+        return;
+    }
+    if (FMT == SNNB_FRAME_P010) {
+        const int Y      = p010_sample(s.plane[0] + n * s.stride[0] + (size_t) y * s.pitch[0] + (size_t) x * 2);
+        const uint8_t* c = s.plane[1] + n * s.stride[1] + (size_t) (y >> 1) * s.pitch[1] + (size_t) (x >> 1) * 4;
+        const int U = p010_sample(c) >> 2, V = p010_sample(c + 2) >> 2;
+        const int y1 = (int) ((uint32_t) ((Y << 6) * s.yg) >> 16);
+        rgba[0] = (float) min(max((-(V * s.vr) + y1 + s.br) >> 4, 0), 1023) * 0.25f;
+        rgba[1] = (float) min(max((-(U * s.ug + V * s.vg) + y1 + s.bg) >> 4, 0), 1023) * 0.25f;
+        rgba[2] = (float) min(max((-(U * s.ub) + y1 + s.bb) >> 4, 0), 1023) * 0.25f;
+        rgba[3] = 255.0f;
         return;
     }
     if (FMT == SNNB_FRAME_RGBA8) {
@@ -1615,7 +1643,7 @@ __device__ __forceinline__ void frame_texel(const FrameV& s, int n, int x, int y
 }
 // The model input of one pixel (C <= 4: one 8-channel group) from its taps `r` in image n of the frames: each tap as libyuv's RGBA8,
 // then resize_u8_kernel's blend (linear, unless the source is sampled directly) and normalisation. Shared by frame_input_kernel and
-// frame_roi_input_kernel.
+// frame_roi_input_kernel. The 10-bit formats blend with blend_rn instead, so that their model input is restatable in float32.
 template <int FMT>
 __device__ __forceinline__ void frame_pixel(const FrameV& s, int n, const ResizeTaps& r, int linear, bool direct, const TV& t, const U8Norm& q, float v[8]) {
     float p00[4];
@@ -1625,6 +1653,12 @@ __device__ __forceinline__ void frame_pixel(const FrameV& s, int n, const Resize
         frame_texel<FMT>(s, n, r.x1, r.y0, p01);
         frame_texel<FMT>(s, n, r.x0, r.y1, p10);
         frame_texel<FMT>(s, n, r.x1, r.y1, p11);
+        if constexpr (frame_10bit(FMT)) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+                v[j] = (j < t.C) ? __fmul_rn(__fsub_rn(blend_rn(r, p00[j & 3], p01[j & 3], p10[j & 3], p11[j & 3]), q.mean[j & 3]), q.norm[j & 3]) : 0.0f;
+            return;
+        }
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = (j < t.C) ? (r.blend(p00[j & 3], p01[j & 3], p10[j & 3], p11[j & 3]) - q.mean[j & 3]) * q.norm[j & 3] : 0.0f;
     } else {
@@ -1655,9 +1689,11 @@ __global__ void __launch_bounds__(256) frame_input_kernel(FrameV s, TV t, U8Norm
 }
 // The kernel-side view of an snnb_frames: planes, size and libyuv's constants of its matrix; and its mean / norm
 static FrameV frame_view(const snnb_frames& fr) {
-    // libyuv row_common.cc:1115-1358: YG, YGB, UB, UG, VG, VR of BT.601 (kYuvI601Constants) and BT.709 (kYuvH709Constants)
-    static const int M[2][6] = {{18997, -1160, -128, 25, 52, -102}, {18997, -1160, -128, 14, 34, -115}};
-    const int* m = M[fr.matrix == SNNB_YUV_BT709 ? 1 : 0];
+    // libyuv row_common.cc:1115-1420: YG, YGB, UB, UG, VG, VR of BT.601 (kYuvI601Constants), BT.709 (kYuvH709Constants), BT.2020
+    // (kYuv2020Constants) and full-range BT.601 (kYuvJPEGConstants). The biases UB * 128 + YGB etc. are libyuv's for all four.
+    static const int M[4][6] = {
+        {18997, -1160, -128, 25, 52, -102}, {18997, -1160, -128, 14, 34, -115}, {19003, -1160, -128, 12, 42, -107}, {16320, 32, -113, 22, 46, -90}};
+    const int* m = M[fr.matrix == SNNB_YUV_BT709 ? 1 : (fr.matrix == SNNB_YUV_BT2020 ? 2 : (fr.matrix == (SNNB_YUV_BT601 | SNNB_YUV_FULL_RANGE) ? 3 : 0))];
     FrameV s;
     for (int i = 0; i < 3; ++i) s.plane[i] = fr.plane[i], s.pitch[i] = fr.pitch[i], s.stride[i] = fr.image_stride[i];
     s.w = fr.width, s.h = fr.height;
@@ -1679,6 +1715,8 @@ int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t,
     if (luma) {
         SNNB_REQUIRE(t->c == 1 && fr.format != SNNB_FRAME_RGBA8, "launch_frame_input: luma input feeds 1 channel from YUV frames (%d channels, format %d)", t->c,
                      fr.format);
+        if (fr.format == SNNB_FRAME_P010)
+            return launch_done(ctx, launch_k(frame_input_kernel<FRAME_LUMA10>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<luma10>");
         return launch_done(ctx, launch_k(frame_input_kernel<FRAME_LUMA>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<luma>");
     }
     switch (fr.format) {
@@ -1690,6 +1728,8 @@ int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t,
         return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<i420>");
     case SNNB_FRAME_RGBA8:
         return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<rgba8>");
+    case SNNB_FRAME_P010:
+        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<p010>");
     }
     SNNB_REQUIRE(false, "launch_frame_input: unknown format %d", fr.format);
 }
@@ -1750,6 +1790,8 @@ int launch_frame_roi_input(snnb_context* ctx, const snnb_frames& fr, int num_fra
         return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<i420>");
     case SNNB_FRAME_RGBA8:
         return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<rgba8>");
+    case SNNB_FRAME_P010:
+        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<p010>");
     }
     SNNB_REQUIRE(false, "launch_frame_roi_input: unknown format %d", fr.format);
 }
@@ -1852,37 +1894,44 @@ struct FrameOutV {
     int w, h;
     float scale, offset;
 };
-// ResizeTaps::blend with every + - * rounded on its own: nothing is contracted into an FMA, so numpy float32 restates it exactly.
-__device__ __forceinline__ float blend_rn(const ResizeTaps& r, float p00, float p01, float p10, float p11) {
-    const float top = __fadd_rn(p00, __fmul_rn(r.ax, __fsub_rn(p01, p00)));
-    const float bot = __fadd_rn(p10, __fmul_rn(r.ax, __fsub_rn(p11, p10)));
-    return __fadd_rn(top, __fmul_rn(r.ay, __fsub_rn(bot, top)));
+// A model output value as 10 bits (P010 output): clamp(rint(4 * (v * scale + offset)), 0, 1023), the product and the sum each rounded
+// on its own, so that numpy float32 restates it exactly. The same scale and offset as for 8-bit output give the same range.
+__device__ __forceinline__ float quant10(float v, float scale, float offset) {
+    return fminf(fmaxf(rintf(4.0f * __fadd_rn(__fmul_rn(v, scale), offset)), 0.0f), 1023.0f);
 }
-// Texel (x, y) of image n of M: C = 4 RGBA, C = 3 RGB + alpha 255, C = 1 grey (R = G = B) + alpha 255
+template <bool TEN>
+__device__ __forceinline__ float quant_out(float v, float scale, float offset) {
+    if constexpr (TEN) return quant10(v, scale, offset);
+    else return quant_u8(v, scale, offset);
+}
+// Texel (x, y) of image n of M: C = 4 RGBA, C = 3 RGB + alpha 255, C = 1 grey (R = G = B) + alpha 255. TEN: 10-bit components (M10).
+template <bool TEN>
 __device__ __forceinline__ void out_texel(const TV& t, int n, int x, int y, float scale, float offset, float rgba[4]) {
     float v[8];
     load8(t.hi, t.lo, (((size_t) n * t.H + y) * t.W + x) * t.Cp, v);
     if (t.C == 1) {
-        rgba[0] = rgba[1] = rgba[2] = quant_u8(v[0], scale, offset);
+        rgba[0] = rgba[1] = rgba[2] = quant_out<TEN>(v[0], scale, offset);
     } else {
 #pragma unroll
-        for (int c = 0; c < 3; ++c) rgba[c] = quant_u8(v[c], scale, offset);
+        for (int c = 0; c < 3; ++c) rgba[c] = quant_out<TEN>(v[c], scale, offset);
     }
-    rgba[3] = t.C == 4 ? quant_u8(v[3], scale, offset) : 255.0f;
+    rgba[3] = t.C == 4 ? quant_out<TEN>(v[3], scale, offset) : 255.0f;
 }
-// Pixel (x, y) of image n of the frame-size RGBA8 image F. A frame of the output's size takes M as it is.
+// Pixel (x, y) of image n of the frame-size RGBA8 image F (TEN: its 10-bit counterpart from M10). A frame of the output's size takes M
+// as it is.
+template <bool TEN>
 __device__ __forceinline__ void frame_out_pixel(const TV& t, const FrameOutV& o, int n, int x, int y, int linear, int rgba[4]) {
     const bool direct = o.w == t.W && o.h == t.H;
     ResizeTaps r;
     if (direct) r.x0 = r.x1 = x, r.y0 = r.y1 = y, r.ax = r.ay = 0.0f;
     else r = resize_taps(resize_pos(x, y, o.w, o.h, t.W, t.H), t.W, t.H, linear);
     float p00[4];
-    out_texel(t, n, r.x0, r.y0, o.scale, o.offset, p00);
+    out_texel<TEN>(t, n, r.x0, r.y0, o.scale, o.offset, p00);
     if (linear && !direct) {
         float p01[4], p10[4], p11[4];
-        out_texel(t, n, r.x1, r.y0, o.scale, o.offset, p01);
-        out_texel(t, n, r.x0, r.y1, o.scale, o.offset, p10);
-        out_texel(t, n, r.x1, r.y1, o.scale, o.offset, p11);
+        out_texel<TEN>(t, n, r.x1, r.y0, o.scale, o.offset, p01);
+        out_texel<TEN>(t, n, r.x0, r.y1, o.scale, o.offset, p10);
+        out_texel<TEN>(t, n, r.x1, r.y1, o.scale, o.offset, p11);
 #pragma unroll
         for (int c = 0; c < 4; ++c) rgba[c] = (int) rintf(blend_rn(r, p00[c], p01[c], p10[c], p11[c]));
     } else {
@@ -1895,10 +1944,17 @@ __device__ __forceinline__ void store_2u8(uint8_t* p, int a, int b) {
     if ((reinterpret_cast<uintptr_t>(p) & 1) == 0) *reinterpret_cast<uint16_t*>(p) = (uint16_t) (a | (b << 8));
     else p[0] = (uint8_t) a, p[1] = (uint8_t) b;
 }
+// Two 10-bit values at p as P010 words (value << 6, low 6 bits zero), in one store where p is 4-byte aligned (p is 2-byte aligned)
+__device__ __forceinline__ void store_2p010(uint8_t* p, int a, int b) {
+    if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) *reinterpret_cast<uint32_t*>(p) = (uint32_t) (a << 6) | ((uint32_t) (b << 6) << 16);
+    else reinterpret_cast<uint16_t*>(p)[0] = (uint16_t) (a << 6), reinterpret_cast<uint16_t*>(p)[1] = (uint16_t) (b << 6);
+}
 // One thread per 2 x 2 block of frame pixels, i.e. per chroma sample: its 4 pixels of F, then 4 Y bytes and the chroma sample (or
-// 4 RGBA8 pixels). Pixels past an odd width or height are not written.
+// 4 RGBA8 pixels). Pixels past an odd width or height are not written. P010: the same from M10, with the 8-bit coefficients and the
+// 10-bit offsets (64 and 512), stored as 16-bit words.
 template <int FMT>
 __global__ void __launch_bounds__(256) frame_output_kernel(TV t, FrameOutV o, int linear) {
+    constexpr bool TEN = FMT == SNNB_FRAME_P010;
     pdl_wait();
     const int cw = (o.w + 1) >> 1, ch = (o.h + 1) >> 1;
     const size_t total = (size_t) t.N * ch * cw;
@@ -1908,10 +1964,25 @@ __global__ void __launch_bounds__(256) frame_output_kernel(TV t, FrameOutV o, in
     const int x = 2 * bx, y = 2 * by;
     const bool has_x1 = x + 1 < o.w, has_y1 = y + 1 < o.h;
     int p[2][2][4];
-    frame_out_pixel(t, o, n, x, y, linear, p[0][0]);
-    if (has_x1) frame_out_pixel(t, o, n, x + 1, y, linear, p[0][1]);
-    if (has_y1) frame_out_pixel(t, o, n, x, y + 1, linear, p[1][0]);
-    if (has_x1 && has_y1) frame_out_pixel(t, o, n, x + 1, y + 1, linear, p[1][1]);
+    frame_out_pixel<TEN>(t, o, n, x, y, linear, p[0][0]);
+    if (has_x1) frame_out_pixel<TEN>(t, o, n, x + 1, y, linear, p[0][1]);
+    if (has_y1) frame_out_pixel<TEN>(t, o, n, x, y + 1, linear, p[1][0]);
+    if (has_x1 && has_y1) frame_out_pixel<TEN>(t, o, n, x + 1, y + 1, linear, p[1][1]);
+    if constexpr (TEN) {
+#pragma unroll
+        for (int dy = 0; dy < 2; ++dy) {
+            if (dy && !has_y1) break;
+            uint8_t* d = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + (size_t) x * 2;
+            const int* a = p[dy][0];
+            const int ya = (66 * a[0] + 129 * a[1] + 25 * a[2] + 0x4080) >> 8;
+            if (has_x1) {
+                const int* b = p[dy][1];
+                store_2p010(d, ya, (66 * b[0] + 129 * b[1] + 25 * b[2] + 0x4080) >> 8);
+            } else {
+                *reinterpret_cast<uint16_t*>(d) = (uint16_t) (ya << 6);
+            }
+        }
+    }
     if (FMT == SNNB_FRAME_RGBA8) {
 #pragma unroll
         for (int dy = 0; dy < 2; ++dy)
@@ -1925,17 +1996,19 @@ __global__ void __launch_bounds__(256) frame_output_kernel(TV t, FrameOutV o, in
             }
         return;
     }
+    if constexpr (!TEN) {
 #pragma unroll
-    for (int dy = 0; dy < 2; ++dy) {
-        if (dy && !has_y1) break;
-        uint8_t* d = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + x;
-        const int* a = p[dy][0];
-        const int ya = (66 * a[0] + 129 * a[1] + 25 * a[2] + 0x1080) >> 8;
-        if (has_x1) {
-            const int* b = p[dy][1];
-            store_2u8(d, ya, (66 * b[0] + 129 * b[1] + 25 * b[2] + 0x1080) >> 8);
-        } else {
-            d[0] = (uint8_t) ya;
+        for (int dy = 0; dy < 2; ++dy) {
+            if (dy && !has_y1) break;
+            uint8_t* d = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + x;
+            const int* a = p[dy][0];
+            const int ya = (66 * a[0] + 129 * a[1] + 25 * a[2] + 0x1080) >> 8;
+            if (has_x1) {
+                const int* b = p[dy][1];
+                store_2u8(d, ya, (66 * b[0] + 129 * b[1] + 25 * b[2] + 0x1080) >> 8);
+            } else {
+                d[0] = (uint8_t) ya;
+            }
         }
     }
     // libyuv pairs an odd last row with itself (ABGRToUVRow with stride 0) and averages an odd last column over its two rows
@@ -1950,8 +2023,11 @@ __global__ void __launch_bounds__(256) frame_output_kernel(TV t, FrameOutV o, in
             avg[c] = (a + cc) >> 1;
         }
     }
-    const int U = (112 * avg[2] - 74 * avg[1] - 38 * avg[0] + 0x8080) >> 8, V = (112 * avg[0] - 94 * avg[1] - 18 * avg[2] + 0x8080) >> 8;
-    if (FMT == SNNB_FRAME_I420) {
+    constexpr int COFF = TEN ? 0x20080 : 0x8080;
+    const int U = (112 * avg[2] - 74 * avg[1] - 38 * avg[0] + COFF) >> 8, V = (112 * avg[0] - 94 * avg[1] - 18 * avg[2] + COFF) >> 8;
+    if (TEN) {
+        store_2p010(o.plane[1] + n * o.stride[1] + (size_t) by * o.pitch[1] + (size_t) bx * 4, U, V);
+    } else if (FMT == SNNB_FRAME_I420) {
         o.plane[1][n * o.stride[1] + (size_t) by * o.pitch[1] + bx] = (uint8_t) U;
         o.plane[2][n * o.stride[2] + (size_t) by * o.pitch[2] + bx] = (uint8_t) V;
     } else {
@@ -1978,6 +2054,8 @@ int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_fram
         return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<i420>");
     case SNNB_FRAME_RGBA8:
         return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<rgba8>");
+    case SNNB_FRAME_P010:
+        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<p010>");
     }
     SNNB_REQUIRE(false, "launch_frame_output: unknown format %d", fr.format);
 }
@@ -1985,32 +2063,43 @@ int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_fram
 // A 1-channel model output 0 -> the Y plane of device video frames, with the source frames' chroma resampled beside it
 // (snnb_model_transform_luma). Y is frame_out_pixel's component 0 from one value per texel; U and V are ImageTexture::resize of the
 // source chroma planes, plane to plane, with the same taps and blend_rn.
-// Texel (x, y) of image n of M for a 1-channel output: its one value, quantised
+// Texel (x, y) of image n of M (TEN: M10) for a 1-channel output: its one value, quantised
+template <bool TEN>
 __device__ __forceinline__ float out_luma_texel(const TV& t, int n, int x, int y, float scale, float offset) {
     const size_t off = (((size_t) n * t.H + y) * t.W + x) * t.Cp;
     const float v    = __half2float(__ldg(t.hi + off)) + (t.lo ? __half2float(__ldg(t.lo + off)) : 0.0f); // = load8's component 0
-    return quant_u8(v, scale, offset);
+    return quant_out<TEN>(v, scale, offset);
 }
+template <bool TEN>
 __device__ __forceinline__ int luma_out_pixel(const TV& t, const FrameOutV& o, int n, int x, int y, int linear) {
     const bool direct = o.w == t.W && o.h == t.H;
     ResizeTaps r;
     if (direct) r.x0 = r.x1 = x, r.y0 = r.y1 = y, r.ax = r.ay = 0.0f;
     else r = resize_taps(resize_pos(x, y, o.w, o.h, t.W, t.H), t.W, t.H, linear);
-    const float p00 = out_luma_texel(t, n, r.x0, r.y0, o.scale, o.offset);
+    const float p00 = out_luma_texel<TEN>(t, n, r.x0, r.y0, o.scale, o.offset);
     if (!linear || direct) return (int) p00;
-    const float p01 = out_luma_texel(t, n, r.x1, r.y0, o.scale, o.offset), p10 = out_luma_texel(t, n, r.x0, r.y1, o.scale, o.offset);
-    const float p11 = out_luma_texel(t, n, r.x1, r.y1, o.scale, o.offset);
+    const float p01 = out_luma_texel<TEN>(t, n, r.x1, r.y0, o.scale, o.offset), p10 = out_luma_texel<TEN>(t, n, r.x0, r.y1, o.scale, o.offset);
+    const float p11 = out_luma_texel<TEN>(t, n, r.x1, r.y1, o.scale, o.offset);
     return (int) rintf(blend_rn(r, p00, p01, p10, p11));
 }
-// Chroma sample (x, y) of image n: U from plane 1, V from plane 2 of `s`, `step` bytes apart along a row (2 in an interleaved plane)
+// Chroma sample (x, y) of image n: U from plane 1, V from plane 2 of `s`, `step` samples apart along a row (2 in an interleaved plane).
+// TEN: 16-bit P010 samples, as their 10-bit values.
+template <bool TEN>
 __device__ __forceinline__ void chroma_texel(const FrameV& s, int step, int n, int x, int y, float& u, float& v) {
-    u = (float) __ldg(s.plane[1] + n * s.stride[1] + (size_t) y * s.pitch[1] + (size_t) x * step);
-    v = (float) __ldg(s.plane[2] + n * s.stride[2] + (size_t) y * s.pitch[2] + (size_t) x * step);
+    if constexpr (TEN) {
+        u = (float) p010_sample(s.plane[1] + n * s.stride[1] + (size_t) y * s.pitch[1] + (size_t) x * step * 2);
+        v = (float) p010_sample(s.plane[2] + n * s.stride[2] + (size_t) y * s.pitch[2] + (size_t) x * step * 2);
+    } else {
+        u = (float) __ldg(s.plane[1] + n * s.stride[1] + (size_t) y * s.pitch[1] + (size_t) x * step);
+        v = (float) __ldg(s.plane[2] + n * s.stride[2] + (size_t) y * s.pitch[2] + (size_t) x * step);
+    }
 }
 // One thread per 2 x 2 block of frame pixels, i.e. per chroma sample, as frame_output_kernel: 4 Y bytes, then the chroma sample resized
 // from the source's chroma planes. A chroma plane of the source's size is copied. Pixels past an odd width or height are not written.
+// P010 (from P010 frames): 10-bit Y from M10 and the source's 10-bit chroma, each stored as value << 6.
 template <int FMT>
 __global__ void __launch_bounds__(256) luma_output_kernel(TV t, FrameV s, int step, FrameOutV o, int linear) {
+    constexpr bool TEN = FMT == SNNB_FRAME_P010;
     pdl_wait();
     const int cw = (o.w + 1) >> 1, ch = (o.h + 1) >> 1;
     const size_t total = (size_t) t.N * ch * cw;
@@ -2022,10 +2111,17 @@ __global__ void __launch_bounds__(256) luma_output_kernel(TV t, FrameV s, int st
 #pragma unroll
     for (int dy = 0; dy < 2; ++dy) {
         if (dy && !has_y1) break;
-        uint8_t* d   = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + x;
-        const int ya = luma_out_pixel(t, o, n, x, y + dy, linear);
-        if (has_x1) store_2u8(d, ya, luma_out_pixel(t, o, n, x + 1, y + dy, linear));
-        else d[0] = (uint8_t) ya;
+        if constexpr (TEN) {
+            uint8_t* d   = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + (size_t) x * 2;
+            const int ya = luma_out_pixel<true>(t, o, n, x, y + dy, linear);
+            if (has_x1) store_2p010(d, ya, luma_out_pixel<true>(t, o, n, x + 1, y + dy, linear));
+            else *reinterpret_cast<uint16_t*>(d) = (uint16_t) (ya << 6);
+        } else {
+            uint8_t* d   = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + x;
+            const int ya = luma_out_pixel<false>(t, o, n, x, y + dy, linear);
+            if (has_x1) store_2u8(d, ya, luma_out_pixel<false>(t, o, n, x + 1, y + dy, linear));
+            else d[0] = (uint8_t) ya;
+        }
     }
     const int scw = (s.w + 1) >> 1, sch = (s.h + 1) >> 1;
     const bool direct = cw == scw && ch == sch;
@@ -2033,16 +2129,18 @@ __global__ void __launch_bounds__(256) luma_output_kernel(TV t, FrameV s, int st
     if (direct) r.x0 = r.x1 = bx, r.y0 = r.y1 = by, r.ax = r.ay = 0.0f;
     else r = resize_taps(resize_pos(bx, by, cw, ch, scw, sch), scw, sch, linear);
     float u00, v00;
-    chroma_texel(s, step, n, r.x0, r.y0, u00, v00);
+    chroma_texel<TEN>(s, step, n, r.x0, r.y0, u00, v00);
     int U = (int) u00, V = (int) v00;
     if (linear && !direct) {
         float u01, v01, u10, v10, u11, v11;
-        chroma_texel(s, step, n, r.x1, r.y0, u01, v01);
-        chroma_texel(s, step, n, r.x0, r.y1, u10, v10);
-        chroma_texel(s, step, n, r.x1, r.y1, u11, v11);
+        chroma_texel<TEN>(s, step, n, r.x1, r.y0, u01, v01);
+        chroma_texel<TEN>(s, step, n, r.x0, r.y1, u10, v10);
+        chroma_texel<TEN>(s, step, n, r.x1, r.y1, u11, v11);
         U = (int) rintf(blend_rn(r, u00, u01, u10, u11)), V = (int) rintf(blend_rn(r, v00, v01, v10, v11));
     }
-    if (FMT == SNNB_FRAME_I420) {
+    if (TEN) {
+        store_2p010(o.plane[1] + n * o.stride[1] + (size_t) by * o.pitch[1] + (size_t) bx * 4, U, V);
+    } else if (FMT == SNNB_FRAME_I420) {
         o.plane[1][n * o.stride[1] + (size_t) by * o.pitch[1] + bx] = (uint8_t) U;
         o.plane[2][n * o.stride[2] + (size_t) by * o.pitch[2] + bx] = (uint8_t) V;
     } else {
@@ -2054,16 +2152,18 @@ __global__ void __launch_bounds__(256) luma_output_kernel(TV t, FrameV s, int st
 int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames& src, const snnb_frames_out& fr) {
     SNNB_REQUIRE(t->c == 1 && t->cp == 8 && !t->feed_only && src.format != SNNB_FRAME_RGBA8,
                  "launch_luma_output: the output tensor has %d channels, source format %d; luma frames are written from 1 channel with YUV chroma", t->c, src.format);
-    // the source chroma as two planes of samples `step` bytes apart: U and V of I420, or the two bytes of an NV12 / NV21 pair
+    SNNB_REQUIRE((src.format == SNNB_FRAME_P010) == (fr.format == SNNB_FRAME_P010), "launch_luma_output: source format %d, out format %d; P010 pairs with P010 only",
+                 src.format, fr.format);
+    // the source chroma as two planes of samples `step` samples apart: U and V of I420, or the two samples of an NV12 / NV21 / P010 pair
     FrameV s {};
     int step = 1;
     s.w = src.width, s.h = src.height;
     if (src.format == SNNB_FRAME_I420) {
         for (int i = 1; i < 3; ++i) s.plane[i] = src.plane[i], s.pitch[i] = src.pitch[i], s.stride[i] = src.image_stride[i];
     } else {
-        const int u = src.format == SNNB_FRAME_NV21 ? 1 : 0;
+        const int u = src.format == SNNB_FRAME_NV21 ? 1 : 0, bytes = src.format == SNNB_FRAME_P010 ? 2 : 1;
         step = 2;
-        s.plane[1] = src.plane[1] + u, s.plane[2] = src.plane[1] + (1 - u);
+        s.plane[1] = src.plane[1] + u * bytes, s.plane[2] = src.plane[1] + (1 - u) * bytes;
         s.pitch[1] = s.pitch[2] = src.pitch[1], s.stride[1] = s.stride[2] = src.image_stride[1];
     }
     FrameOutV o;
@@ -2079,8 +2179,10 @@ int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame
         return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<nv21>");
     case SNNB_FRAME_I420:
         return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<i420>");
+    case SNNB_FRAME_P010:
+        return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<p010>");
     }
-    SNNB_REQUIRE(false, "launch_luma_output: out format %d; luma frames are written as NV12, NV21 or I420", fr.format);
+    SNNB_REQUIRE(false, "launch_luma_output: out format %d; luma frames are written as NV12, NV21, I420 or P010", fr.format);
 }
 
 // Model output 0 -> an 8-bit label plane (snnb_model_segment_frames): the fp32 scores hi + lo resampled to the plane with

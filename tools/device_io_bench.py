@@ -2,7 +2,8 @@
 
     python tools/device_io_bench.py --out DIR [--seconds 2] [--rounds 3]
 
-Writes DIR/device_io_bench.json and prints it. Four parts, all in one process:
+Writes DIR/device_io_bench.json and prints it. Four parts by default, and opt-in ones (see --parts; p010 compares 10-bit frames with
+NV12 on detect_frames, transform_luma and transform_frames, with each frame kernel's time and bytes/s), all in one process:
 
   throughput   ResNet-18 224x224 batch 32 fed with uint8 NCHW images already on the GPU (what a GPU JPEG decoder returns), device
                classes and logits out, against snnb_model_submit_u8 / snnb_model_wait from pinned host uint8 NHWC images; and Candy 720x720
@@ -678,6 +679,95 @@ def rois(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def p010_surface(torch, batch, H, W, seed):
+    """Random 10-bit frames as P010 words [N, H * 3 // 2, W] uint16 on the device (limited-range values, low 6 bits zero)."""
+    rng = np.random.default_rng(seed)
+    return torch.from_numpy((rng.integers(64, 941, (batch, H * 3 // 2, W)).astype(np.uint16) << 6)).cuda()
+
+
+def torch_p010_to_nv12(torch, p010):
+    """Today's workaround for 10-bit frames: every word's top 8 bits, as NV12 uint8 (one pass over the frame; the low 2 bits are lost)."""
+    return ((p010.view(torch.int16) >> 8) & 0xFF).to(torch.uint8)
+
+
+def alternate(torch, fns, seconds, batch, rounds):
+    """Rounds of timed(fn) for each named fn, alternating, and the median frames/s of each."""
+    for _ in range(5):
+        for fn in fns.values():
+            fn()
+    torch.cuda.synchronize()
+    runs = [{k: timed(fn, seconds, batch, torch.cuda.synchronize) for k, fn in fns.items()} for _ in range(rounds)]
+    return runs, {k: float(np.median([r[k]["frames_per_s"] for r in runs])) for k in fns}
+
+
+def with_rate(kt, read, written):
+    kt["us_per_launch"] = kt["us_per_batch"] * 50 / kt["launches"]
+    kt.update({"bytes_read": read, "bytes_written": written, "bytes_per_s": (read + written) / (kt["us_per_launch"] * 1e-6)})
+    kt["share_of_hbm_peak"] = kt["bytes_per_s"] / HBM_BYTES_PER_S
+    return kt
+
+
+def p010(torch, ctx, core, modelzoo, d, args):
+    """10-bit frames against 8-bit NV12 on the same sizes: detect_frames (YOLOv3-tiny 416 x 16), transform_luma (ESPCN) and
+    transform_frames (Candy 720 x 8), 1920 x 1080 frames."""
+    H, W = 1080, 1920
+    res = []
+    # YOLOv3-tiny: P010 in, against the workaround of repacking the top 8 bits as NV12
+    hw, batch, mean4, norm4 = (416, 416), 16, [127.5] * 4, [1.0 / 127.5] * 4
+    path, _ = modelzoo.build("yolov3tiny", os.path.join(d, "p010_yolo"), input_hw=hw)
+    m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+    src = p010_surface(torch, batch, H, W, 7)
+    nv12 = torch_p010_to_nv12(torch, src)
+    fns = {"p010": lambda: m.detect_frames(src, format="p010", mean4=mean4, norm4=norm4),
+           "torch_repack_nv12": lambda: m.detect_frames(torch_p010_to_nv12(torch, src), mean4=mean4, norm4=norm4)}
+    runs, med = alternate(torch, fns, args.seconds, batch, args.rounds)
+    sampled = lambda bps: batch * (min(4 * hw[0] * hw[1], H * W) * bps + min(4 * hw[0] * hw[1], (H // 2) * (W // 2)) * 2 * bps)  # noqa: E731
+    written = batch * hw[0] * hw[1] * 32
+    k10 = with_rate(frame_kernel_us(torch, fns["p010"], 50), sampled(2), written)
+    k8 = with_rate(frame_kernel_us(torch, lambda: m.detect_frames(nv12, mean4=mean4, norm4=norm4), 50), sampled(1), written)
+    res.append({"case": "yolov3tiny 416x416 batch 16 from 1920x1080 P010", "p010_frames_per_s_median": med["p010"],
+                "torch_repack_frames_per_s_median": med["torch_repack_nv12"], "p010_over_torch_repack": med["p010"] / med["torch_repack_nv12"],
+                "rounds": runs, "frame_input_kernel_p010": k10, "frame_input_kernel_nv12": k8})
+    m.close()
+    # ESPCN: P010 -> P010 against NV12 -> NV12, 2x up
+    path, _ = modelzoo.build("espcn", os.path.join(d, "p010_espcn"), input_hw=(H, W))
+    m = core.MixedInferenceCore(ctx, path, batch=1, input_hw=(H, W), fuse=True, use_cuda_graph=True)
+    src = p010_surface(torch, 1, H, W, 8)
+    nv12 = torch_p010_to_nv12(torch, src)
+    out10 = torch.empty((1, 2 * H * 3 // 2, 2 * W), dtype=torch.uint16, device="cuda")
+    out8 = torch.empty((1, 2 * H * 3 // 2, 2 * W), dtype=torch.uint8, device="cuda")
+    kw = dict(norm=1.0 / 255.0, out_hw=(2 * H, 2 * W), out_scale=255.0)
+    fns = {"p010": lambda: m.transform_luma(src, format="p010", out=out10, **kw), "nv12": lambda: m.transform_luma(nv12, out=out8, **kw)}
+    runs, med = alternate(torch, fns, args.seconds, 1, args.rounds)
+    entry = {"case": "espcn 1080x1920 batch 1, 1920x1080 to 3840x2160, P010 -> P010 against NV12 -> NV12",
+             "p010_frames_per_s_median": med["p010"], "nv12_frames_per_s_median": med["nv12"], "p010_over_nv12": med["p010"] / med["nv12"], "rounds": runs}
+    for fmt, bps in (("p010", 2), ("nv12", 1)):
+        entry["frame_input_kernel_" + fmt] = with_rate(frame_kernel_us(torch, fns[fmt], 50), H * W * bps, H * W * 32)
+        entry["luma_output_kernel_" + fmt] = with_rate(frame_kernel_us(torch, fns[fmt], 50, "luma_output_kernel"),
+                                                       4 * H * W * 32 + H * W // 2 * bps, 4 * H * W * 3 // 2 * bps)
+    res.append(entry)
+    m.close()
+    # Candy: P010 -> P010 against NV12 -> NV12, 720x720 x 8, 1080p in and out
+    hw, batch = (720, 720), 8
+    path, _ = modelzoo.build("candy", os.path.join(d, "p010_candy"), input_hw=hw)
+    m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+    src = p010_surface(torch, batch, H, W, 9)
+    nv12 = torch_p010_to_nv12(torch, src)
+    out10, out8 = torch.empty_like(src), torch.empty_like(nv12)
+    fns = {"p010": lambda: m.transform_frames(src, format="p010", out=out10), "nv12": lambda: m.transform_frames(nv12, out=out8)}
+    runs, med = alternate(torch, fns, args.seconds, batch, args.rounds)
+    entry = {"case": "candy 720x720 batch 8, 1920x1080 P010 -> 1920x1080 P010 against NV12 -> NV12",
+             "p010_frames_per_s_median": med["p010"], "nv12_frames_per_s_median": med["nv12"], "p010_over_nv12": med["p010"] / med["nv12"], "rounds": runs}
+    for fmt, bps in (("p010", 2), ("nv12", 1)):
+        entry["frame_input_kernel_" + fmt] = with_rate(frame_kernel_us(torch, fns[fmt], 50),
+                                                       batch * (H * W + H * W // 2) * bps, batch * hw[0] * hw[1] * 32)
+        entry["frame_output_kernel_" + fmt] = with_rate(frame_kernel_us(torch, fns[fmt], 50, "frame_output_kernel"),
+                                                        batch * hw[0] * hw[1] * 2 * 8 * 2, batch * (H * W + H * W // 2) * bps)
+    res.append(entry)
+    m.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
@@ -685,7 +775,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
                     help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in), "
-                         "segment (opt-in)")
+                         "segment (opt-in), p010 (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -712,6 +802,8 @@ def main():
         result["luma"] = luma(torch, ctx, core, modelzoo, d, args)
     if "segment" in parts:
         result["segment"] = segment(torch, ctx, core, modelzoo, d, args)
+    if "p010" in parts:
+        result["p010"] = p010(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
