@@ -40,9 +40,21 @@ argument moves the result by at most L e: L = 1 (none, relu, relu6, tanh), max(1
 
 Output storage: hi = fp16_rn(v), lo = fp16_rn(v - hi) stores v to 2^-22 |v| + 2^-25 (the half ulp of lo, also at fp16's smallest
 subnormal); the fp16 storage mode stores v to 2^-11 |v| + 2^-25. Second-order terms (an error times u) are covered by SLACK.
+
+Chosen output pixels. Every function of a layer with a spatial output takes an optional at = (n_idx, oy_idx, ox_idx), integer arrays
+of equal length; with it, it returns (ref, bound) at those output pixels only, for all channels, shaped [len(at), C]. The full
+restatement is the same code run at every pixel: a pixel's operands are gathered from the input by the same index arithmetic, and
+its float64 operations are the same ones in the same order. The one place where the order could depend on the other pixels is a
+BLAS matrix product, whose kernel (and with it the order of a dot product's additions) depends on the matrix shape; conv2d
+therefore multiplies in blocks of exactly ROWS pixel rows, the last one zero-filled, so a pixel's value is the same bits whichever
+pixels are evaluated with it. InstanceNorm's per-(image, channel) statistics are computed over the whole plane either way.
 """
 import numpy as np
 
+# Pixel rows per matrix product of conv2d (module docstring, "Chosen output pixels"). It cannot follow the number of pixels asked
+# for, so a small restatement (a dense head of a few images, a tiny test layer) pays for a whole zero-filled block: negligible next to
+# the Python overhead of its K steps. A smaller block would multiply that overhead on the large restatements instead.
+ROWS = 2048
 U = 2.0 ** -24          # fp32 unit roundoff
 KAPPA = 24 * 2.0 ** -23  # one m64nNk16 wgmma, relative to |c_in| + sum |p| (module docstring)
 ACT_ULPS = 4
@@ -128,26 +140,38 @@ def weight_operand(wv, form):
     return np.asarray(wv, np.float64), None  # simt
 
 
-def pad_input(x, pad_top, pad_left, need_h, need_w, mode="constant"):
-    """x [n, h, w, c] -> [n, need_h, need_w, c] with x at (pad_top, pad_left): zeros, or the kernels' replicate / single reflection
-    (src_coord in kernels_simt.cu; a coordinate still outside after one reflection reads zero)."""
+def src_coord(s, size, mode="constant"):
+    """The input coordinate an outside coordinate s reads: replicate, a single reflection, or -1 (zero) for constant padding and
+    for a coordinate still outside after one reflection (src_coord in kernels_simt.cu)."""
+    s = np.asarray(s)
+    if mode == "replicate":
+        return np.clip(s, 0, size - 1)
+    if mode == "reflect":
+        s = np.where(s < 0, -s, s)
+        s = np.where(s >= size, 2 * size - 2 - s, s)
+    return np.where((s >= 0) & (s < size), s, -1)
+
+
+def pixels(at, n, oh, ow):
+    """(n_idx, oy_idx, ox_idx) of the chosen output pixels, or of every pixel in NHWC order when at is None."""
+    if at is None:
+        return tuple(np.indices((n, oh, ow)).reshape(3, -1))
+    return tuple(np.asarray(a, np.int64).reshape(-1) for a in at)
+
+
+def shaped(v, at, n, oh, ow):
+    """Rows of per-pixel values -> [n, oh, ow, C] for a full restatement, [len(at), C] for chosen pixels."""
+    return v.reshape(n, oh, ow, -1) if at is None else v.reshape(len(at[0]), -1)
+
+
+def gather(x, ni, iy, ix, mode="constant", dtype=np.float64):
+    """x[ni, iy, ix, :] as [len(ni), C]; coordinates outside x read as padding mode `mode` does (src_coord)."""
     n, h, w, c = x.shape
-    ys = np.arange(need_h) - pad_top
-    xs = np.arange(need_w) - pad_left
-
-    def src(s, size):
-        if mode == "replicate":
-            return np.clip(s, 0, size - 1)
-        if mode == "reflect":
-            s = np.where(s < 0, -s, s)
-            s = np.where(s >= size, 2 * size - 2 - s, s)
-        return np.where((s >= 0) & (s < size), s, -1)
-
-    sy, sx = src(ys, h), src(xs, w)
-    out = x[:, np.clip(sy, 0, h - 1)][:, :, np.clip(sx, 0, w - 1)].copy()
-    out[:, sy < 0] = 0
-    out[:, :, sx < 0] = 0
-    return out
+    sy, sx = src_coord(iy, h, mode), src_coord(ix, w, mode)
+    ok = (sy >= 0) & (sx >= 0)
+    v = np.asarray(x[ni, np.where(ok, sy, 0), np.where(ok, sx, 0)], dtype)
+    v[~ok] = 0
+    return v
 
 
 def row_plan_steps(k, stride, pad_x):
@@ -190,69 +214,75 @@ def k_blocks(kernel, k, stride, pad_x, ic):
 
 
 def conv2d(x, w_oihw, bias, bn, stride, pad_x, pad_y, out_hw, act="", alpha=0.0, residual=None, form="fp32x3", kernel="igemm",
-           half_out=False, pad_mode="constant"):
+           half_out=False, pad_mode="constant", at=None):
     """Conv2D as the engine runs it: output column ox reads input column ox * stride + kx - pad_x, row oy * stride + ky - pad_y
     (the kernels' (pad_x, pad_y) = the layer's (T, L) offsets). kernel: "igemm" (conv_umma_kernel), "rowwin" / "feed"
-    (conv_rowwin_kernel, regular or feed mode) or "simt". Returns (ref, bound) [n, oh, ow, oc]."""
-    x = np.asarray(x, np.float64)
-    n, h, w, ic = x.shape
+    (conv_rowwin_kernel, regular or feed mode) or "simt". residual: [n, oh, ow, oc]. Returns (ref, bound) [n, oh, ow, oc], or
+    [len(at), oc] at the output pixels `at`."""
+    n, h, w, ic = np.shape(x)
     wv, shift = fold(w_oihw, bias, bn)
     oc, _, k, _ = wv.shape
     oh, ow = out_hw
     s = int(stride)
     T = TERMS.get(form, 0)
     wq, wlo = weight_operand(wv, form)
-    xp = pad_input(x, pad_y, pad_x, (oh - 1) * s + k, (ow - 1) * s + k, pad_mode)
-    M = n * oh * ow
-    taps = {}
-    for ky in range(k):
-        for kx in range(k):
-            X = xp[:, ky:ky + (oh - 1) * s + 1:s, kx:kx + (ow - 1) * s + 1:s, :].reshape(M, ic)
-            taps[ky, kx] = (X, np.abs(X), wq[:, :, ky, kx].T)
+    ni, oy, ox = pixels(at, n, oh, ow)
+    M = len(ni)
     y = np.zeros((M, oc))
     e_acc = np.zeros((M, oc))
-    if kernel == "simt":
-        a_all = np.zeros((M, oc))
-        for X, aX, W in taps.values():
-            y += X @ W
-            a_all += aX @ np.abs(W)
-        e_acc = gamma(k * k * ic) * a_all
-    else:
-        blocks_abs = np.zeros((M, oc))
-        blocks = k_blocks(kernel, k, s, pad_x, ic)
-        for block in blocks:
-            c = np.zeros((M, oc))
-            for step in block:
-                A = np.zeros((M, oc))
-                P = np.zeros((M, oc))
-                for ky, kx, ch in step:
-                    X, aX, W = taps[ky, kx]
-                    A += aX[:, ch] @ np.abs(W[ch])
-                    P += X[:, ch] @ W[ch]
-                e_acc += T * STEP_SLACK * KAPPA * (np.abs(c) + A)
-                c += P
-            y += c
-            blocks_abs += np.abs(c)
-        e_acc += max(len(blocks) - 1, 0) * U * blocks_abs
-    if wlo is not None:
-        for (ky, kx), (X, aX, W) in taps.items():
-            e_acc += (aX * (2.0 ** -11 * SLACK) + 2.0 ** -25) @ wlo[:, :, ky, kx].T
+    blocks = None if kernel == "simt" else k_blocks(kernel, k, s, pad_x, ic)
+    for r0 in range(0, M, ROWS):  # ROWS pixel rows per product, whatever else is evaluated (module docstring)
+        r1 = min(r0 + ROWS, M)
+        taps = {}
+        for ky in range(k):
+            for kx in range(k):
+                X = np.zeros((ROWS, ic))
+                X[:r1 - r0] = gather(x, ni[r0:r1], oy[r0:r1] * s + ky - pad_y, ox[r0:r1] * s + kx - pad_x, pad_mode)
+                taps[ky, kx] = (X, np.abs(X), wq[:, :, ky, kx].T)
+        yc = np.zeros((ROWS, oc))
+        ec = np.zeros((ROWS, oc))
+        if kernel == "simt":
+            a_all = np.zeros((ROWS, oc))
+            for X, aX, W in taps.values():
+                yc += X @ W
+                a_all += aX @ np.abs(W)
+            ec = gamma(k * k * ic) * a_all
+        else:
+            blocks_abs = np.zeros((ROWS, oc))
+            for block in blocks:
+                c = np.zeros((ROWS, oc))
+                for step in block:
+                    A = np.zeros((ROWS, oc))
+                    P = np.zeros((ROWS, oc))
+                    for ky, kx, ch in step:
+                        X, aX, W = taps[ky, kx]
+                        A += aX[:, ch] @ np.abs(W[ch])
+                        P += X[:, ch] @ W[ch]
+                    ec += T * STEP_SLACK * KAPPA * (np.abs(c) + A)
+                    c += P
+                yc += c
+                blocks_abs += np.abs(c)
+            ec += max(len(blocks) - 1, 0) * U * blocks_abs
+        if wlo is not None:
+            for (ky, kx), (X, aX, W) in taps.items():
+                ec += (aX * (2.0 ** -11 * SLACK) + 2.0 ** -25) @ wlo[:, :, ky, kx].T
+        y[r0:r1], e_acc[r0:r1] = yc[:r1 - r0], ec[:r1 - r0]
     pre = y + shift.astype(np.float64)
     e_pre = e_acc * SLACK + U * np.abs(pre)
     if residual is not None:
-        pre = pre + np.asarray(residual, np.float64).reshape(M, oc)
+        pre = pre + np.asarray(residual).reshape(n, oh, ow, oc)[ni, oy, ox].astype(np.float64)
         e_pre += U * np.abs(pre)
     ref = act64(pre, act, alpha)
     bound = act_bound(pre, e_pre, ref, act, alpha) * SLACK + store_bound(ref, half_out)
-    return ref.reshape(n, oh, ow, oc), bound.reshape(n, oh, ow, oc)
+    return shaped(ref, at, n, oh, ow), shaped(bound, at, n, oh, ow)
 
 
-def dense(x, kernel_out_in, bias, act="", form="fp32x3", half_out=False):
-    """Dense on a 1 x 1 map (or flattened HWC): a 1x1 conv_umma_kernel launch."""
+def dense(x, kernel_out_in, bias, act="", form="fp32x3", half_out=False, at=None):
+    """Dense on a 1 x 1 map (or flattened HWC): a 1x1 conv_umma_kernel launch. at: output pixels (n_idx, 0, 0)."""
     n = x.shape[0]
     x1 = np.asarray(x, np.float64).reshape(n, 1, 1, -1)
     kern = np.asarray(kernel_out_in, np.float32)
-    return conv2d(x1, kern[:, :, None, None], bias, None, 1, 0, 0, (1, 1), act, 0.0, form=form, half_out=half_out)
+    return conv2d(x1, kern[:, :, None, None], bias, None, 1, 0, 0, (1, 1), act, 0.0, form=form, half_out=half_out, at=at)
 
 
 def gap_dense(x, kernel_out_in, bias, act="", alpha=0.0, softmax_out=False, half_out=False):
@@ -297,41 +327,81 @@ def softmax(x, half_out=False):
     return ref, bound + store_bound(ref, half_out)
 
 
-def depthwise(x, w_chw, bias, bn, stride, pad_x, pad_y, out_hw, act="", alpha=0.0, half_out=False):
+def depthwise(x, w_chw, bias, bn, stride, pad_x, pad_y, out_hw, act="", alpha=0.0, half_out=False, at=None):
     """Depthwise k x k on the fp32 folded weights (depthwise kernels: fp32 FMAs started from the bias, window clipped to the input)."""
-    x = np.asarray(x, np.float64)
-    n, h, w, c = x.shape
+    n, h, w, c = np.shape(x)
     wk = np.asarray(w_chw, np.float32)
     k = wk.shape[-1]
     wv, shift = fold(wk[:, None], bias, bn)
     wv = wv[:, 0].astype(np.float64)
     oh, ow = out_hw
     s = int(stride)
-    xp = pad_input(x, pad_y, pad_x, (oh - 1) * s + k, (ow - 1) * s + k)
-    acc = np.zeros((n, oh, ow, c))
-    aab = np.zeros((n, oh, ow, c))
+    ni, oy, ox = pixels(at, n, oh, ow)
+    acc = np.zeros((len(ni), c))
+    aab = np.zeros((len(ni), c))
     for ky in range(k):
         for kx in range(k):
-            X = xp[:, ky:ky + (oh - 1) * s + 1:s, kx:kx + (ow - 1) * s + 1:s, :]
+            X = gather(x, ni, oy * s + ky - pad_y, ox * s + kx - pad_x)
             acc += X * wv[:, ky, kx]
             aab += np.abs(X * wv[:, ky, kx])
     pre = acc + shift
     e_pre = gamma(k * k) * (aab + np.abs(shift))
     ref = act64(pre, act, alpha)
-    return ref, act_bound(pre, e_pre, ref, act, alpha) * SLACK + store_bound(ref, half_out)
+    bound = act_bound(pre, e_pre, ref, act, alpha) * SLACK + store_bound(ref, half_out)
+    return shaped(ref, at, n, oh, ow), shaped(bound, at, n, oh, ow)
 
 
-def add(a, b, act="", alpha=0.0, half_out=False):
-    pre = np.asarray(a, np.float64) + np.asarray(b, np.float64)
+def box_grid(n, oh, ow, box):
+    """The boxes of a (tw, th, tn) tile grid laid over [n, oh, ow] from pixel (0, 0) of image 0, boxes past the edges clipped:
+    (n0, y0, x0, nn, hy, wx) arrays, one entry per box, in the kernels' tile order (x fastest, then y, then images)."""
+    tw, th, tn = box
+    bn, by, bx = np.indices((-(-n // tn), -(-oh // th), -(-ow // tw))).reshape(3, -1)
+    n0, y0, x0 = bn * tn, by * th, bx * tw
+    return n0, y0, x0, np.minimum(tn, n - n0), np.minimum(th, oh - y0), np.minimum(tw, ow - x0)
+
+
+def sample_pixels(n, oh, ow, boxes, seed, per_box=2):
+    """Output pixels to restate for one layer: every pixel of the first and last row and column of each image, and per_box seeded
+    random pixels in every box of each (tw, th, tn) grid in `boxes` (all of a box's pixels when it has fewer). The same (n, oh,
+    ow, boxes, seed) give the same pixels. Returns (n_idx, oy_idx, ox_idx) in NHWC order, without repeats."""
+    rng = np.random.default_rng(seed)
+    lin = []
+    for i in range(n):
+        rows = np.concatenate([np.zeros(ow, np.int64), np.full(ow, oh - 1), np.arange(oh), np.arange(oh)])
+        cols = np.concatenate([np.arange(ow), np.arange(ow), np.zeros(oh, np.int64), np.full(oh, ow - 1)])
+        lin.append((i * oh + rows) * ow + cols)
+    for box in boxes:
+        n0, y0, x0, nn, hy, wx = box_grid(n, oh, ow, box)
+        cnt = nn * hy * wx
+        keys = rng.random((len(cnt), int(cnt.max())))
+        keys[np.arange(keys.shape[1])[None, :] >= cnt[:, None]] = np.inf  # positions past a clipped box's pixels never win
+        q = np.argsort(keys, axis=1)[:, :per_box]
+        keep = np.arange(q.shape[1])[None, :] < np.minimum(cnt, per_box)[:, None]
+        q, b = q[keep], np.nonzero(keep)[0]
+        lin.append(((n0[b] + q // (wx[b] * hy[b])) * oh + y0[b] + (q // wx[b]) % hy[b]) * ow + x0[b] + q % wx[b])
+    u = np.unique(np.concatenate(lin))
+    return u // (oh * ow), (u // ow) % oh, u % ow
+
+
+def elementwise_operand(x, at):
+    """The operand of an elementwise layer as float64: whole, or [len(at), C] at the pixels `at`."""
+    if at is None:
+        return np.asarray(x, np.float64)
+    ni, oy, ox = pixels(at, 0, 0, 0)
+    return np.asarray(x[ni, oy, ox], np.float64)
+
+
+def add(a, b, act="", alpha=0.0, half_out=False, at=None):
+    pre = elementwise_operand(a, at) + elementwise_operand(b, at)
     ref = act64(pre, act, alpha)
     return ref, act_bound(pre, U * np.abs(pre), ref, act, alpha) * SLACK + store_bound(ref, half_out)
 
 
-def batchnorm(x, bn, act="", alpha=0.0, half_out=False):
+def batchnorm(x, bn, act="", alpha=0.0, half_out=False, at=None):
     """chanwise_kernel: scale * (x - mean) + beta with scale = gamma / max(sqrt(var + 1e-3), 1e-4) in fp32 (pack.cpp); three roundings."""
     g, be, m, v = (np.asarray(bn[k], np.float32) for k in ("gamma", "beta", "mean", "var"))
     scale = (g / np.maximum(np.sqrt(v + np.float32(0.001)), np.float32(0.0001))).astype(np.float64)
-    x = np.asarray(x, np.float64)
+    x = elementwise_operand(x, at)
     d = x - m
     pre = scale * d + be
     e_pre = U * np.abs(d) * np.abs(scale) * 2 + U * np.abs(pre)
@@ -339,61 +409,60 @@ def batchnorm(x, bn, act="", alpha=0.0, half_out=False):
     return ref, act_bound(pre, e_pre * SLACK, ref, act, alpha) * SLACK + store_bound(ref, half_out)
 
 
-def activation(x, act, alpha=0.0, half_out=False):
-    pre = np.asarray(x, np.float64)
+def activation(x, act, alpha=0.0, half_out=False, at=None):
+    pre = elementwise_operand(x, at)
     ref = act64(pre, act, alpha)
     return ref, act_bound(pre, 0.0, ref, act, alpha) * SLACK + store_bound(ref, half_out)
 
 
-def maxpool(x, k, stride, out_hw):
+def maxpool(x, k, stride, out_hw, at=None):
     """Windows start inside the input and are clipped at the bottom / right edge. A maximum is one of the stored inputs: bit-identical."""
-    x = np.asarray(x, np.float32)
-    n, h, w, c = x.shape
+    n, h, w, c = np.shape(x)
     oh, ow = out_hw
-    y = np.full((n, oh, ow, c), -np.inf, np.float32)
+    ni, oy, ox = pixels(at, n, oh, ow)
+    y = np.full((len(ni), c), -np.inf, np.float32)
     for ky in range(k):
         for kx in range(k):
-            ys = np.arange(oh) * stride + ky
-            xs = np.arange(ow) * stride + kx
-            iy, ix = np.nonzero(ys < h)[0], np.nonzero(xs < w)[0]
-            blk = np.full((n, oh, ow, c), -np.inf, np.float32)
-            blk[:, iy[:, None], ix[None, :]] = x[:, ys[iy]][:, :, xs[ix]]
+            ys, xs = oy * stride + ky, ox * stride + kx
+            inside = (ys < h) & (xs < w)
+            blk = gather(x, ni, np.where(inside, ys, 0), np.where(inside, xs, 0), dtype=np.float32)
+            blk[~inside] = -np.inf
             y = np.maximum(y, blk)
-    return y.astype(np.float64), np.zeros(y.shape)
+    return shaped(y.astype(np.float64), at, n, oh, ow), shaped(np.zeros(y.shape), at, n, oh, ow)
 
 
-def avgpool(x, k, stride, out_hw, half_out=False):
+def avgpool(x, k, stride, out_hw, half_out=False, at=None):
     """Clipped windows averaged over the pixels inside the input (fp32 sum of at most k*k terms, one division)."""
-    x = np.asarray(x, np.float64)
-    n, h, w, c = x.shape
+    n, h, w, c = np.shape(x)
     oh, ow = out_hw
-    s = np.zeros((n, oh, ow, c))
-    a = np.zeros((n, oh, ow, c))
-    cnt = np.zeros((oh, ow))
+    ni, oy, ox = pixels(at, n, oh, ow)
+    s = np.zeros((len(ni), c))
+    a = np.zeros((len(ni), c))
+    cnt = np.zeros((len(ni), 1))
     for ky in range(k):
         for kx in range(k):
-            ys = np.arange(oh) * stride + ky
-            xs = np.arange(ow) * stride + kx
-            vy, vx = ys < h, xs < w
-            sub = x[:, ys[vy]][:, :, xs[vx]]
-            idx_y, idx_x = np.nonzero(vy)[0], np.nonzero(vx)[0]
-            s[:, idx_y[:, None], idx_x[None, :]] += sub
-            a[:, idx_y[:, None], idx_x[None, :]] += np.abs(sub)
-            cnt[idx_y[:, None], idx_x[None, :]] += 1
-    ref = s / cnt[None, :, :, None]
-    bound = (gamma(k * k + 1) * a / cnt[None, :, :, None]) * SLACK + store_bound(ref, half_out)
-    return ref, bound
+            ys, xs = oy * stride + ky, ox * stride + kx
+            inside = (ys < h) & (xs < w)
+            sub = gather(x, ni[inside], ys[inside], xs[inside])
+            s[inside] += sub
+            a[inside] += np.abs(sub)
+            cnt[inside] += 1
+    ref = s / cnt
+    bound = (gamma(k * k + 1) * a / cnt) * SLACK + store_bound(ref, half_out)
+    return shaped(ref, at, n, oh, ow), shaped(bound, at, n, oh, ow)
 
 
-def pad(x, pad_x, pad_y, out_hw, mode="constant"):
+def pad(x, pad_x, pad_y, out_hw, mode="constant", at=None):
     """pad_kernel: input column x lands at x + pad_x, row y at y + pad_y (the layer's (T, L) offsets, as the kernel is handed them)."""
-    y = pad_input(np.asarray(x, np.float32), pad_y, pad_x, out_hw[0], out_hw[1], mode)
-    return y.astype(np.float64), np.zeros(y.shape)
+    n = np.shape(x)[0]
+    ni, oy, ox = pixels(at, n, *out_hw)
+    y = gather(x, ni, oy - pad_y, ox - pad_x, mode)
+    return shaped(y, at, n, *out_hw), shaped(np.zeros(y.shape), at, n, *out_hw)
 
 
-def concat(a, b):
-    y = np.concatenate([np.asarray(a, np.float32), np.asarray(b, np.float32)], axis=-1)
-    return y.astype(np.float64), np.zeros(y.shape)
+def concat(a, b, at=None):
+    y = np.concatenate([elementwise_operand(a, at), elementwise_operand(b, at)], axis=-1)
+    return y, np.zeros(y.shape)
 
 
 def flatten(x):
@@ -402,30 +471,29 @@ def flatten(x):
     return y.astype(np.float64), np.zeros(y.shape)
 
 
-def upsample_nearest(x, out_hw):
+def upsample_nearest(x, out_hw, at=None):
     """Nearest upsampling: output (y, x) reads input (floor(y h / oh), floor(x w / ow)) - for the integer scales of the zoo, y // s."""
-    x = np.asarray(x, np.float32)
-    n, h, w, c = x.shape
+    n, h, w, c = np.shape(x)
     oh, ow = out_hw
-    ys = (np.arange(oh) * h) // oh
-    xs = (np.arange(ow) * w) // ow
-    y = x[:, ys][:, :, xs]
-    return y.astype(np.float64), np.zeros(y.shape)
+    ni, oy, ox = pixels(at, n, oh, ow)
+    y = gather(x, ni, (oy * h) // oh, (ox * w) // ow)
+    return shaped(y, at, n, oh, ow), shaped(np.zeros(y.shape), at, n, oh, ow)
 
 
-def subpixel(x, r, half_out=False):
+def subpixel(x, r, half_out=False, at=None):
     """Depth-to-space of r*r channels into one, through tanh as the reference's subpixel shader does: output (y r + i, x r + j) =
     tanhf(input (y, x, i r + j))."""
-    x = np.asarray(x, np.float64)
-    n, h, w, c = x.shape
-    v = x.reshape(n, h, w, r, r).transpose(0, 1, 3, 2, 4).reshape(n, h * r, w * r, 1)
+    n, h, w, c = np.shape(x)
+    ni, oy, ox = pixels(at, n, h * r, w * r)
+    v = np.asarray(x[ni, oy // r, ox // r, (oy % r) * r + ox % r], np.float64)[:, None]
     ref = np.tanh(v)
-    return ref, act_bound(v, 0.0, ref, "tanh", 0.0) * SLACK + store_bound(ref, half_out)
+    bound = act_bound(v, 0.0, ref, "tanh", 0.0) * SLACK + store_bound(ref, half_out)
+    return shaped(ref, at, n, h * r, w * r), shaped(bound, at, n, h * r, w * r)
 
 
-def model_input(x, half):
+def model_input(x, half, at=None):
     """The input upload (split_f32_kernel, and the stem's feed copy): fp32 -> hi + lo, or fp16 alone. Restated exactly."""
-    y = stored(np.asarray(x, np.float32), half)
+    y = stored(elementwise_operand(np.asarray(x, np.float32), at), half)
     return y.astype(np.float64), np.zeros(y.shape)
 
 
@@ -439,25 +507,26 @@ def check(got, ref, bound, what):
     return ratio, bad
 
 
-def instancenorm(x, gamma_c, beta_c, act="", alpha=0.0, half_out=False):
+def instancenorm(x, gamma_c, beta_c, act="", alpha=0.0, half_out=False, at=None):
     """InstanceNorm (instnorm_*_kernel): per (image, channel) mean and biased variance over H W of d = x - x[first pixel], summed in
     fp32 (sum d with adds, sum d^2 with FMAs, any order: gamma_{HW+2}); m = S1 / HW, var = max(S2 / HW - m^2, 0), mean = x0 + m,
     rstd = 1 / sqrtf(var + 1e-5) (correctly rounded sqrt and division), y = (x - mean) * (gamma rstd) + beta, then the activation.
     ref evaluates the same formula in float64 with the exact mean and variance. The bound follows each rounding: e_m of m,
     e_var of the variance, e_r of rstd by the mean value theorem on (v + eps)^-1/2 over [v + eps - e_var, v + eps], then the
-    elementwise part."""
-    x = np.asarray(x, np.float64)
-    n, h, w, c = x.shape
+    elementwise part. The statistics always cover the whole plane; at only chooses the output pixels evaluated."""
+    n, h, w, c = np.shape(x)
     hw = h * w
     g = np.asarray(gamma_c, np.float32).astype(np.float64)
     b = np.asarray(beta_c, np.float32).astype(np.float64)
-    xs = x.reshape(n, hw, c)
-    d = xs - xs[:, :1]
-    s1, s2 = d.sum(axis=1), (d * d).sum(axis=1)
+    x0 = np.asarray(x[:, 0, 0], np.float64)
+    s1, s2, sa = np.zeros((n, c)), np.zeros((n, c)), np.zeros((n, c))
+    for i in range(n):  # one image at a time: a 720 x 720 plane in float64 is large enough
+        d = np.asarray(x[i], np.float64).reshape(hw, c) - x0[i]
+        s1[i], s2[i], sa[i] = d.sum(axis=0), (d * d).sum(axis=0), np.abs(d).sum(axis=0)
     m = s1 / hw
-    mu = xs[:, :1, :][:, 0] + m
+    mu = x0 + m
     var = s2 / hw - m * m
-    e_s1 = gamma(hw + 1) * np.abs(d).sum(axis=1)
+    e_s1 = gamma(hw + 1) * sa
     e_s2 = gamma(hw + 3) * s2
     e_m = e_s1 / hw + U * np.abs(m)
     e_mean = e_m + U * np.abs(mu)
@@ -468,10 +537,11 @@ def instancenorm(x, gamma_c, beta_c, act="", alpha=0.0, half_out=False):
     e_r = 0.5 * r_lo ** 3 * e_var * SLACK + 2.5 * U * r_lo + U * 1e-5 * 0.5 * r_lo ** 3
     mul = g * r
     e_mul = np.abs(g) * e_r + U * np.abs(mul) * SLACK
-    xm = xs - mu[:, None, :]
-    e_xm = e_mean[:, None, :] + U * (np.abs(xm) + e_mean[:, None, :])
-    pre = xm * mul[:, None, :] + b
-    e_pre = (np.abs(xm) * e_mul[:, None, :] + np.abs(mul[:, None, :]) * e_xm + U * np.abs(xm * mul[:, None, :]) + U * np.abs(pre)) * SLACK
+    ni, oy, ox = pixels(at, n, h, w)
+    xm = np.asarray(x[ni, oy, ox], np.float64) - mu[ni]
+    e_xm = e_mean[ni] + U * (np.abs(xm) + e_mean[ni])
+    pre = xm * mul[ni] + b
+    e_pre = (np.abs(xm) * e_mul[ni] + np.abs(mul[ni]) * e_xm + U * np.abs(xm * mul[ni]) + U * np.abs(pre)) * SLACK
     ref = act64(pre, act, alpha)
     bound = act_bound(pre, e_pre, ref, act, alpha) * SLACK + store_bound(ref, half_out)
-    return ref.reshape(n, h, w, c), bound.reshape(n, h, w, c)
+    return shaped(ref, at, n, h, w), shaped(bound, at, n, h, w)

@@ -246,16 +246,17 @@ def test_every_tensor_core_instantiation(ctx, tmp_path):
 
 
 # ---- whole models, teacher-forced -------------------------------------------------------------------------------------------
-def restate(om, i, outs, kernels, precision, half, x):
+def restate(om, i, outs, kernels, precision, half, x, at=None):
     """exact.* for layer i of oracle.Model om from the engine outputs `outs` of its producers (None where fusion hid them).
-    Returns (ref, bound), or None when a hidden producer makes the layer one this restatement does not cover."""
+    Returns (ref, bound), or None when a hidden producer makes the layer one this restatement does not cover. at: the output
+    pixels to restate (exact.py); the classifier heads (GAP + dense, dense, soft-max) and Flatten are always restated whole."""
     l = om.layers[i]
     t = om.type_of(l)
     w = om.w[i]
     act = l.get("activation", "linear")
     ins = [int(v) for v in l.get("inputId", [])][:int(l.get("numInputs", 0))]
     if t == "InputLayer":
-        return exact.model_input(x, half)
+        return exact.model_input(x, half, at)
     outs = list(outs)
     for j in ins:  # a constant Pad folded into its consumer: zero padding composes, so restate it as a tensor (pure data movement)
         p = om.layers[j]
@@ -271,7 +272,7 @@ def restate(om, i, outs, kernels, precision, half, x):
         if om.type_of(om.layers[j]) != "Conv2D" or outs[other] is None:
             return None
         return restate_conv(om, j, outs, kernels, precision, half, act=act, alpha=float(l.get("leakyReluAlpha", l.get("alpha", 0.3))),
-                            residual=outs[other], shape_of=i)
+                            residual=outs[other], shape_of=i, at=at)
     if t == "Dense" and any(outs[j] is None for j in ins):
         # the fused global average pool + dense (+ soft-max) head
         j = ins[0]
@@ -283,7 +284,7 @@ def restate(om, i, outs, kernels, precision, half, x):
             return None
         return exact.gap_dense(outs[j], w["kernel"], w.get("bias"), "" if act == "softmax" else act, softmax_out=act == "softmax", half_out=half)
     if t == "Conv2D":
-        return restate_conv(om, i, outs, kernels, precision, half, act=act, alpha=float(l.get("leakyReluAlpha", l.get("alpha", 0.0))))
+        return restate_conv(om, i, outs, kernels, precision, half, act=act, alpha=float(l.get("leakyReluAlpha", l.get("alpha", 0.0))), at=at)
     if any(outs[j] is None for j in ins):
         return None
     a = outs[ins[0]]
@@ -292,25 +293,25 @@ def restate(om, i, outs, kernels, precision, half, x):
     if t == "SeparableConv2D":
         k, s = int(l["kernel_size"]), int(l["strides"])
         o = om._offsets(l, k)
-        return exact.depthwise(a, w["kernel"], w.get("bias"), w.get("bn"), s, o[0], o[2], shape[1:3], act, float(l.get("leakyReluAlpha", l.get("alpha", 0.0))), half)
+        return exact.depthwise(a, w["kernel"], w.get("bias"), w.get("bn"), s, o[0], o[2], shape[1:3], act, float(l.get("leakyReluAlpha", l.get("alpha", 0.0))), half, at)
     if t == "MaxPooling2D":
         pool = l.get("pool", l.get("pool_size"))
         k = int(pool[0] if isinstance(pool, list) else pool)
         s = l.get("stride", l.get("strides", k))
-        return exact.maxpool(a, k, int(s[0] if isinstance(s, list) else s), shape[1:3])
+        return exact.maxpool(a, k, int(s[0] if isinstance(s, list) else s), shape[1:3], at)
     if t == "AveragePooling2D":
         pool = l.get("pool", l.get("pool_size"))
         k = int(pool[0] if isinstance(pool, list) else pool)
         s = l.get("stride", k)
-        return exact.avgpool(a, k, int(s[0] if isinstance(s, list) else s), shape[1:3], half)
+        return exact.avgpool(a, k, int(s[0] if isinstance(s, list) else s), shape[1:3], half, at)
     if t == "Add":
-        return exact.add(a, outs[ins[1]], act, float(l.get("leakyReluAlpha", l.get("alpha", 0.3))), half)
+        return exact.add(a, outs[ins[1]], act, float(l.get("leakyReluAlpha", l.get("alpha", 0.3))), half, at)
     if t == "InstanceNorm":
-        return exact.instancenorm(a, w["gamma"], w["beta"], act, float(l.get("leakyReluAlpha", 0.0)), half)
+        return exact.instancenorm(a, w["gamma"], w["beta"], act, float(l.get("leakyReluAlpha", 0.0)), half, at)
     if t == "BatchNormalization":
-        return exact.batchnorm(a, w["bn"], act, float(l.get("leakyReluAlpha", l.get("alpha", 0.0))), half)
+        return exact.batchnorm(a, w["bn"], act, float(l.get("leakyReluAlpha", l.get("alpha", 0.0))), half, at)
     if t == "Activation":
-        return exact.activation(a, act, float(l.get("leakyReluAlpha", 0.3)), half)
+        return exact.activation(a, act, float(l.get("leakyReluAlpha", 0.3)), half, at)
     if t == "Flatten":
         if act not in ("", "linear"):
             return None
@@ -324,24 +325,24 @@ def restate(om, i, outs, kernels, precision, half, x):
             ref, bound = ref.reshape(n, 1, 1, -1), bound.reshape(n, 1, 1, -1) + exact.store_bound(ref.reshape(n, 1, 1, -1), half)
         return ref, bound
     if t == "Concatenate":
-        return exact.concat(a, outs[ins[1]])
+        return exact.concat(a, outs[ins[1]], at)
     if t == "UpSampling2D":
         if l.get("interpolation") == "bilinear":
             return None
-        return exact.upsample_nearest(a, shape[1:3])
+        return exact.upsample_nearest(a, shape[1:3], at)
     if t == "Pad":
         if "pads" in l:
             p = l["pads"]
             o = [int(p[2]), int(p[6]), int(p[3]), int(p[7])]
         else:
             o = om._offsets(l, 0, False)
-        return exact.pad(a, o[0], o[2], shape[1:3], l.get("mode", "constant"))
+        return exact.pad(a, o[0], o[2], shape[1:3], l.get("mode", "constant"), at)
     if t == "Subpixel":
-        return exact.subpixel(a, int(l.get("kernel_size", 2)), half)
+        return exact.subpixel(a, int(l.get("kernel_size", 2)), half, at)
     return None
 
 
-def restate_conv(om, j, outs, kernels, precision, half, act, alpha, residual=None, shape_of=None):
+def restate_conv(om, j, outs, kernels, precision, half, act, alpha, residual=None, shape_of=None, at=None):
     l = om.layers[j]
     k, s = int(l["kernel_size"]), int(l["strides"])
     src = [int(v) for v in l["inputId"]][0]
@@ -353,7 +354,7 @@ def restate_conv(om, j, outs, kernels, precision, half, act, alpha, residual=Non
     w = om.w[j]
     shape = kernels["shapes"][shape_of if shape_of is not None else j]
     return exact.conv2d(x, w["kernel"], w.get("bias"), w.get("bn"), s, px, py, shape[1:3], act, alpha, residual=residual,
-                        form=conv_form(kernels["names"][j], precision), kernel=kern, half_out=half, pad_mode=mode)
+                        form=conv_form(kernels["names"][j], precision), kernel=kern, half_out=half, pad_mode=mode, at=at)
 
 
 def teacher_forced(ctx, name, hw, batch, model_dir, precision, fuse, conv_algo="auto", **kw):
