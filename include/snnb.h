@@ -453,6 +453,52 @@ typedef struct {
  * num_frames >= 1, 1 <= max_rows <= 100, frame size >= 1, capacity >= 1, expand finite and >= 0, a stream that is not capturing. */
 int snnb_rois_from_detections(snnb_context* ctx, const float* rows_dev, const int* counts_dev, int num_frames, int max_rows, int frame_width,
                               int frame_height, const snnb_roi_select* sel, snnb_roi* rois_dev, int capacity, int* count_dev, void* stream);
+/* Frame lists: a batch of separately allocated device frames of mixed sizes, one descriptor per image (the decoded pictures of several
+ * video streams, each from its own decoder's surface pool, at 720p, 1080p and 2160p side by side). An snnb_frames batch is one
+ * allocation of equally sized images at a constant stride; a list lifts all three restrictions. One pixel format for the whole list;
+ * each image has its own planes, pitches, size and matrix. The descriptors are read on the host during the call only: they travel to
+ * the kernel by value, as a kernel parameter, so nothing is allocated or copied and the host array may be reused at once. */
+typedef struct {
+    const uint8_t* plane[3]; /* as snnb_frames.plane, for this image only */
+    int pitch[3];            /* as snnb_frames.pitch */
+    int width, height;       /* this image's size, any >= 1 (odd allowed) */
+    int matrix;              /* SNNB_YUV_* for this image (ignored for RGBA8) */
+} snnb_frame_image;
+typedef struct {
+    int format;                     /* SNNB_FRAME_*: one format for every image */
+    int count;                      /* number of images */
+    const snnb_frame_image* images; /* HOST array of `count` descriptors */
+    int linear_filter;              /* as snnb_frames */
+    float mean4[4], norm4[4];       /* as snnb_frames */
+} snnb_frame_list;
+enum { SNNB_FRAME_LIST_MAX = 256 }; /* images per list */
+/* snnb_model_run_frames / snnb_model_detect_frames with a frame list of exactly the loaded batch of images: the model input of slot i is
+ * bit for bit what snnb_model_run_frames computes for a batch made only of image i, with image i's matrix (direct sampling when image i
+ * has the model's size, every format, both filters). Outputs, classes, rows, counts, the stream contract and the fences are exactly
+ * those of run_frames / detect_frames; run_frame_list refuses YOLO models, detect_frame_list requires them. Checked on the host before
+ * anything is enqueued, each error naming the image: a known format, a non-null `images`, count == the loaded batch (<= 256); per
+ * image, width and height >= 1, a known matrix (full range with BT.601 only), each used pitch >= its row's bytes, each used plane
+ * device or managed memory of the context's device (P010: even pitches, 2-byte-aligned planes); a model with one input of <= 4
+ * channels and a stream that is not capturing. A plane's size cannot be checked: it must hold its image. Cost beyond the forward pass:
+ * one kernel launch for the input, as run_frames (1920x1080 NV12 to YOLOv3-tiny 416x416 x 16: 58 us, against 50 us for run_frames'
+ * kernel on the same frames as one batch; NVIDIA H100 80GB HBM3, 700 W power limit). */
+int snnb_model_run_frame_list(snnb_model* m, const snnb_frame_list* frames, const snnb_device_buffer* outputs, int num_outputs,
+                              int* classes_1based_dev, void* stream);
+int snnb_model_detect_frame_list(snnb_model* m, const snnb_frame_list* frames, float* rows_dev, int max_rows, int* counts_dev, void* stream);
+/* snnb_model_run_rois on a frame list of 1..256 source frames (frames->count of them, independent of the batch): a used slot is valid
+ * when 0 <= frame < frames->count and the rectangle lies inside frames->images[frame], its OWN frame's size (a rectangle that fits a
+ * 1080p frame but not the 720p frame it names is invalid: all-zero outputs, class 0). Chroma is sited in that frame's coordinates and
+ * the colour conversion uses that frame's matrix. Every other rule, the checks (the list's, as for run_frame_list, with 1 <= count <=
+ * 256, then run_rois' own), the stream contract and the cost are those of snnb_model_run_rois. */
+int snnb_model_run_rois_list(snnb_model* m, const snnb_frame_list* frames, const snnb_roi* rois_dev, const int* count_dev,
+                             const snnb_device_buffer* outputs, int num_outputs, int* classes_1based_dev, void* stream);
+/* snnb_rois_from_detections with a size per frame: frame_wh is a HOST array [num_frames][2] of {width, height}, read during the call
+ * only, 1 <= num_frames <= 256. Row r of frame n is mapped with frame n's own W and H in snnb_rois_from_detections' float32 formula, so
+ * with every size equal the regions are byte for byte snnb_rois_from_detections'. Checked on the host before anything is enqueued:
+ * everything snnb_rois_from_detections checks, a non-null frame_wh and every width and height >= 1. */
+int snnb_rois_from_detections_list(snnb_context* ctx, const float* rows_dev, const int* counts_dev, int num_frames, int max_rows,
+                                   const int* frame_wh, const snnb_roi_select* sel, snnb_roi* rois_dev, int capacity, int* count_dev,
+                                   void* stream);
 /* Device-resident variant: inputs already uploaded with snnb_model_set_input(); forward only, asynchronous. */
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input_nhwc);
 int snnb_model_forward(snnb_model* m);

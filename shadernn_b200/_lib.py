@@ -126,6 +126,32 @@ class LabelsOut(C.Structure):
     ]
 
 
+class FrameImage(C.Structure):
+    """snnb_frame_image"""
+    _fields_ = [
+        ("plane", C.c_void_p * 3),
+        ("pitch", C.c_int * 3),
+        ("width", C.c_int),
+        ("height", C.c_int),
+        ("matrix", C.c_int),
+    ]
+
+
+class FrameList(C.Structure):
+    """snnb_frame_list"""
+    _fields_ = [
+        ("format", C.c_int),
+        ("count", C.c_int),
+        ("images", C.POINTER(FrameImage)),
+        ("linear_filter", C.c_int),
+        ("mean4", C.c_float * 4),
+        ("norm4", C.c_float * 4),
+    ]
+
+
+FRAME_LIST_MAX = 256
+
+
 class Roi(C.Structure):
     """snnb_roi"""
     _fields_ = [
@@ -217,6 +243,10 @@ SIGNATURES = {
     "snnb_model_segment_frames": (C.c_int, [vp, C.POINTER(Frames), C.c_int, C.POINTER(LabelsOut), vp]),
     "snnb_model_run_rois": (C.c_int, [vp, C.POINTER(Frames), C.c_int, vp, vp, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
     "snnb_rois_from_detections": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(RoiSelect), vp, C.c_int, vp, vp]),
+    "snnb_model_run_frame_list": (C.c_int, [vp, C.POINTER(FrameList), C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
+    "snnb_model_detect_frame_list": (C.c_int, [vp, C.POINTER(FrameList), vp, C.c_int, vp, vp]),
+    "snnb_model_run_rois_list": (C.c_int, [vp, C.POINTER(FrameList), vp, vp, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
+    "snnb_rois_from_detections_list": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, C.POINTER(RoiSelect), vp, C.c_int, vp, vp]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),

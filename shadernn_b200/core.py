@@ -66,7 +66,9 @@ class GpuContext:
         regions of frame_hw = (H, W) frames for MixedInferenceCore.run_rois, on the device, ordered on the current torch stream and
         never synchronising. Rows with score >= min_score and of class class_id (-1: any) are kept, each box grown by `expand` times its
         width (height) on each side and clipped to the frame, in frame order then row order. Returns (rois, count): an int32 CUDA tensor
-        [capacity, 6] of {frame, row, x, y, width, height}, zero past the count, and an int32 CUDA tensor [1] with min(kept, capacity)."""
+        [capacity, 6] of {frame, row, x, y, width, height}, zero past the count, and an int32 CUDA tensor [1] with min(kept, capacity).
+        frame_hw may also be a list of one (H, W) per frame (snnb_rois_from_detections_list: each frame's rows are mapped with its own
+        size, for MixedInferenceCore.run_rois_list on frames of mixed sizes)."""
         import torch
         if not (isinstance(rows, torch.Tensor) and rows.is_cuda and rows.dtype == torch.float32 and rows.dim() == 3 and rows.shape[2] == 6):
             raise ValueError("rois_from_detections: rows must be a float32 CUDA tensor [N, max_rows, 6]")
@@ -78,6 +80,14 @@ class GpuContext:
         count = torch.empty(1, dtype=torch.int32, device=device)
         sel = _lib.RoiSelect(float(min_score), int(class_id), float(expand))
         stream = torch.cuda.current_stream(device).cuda_stream or 1  # the legacy default stream is cudaStreamLegacy (1), not NULL
+        if np.ndim(frame_hw) == 2:
+            if len(frame_hw) != rows.shape[0]:
+                raise ValueError("rois_from_detections: %d frame sizes for rows of %d frames" % (len(frame_hw), rows.shape[0]))
+            wh = np.ascontiguousarray(np.asarray(frame_hw, np.int32)[:, ::-1])  # (H, W) -> {width, height}
+            check(lib().snnb_rois_from_detections_list(self.h, rows.data_ptr() or None, counts.data_ptr() or None, rows.shape[0], rows.shape[1],
+                                                       wh.ctypes.data_as(vp), C.byref(sel), rois.data_ptr() or None, int(capacity), count.data_ptr(), stream),
+                  "snnb_rois_from_detections_list")
+            return rois, count
         check(lib().snnb_rois_from_detections(self.h, rows.data_ptr() or None, counts.data_ptr() or None, rows.shape[0], rows.shape[1], int(frame_hw[1]),
                                               int(frame_hw[0]), C.byref(sel), rois.data_ptr() or None, int(capacity), count.data_ptr(), stream),
               "snnb_rois_from_detections")
@@ -637,6 +647,74 @@ class MixedInferenceCore:
         check(lib().snnb_model_run_rois(self.h, C.byref(f), n, rois.data_ptr(), count.data_ptr() if count is not None else None, obufs, len(outs),
                                         classes.data_ptr() if want_classes else None, self._torch_stream()),
               "snnb_model_run_rois")
+        result = outs[0] if len(outs) == 1 else outs
+        return (result, classes) if want_classes else result
+
+    def _frame_list(self, who, frames, format, matrix, linear, mean4, norm4):
+        """The snnb_frame_list of a Python list of CUDA tensors, one frame each, in _frames' layouts without the batch dimension (each
+        tensor its own allocation, with its own size and pitch). matrix: one name for every frame, or a list with one per frame.
+        Returns (the list, its descriptor array, which must stay alive until the call returns)."""
+        frames = list(frames)
+        matrices = [matrix] * len(frames) if isinstance(matrix, str) else list(matrix)
+        if format not in self._FRAME_FORMATS or len(matrices) != len(frames) or any(m not in self._YUV_MATRICES for m in matrices):
+            raise ValueError("%s: format %r / matrix %r for %d frames: expected one of %s and one of %s (or a list with one per frame)" % (
+                who, format, matrix, len(frames), sorted(self._FRAME_FORMATS), sorted(self._YUV_MATRICES)))
+        images = (_lib.FrameImage * max(1, len(frames)))()
+        for i, (x, m) in enumerate(zip(frames, matrices)):
+            f = _lib.Frames()
+            if not hasattr(x, "unsqueeze"):
+                raise ValueError("%s: frame %d must be a CUDA tensor" % (who, i))
+            self._frame_planes(who, "frame %d" % i, x.unsqueeze(0), format, f)
+            images[i].plane, images[i].pitch = f.plane, f.pitch
+            images[i].width, images[i].height, images[i].matrix = f.width, f.height, self._YUV_MATRICES[m]
+        fl = _lib.FrameList()
+        fl.format, fl.count, fl.images, fl.linear_filter = self._FRAME_FORMATS[format], len(frames), images, int(bool(linear))
+        fl.mean4 = (C.c_float * 4)(*[float(v) for v in (mean4 if mean4 is not None else [0.0] * 4)])
+        fl.norm4 = (C.c_float * 4)(*[float(v) for v in (norm4 if norm4 is not None else [1.0] * 4)])
+        return fl, images
+
+    def run_frame_list(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_dtype=None, out_layout="nhwc",
+                       out_scale=1.0, out_offset=0.0, want_classes=False):
+        """snnb_model_run_frame_list: run_frames on a list of separately allocated frames of mixed sizes, one per batch slot (see
+        _frame_list; matrix may name one matrix per frame). Slot i is exactly what run_frames computes for a batch of frame i alone.
+        Outputs, classes and the stream contract as run_frames."""
+        if len(frames) != self.batch:
+            raise ValueError("run_frame_list: %d frames given, the model's batch is %d" % (len(frames), self.batch))
+        outs, obufs, classes = self._device_outputs("run_frame_list", out_dtype, out_layout, out_scale, out_offset, want_classes)
+        fl, images = self._frame_list("run_frame_list", frames, format, matrix, linear, mean4, norm4)
+        check(lib().snnb_model_run_frame_list(self.h, C.byref(fl), obufs, len(outs), classes.data_ptr() if want_classes else None, self._torch_stream()),
+              "snnb_model_run_frame_list")
+        result = outs[0] if len(outs) == 1 else outs
+        return (result, classes) if want_classes else result
+
+    def detect_frame_list(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, max_rows=100):
+        """snnb_model_detect_frame_list: detect_frames on a list of frames as run_frame_list takes it. Returns (rows, counts)."""
+        import torch
+        if len(frames) != self.batch:
+            raise ValueError("detect_frame_list: %d frames given, the model's batch is %d" % (len(frames), self.batch))
+        fl, images = self._frame_list("detect_frame_list", frames, format, matrix, linear, mean4, norm4)
+        device = torch.device("cuda", self.ctx.device)
+        rows = torch.empty((self.batch, max(int(max_rows), 0), 6), dtype=torch.float32, device=device)
+        counts = torch.empty(self.batch, dtype=torch.int32, device=device)
+        check(lib().snnb_model_detect_frame_list(self.h, C.byref(fl), rows.data_ptr() or None, int(max_rows), counts.data_ptr(), self._torch_stream()),
+              "snnb_model_detect_frame_list")
+        return rows, counts
+
+    def run_rois_list(self, frames, rois, count=None, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_dtype=None,
+                      out_layout="nhwc", out_scale=1.0, out_offset=0.0, want_classes=False):
+        """snnb_model_run_rois_list: run_rois on a list of 1 to 256 frames of mixed sizes as run_frame_list takes it. A region is valid
+        against the size of its own frame. rois, count, outputs, classes and the stream contract as run_rois."""
+        import torch
+        if not (isinstance(rois, torch.Tensor) and rois.is_cuda and rois.dtype == torch.int32 and tuple(rois.shape) == (self.batch, 6)):
+            raise ValueError("run_rois_list: rois must be an int32 CUDA tensor [%d, 6] (the model's batch)" % self.batch)
+        if count is not None and not (isinstance(count, torch.Tensor) and count.is_cuda and count.dtype == torch.int32 and count.numel() == 1):
+            raise ValueError("run_rois_list: count must be None or an int32 CUDA tensor of one element")
+        outs, obufs, classes = self._device_outputs("run_rois_list", out_dtype, out_layout, out_scale, out_offset, want_classes)
+        fl, images = self._frame_list("run_rois_list", frames, format, matrix, linear, mean4, norm4)
+        rois = rois.contiguous()
+        check(lib().snnb_model_run_rois_list(self.h, C.byref(fl), rois.data_ptr(), count.data_ptr() if count is not None else None, obufs, len(outs),
+                                             classes.data_ptr() if want_classes else None, self._torch_stream()),
+              "snnb_model_run_rois_list")
         result = outs[0] if len(outs) == 1 else outs
         return (result, classes) if want_classes else result
 

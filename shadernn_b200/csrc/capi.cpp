@@ -139,6 +139,12 @@ int snnb_rois_from_detections(snnb_context* ctx, const float* rows_dev, const in
     return rois_from_detections(ctx, rows_dev, counts_dev, num_frames, max_rows, frame_width, frame_height, sel, rois_dev, capacity, count_dev,
                                 static_cast<cudaStream_t>(stream));
 }
+int snnb_rois_from_detections_list(snnb_context* ctx, const float* rows_dev, const int* counts_dev, int num_frames, int max_rows, const int* frame_wh,
+                                   const snnb_roi_select* sel, snnb_roi* rois_dev, int capacity, int* count_dev, void* stream) {
+    SNNB_REQUIRE(ctx, "snnb_rois_from_detections_list: null context");
+    SNNB_CUDA_OK(cudaSetDevice(ctx->device));
+    return rois_from_detections_list(ctx, rows_dev, counts_dev, num_frames, max_rows, frame_wh, sel, rois_dev, capacity, count_dev, static_cast<cudaStream_t>(stream));
+}
 
 // ---- tensors ----
 int snnb_tensor_alloc(snnb_context* ctx, int n, int h, int w, int c, snnb_tensor** out) { return tensor_alloc(ctx, n, h, w, c, out); }

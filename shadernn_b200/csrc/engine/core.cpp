@@ -2,6 +2,7 @@
 // Counterpart of core/src/ic2/core.cpp:294-410 (init) and :97-245 (run).
 #include <algorithm>
 #include <cmath>
+#include <cstdio>
 #include <cstring>
 #include <unordered_map>
 #include <unordered_set>
@@ -692,24 +693,56 @@ static int checkCallerStream(const char* api, cudaStream_t stream) {
     return 0;
 }
 
+// The matrix (YUV formats) and size of one frame description. `image` prefixes each message: "" for an snnb_frames batch, "image 3: "
+// for entry 3 of a frame list.
+static int checkFrameImage(const char* api, const char* image, int format, int matrix, int width, int height) {
+    if (format != SNNB_FRAME_RGBA8) {
+        const int base = matrix & ~SNNB_YUV_FULL_RANGE;
+        SNNB_REQUIRE(base == SNNB_YUV_BT601 || base == SNNB_YUV_BT709 || base == SNNB_YUV_BT2020, "%s: %sunknown YUV matrix %d", api, image, matrix);
+        SNNB_REQUIRE(base == SNNB_YUV_BT601 || !(matrix & SNNB_YUV_FULL_RANGE), "%s: %sYUV matrix %d: full range is defined for BT.601 only", api, image, matrix);
+    }
+    SNNB_REQUIRE(width >= 1 && height >= 1, "%s: %sframe size %d x %d; width and height must be >= 1", api, image, width, height);
+    return 0;
+}
+
 int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, cudaStream_t stream) {
-    if (in.frames) {
-        const snnb_frames& f = *in.frames;
-        SNNB_REQUIRE(knownFrameFormat(f.format), "%s: unknown frame format %d", api, f.format);
-        if (f.format != SNNB_FRAME_RGBA8) {
-            const int base = f.matrix & ~SNNB_YUV_FULL_RANGE;
-            SNNB_REQUIRE(base == SNNB_YUV_BT601 || base == SNNB_YUV_BT709 || base == SNNB_YUV_BT2020, "%s: unknown YUV matrix %d", api, f.matrix);
-            SNNB_REQUIRE(base == SNNB_YUV_BT601 || !(f.matrix & SNNB_YUV_FULL_RANGE), "%s: YUV matrix %d: full range is defined for BT.601 only", api, f.matrix);
+    if (in.frames || in.list) {
+        // one snnb_frames (its batch shares one description) or each image of a list, in run_frames' order of checks: the format,
+        // each image's matrix and size, the model's input, then each image's planes
+        static const long long noStride[3] = {0, 0, 0};
+        const int format = in.frames ? in.frames->format : in.list->format;
+        SNNB_REQUIRE(knownFrameFormat(format), "%s: unknown frame format %d", api, format);
+        if (in.list) {
+            SNNB_REQUIRE(in.list->images, "%s: null images", api);
+            const int n = in.list->count;
+            if (in.rois)
+                SNNB_REQUIRE(n >= 1 && n <= SNNB_FRAME_LIST_MAX, "%s: count %d; a list holds 1 to %d frames", api, n, (int) SNNB_FRAME_LIST_MAX);
+            else
+                SNNB_REQUIRE(n == (int) options.batch && n <= SNNB_FRAME_LIST_MAX, "%s: count %d; the list must hold the model's batch of %u images (at most %d)", api,
+                             n, options.batch, (int) SNNB_FRAME_LIST_MAX);
         }
-        SNNB_REQUIRE(f.width >= 1 && f.height >= 1, "%s: frame size %d x %d; width and height must be >= 1", api, f.width, f.height);
+        const int images = in.frames ? 1 : in.list->count;
+        char image[32] = "", planes[32] = "plane";
+        for (int i = 0; i < images; ++i) {
+            if (in.list) std::snprintf(image, sizeof(image), "image %d: ", i);
+            const int rc = in.frames ? checkFrameImage(api, image, format, in.frames->matrix, in.frames->width, in.frames->height)
+                                     : checkFrameImage(api, image, format, in.list->images[i].matrix, in.list->images[i].width, in.list->images[i].height);
+            if (rc) return rc;
+        }
         SNNB_REQUIRE(inputLayers.size() == 1, "%s: the model has %d inputs; frames feed a model with exactly one", api, (int) inputLayers.size());
         const snnb_tensor* t = inputLayers[0]->output;
         SNNB_REQUIRE(t->c >= 1 && t->c <= 4, "%s: the model input has %d channels; frames feed 1 to 4 (RGBA components)", api, t->c);
         if (in.luma) {
-            SNNB_REQUIRE(f.format != SNNB_FRAME_RGBA8, "%s: RGBA8 frames have no Y plane; luma input takes NV12, NV21, I420 or P010 frames", api);
+            SNNB_REQUIRE(format != SNNB_FRAME_RGBA8, "%s: RGBA8 frames have no Y plane; luma input takes NV12, NV21, I420 or P010 frames", api);
             SNNB_REQUIRE(t->c == 1, "%s: the model input has %d channels; the Y plane feeds exactly 1", api, t->c);
         }
-        if (int rc = checkFramePlanes(api, "plane", f.format, f.width, f.plane, f.pitch, f.image_stride, ctx->device)) return rc;
+        for (int i = 0; i < images; ++i) {
+            if (in.list) std::snprintf(planes, sizeof(planes), "image %d plane", i);
+            const int rc = in.frames ? checkFramePlanes(api, planes, format, in.frames->width, in.frames->plane, in.frames->pitch, in.frames->image_stride, ctx->device)
+                                     : checkFramePlanes(api, planes, format, in.list->images[i].width, in.list->images[i].plane, in.list->images[i].pitch, noStride,
+                                                        ctx->device);
+            if (rc) return rc;
+        }
         if (in.rois) {
             SNNB_REQUIRE(in.numFrames >= 1, "%s: num_frames %d; at least one frame is required", api, in.numFrames);
             SNNB_REQUIRE(options.batch <= 65535, "%s: batch %u; regions fill at most 65535 slots", api, options.batch);
@@ -734,8 +767,12 @@ int MixedInferenceCore::enqueueDeviceForward(const DeviceFeed& in, cudaStream_t 
         SNNB_CUDA_OK(cudaEventRecord(callerReady, stream));
         SNNB_CUDA_OK(cudaStreamWaitEvent(ctx->stream, callerReady, 0));
     }
-    if (in.rois) {
+    if (in.rois && in.list) {
+        if (launch_frame_list_roi_input(ctx, *in.list, in.rois, in.roiCount, inputLayers[0]->output)) return 1;
+    } else if (in.rois) {
         if (launch_frame_roi_input(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, inputLayers[0]->output)) return 1;
+    } else if (in.list) {
+        if (launch_frame_list_input(ctx, *in.list, inputLayers[0]->output)) return 1;
     } else if (in.frames) {
         if (launch_frame_input(ctx, *in.frames, inputLayers[0]->output, in.luma)) return 1;
     } else {
@@ -774,6 +811,20 @@ int MixedInferenceCore::runRois(const snnb_frames* frames, int numFrames, const 
     in.frames = frames, in.rois = roisDev, in.roiCount = countDev, in.numFrames = numFrames;
     return runDeviceFeed("snnb_model_run_rois", in, outputs, numOutputs, classes1Dev, stream);
 }
+int MixedInferenceCore::runFrameList(const snnb_frame_list* frames, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_run_frame_list: null frames");
+    DeviceFeed in;
+    in.list = frames;
+    return runDeviceFeed("snnb_model_run_frame_list", in, outputs, numOutputs, classes1Dev, stream);
+}
+int MixedInferenceCore::runRoisList(const snnb_frame_list* frames, const snnb_roi* roisDev, const int* countDev, const snnb_device_buffer* outputs,
+                                    int numOutputs, int* classes1Dev, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_run_rois_list: null frames");
+    SNNB_REQUIRE(roisDev, "snnb_model_run_rois_list: null rois");
+    DeviceFeed in;
+    in.list = frames, in.rois = roisDev, in.roiCount = countDev, in.numFrames = frames->count;
+    return runDeviceFeed("snnb_model_run_rois_list", in, outputs, numOutputs, classes1Dev, stream);
+}
 
 int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev,
                                       cudaStream_t stream) {
@@ -785,7 +836,7 @@ int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, con
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO",
                  "%s: output 0 is a YOLO detection list; use %s for device detections, or snnb_model_run or "
                  "snnb_model_submit / snnb_model_wait and read the boxes with snnb_model_get_boxes",
-                 api, in.frames ? "snnb_model_detect_frames" : "snnb_model_detect_device");
+                 api, in.list ? "snnb_model_detect_frame_list" : (in.frames ? "snnb_model_detect_frames" : "snnb_model_detect_device"));
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
     const int device = ctx->device;
     for (int j = 0; j < numOutputs; ++j) {
@@ -804,13 +855,17 @@ int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, con
     if (classes1Dev && launch_argmax(ctx, outputLayers[0]->output, classes1Dev, 1)) return 1; // core.cpp:228-233: argmax + 1
     if (in.rois) { // the slots without a valid region: every output byte and the class zero
         const int B = (int) options.batch;
+        auto clear = [&](void* dst, long long slotBytes) {
+            return in.list ? launch_roi_list_clear(ctx, *in.list, in.rois, in.roiCount, B, dst, slotBytes)
+                           : launch_roi_clear(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, B, dst, slotBytes);
+        };
         for (int j = 0; j < numOutputs; ++j) {
             if (!outputs[j].data) continue;
             const snnb_tensor* t = outputLayers[j]->output;
             const long long elem = outputs[j].dtype == SNNB_DTYPE_F32 ? 4 : (outputs[j].dtype == SNNB_DTYPE_F16 ? 2 : 1);
-            if (launch_roi_clear(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, B, outputs[j].data, (long long) t->h * t->w * t->c * elem)) return 1;
+            if (clear(outputs[j].data, (long long) t->h * t->w * t->c * elem)) return 1;
         }
-        if (classes1Dev && launch_roi_clear(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, B, classes1Dev, (long long) sizeof(int))) return 1;
+        if (classes1Dev && clear(classes1Dev, (long long) sizeof(int))) return 1;
     }
     return fenceToCaller(stream);
 }
@@ -828,9 +883,16 @@ int MixedInferenceCore::detectFrames(const snnb_frames* frames, float* rowsDev, 
     in.frames = frames;
     return detectDeviceFeed("snnb_model_detect_frames", in, rowsDev, maxRows, countsDev, stream);
 }
+int MixedInferenceCore::detectFrameList(const snnb_frame_list* frames, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_detect_frame_list: null frames");
+    DeviceFeed in;
+    in.list = frames;
+    return detectDeviceFeed("snnb_model_detect_frame_list", in, rowsDev, maxRows, countsDev, stream);
+}
 
 int MixedInferenceCore::detectDeviceFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
-    SNNB_REQUIRE(yolo, "%s: the model has no YOLO output; use %s", api, in.frames ? "snnb_model_run_frames" : "snnb_model_run_device");
+    SNNB_REQUIRE(yolo, "%s: the model has no YOLO output; use %s", api,
+                 in.list ? "snnb_model_run_frame_list" : (in.frames ? "snnb_model_run_frames" : "snnb_model_run_device"));
     SNNB_REQUIRE(maxRows >= 1 && maxRows <= 100, "%s: max_rows %d is outside 1..100", api, maxRows);
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
     if (int rc = checkDevicePointer(api, rowsDev, sizeof(float), ctx->device, "rows", 0)) return rc;
@@ -999,15 +1061,22 @@ int MixedInferenceCore::dumpOutputs(const std::string& dir) {
 
 } // namespace snn
 
-// snnb_rois_from_detections: a context-level call with no model state, so its one kernel runs on the caller's stream itself.
-int snnb::rois_from_detections(snnb_context* ctx, const float* rows, const int* counts, int numFrames, int maxRows, int fw, int fh, const snnb_roi_select* sel,
-                               snnb_roi* rois, int capacity, int* count, cudaStream_t stream) {
-    static const char* api = "snnb_rois_from_detections";
+// snnb_rois_from_detections and its per-frame-size form: context-level calls with no model state, so their one kernel runs on the
+// caller's stream itself. frameWh == nullptr: every frame is fw x fh; else frame n is frameWh[2n] x frameWh[2n + 1].
+static int roisFromDetections(const char* api, snnb_context* ctx, const float* rows, const int* counts, int numFrames, int maxRows, int fw, int fh,
+                              const int* frameWh, const snnb_roi_select* sel, snnb_roi* rois, int capacity, int* count, cudaStream_t stream) {
     SNNB_REQUIRE(sel, "%s: null sel", api);
     SNNB_REQUIRE(numFrames >= 1, "%s: num_frames %d; at least one frame is required", api, numFrames);
     SNNB_REQUIRE(maxRows >= 1 && maxRows <= 100, "%s: max_rows %d is outside 1..100", api, maxRows);
     SNNB_REQUIRE((long long) numFrames * maxRows <= 0x7fffffffLL, "%s: %d frames of %d rows", api, numFrames, maxRows);
-    SNNB_REQUIRE(fw >= 1 && fh >= 1, "%s: frame size %d x %d; width and height must be >= 1", api, fw, fh);
+    if (frameWh) {
+        SNNB_REQUIRE(numFrames <= SNNB_FRAME_LIST_MAX, "%s: num_frames %d is more than %d", api, numFrames, (int) SNNB_FRAME_LIST_MAX);
+        for (int n = 0; n < numFrames; ++n)
+            SNNB_REQUIRE(frameWh[2 * n] >= 1 && frameWh[2 * n + 1] >= 1, "%s: frame %d: size %d x %d; width and height must be >= 1", api, n, frameWh[2 * n],
+                         frameWh[2 * n + 1]);
+    } else {
+        SNNB_REQUIRE(fw >= 1 && fh >= 1, "%s: frame size %d x %d; width and height must be >= 1", api, fw, fh);
+    }
     SNNB_REQUIRE(capacity >= 1, "%s: capacity %d; at least one region is required", api, capacity);
     SNNB_REQUIRE(std::isfinite(sel->expand) && sel->expand >= 0.0f, "%s: expand %g; a finite value >= 0 is required", api, (double) sel->expand);
     if (int rc = snn::checkDevicePointer(api, rows, sizeof(float), ctx->device, "rows", 0)) return rc;
@@ -1015,5 +1084,16 @@ int snnb::rois_from_detections(snnb_context* ctx, const float* rows, const int* 
     if (int rc = snn::checkDevicePointer(api, rois, sizeof(int), ctx->device, "rois", 0)) return rc;
     if (int rc = snn::checkDevicePointer(api, count, sizeof(int), ctx->device, "count", 0)) return rc;
     if (int rc = snn::checkCallerStream(api, stream)) return rc;
-    return launch_rois_from_detections(ctx, stream ? stream : ctx->stream, rows, counts, numFrames, maxRows, fw, fh, *sel, rois, capacity, count);
+    if (frameWh)
+        return snnb::launch_rois_from_detections_list(ctx, stream ? stream : ctx->stream, rows, counts, numFrames, maxRows, frameWh, *sel, rois, capacity, count);
+    return snnb::launch_rois_from_detections(ctx, stream ? stream : ctx->stream, rows, counts, numFrames, maxRows, fw, fh, *sel, rois, capacity, count);
+}
+int snnb::rois_from_detections(snnb_context* ctx, const float* rows, const int* counts, int numFrames, int maxRows, int fw, int fh, const snnb_roi_select* sel,
+                               snnb_roi* rois, int capacity, int* count, cudaStream_t stream) {
+    return roisFromDetections("snnb_rois_from_detections", ctx, rows, counts, numFrames, maxRows, fw, fh, nullptr, sel, rois, capacity, count, stream);
+}
+int snnb::rois_from_detections_list(snnb_context* ctx, const float* rows, const int* counts, int numFrames, int maxRows, const int* frameWh,
+                                    const snnb_roi_select* sel, snnb_roi* rois, int capacity, int* count, cudaStream_t stream) {
+    SNNB_REQUIRE(frameWh, "snnb_rois_from_detections_list: null frame_wh");
+    return roisFromDetections("snnb_rois_from_detections_list", ctx, rows, counts, numFrames, maxRows, 0, 0, frameWh, sel, rois, capacity, count, stream);
 }

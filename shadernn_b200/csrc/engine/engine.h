@@ -362,6 +362,11 @@ public:
     // snnb_model_run_rois: runFrames with regions of numFrames frames as the batch; slots without a valid region come out zero
     int runRois(const snnb_frames* frames, int numFrames, const snnb_roi* roisDev, const int* countDev, const snnb_device_buffer* outputs, int numOutputs,
                 int* classes1Dev, cudaStream_t stream);
+    // snnb_model_run_frame_list / detect_frame_list / run_rois_list: runFrames / detectFrames / runRois with one descriptor per image
+    int runFrameList(const snnb_frame_list* frames, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
+    int detectFrameList(const snnb_frame_list* frames, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
+    int runRoisList(const snnb_frame_list* frames, const snnb_roi* roisDev, const int* countDev, const snnb_device_buffer* outputs, int numOutputs,
+                    int* classes1Dev, cudaStream_t stream);
     int layerOutput(int layerId, float* host, size_t capacityFloats);
     int timeLayers(std::vector<float>& ms);
     int dumpOutputs(const std::string& dir);
@@ -420,18 +425,20 @@ private:
     cudaEvent_t callerReady = nullptr, deviceDone = nullptr;
     // What a device-resident call feeds the model: one snnb_device_buffer per input, or (frames != NULL) a batch of frames into input 0,
     // or (rois != NULL as well) regions of numFrames frames, one per batch slot, with roiCount (NULL: all slots) of them used, or
-    // (luma) the frames' Y plane alone into a 1-channel input.
+    // (luma) the frames' Y plane alone into a 1-channel input, or (list != NULL, in place of frames) a frame list: one descriptor per
+    // image, the loaded batch of them, or with rois its list->count (= numFrames) source frames.
     // The input staging (and, for regions, the clearing of the slots without one) is the only step in which these entry points differ.
     struct DeviceFeed {
         const snnb_device_buffer* inputs = nullptr;
         int numInputs = 0;
         const snnb_frames* frames = nullptr;
+        const snnb_frame_list* list = nullptr;
         const snnb_roi* rois = nullptr;
         const int* roiCount = nullptr;
         int numFrames = 0;
         bool luma = false;
     };
-    // shared by runDevice, detectDevice, runFrames, detectFrames and runRois: the host-side checks of the feed and the stream (nothing
+    // shared by runDevice, detectDevice, runFrames, detectFrames, runRois and their frame-list forms: the host-side checks of the feed and the stream (nothing
     // enqueued), then the fenced input staging + forward pass, the outputs or the detections, and the fence back to the caller's stream
     int runDeviceFeed(const char* api, const DeviceFeed& in, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
     int detectDeviceFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);

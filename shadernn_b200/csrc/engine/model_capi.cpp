@@ -165,6 +165,23 @@ int snnb_model_run_rois(snnb_model* m, const snnb_frames* frames, int num_frames
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->runRois(frames, num_frames, rois_dev, count_dev, outputs, num_outputs, classes_1based_dev, static_cast<cudaStream_t>(stream));
 }
+int snnb_model_run_frame_list(snnb_model* m, const snnb_frame_list* frames, const snnb_device_buffer* outputs, int num_outputs, int* classes_1based_dev,
+                              void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_run_frame_list: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->runFrameList(frames, outputs, num_outputs, classes_1based_dev, static_cast<cudaStream_t>(stream));
+}
+int snnb_model_detect_frame_list(snnb_model* m, const snnb_frame_list* frames, float* rows_dev, int max_rows, int* counts_dev, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_detect_frame_list: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->detectFrameList(frames, rows_dev, max_rows, counts_dev, static_cast<cudaStream_t>(stream));
+}
+int snnb_model_run_rois_list(snnb_model* m, const snnb_frame_list* frames, const snnb_roi* rois_dev, const int* count_dev, const snnb_device_buffer* outputs,
+                             int num_outputs, int* classes_1based_dev, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_run_rois_list: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->runRoisList(frames, rois_dev, count_dev, outputs, num_outputs, classes_1based_dev, static_cast<cudaStream_t>(stream));
+}
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input) {
     SNNB_REQUIRE(m, "snnb_model_set_input: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));

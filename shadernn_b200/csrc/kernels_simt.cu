@@ -10,6 +10,7 @@
 // core/data/assets/shaders/).
 #include <algorithm>
 #include <cstdlib>
+#include <cstring>
 
 #include "snnb_internal.h"
 
@@ -1819,6 +1820,150 @@ int launch_roi_clear(snnb_context* ctx, const snnb_frames& fr, int num_frames, c
                        "roi_clear_kernel");
 }
 
+// Frame lists (snnb_model_run_frame_list): one FrameV per image, filled by frame_view, passed by value as a __grid_constant__ kernel
+// parameter (26.6 KB at SNNB_FRAME_LIST_MAX images; CUDA 12.1+ allows 32,764 bytes). No allocation, no host-to-device copy, nothing
+// that must outlive the launch, and a launch that a CUDA graph may capture. Indexed by a register, an entry is read from the constant
+// bank (LDC). Each kernel below is its snnb_frames form with s = img[n] and image index 0, through the same frame_pixel and stores.
+struct FrameListV {
+    FrameV img[SNNB_FRAME_LIST_MAX];
+};
+template <int FMT>
+__global__ void __launch_bounds__(256) frame_list_input_kernel(const __grid_constant__ FrameListV L, TV t, U8Norm q, int linear, FeedV f) {
+    pdl_wait();
+    const size_t total = (size_t) t.N * t.H * t.W;
+    const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (px >= total) return;
+    const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
+    const FrameV& s   = L.img[n];
+    const bool direct = s.w == t.W && s.h == t.H;
+    ResizeTaps r;
+    if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
+    else r = resize_taps(resize_pos(ox, oy, t.W, t.H, s.w, s.h), s.w, s.h, linear);
+    float v[8];
+    frame_pixel<FMT>(s, 0, r, linear, direct, t, q, v);
+    store_input_pixel(t, f, px, v);
+}
+// roi_slot against the size of the region's own frame: the one validity test of frame_list_roi_input_kernel and roi_list_clear_kernel.
+// A frame index outside the list fails roi_slot's own test, so the size looked up for it does not matter.
+__device__ __forceinline__ bool roi_list_slot(const FrameListV& L, const RoiV& g, int slot, int N, snnb_roi& r) {
+    const int frame = __ldg(reinterpret_cast<const int*>(g.rois + slot));
+    const FrameV& s = L.img[min(max(frame, 0), g.num_frames - 1)];
+    return roi_slot(g, slot, N, s.w, s.h, r);
+}
+template <int FMT>
+__global__ void __launch_bounds__(256) frame_list_roi_input_kernel(const __grid_constant__ FrameListV L, RoiV g, TV t, U8Norm q, int linear, FeedV f) {
+    pdl_wait();
+    const size_t total = (size_t) t.N * t.H * t.W;
+    const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (px >= total) return;
+    const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
+    snnb_roi roi;
+    float v[8];
+    if (roi_list_slot(L, g, n, t.N, roi)) {
+        const bool direct = roi.width == t.W && roi.height == t.H;
+        ResizeTaps r;
+        if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
+        else r = resize_taps(resize_pos(ox, oy, t.W, t.H, roi.width, roi.height), roi.width, roi.height, linear);
+        r.x0 += roi.x, r.x1 += roi.x, r.y0 += roi.y, r.y1 += roi.y;
+        frame_pixel<FMT>(L.img[roi.frame], 0, r, linear, direct, t, q, v);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = 0.0f;
+    }
+    store_input_pixel(t, f, px, v);
+}
+__global__ void __launch_bounds__(256) roi_list_clear_kernel(const __grid_constant__ FrameListV L, RoiV g, int N, uint8_t* __restrict__ dst, long long slot_bytes) {
+    pdl_wait();
+    snnb_roi roi;
+    if (roi_list_slot(L, g, (int) blockIdx.y, N, roi)) return;
+    uint8_t* p = dst + (long long) blockIdx.y * slot_bytes;
+    for (long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * 16; i < slot_bytes; i += (long long) gridDim.x * blockDim.x * 16) {
+        if ((reinterpret_cast<uintptr_t>(p + i) & 15) == 0 && i + 16 <= slot_bytes) {
+            *reinterpret_cast<uint4*>(p + i) = make_uint4(0u, 0u, 0u, 0u);
+        } else {
+            for (long long k = i; k < i + 16 && k < slot_bytes; ++k) p[k] = 0;
+        }
+    }
+}
+// The table of a list (checked by the caller: 1 <= count <= SNNB_FRAME_LIST_MAX); each entry is frame_view of the image as a one-image
+// snnb_frames, so the matrix constants come from the same code. Entries past the count stay zero and are never read.
+static void frame_list_view(const snnb_frame_list& fl, FrameListV& L) {
+    std::memset(&L, 0, sizeof(L));
+    for (int i = 0; i < fl.count; ++i) {
+        const snnb_frame_image& im = fl.images[i];
+        snnb_frames fr {};
+        fr.format = fl.format, fr.matrix = im.matrix, fr.width = im.width, fr.height = im.height;
+        for (int p = 0; p < 3; ++p) fr.plane[p] = im.plane[p], fr.pitch[p] = im.pitch[p];
+        L.img[i] = frame_view(fr);
+    }
+}
+static U8Norm frame_list_norm(const snnb_frame_list& fl) {
+    U8Norm q;
+    for (int i = 0; i < 4; ++i) q.mean[i] = fl.mean4[i], q.norm[i] = fl.norm4[i];
+    return q;
+}
+int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t) {
+    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_list_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
+    SNNB_REQUIRE(fl.count == t->n && fl.count <= SNNB_FRAME_LIST_MAX, "launch_frame_list_input: %d images for a batch of %d", fl.count, t->n);
+    FrameListV L;
+    frame_list_view(fl, L);
+    const U8Norm q   = frame_list_norm(fl);
+    const int linear = fl.linear_filter ? 1 : 0;
+    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
+    switch (fl.format) {
+    case SNNB_FRAME_NV12:
+        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<nv12>");
+    case SNNB_FRAME_NV21:
+        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<nv21>");
+    case SNNB_FRAME_I420:
+        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<i420>");
+    case SNNB_FRAME_RGBA8:
+        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<rgba8>");
+    case SNNB_FRAME_P010:
+        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<p010>");
+    }
+    SNNB_REQUIRE(false, "launch_frame_list_input: unknown format %d", fl.format);
+}
+int launch_frame_list_roi_input(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, snnb_tensor* t) {
+    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_list_roi_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
+    SNNB_REQUIRE(fl.count >= 1 && fl.count <= SNNB_FRAME_LIST_MAX, "launch_frame_list_roi_input: %d frames", fl.count);
+    FrameListV L;
+    frame_list_view(fl, L);
+    const U8Norm q   = frame_list_norm(fl);
+    const RoiV g {rois, count, fl.count};
+    const int linear = fl.linear_filter ? 1 : 0;
+    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
+    switch (fl.format) {
+    case SNNB_FRAME_NV12:
+        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
+                           "frame_list_roi_input_kernel<nv12>");
+    case SNNB_FRAME_NV21:
+        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
+                           "frame_list_roi_input_kernel<nv21>");
+    case SNNB_FRAME_I420:
+        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
+                           "frame_list_roi_input_kernel<i420>");
+    case SNNB_FRAME_RGBA8:
+        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
+                           "frame_list_roi_input_kernel<rgba8>");
+    case SNNB_FRAME_P010:
+        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
+                           "frame_list_roi_input_kernel<p010>");
+    }
+    SNNB_REQUIRE(false, "launch_frame_list_roi_input: unknown format %d", fl.format);
+}
+int launch_roi_list_clear(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes) {
+    SNNB_REQUIRE(batch >= 1 && batch <= 65535 && slot_bytes >= 1, "launch_roi_list_clear: batch %d, %lld bytes per slot", batch, slot_bytes);
+    SNNB_REQUIRE(fl.count >= 1 && fl.count <= SNNB_FRAME_LIST_MAX, "launch_roi_list_clear: %d frames", fl.count);
+    FrameListV L;
+    frame_list_view(fl, L);
+    const RoiV g {rois, count, fl.count};
+    const long long chunks = (slot_bytes + 16 * 256 - 1) / (16 * 256);
+    const dim3 grid((unsigned) std::min(chunks, 1024LL), (unsigned) batch);
+    return launch_done(ctx, launch_k(roi_list_clear_kernel, grid, dim3(256), 0, ctx->stream, L, g, batch, static_cast<uint8_t*>(dst), slot_bytes),
+                       "roi_list_clear_kernel");
+}
+
 // Detection rows -> regions (snnb_rois_from_detections). The rectangle of one row, every operation IEEE-rounded on its own (no FMA
 // contraction), so that a float32 restatement reproduces it; false when the row is not kept.
 __device__ __forceinline__ bool roi_from_row(const float* __restrict__ row, float W, float H, const snnb_roi_select& sel, snnb_roi& r) {
@@ -1881,6 +2026,59 @@ int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const fl
     return launch_done(ctx, launch_k(rois_from_detections_kernel, dim3(1), dim3(ROI_THREADS), 0, stream, rows, counts, num_frames, max_rows, fw, fh, sel, rois,
                                      capacity, count),
                        "rois_from_detections_kernel");
+}
+// snnb_rois_from_detections_list: rois_from_detections_kernel's scan with frame n's own size, from a table passed by value as FrameListV
+// is (2 KB).
+struct FrameSizesV {
+    int wh[SNNB_FRAME_LIST_MAX][2];
+};
+__global__ void __launch_bounds__(ROI_THREADS) rois_from_detections_list_kernel(const float* __restrict__ rows, const int* __restrict__ counts, int num_frames,
+                                                                              int max_rows, const __grid_constant__ FrameSizesV S, snnb_roi_select sel,
+                                                                              snnb_roi* __restrict__ out, int capacity, int* __restrict__ count_out) {
+    pdl_wait();
+    __shared__ int warp_incl[ROI_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = ROI_THREADS / 32;
+    const int total = num_frames * max_rows;
+    int kept = 0; // rows kept before the current chunk (uniform over the CTA)
+    for (int c0 = 0; c0 < total; c0 += ROI_THREADS) {
+        const int i = c0 + threadIdx.x;
+        snnb_roi r;
+        bool keep = false;
+        if (i < total) {
+            const int n = i / max_rows, k = i - n * max_rows;
+            if (k < min(__ldg(counts + n), max_rows)) keep = roi_from_row(rows + (size_t) i * 6, (float) S.wh[n][0], (float) S.wh[n][1], sel, r);
+            r.frame = n, r.row = k;
+        }
+        const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) warp_incl[warp] = __popc(ballot);
+        __syncthreads();
+        if (warp == 0) {
+            int v = warp_incl[lane];
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int u = __shfl_up_sync(0xffffffffu, v, d);
+                if (lane >= d) v += u;
+            }
+            warp_incl[lane] = v;
+        }
+        __syncthreads();
+        const int rank = kept + (warp ? warp_incl[warp - 1] : 0) + __popc(ballot & ((1u << lane) - 1u));
+        if (keep && rank < capacity) out[rank] = r;
+        kept += warp_incl[warps - 1];
+        __syncthreads(); // warp_incl is rewritten by the next chunk
+    }
+    const int written = min(kept, capacity);
+    for (int i = written + threadIdx.x; i < capacity; i += ROI_THREADS) out[i] = snnb_roi {0, 0, 0, 0, 0, 0};
+    if (threadIdx.x == 0) *count_out = written;
+}
+int launch_rois_from_detections_list(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows,
+                                     const int* frame_wh, const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count) {
+    SNNB_REQUIRE(num_frames >= 1 && num_frames <= SNNB_FRAME_LIST_MAX, "launch_rois_from_detections_list: %d frames", num_frames);
+    FrameSizesV S {};
+    for (int n = 0; n < num_frames; ++n) S.wh[n][0] = frame_wh[2 * n], S.wh[n][1] = frame_wh[2 * n + 1];
+    return launch_done(ctx, launch_k(rois_from_detections_list_kernel, dim3(1), dim3(ROI_THREADS), 0, stream, rows, counts, num_frames, max_rows, S, sel, rois,
+                                     capacity, count),
+                       "rois_from_detections_list_kernel");
 }
 
 // Model output 0 -> device video frames (snnb_model_transform_frames), the reverse of frame_input_kernel. Each frame pixel is

@@ -266,9 +266,19 @@ int launch_roi_clear(snnb_context* ctx, const snnb_frames& f, int num_frames, co
 // Detection rows -> regions (snnb_rois_from_detections, checked by the caller), one CTA on `stream`
 int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh,
                                 const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count);
+// Frame lists (snnb_model_run_frame_list / run_rois_list, checked by the caller): launch_frame_input, launch_frame_roi_input and
+// launch_roi_clear with one descriptor per image, passed to the kernel by value (fl.count <= SNNB_FRAME_LIST_MAX)
+int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t);
+int launch_frame_list_roi_input(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, snnb_tensor* t);
+int launch_roi_list_clear(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes);
+// launch_rois_from_detections with frame n's size at frame_wh[2n], frame_wh[2n + 1] (host, num_frames <= SNNB_FRAME_LIST_MAX)
+int launch_rois_from_detections_list(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows,
+                                     const int* frame_wh, const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count);
 // The host-side checks of snnb_rois_from_detections, then its launch (engine/core.cpp, beside the device-feed checks)
 int rois_from_detections(snnb_context* ctx, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh, const snnb_roi_select* sel,
                          snnb_roi* rois, int capacity, int* count, cudaStream_t stream);
+int rois_from_detections_list(snnb_context* ctx, const float* rows, const int* counts, int num_frames, int max_rows, const int* frame_wh,
+                              const snnb_roi_select* sel, snnb_roi* rois, int capacity, int* count, cudaStream_t stream);
 
 // ---- host-side weight folding/packing (pack.cpp) -----------------------------------------------------------
 // K ordering of the row-window convolution kernel (kernels_umma.cu): for stride s the taps of one filter row fall

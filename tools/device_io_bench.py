@@ -49,6 +49,12 @@ NV12 on detect_frames, transform_luma and transform_frames, with each frame kern
                the arg-max (or the 0.5 threshold) + .to(uint8); alternating as above. And segment_output_kernel's time per batch from
                CUDA events (segment_frames calls less calls that run only the same input and forward pass) and from torch.profiler, with
                bytes/s from the labels written plus the model-output planes read once.
+  framelist   (opt-in) Sixteen streams of mixed sizes, each frame its own allocation (4 x 3840x2160, 8 x 1920x1080, 4 x 1280x720 NV12):
+               YOLOv3-tiny 416x416 batch 16 with all-pass heads detect_frame_list -> rois_from_detections with per-frame sizes ->
+               ResNet-18 112x112 batch 64 run_rois_list, against what a user does without frame lists: per frame a torch NV12 -> RGB
+               conversion and F.interpolate into one batch, detect_torch, rows to the host, crops as in `rois`, run_torch; alternating
+               as above. The device time of each kernel of the chain from torch.profiler over 50 calls, and frame_list_input_kernel
+               against frame_input_kernel on one uniform 1920x1080 batch of 16 (the cost of the per-image descriptor).
   card        name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -679,6 +685,75 @@ def rois(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+FRAMELIST_SIZES = [(2160, 3840)] * 4 + [(1080, 1920)] * 8 + [(720, 1280)] * 4  # (H, W) of the 16 streams
+
+
+def framelist(torch, ctx, core, modelzoo, d, args):
+    import torch.nn.functional as F
+    dhw, chw, cbatch = (416, 416), (112, 112), 64
+    dbatch = len(FRAMELIST_SIZES)
+    dmean, dnorm = [127.5] * 4, [1.0 / 127.5] * 4
+    mean4, norm4 = [127.5] * 4, [1.0 / 127.5] * 4
+    path, layers = modelzoo.build("yolov3tiny", os.path.join(d, "list_yolov3tiny"), input_hw=dhw)
+    for head in [l for l in layers if l["type"] == "Conv2D" and l["outputPlanes"] == 18]:  # all-pass heads (see `detector`)
+        head["_w"]["bias"][:] = 0
+        head["_w"]["bias"][[4, 5, 10, 11, 16, 17]] = 8.0
+    det = core.MixedInferenceCore(ctx, modelzoo.write_model(layers, os.path.join(d, "list_allpass.json"), split=True), batch=dbatch, input_hw=dhw,
+                                  fuse=True, use_cuda_graph=True)
+    cpath, _ = modelzoo.build("resnet18", os.path.join(d, "list_resnet18"), input_hw=chw)
+    cls = core.MixedInferenceCore(ctx, cpath, batch=cbatch, input_hw=chw, fuse=True, use_cuda_graph=True)
+    g = torch.Generator().manual_seed(7)
+    frames = [torch.randint(16, 236, (h * 3 // 2, w), dtype=torch.uint8, generator=g).cuda() for h, w in FRAMELIST_SIZES]  # one allocation each
+    mean_t = torch.tensor(mean4[:3], device="cuda").view(1, 3, 1, 1)
+    norm_t = torch.tensor(norm4[:3], device="cuda").view(1, 3, 1, 1)
+
+    def chain():
+        r, c = det.detect_frame_list(frames, mean4=dmean, norm4=dnorm)
+        regions, count = ctx.rois_from_detections(r, c, FRAMELIST_SIZES, cbatch)
+        return cls.run_rois_list(frames, regions, count, mean4=mean4, norm4=norm4, want_classes=True)
+
+    def today():
+        rgb = [torch_nv12_to_rgb(torch, f[None]) for f in frames]
+        x = torch.cat([F.interpolate(t, size=dhw, mode="bilinear", align_corners=False) for t in rgb])
+        r, c = det.detect_torch(((x - mean_t) * norm_t).contiguous(), layout="nchw")
+        hr, hc = r.cpu().numpy(), c.cpu().numpy()  # synchronises
+        regions = []
+        for n, (h, w) in enumerate(FRAMELIST_SIZES):
+            regions += [(n,) + reg[1:] for reg in host_regions(hr[n:n + 1], hc[n:n + 1], h, w, cbatch)]
+        crops = [F.interpolate(rgb[n][:, :, y0:y1, x0:x1], size=chw, mode="bilinear", align_corners=False) for n, x0, y0, x1, y1 in regions[:cbatch]]
+        crops += [torch.zeros((cbatch - len(crops), 3) + chw, device="cuda")] if len(crops) < cbatch else []
+        return cls.run_torch(((torch.cat(crops) - mean_t) * norm_t).contiguous(), layout="nchw", want_classes=True)
+
+    runs, med = alternate(torch, {"chain": chain, "today": today}, args.seconds, dbatch, args.rounds)
+    kept = int(ctx.rois_from_detections(*det.detect_frame_list(frames, mean4=dmean, norm4=dnorm), FRAMELIST_SIZES, cbatch)[1].item())
+    mix = "4 x 3840x2160 + 8 x 1920x1080 + 4 x 1280x720 NV12, each its own allocation"
+    res = {"chain": {
+        "case": "yolov3tiny all-pass heads %dx%d batch %d from %s -> %d regions -> resnet18 %dx%d batch %d" % (dhw[0], dhw[1], dbatch, mix, kept, chw[0],
+                                                                                                           chw[1], cbatch),
+        "chain_path": "detect_frame_list -> rois_from_detections (per-frame sizes) -> run_rois_list (+ device classes); no host synchronisation",
+        "today_path": "per frame torch NV12 -> RGB + F.interpolate into one batch, normalise, detect_torch; rows + counts to the host; per-box crop + "
+                      "F.interpolate, stack + normalise, run_torch",
+        "regions_per_batch": kept,
+        "chain_frames_per_s_median": med["chain"],
+        "today_frames_per_s_median": med["today"],
+        "chain_over_today": med["chain"] / med["today"],
+        "rounds": runs,
+        "kernels": {k: frame_kernel_us(torch, chain, 50, k) for k in ("frame_list_input_kernel", "rois_from_detections_list_kernel", "frame_list_roi_input_kernel",
+                                                                     "roi_list_clear_kernel")},
+    }}
+    # the cost of the per-image descriptor: the same uniform 1080p batch through frame_input_kernel and frame_list_input_kernel
+    nv12 = torch.randint(16, 236, (dbatch, 1080 * 3 // 2, 1920), dtype=torch.uint8, generator=g).cuda()
+    views = [nv12[n] for n in range(dbatch)]
+    batch_kt = frame_kernel_us(torch, lambda: det.detect_frames(nv12, mean4=dmean, norm4=dnorm), 50, "frame_input_kernel")
+    list_kt = frame_kernel_us(torch, lambda: det.detect_frame_list(views, mean4=dmean, norm4=dnorm), 50, "frame_list_input_kernel")
+    res["uniform_1080p"] = {"case": "yolov3tiny %dx%d batch %d from 1920x1080 NV12: the input kernel alone" % (dhw[0], dhw[1], dbatch),
+                            "frame_input_kernel": batch_kt, "frame_list_input_kernel": list_kt,
+                            "list_over_batch_time": list_kt["us_per_batch"] / batch_kt["us_per_batch"]}
+    det.close()
+    cls.close()
+    return res
+
+
 def p010_surface(torch, batch, H, W, seed):
     """Random 10-bit frames as P010 words [N, H * 3 // 2, W] uint16 on the device (limited-range values, low 6 bits zero)."""
     rng = np.random.default_rng(seed)
@@ -775,7 +850,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
                     help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in), "
-                         "segment (opt-in), p010 (opt-in)")
+                         "segment (opt-in), p010 (opt-in), framelist (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -802,6 +877,8 @@ def main():
         result["luma"] = luma(torch, ctx, core, modelzoo, d, args)
     if "segment" in parts:
         result["segment"] = segment(torch, ctx, core, modelzoo, d, args)
+    if "framelist" in parts:
+        result["framelist"] = framelist(torch, ctx, core, modelzoo, d, args)
     if "p010" in parts:
         result["p010"] = p010(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
