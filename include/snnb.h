@@ -499,6 +499,51 @@ int snnb_model_run_rois_list(snnb_model* m, const snnb_frame_list* frames, const
 int snnb_rois_from_detections_list(snnb_context* ctx, const float* rows_dev, const int* counts_dev, int num_frames, int max_rows,
                                    const int* frame_wh, const snnb_roi_select* sel, snnb_roi* rois_dev, int capacity, int* count_dev,
                                    void* stream);
+/* Output lists: the frame-writing paths with one output descriptor per image, so that each stream of a multi-stream service gets its
+ * result in its own surface (its encoder's, or the decoded frame itself) at its own size. As for snnb_frame_list, the descriptors are a
+ * HOST array read during the call only; they reach the kernel by value. */
+typedef struct {
+    uint8_t* plane[3];  /* as snnb_frames_out.plane, for this image only */
+    int pitch[3];       /* as snnb_frames_out.pitch */
+    int width, height;  /* this image's output size, any >= 1 (odd allowed) */
+} snnb_frame_out_image;
+typedef struct {
+    int format;                         /* SNNB_FRAME_*: one format for every image */
+    int count;                          /* number of images */
+    const snnb_frame_out_image* images; /* HOST array of `count` descriptors */
+    int linear_filter;                  /* as snnb_frames_out */
+    float scale, offset;                /* as snnb_frames_out */
+} snnb_frame_out_list;
+typedef struct {
+    uint8_t* plane;     /* as snnb_labels_out.plane, for this image only */
+    int pitch;          /* bytes per row, >= width */
+    int width, height;  /* this image's label plane size, any >= 1 */
+} snnb_labels_image;
+typedef struct {
+    int count;                       /* number of images */
+    const snnb_labels_image* images; /* HOST array of `count` descriptors */
+    int linear_filter;               /* as snnb_labels_out */
+    float threshold;                 /* as snnb_labels_out */
+} snnb_labels_list;
+/* snnb_model_transform_frames / snnb_model_transform_luma / snnb_model_segment_frames with a frame list in and an output list out, both
+ * of exactly the loaded batch of images (<= SNNB_FRAME_LIST_MAX). Out image i is bit for bit what the batch call writes for image i when
+ * it is fed a batch whose every frame is input image i and writes an output of out image i's size: every rule of the batch calls holds
+ * per image (quantisation, resize taps, blend, libyuv rows, the P010 steps, arg-max and threshold, pixels past an odd width or height;
+ * bytes outside the rows are never written). The stream contract and the fences are those of the batch calls; a capturing stream is
+ * refused. Checked on the host before anything is enqueued, each error naming the image: everything snnb_model_run_frame_list checks on
+ * the input (with luma, also the Y-plane rules of snnb_model_transform_luma), a non-null out with non-null `images` and count == the
+ * input's count; per out image, width and height >= 1, each used pitch >= its row's bytes (labels: pitch >= width), each used plane
+ * device or managed memory of the context's device (P010: even pitches, 2-byte-aligned planes); output 0's channel count and the YOLO
+ * rule exactly as the batch calls check them.
+ * Aliasing: transform_frame_list and segment_frame_list write after the forward pass, so their outputs may overlap the input frames.
+ * transform_luma_list reads the source chroma while it writes and runs every image in one kernel: out image i may be input image i
+ * itself (same format, size, planes and pitches: an in-place luma filter); otherwise no out plane of any image may overlap a source
+ * chroma plane of any image, image j != i included. P010 pairs with P010 only, for the whole list.
+ * Cost beyond the forward pass: one kernel launch for the input and one for the output, the output grid sized by each image's own
+ * output (DESIGN.md section 4 has the measured cost). */
+int snnb_model_transform_frame_list(snnb_model* m, const snnb_frame_list* frames, const snnb_frame_out_list* out, void* stream);
+int snnb_model_transform_luma_list(snnb_model* m, const snnb_frame_list* frames, const snnb_frame_out_list* out, void* stream);
+int snnb_model_segment_frame_list(snnb_model* m, const snnb_frame_list* frames, int luma, const snnb_labels_list* out, void* stream);
 /* Device-resident variant: inputs already uploaded with snnb_model_set_input(); forward only, asynchronous. */
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input_nhwc);
 int snnb_model_forward(snnb_model* m);

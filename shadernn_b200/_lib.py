@@ -152,6 +152,48 @@ class FrameList(C.Structure):
 FRAME_LIST_MAX = 256
 
 
+class FrameOutImage(C.Structure):
+    """snnb_frame_out_image"""
+    _fields_ = [
+        ("plane", C.c_void_p * 3),
+        ("pitch", C.c_int * 3),
+        ("width", C.c_int),
+        ("height", C.c_int),
+    ]
+
+
+class FrameOutList(C.Structure):
+    """snnb_frame_out_list"""
+    _fields_ = [
+        ("format", C.c_int),
+        ("count", C.c_int),
+        ("images", C.POINTER(FrameOutImage)),
+        ("linear_filter", C.c_int),
+        ("scale", C.c_float),
+        ("offset", C.c_float),
+    ]
+
+
+class LabelsImage(C.Structure):
+    """snnb_labels_image"""
+    _fields_ = [
+        ("plane", C.c_void_p),
+        ("pitch", C.c_int),
+        ("width", C.c_int),
+        ("height", C.c_int),
+    ]
+
+
+class LabelsList(C.Structure):
+    """snnb_labels_list"""
+    _fields_ = [
+        ("count", C.c_int),
+        ("images", C.POINTER(LabelsImage)),
+        ("linear_filter", C.c_int),
+        ("threshold", C.c_float),
+    ]
+
+
 class Roi(C.Structure):
     """snnb_roi"""
     _fields_ = [
@@ -247,6 +289,9 @@ SIGNATURES = {
     "snnb_model_detect_frame_list": (C.c_int, [vp, C.POINTER(FrameList), vp, C.c_int, vp, vp]),
     "snnb_model_run_rois_list": (C.c_int, [vp, C.POINTER(FrameList), vp, vp, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
     "snnb_rois_from_detections_list": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, C.POINTER(RoiSelect), vp, C.c_int, vp, vp]),
+    "snnb_model_transform_frame_list": (C.c_int, [vp, C.POINTER(FrameList), C.POINTER(FrameOutList), vp]),
+    "snnb_model_transform_luma_list": (C.c_int, [vp, C.POINTER(FrameList), C.POINTER(FrameOutList), vp]),
+    "snnb_model_segment_frame_list": (C.c_int, [vp, C.POINTER(FrameList), C.c_int, C.POINTER(LabelsList), vp]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),

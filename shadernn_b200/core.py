@@ -822,6 +822,96 @@ class MixedInferenceCore:
         check(lib().snnb_model_segment_frames(self.h, C.byref(f), int(bool(luma)), C.byref(o), self._torch_stream()), "snnb_model_segment_frames")
         return out
 
+    def _frame_out_list(self, who, frames, out, out_format, out_hw, luma):
+        """Output frames of transform_frame_list / transform_luma_list: `out` (one CUDA tensor per image in _frames' layouts without the
+        batch dimension, any sizes), or when None one allocated per image at out_hw[i] (default: frame i's own size). Returns (out,
+        the snnb_frame_out_image array, which must stay alive until the call returns)."""
+        import torch
+        if out_format not in self._FRAME_FORMATS or (luma and out_format == "rgba8"):
+            raise ValueError("%s: out_format %r: expected one of %s" % (who, out_format, sorted(set(self._FRAME_FORMATS) - ({"rgba8"} if luma else set()))))
+        if out is None:
+            sizes = [self._frame_hw(who, x) for x in frames] if out_hw is None else [(int(h), int(w)) for h, w in out_hw]
+            if len(sizes) != len(frames):
+                raise ValueError("%s: %d out sizes for %d frames" % (who, len(sizes), len(frames)))
+            if out_format != "rgba8" and any(h % 2 or w % 2 for h, w in sizes):
+                raise ValueError("%s: %s frames of sizes %s: the packed layout needs H and W even" % (who, out_format, sizes))
+            dtype = torch.uint16 if out_format == "p010" else torch.uint8
+            device = torch.device("cuda", self.ctx.device)
+            out = [torch.empty((h, w, 4) if out_format == "rgba8" else (h * 3 // 2, w), dtype=dtype, device=device) for h, w in sizes]
+        out = list(out)
+        if len(out) != len(frames):
+            raise ValueError("%s: %d out frames for %d frames" % (who, len(out), len(frames)))
+        images = (_lib.FrameOutImage * max(1, len(out)))()
+        for i, x in enumerate(out):
+            o = _lib.FramesOut()
+            if not hasattr(x, "unsqueeze"):
+                raise ValueError("%s: out frame %d must be a CUDA tensor" % (who, i))
+            self._frame_planes(who, "out frame %d" % i, x.unsqueeze(0), out_format, o)
+            if out_hw is not None and (o.height, o.width) != tuple(int(v) for v in out_hw[i]):
+                raise ValueError("%s: out frame %d is %d x %d; expected %d x %d" % (who, i, o.height, o.width, out_hw[i][0], out_hw[i][1]))
+            images[i].plane, images[i].pitch, images[i].width, images[i].height = o.plane, o.pitch, o.width, o.height
+        return out, images
+
+    def _frame_hw(self, who, x):
+        """(H, W) of one frame tensor in _frames' layouts without the batch dimension"""
+        if not hasattr(x, "dim") or x.dim() not in (2, 3):
+            raise ValueError("%s: each frame must be a CUDA tensor [H * 3 // 2, W] or [H, W, 4]" % who)
+        return (x.shape[0], x.shape[1]) if x.dim() == 3 else (x.shape[0] // 3 * 2, x.shape[1])
+
+    def transform_frame_list(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_format=None, out_hw=None,
+                             out_linear=True, out_scale=1.0, out_offset=0.0, out=None):
+        """snnb_model_transform_frame_list: transform_frames on a list of separately allocated frames of mixed sizes (as run_frame_list
+        takes them), each image written to its own out frame. out: a list of one CUDA tensor per image in _frames' layouts without the
+        batch dimension, or None to allocate one per image at out_hw[i] (default: frame i's own size); it may be `frames` itself. Out
+        image i is exactly what transform_frames writes for a batch of frame i alone. Returns the list of out frames."""
+        if len(frames) != self.batch:
+            raise ValueError("transform_frame_list: %d frames given, the model's batch is %d" % (len(frames), self.batch))
+        out_format = format if out_format is None else out_format
+        fl, keep = self._frame_list("transform_frame_list", frames, format, matrix, linear, mean4, norm4)
+        out, images = self._frame_out_list("transform_frame_list", frames, out, out_format, out_hw, False)
+        ol = _lib.FrameOutList(self._FRAME_FORMATS[out_format], len(out), images, int(bool(out_linear)), float(out_scale), float(out_offset))
+        check(lib().snnb_model_transform_frame_list(self.h, C.byref(fl), C.byref(ol), self._torch_stream()), "snnb_model_transform_frame_list")
+        return out
+
+    def transform_luma_list(self, frames, format="nv12", linear=True, mean=0.0, norm=1.0, out_format=None, out_hw=None, out_linear=True, out_scale=1.0,
+                            out_offset=0.0, out=None):
+        """snnb_model_transform_luma_list: transform_luma on a list of frames of mixed sizes, out as transform_frame_list takes it.
+        out=frames is the in-place luma filter; otherwise no out frame may overlap the chroma of any source frame."""
+        if len(frames) != self.batch:
+            raise ValueError("transform_luma_list: %d frames given, the model's batch is %d" % (len(frames), self.batch))
+        out_format = format if out_format is None else out_format
+        fl, keep = self._frame_list("transform_luma_list", frames, format, "bt601", linear, [float(mean)] * 4, [float(norm)] * 4)
+        out, images = self._frame_out_list("transform_luma_list", frames, out, out_format, out_hw, True)
+        ol = _lib.FrameOutList(self._FRAME_FORMATS[out_format], len(out), images, int(bool(out_linear)), float(out_scale), float(out_offset))
+        check(lib().snnb_model_transform_luma_list(self.h, C.byref(fl), C.byref(ol), self._torch_stream()), "snnb_model_transform_luma_list")
+        return out
+
+    def segment_frame_list(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, luma=False, out_hw=None, out_linear=True,
+                           threshold=0.5, out=None):
+        """snnb_model_segment_frame_list: segment_frames on a list of frames of mixed sizes. out: a list of one uint8 CUDA tensor [H, W]
+        (dense pixels, any row stride) per image, or None to allocate one per image at out_hw[i] (default: frame i's own size). Image i's
+        labels are exactly what segment_frames writes for a batch of frame i alone. Returns the list of label planes."""
+        import torch
+        if len(frames) != self.batch:
+            raise ValueError("segment_frame_list: %d frames given, the model's batch is %d" % (len(frames), self.batch))
+        fl, keep = self._frame_list("segment_frame_list", frames, format, matrix, linear, mean4, norm4)
+        if out is None:
+            sizes = [self._frame_hw("segment_frame_list", x) for x in frames] if out_hw is None else [(int(h), int(w)) for h, w in out_hw]
+            out = [torch.empty(hw, dtype=torch.uint8, device=torch.device("cuda", self.ctx.device)) for hw in sizes]
+        out = list(out)
+        if len(out) != len(frames):
+            raise ValueError("segment_frame_list: %d label planes for %d frames" % (len(out), len(frames)))
+        images = (_lib.LabelsImage * max(1, len(out)))()
+        for i, x in enumerate(out):
+            if not (isinstance(x, torch.Tensor) and x.dtype == torch.uint8 and x.dim() == 2 and x.stride(1) == 1):
+                raise ValueError("segment_frame_list: label plane %d must be a uint8 CUDA tensor [H, W] with dense pixels" % i)
+            if out_hw is not None and tuple(x.shape) != tuple(int(v) for v in out_hw[i]):
+                raise ValueError("segment_frame_list: label plane %d is %d x %d; expected %d x %d" % (i, x.shape[0], x.shape[1], out_hw[i][0], out_hw[i][1]))
+            images[i].plane, images[i].pitch, images[i].height, images[i].width = x.data_ptr(), x.stride(0), x.shape[0], x.shape[1]
+        ol = _lib.LabelsList(len(out), images, int(bool(out_linear)), float(threshold))
+        check(lib().snnb_model_segment_frame_list(self.h, C.byref(fl), int(bool(luma)), C.byref(ol), self._torch_stream()), "snnb_model_segment_frame_list")
+        return out
+
     def set_input(self, images, idx=0):
         images = _f32(images)
         check(lib().snnb_model_set_input(self.h, idx, _ptr(images)), "snnb_model_set_input")

@@ -772,7 +772,7 @@ int MixedInferenceCore::enqueueDeviceForward(const DeviceFeed& in, cudaStream_t 
     } else if (in.rois) {
         if (launch_frame_roi_input(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, inputLayers[0]->output)) return 1;
     } else if (in.list) {
-        if (launch_frame_list_input(ctx, *in.list, inputLayers[0]->output)) return 1;
+        if (launch_frame_list_input(ctx, *in.list, inputLayers[0]->output, in.luma)) return 1;
     } else if (in.frames) {
         if (launch_frame_input(ctx, *in.frames, inputLayers[0]->output, in.luma)) return 1;
     } else {
@@ -906,26 +906,55 @@ int MixedInferenceCore::detectDeviceFeed(const char* api, const DeviceFeed& in, 
     return fenceToCaller(stream);
 }
 
+// The out frames of transform / transform_luma: one snnb_frames_out, or (ol) each image of an output list, which must hold one image per
+// frame of the input list. Each size, then each image's planes, in transform_frames' order of checks; list errors name the image.
+static int checkFramesOut(const char* api, const snnb_frames_out* o, const snnb_frame_out_list* ol, int frames, int device) {
+    static const long long noStride[3] = {0, 0, 0};
+    if (ol) {
+        SNNB_REQUIRE(ol->images, "%s: null out images", api);
+        SNNB_REQUIRE(ol->count == frames, "%s: out count %d; the out list must hold one image per frame (%d)", api, ol->count, frames);
+    }
+    const int format = o ? o->format : ol->format;
+    char image[32] = "", planes[40] = "out plane";
+    for (int i = 0; i < (o ? 1 : ol->count); ++i) {
+        if (ol) std::snprintf(image, sizeof(image), "image %d: ", i), std::snprintf(planes, sizeof(planes), "image %d out plane", i);
+        const int w = o ? o->width : ol->images[i].width, h = o ? o->height : ol->images[i].height;
+        SNNB_REQUIRE(w >= 1 && h >= 1, "%s: %sout frame size %d x %d; width and height must be >= 1", api, image, w, h);
+        const int rc = o ? checkFramePlanes(api, planes, format, w, o->plane, o->pitch, o->image_stride, device)
+                         : checkFramePlanes(api, planes, format, w, ol->images[i].plane, ol->images[i].pitch, noStride, device);
+        if (rc) return rc;
+    }
+    return 0;
+}
+
 // Frames in, frames out: runFrames' input staging and forward pass, then output 0 quantised, resized and colour-converted into `out` in
 // one kernel. The output kernel runs after the forward pass on the context's stream, so `out` may alias the input frames.
 int MixedInferenceCore::transformFrames(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream) {
-    static const char* api = "snnb_model_transform_frames";
     SNNB_REQUIRE(frames, "snnb_model_transform_frames: null frames");
     SNNB_REQUIRE(out, "snnb_model_transform_frames: null out");
     DeviceFeed in;
     in.frames = frames;
+    return transformDeviceFeed("snnb_model_transform_frames", in, out, nullptr, stream);
+}
+int MixedInferenceCore::transformFrameList(const snnb_frame_list* frames, const snnb_frame_out_list* out, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_transform_frame_list: null frames");
+    SNNB_REQUIRE(out, "snnb_model_transform_frame_list: null out");
+    DeviceFeed in;
+    in.list = frames;
+    return transformDeviceFeed("snnb_model_transform_frame_list", in, nullptr, out, stream);
+}
+int MixedInferenceCore::transformDeviceFeed(const char* api, const DeviceFeed& in, const snnb_frames_out* o, const snnb_frame_out_list* ol, cudaStream_t stream) {
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
-    const snnb_frames_out& o = *out;
-    SNNB_REQUIRE(knownFrameFormat(o.format), "%s: unknown out frame format %d", api, o.format);
-    SNNB_REQUIRE(o.width >= 1 && o.height >= 1, "%s: out frame size %d x %d; width and height must be >= 1", api, o.width, o.height);
-    if (int rc = checkFramePlanes(api, "out plane", o.format, o.width, o.plane, o.pitch, o.image_stride, ctx->device)) return rc;
+    const int format = o ? o->format : ol->format;
+    SNNB_REQUIRE(knownFrameFormat(format), "%s: unknown out frame format %d", api, format);
+    if (int rc = checkFramesOut(api, o, ol, in.list ? in.list->count : 1, ctx->device)) return rc;
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; frames are written from an image output", api);
     const snnb_tensor* t = outputLayers[0]->output;
     SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
     SNNB_REQUIRE(t->c == 1 || t->c == 3 || t->c == 4, "%s: output 0 has %d channels; frames are written from 1 (grey), 3 (RGB) or 4 (RGBA)", api, t->c);
 
     if (enqueueDeviceForward(in, stream)) return 1;
-    if (launch_frame_output(ctx, t, o)) return 1;
+    if (o ? launch_frame_output(ctx, t, *o) : launch_frame_list_output(ctx, t, *ol)) return 1;
     return fenceToCaller(stream);
 }
 
@@ -942,45 +971,80 @@ static bool planeExtent(int format, int width, int height, const uint8_t* plane,
 
 // Luma frames in, luma frames out: the Y plane feeds a 1-channel model, output 0 (1 channel) becomes the Y plane of `out`, and the same
 // output kernel resamples the source frames' chroma into out's chroma. The kernel reads the source chroma while it writes, so out must
-// keep clear of it unless out is the source frames themselves (each chroma sample is then read and written by one thread).
+// keep clear of it unless out is the source frames themselves (each chroma sample is then read and written by one thread). A list runs
+// every image in one kernel: out image i may be source image i itself, and must keep clear of every other image's source chroma.
 int MixedInferenceCore::transformLuma(const snnb_frames* frames, const snnb_frames_out* out, cudaStream_t stream) {
-    static const char* api = "snnb_model_transform_luma";
     SNNB_REQUIRE(frames, "snnb_model_transform_luma: null frames");
     SNNB_REQUIRE(out, "snnb_model_transform_luma: null out");
     DeviceFeed in;
     in.frames = frames, in.luma = true;
+    return transformLumaDeviceFeed("snnb_model_transform_luma", in, out, nullptr, stream);
+}
+int MixedInferenceCore::transformLumaList(const snnb_frame_list* frames, const snnb_frame_out_list* out, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_transform_luma_list: null frames");
+    SNNB_REQUIRE(out, "snnb_model_transform_luma_list: null out");
+    DeviceFeed in;
+    in.list = frames, in.luma = true;
+    return transformLumaDeviceFeed("snnb_model_transform_luma_list", in, nullptr, out, stream);
+}
+int MixedInferenceCore::transformLumaDeviceFeed(const char* api, const DeviceFeed& in, const snnb_frames_out* o, const snnb_frame_out_list* ol,
+                                                cudaStream_t stream) {
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
-    const snnb_frames& f     = *frames;
-    const snnb_frames_out& o = *out;
-    SNNB_REQUIRE(knownFrameFormat(o.format), "%s: unknown out frame format %d", api, o.format);
-    SNNB_REQUIRE(o.format != SNNB_FRAME_RGBA8, "%s: out format RGBA8 has no Y plane; luma frames are written as NV12, NV21, I420 or P010", api);
-    SNNB_REQUIRE((o.format == SNNB_FRAME_P010) == (f.format == SNNB_FRAME_P010),
-                 "%s: frames format %d, out format %d: the bit depths differ; P010 frames are written from P010 frames only", api, f.format, o.format);
-    SNNB_REQUIRE(o.width >= 1 && o.height >= 1, "%s: out frame size %d x %d; width and height must be >= 1", api, o.width, o.height);
-    if (int rc = checkFramePlanes(api, "out plane", o.format, o.width, o.plane, o.pitch, o.image_stride, ctx->device)) return rc;
+    const snnb_frames* f = in.frames;
+    const snnb_frame_list* fl = in.list;
+    const int format = f ? f->format : fl->format, oformat = o ? o->format : ol->format;
+    SNNB_REQUIRE(knownFrameFormat(oformat), "%s: unknown out frame format %d", api, oformat);
+    SNNB_REQUIRE(oformat != SNNB_FRAME_RGBA8, "%s: out format RGBA8 has no Y plane; luma frames are written as NV12, NV21, I420 or P010", api);
+    SNNB_REQUIRE((oformat == SNNB_FRAME_P010) == (format == SNNB_FRAME_P010),
+                 "%s: frames format %d, out format %d: the bit depths differ; P010 frames are written from P010 frames only", api, format, oformat);
+    const int images = fl ? fl->count : 1;
+    if (int rc = checkFramesOut(api, o, ol, images, ctx->device)) return rc;
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; frames are written from an image output", api);
     const snnb_tensor* t = outputLayers[0]->output;
     SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
     SNNB_REQUIRE(t->c == 1, "%s: output 0 has %d channels; the Y plane is written from exactly 1", api, t->c);
-    bool same = o.format == f.format && o.width == f.width && o.height == f.height;
-    for (int p = 0; p < 3 && same; ++p)
-        if (frameRowBytes(f.format, f.width, p)) same = o.plane[p] == f.plane[p] && o.pitch[p] == f.pitch[p] && o.image_stride[p] == f.image_stride[p];
-    if (!same) {
-        const int n = (int) options.batch;
-        for (int p = 0; p < 3; ++p) {
-            uintptr_t ob, oe;
-            if (!planeExtent(o.format, o.width, o.height, o.plane[p], o.pitch[p], o.image_stride[p], n, p, ob, oe)) continue;
-            for (int q = 1; q < 3; ++q) {
-                uintptr_t sb, se;
-                if (!planeExtent(f.format, f.width, f.height, f.plane[q], f.pitch[q], f.image_stride[q], n, q, sb, se)) continue;
-                SNNB_REQUIRE(oe <= sb || se <= ob, "%s: out plane %d overlaps source chroma plane %d; out may alias the source chroma only as the source frames themselves",
-                             api, p, q);
+    // image i of either side: a batch is one image of `n` at its image strides, a list image is one image of its own (stride 0)
+    const int n = f ? (int) options.batch : 1;
+    auto outExtent = [&](int i, int p, uintptr_t& b, uintptr_t& e) {
+        return o ? planeExtent(oformat, o->width, o->height, o->plane[p], o->pitch[p], o->image_stride[p], n, p, b, e)
+                 : planeExtent(oformat, ol->images[i].width, ol->images[i].height, ol->images[i].plane[p], ol->images[i].pitch[p], 0, 1, p, b, e);
+    };
+    auto srcExtent = [&](int j, int q, uintptr_t& b, uintptr_t& e) {
+        return f ? planeExtent(format, f->width, f->height, f->plane[q], f->pitch[q], f->image_stride[q], n, q, b, e)
+                 : planeExtent(format, fl->images[j].width, fl->images[j].height, fl->images[j].plane[q], fl->images[j].pitch[q], 0, 1, q, b, e);
+    };
+    auto inPlace = [&](int i) {
+        const int ow = o ? o->width : ol->images[i].width, oh = o ? o->height : ol->images[i].height;
+        const int sw = f ? f->width : fl->images[i].width, sh = f ? f->height : fl->images[i].height;
+        bool same = oformat == format && ow == sw && oh == sh;
+        for (int p = 0; p < 3 && same; ++p)
+            if (frameRowBytes(format, sw, p))
+                same = f ? o->plane[p] == f->plane[p] && o->pitch[p] == f->pitch[p] && o->image_stride[p] == f->image_stride[p]
+                         : ol->images[i].plane[p] == fl->images[i].plane[p] && ol->images[i].pitch[p] == fl->images[i].pitch[p];
+        return same;
+    };
+    char oname[24] = "", sname[24] = "";
+    for (int i = 0; i < images; ++i) {
+        const bool same = inPlace(i);
+        for (int j = 0; j < images; ++j) {
+            if (j == i && same) continue;
+            if (fl) std::snprintf(oname, sizeof(oname), "image %d ", i), std::snprintf(sname, sizeof(sname), "image %d ", j);
+            for (int p = 0; p < 3; ++p) {
+                uintptr_t ob, oe;
+                if (!outExtent(i, p, ob, oe)) continue;
+                for (int q = 1; q < 3; ++q) {
+                    uintptr_t sb, se;
+                    if (!srcExtent(j, q, sb, se)) continue;
+                    SNNB_REQUIRE(oe <= sb || se <= ob,
+                                 "%s: %sout plane %d overlaps %ssource chroma plane %d; out may alias the source chroma only as the source frames themselves", api,
+                                 oname, p, sname, q);
+                }
             }
         }
     }
 
     if (enqueueDeviceForward(in, stream)) return 1;
-    if (launch_luma_output(ctx, t, f, o)) return 1;
+    if (f ? launch_luma_output(ctx, t, *f, *o) : launch_luma_list_output(ctx, t, *fl, *ol)) return 1;
     return fenceToCaller(stream);
 }
 
@@ -988,23 +1052,40 @@ int MixedInferenceCore::transformLuma(const snnb_frames* frames, const snnb_fram
 // to the label plane and reduced to one byte per pixel in one kernel. The kernel reads only the model's tensor, so the plane may alias
 // the input frames.
 int MixedInferenceCore::segmentFrames(const snnb_frames* frames, bool luma, const snnb_labels_out* out, cudaStream_t stream) {
-    static const char* api = "snnb_model_segment_frames";
     SNNB_REQUIRE(frames, "snnb_model_segment_frames: null frames");
     SNNB_REQUIRE(out, "snnb_model_segment_frames: null out");
     DeviceFeed in;
     in.frames = frames, in.luma = luma;
+    return segmentDeviceFeed("snnb_model_segment_frames", in, out, nullptr, stream);
+}
+int MixedInferenceCore::segmentFrameList(const snnb_frame_list* frames, bool luma, const snnb_labels_list* out, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_segment_frame_list: null frames");
+    SNNB_REQUIRE(out, "snnb_model_segment_frame_list: null out");
+    DeviceFeed in;
+    in.list = frames, in.luma = luma;
+    return segmentDeviceFeed("snnb_model_segment_frame_list", in, nullptr, out, stream);
+}
+int MixedInferenceCore::segmentDeviceFeed(const char* api, const DeviceFeed& in, const snnb_labels_out* o, const snnb_labels_list* ol, cudaStream_t stream) {
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
-    const snnb_labels_out& o = *out;
-    SNNB_REQUIRE(o.width >= 1 && o.height >= 1, "%s: label plane size %d x %d; width and height must be >= 1", api, o.width, o.height);
-    SNNB_REQUIRE(o.pitch >= o.width, "%s: label plane pitch %d is less than its width %d", api, o.pitch, o.width);
-    if (int rc = checkDevicePointer(api, o.plane, 1, ctx->device, "label plane", 0)) return rc;
+    if (ol) {
+        SNNB_REQUIRE(ol->images, "%s: null out images", api);
+        SNNB_REQUIRE(ol->count == in.list->count, "%s: out count %d; the out list must hold one image per frame (%d)", api, ol->count, in.list->count);
+    }
+    char image[32] = "", plane[40] = "label plane";
+    for (int i = 0; i < (o ? 1 : ol->count); ++i) {
+        if (ol) std::snprintf(image, sizeof(image), "image %d: ", i), std::snprintf(plane, sizeof(plane), "image %d label plane", i);
+        const int w = o ? o->width : ol->images[i].width, h = o ? o->height : ol->images[i].height, pitch = o ? o->pitch : ol->images[i].pitch;
+        SNNB_REQUIRE(w >= 1 && h >= 1, "%s: %slabel plane size %d x %d; width and height must be >= 1", api, image, w, h);
+        SNNB_REQUIRE(pitch >= w, "%s: %slabel plane pitch %d is less than its width %d", api, image, pitch, w);
+        if (int rc = checkDevicePointer(api, o ? o->plane : ol->images[i].plane, 1, ctx->device, plane, 0)) return rc;
+    }
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; labels are written from per-pixel class scores", api);
     const snnb_tensor* t = outputLayers[0]->output;
     SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
     SNNB_REQUIRE(t->c >= 1 && t->c <= 256, "%s: output 0 has %d channels; an 8-bit label plane is written from 1 to 256", api, t->c);
 
     if (enqueueDeviceForward(in, stream)) return 1;
-    if (launch_segment_output(ctx, t, o)) return 1;
+    if (o ? launch_segment_output(ctx, t, *o) : launch_segment_list_output(ctx, t, *ol)) return 1;
     return fenceToCaller(stream);
 }
 

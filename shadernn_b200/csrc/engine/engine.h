@@ -367,6 +367,11 @@ public:
     int detectFrameList(const snnb_frame_list* frames, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
     int runRoisList(const snnb_frame_list* frames, const snnb_roi* roisDev, const int* countDev, const snnb_device_buffer* outputs, int numOutputs,
                     int* classes1Dev, cudaStream_t stream);
+    // snnb_model_transform_frame_list / transform_luma_list / segment_frame_list: transformFrames / transformLuma / segmentFrames with a
+    // frame list in and one output descriptor per image out
+    int transformFrameList(const snnb_frame_list* frames, const snnb_frame_out_list* out, cudaStream_t stream);
+    int transformLumaList(const snnb_frame_list* frames, const snnb_frame_out_list* out, cudaStream_t stream);
+    int segmentFrameList(const snnb_frame_list* frames, bool luma, const snnb_labels_list* out, cudaStream_t stream);
     int layerOutput(int layerId, float* host, size_t capacityFloats);
     int timeLayers(std::vector<float>& ms);
     int dumpOutputs(const std::string& dir);
@@ -442,6 +447,11 @@ private:
     // enqueued), then the fenced input staging + forward pass, the outputs or the detections, and the fence back to the caller's stream
     int runDeviceFeed(const char* api, const DeviceFeed& in, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
     int detectDeviceFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
+    // shared by the frame-writing calls and their list forms: the feed's checks, then out's (one batch description `o`, or the output
+    // list `ol`), output 0's, the forward pass, the output kernel and the fence
+    int transformDeviceFeed(const char* api, const DeviceFeed& in, const snnb_frames_out* o, const snnb_frame_out_list* ol, cudaStream_t stream);
+    int transformLumaDeviceFeed(const char* api, const DeviceFeed& in, const snnb_frames_out* o, const snnb_frame_out_list* ol, cudaStream_t stream);
+    int segmentDeviceFeed(const char* api, const DeviceFeed& in, const snnb_labels_out* o, const snnb_labels_list* ol, cudaStream_t stream);
     int checkDeviceFeed(const char* api, const DeviceFeed& in, cudaStream_t stream);
     int enqueueDeviceForward(const DeviceFeed& in, cudaStream_t stream);
     int fenceToCaller(cudaStream_t stream);

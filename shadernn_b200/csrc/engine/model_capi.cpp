@@ -182,6 +182,21 @@ int snnb_model_run_rois_list(snnb_model* m, const snnb_frame_list* frames, const
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->runRoisList(frames, rois_dev, count_dev, outputs, num_outputs, classes_1based_dev, static_cast<cudaStream_t>(stream));
 }
+int snnb_model_transform_frame_list(snnb_model* m, const snnb_frame_list* frames, const snnb_frame_out_list* out, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_transform_frame_list: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->transformFrameList(frames, out, static_cast<cudaStream_t>(stream));
+}
+int snnb_model_transform_luma_list(snnb_model* m, const snnb_frame_list* frames, const snnb_frame_out_list* out, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_transform_luma_list: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->transformLumaList(frames, out, static_cast<cudaStream_t>(stream));
+}
+int snnb_model_segment_frame_list(snnb_model* m, const snnb_frame_list* frames, int luma, const snnb_labels_list* out, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_segment_frame_list: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->segmentFrameList(frames, luma != 0, out, static_cast<cudaStream_t>(stream));
+}
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input) {
     SNNB_REQUIRE(m, "snnb_model_set_input: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));

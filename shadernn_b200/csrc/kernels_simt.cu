@@ -1902,7 +1902,7 @@ static U8Norm frame_list_norm(const snnb_frame_list& fl) {
     for (int i = 0; i < 4; ++i) q.mean[i] = fl.mean4[i], q.norm[i] = fl.norm4[i];
     return q;
 }
-int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t) {
+int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t, bool luma) {
     SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_list_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
     SNNB_REQUIRE(fl.count == t->n && fl.count <= SNNB_FRAME_LIST_MAX, "launch_frame_list_input: %d images for a batch of %d", fl.count, t->n);
     FrameListV L;
@@ -1910,6 +1910,15 @@ int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_t
     const U8Norm q   = frame_list_norm(fl);
     const int linear = fl.linear_filter ? 1 : 0;
     const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
+    if (luma) {
+        SNNB_REQUIRE(t->c == 1 && fl.format != SNNB_FRAME_RGBA8, "launch_frame_list_input: luma input feeds 1 channel from YUV frames (%d channels, format %d)",
+                     t->c, fl.format);
+        if (fl.format == SNNB_FRAME_P010)
+            return launch_done(ctx, launch_k(frame_list_input_kernel<FRAME_LUMA10>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)),
+                               "frame_list_input_kernel<luma10>");
+        return launch_done(ctx, launch_k(frame_list_input_kernel<FRAME_LUMA>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)),
+                           "frame_list_input_kernel<luma>");
+    }
     switch (fl.format) {
     case SNNB_FRAME_NV12:
         return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<nv12>");
@@ -2147,18 +2156,12 @@ __device__ __forceinline__ void store_2p010(uint8_t* p, int a, int b) {
     if ((reinterpret_cast<uintptr_t>(p) & 3) == 0) *reinterpret_cast<uint32_t*>(p) = (uint32_t) (a << 6) | ((uint32_t) (b << 6) << 16);
     else reinterpret_cast<uint16_t*>(p)[0] = (uint16_t) (a << 6), reinterpret_cast<uint16_t*>(p)[1] = (uint16_t) (b << 6);
 }
-// One thread per 2 x 2 block of frame pixels, i.e. per chroma sample: its 4 pixels of F, then 4 Y bytes and the chroma sample (or
-// 4 RGBA8 pixels). Pixels past an odd width or height are not written. P010: the same from M10, with the 8-bit coefficients and the
-// 10-bit offsets (64 and 512), stored as 16-bit words.
+// The 2 x 2 block (bx, by) of frame pixels of image n, i.e. one chroma sample: its 4 pixels of F, then 4 Y bytes and the chroma sample
+// (or 4 RGBA8 pixels). Pixels past an odd width or height are not written. P010: the same from M10, with the 8-bit coefficients and the
+// 10-bit offsets (64 and 512), stored as 16-bit words. Shared by frame_output_kernel and frame_list_output_kernel.
 template <int FMT>
-__global__ void __launch_bounds__(256) frame_output_kernel(TV t, FrameOutV o, int linear) {
+__device__ __forceinline__ void frame_out_block(const TV& t, const FrameOutV& o, int n, int bx, int by, int linear) {
     constexpr bool TEN = FMT == SNNB_FRAME_P010;
-    pdl_wait();
-    const int cw = (o.w + 1) >> 1, ch = (o.h + 1) >> 1;
-    const size_t total = (size_t) t.N * ch * cw;
-    const size_t gid   = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (gid >= total) return;
-    const int bx = (int) (gid % cw), by = (int) ((gid / cw) % ch), n = (int) (gid / ((size_t) cw * ch));
     const int x = 2 * bx, y = 2 * by;
     const bool has_x1 = x + 1 < o.w, has_y1 = y + 1 < o.h;
     int p[2][2][4];
@@ -2234,6 +2237,17 @@ __global__ void __launch_bounds__(256) frame_output_kernel(TV t, FrameOutV o, in
         else store_2u8(d, V, U);
     }
 }
+// One thread per 2 x 2 block of frame pixels (frame_out_block)
+template <int FMT>
+__global__ void __launch_bounds__(256) frame_output_kernel(TV t, FrameOutV o, int linear) {
+    pdl_wait();
+    const int cw = (o.w + 1) >> 1, ch = (o.h + 1) >> 1;
+    const size_t total = (size_t) t.N * ch * cw;
+    const size_t gid   = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= total) return;
+    const int bx = (int) (gid % cw), by = (int) ((gid / cw) % ch), n = (int) (gid / ((size_t) cw * ch));
+    frame_out_block<FMT>(t, o, n, bx, by, linear);
+}
 int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames_out& fr) {
     SNNB_REQUIRE((t->c == 1 || t->c == 3 || t->c == 4) && t->cp == 8 && !t->feed_only, "launch_frame_output: the output tensor has %d channels; frames are written from 1, 3 or 4",
                  t->c);
@@ -2290,6 +2304,55 @@ __device__ __forceinline__ void chroma_texel(const FrameV& s, int step, int n, i
     } else {
         u = (float) __ldg(s.plane[1] + n * s.stride[1] + (size_t) y * s.pitch[1] + (size_t) x * step);
         v = (float) __ldg(s.plane[2] + n * s.stride[2] + (size_t) y * s.pitch[2] + (size_t) x * step);
+    }
+}
+// The 2 x 2 block (bx, by) of frame pixels of image n for luma_list_output_kernel: luma_output_kernel's body below, through the same
+// helpers. It is written out twice because luma_output_kernel calling it compiles to different register allocation.
+template <int FMT>
+__device__ __forceinline__ void luma_out_block(const TV& t, const FrameV& s, int step, const FrameOutV& o, int n, int bx, int by, int linear) {
+    constexpr bool TEN = FMT == SNNB_FRAME_P010;
+    const int cw = (o.w + 1) >> 1, ch = (o.h + 1) >> 1;
+    const int x = 2 * bx, y = 2 * by;
+    const bool has_x1 = x + 1 < o.w, has_y1 = y + 1 < o.h;
+#pragma unroll
+    for (int dy = 0; dy < 2; ++dy) {
+        if (dy && !has_y1) break;
+        if constexpr (TEN) {
+            uint8_t* d   = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + (size_t) x * 2;
+            const int ya = luma_out_pixel<true>(t, o, n, x, y + dy, linear);
+            if (has_x1) store_2p010(d, ya, luma_out_pixel<true>(t, o, n, x + 1, y + dy, linear));
+            else *reinterpret_cast<uint16_t*>(d) = (uint16_t) (ya << 6);
+        } else {
+            uint8_t* d   = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + x;
+            const int ya = luma_out_pixel<false>(t, o, n, x, y + dy, linear);
+            if (has_x1) store_2u8(d, ya, luma_out_pixel<false>(t, o, n, x + 1, y + dy, linear));
+            else d[0] = (uint8_t) ya;
+        }
+    }
+    const int scw = (s.w + 1) >> 1, sch = (s.h + 1) >> 1;
+    const bool direct = cw == scw && ch == sch;
+    ResizeTaps r;
+    if (direct) r.x0 = r.x1 = bx, r.y0 = r.y1 = by, r.ax = r.ay = 0.0f;
+    else r = resize_taps(resize_pos(bx, by, cw, ch, scw, sch), scw, sch, linear);
+    float u00, v00;
+    chroma_texel<TEN>(s, step, n, r.x0, r.y0, u00, v00);
+    int U = (int) u00, V = (int) v00;
+    if (linear && !direct) {
+        float u01, v01, u10, v10, u11, v11;
+        chroma_texel<TEN>(s, step, n, r.x1, r.y0, u01, v01);
+        chroma_texel<TEN>(s, step, n, r.x0, r.y1, u10, v10);
+        chroma_texel<TEN>(s, step, n, r.x1, r.y1, u11, v11);
+        U = (int) rintf(blend_rn(r, u00, u01, u10, u11)), V = (int) rintf(blend_rn(r, v00, v01, v10, v11));
+    }
+    if (TEN) {
+        store_2p010(o.plane[1] + n * o.stride[1] + (size_t) by * o.pitch[1] + (size_t) bx * 4, U, V);
+    } else if (FMT == SNNB_FRAME_I420) {
+        o.plane[1][n * o.stride[1] + (size_t) by * o.pitch[1] + bx] = (uint8_t) U;
+        o.plane[2][n * o.stride[2] + (size_t) by * o.pitch[2] + bx] = (uint8_t) V;
+    } else {
+        uint8_t* d = o.plane[1] + n * o.stride[1] + (size_t) by * o.pitch[1] + (size_t) bx * 2;
+        if (FMT == SNNB_FRAME_NV12) store_2u8(d, U, V);
+        else store_2u8(d, V, U);
     }
 }
 // One thread per 2 x 2 block of frame pixels, i.e. per chroma sample, as frame_output_kernel: 4 Y bytes, then the chroma sample resized
@@ -2463,6 +2526,220 @@ int launch_segment_output(snnb_context* ctx, const snnb_tensor* t, const snnb_la
         block(SEG_THREADS);
     if (t->c == 1) return launch_done(ctx, launch_k(segment_output_kernel<true>, grid, block, 0, ctx->stream, view(t), o, linear), "segment_output_kernel<threshold>");
     return launch_done(ctx, launch_k(segment_output_kernel<false>, grid, block, 0, ctx->stream, view(t), o, linear), "segment_output_kernel<argmax>");
+}
+
+// Output lists (snnb_model_transform_frame_list / transform_luma_list / segment_frame_list): slot n of the model's output 0 written to
+// out image n, each image its own allocation and size. Each table is a __grid_constant__ parameter, as FrameListV, with compact entries
+// (no image strides) so that the luma kernel's source chroma and destination tables for 256 images fit the 32,764-byte parameter limit
+// together. The work per image differs (a 2160p image has 9x the 2 x 2 blocks of a 720p one), so the grid is the sum of each image's own
+// CTA count: first[n] is image n's first CTA, and a CTA finds its image by a binary search on blockIdx.x. The search is uniform across
+// the CTA, so its constant-bank reads broadcast. Inside the image, indexing is the batch kernel's, through the same per-pixel helpers,
+// with slot n for the model tensor and image 0 (stride 0) for the planes.
+struct OutImageV {
+    uint8_t* plane[3];
+    int pitch[3];
+    int w, h;
+};
+struct ChromaImageV { // the source chroma of transform_luma_list: U and V as launch_luma_output's planes 1 and 2 of FrameV
+    const uint8_t* u;
+    const uint8_t* v;
+    int pitch_u, pitch_v;
+    int w, h; // the source frame's size
+};
+struct LabelsImageV {
+    uint8_t* plane;
+    int pitch;
+    int w, h;
+};
+struct FrameOutListV {
+    int count;
+    unsigned first[SNNB_FRAME_LIST_MAX];
+    OutImageV img[SNNB_FRAME_LIST_MAX];
+};
+struct ChromaListV {
+    ChromaImageV img[SNNB_FRAME_LIST_MAX];
+};
+struct LabelsListV {
+    int count;
+    unsigned first[SNNB_FRAME_LIST_MAX];
+    LabelsImageV img[SNNB_FRAME_LIST_MAX];
+};
+constexpr size_t KERNEL_PARAM_BYTES = 32764; // CUDA 12.1+ on Volta and later
+static_assert(sizeof(FrameOutListV) <= KERNEL_PARAM_BYTES - sizeof(TV) - 3 * sizeof(float), "frame_list_output_kernel's parameters");
+static_assert(sizeof(FrameOutListV) + sizeof(ChromaListV) <= KERNEL_PARAM_BYTES - sizeof(TV) - 4 * sizeof(float), "luma_list_output_kernel's parameters");
+static_assert(sizeof(LabelsListV) <= KERNEL_PARAM_BYTES - sizeof(TV) - 2 * sizeof(float), "segment_list_output_kernel's parameters");
+
+// The image of this CTA: the last n < count with first[n] <= blockIdx.x (first[0] = 0, strictly increasing)
+__device__ __forceinline__ int list_image(const unsigned* first, int count) {
+    int lo = 0, hi = count - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (first[mid] <= blockIdx.x) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+// 256 threads per CTA, one per 2 x 2 block of image n's output (frame_out_block)
+template <int FMT>
+__global__ void __launch_bounds__(256) frame_list_output_kernel(TV t, const __grid_constant__ FrameOutListV L, float scale, float offset, int linear) {
+    pdl_wait();
+    const int n         = list_image(L.first, L.count);
+    const OutImageV& e  = L.img[n];
+    const int cw = (e.w + 1) >> 1, ch = (e.h + 1) >> 1;
+    const size_t gid = (size_t) (blockIdx.x - L.first[n]) * blockDim.x + threadIdx.x;
+    if (gid >= (size_t) cw * ch) return;
+    FrameOutV o;
+#pragma unroll
+    for (int p = 0; p < 3; ++p) o.plane[p] = e.plane[p], o.pitch[p] = e.pitch[p], o.stride[p] = 0;
+    o.w = e.w, o.h = e.h, o.scale = scale, o.offset = offset;
+    frame_out_block<FMT>(t, o, n, (int) (gid % cw), (int) (gid / cw), linear);
+}
+// As frame_list_output_kernel, with luma_out_block and image n's source chroma from S
+template <int FMT>
+__global__ void __launch_bounds__(256) luma_list_output_kernel(TV t, const __grid_constant__ FrameOutListV L, const __grid_constant__ ChromaListV S, int step,
+                                                               float scale, float offset, int linear) {
+    pdl_wait();
+    const int n         = list_image(L.first, L.count);
+    const OutImageV& e  = L.img[n];
+    const int cw = (e.w + 1) >> 1, ch = (e.h + 1) >> 1;
+    const size_t gid = (size_t) (blockIdx.x - L.first[n]) * blockDim.x + threadIdx.x;
+    if (gid >= (size_t) cw * ch) return;
+    FrameOutV o;
+#pragma unroll
+    for (int p = 0; p < 3; ++p) o.plane[p] = e.plane[p], o.pitch[p] = e.pitch[p], o.stride[p] = 0;
+    o.w = e.w, o.h = e.h, o.scale = scale, o.offset = offset;
+    const ChromaImageV& c = S.img[n];
+    FrameV s {};
+    s.plane[1] = c.u, s.plane[2] = c.v, s.pitch[1] = c.pitch_u, s.pitch[2] = c.pitch_v, s.w = c.w, s.h = c.h;
+    luma_out_block<FMT>(t, s, step, o, n, (int) (gid % cw), (int) (gid / cw), linear);
+}
+// SEG_THREADS pixels of one row of image n's label plane per CTA, x fastest, as segment_output_kernel
+template <bool THRESH>
+__global__ void __launch_bounds__(SEG_THREADS) segment_list_output_kernel(TV t, const __grid_constant__ LabelsListV L, float threshold, int linear) {
+    pdl_wait();
+    const int n           = list_image(L.first, L.count);
+    const LabelsImageV& e = L.img[n];
+    const int row_ctas = (e.w + SEG_THREADS - 1) / SEG_THREADS;
+    const int local    = (int) (blockIdx.x - L.first[n]);
+    const int y = local / row_ctas, x = (local - y * row_ctas) * SEG_THREADS + threadIdx.x;
+    if (x >= e.w) return;
+    LabelsV o;
+    o.plane = e.plane, o.pitch = e.pitch, o.stride = 0, o.w = e.w, o.h = e.h, o.threshold = threshold;
+    segment_pixel<THRESH>(t, o, linear, n, x, y);
+}
+
+// first[] of a list whose image n takes ctas(n) CTAs; false when the grid would exceed 2^31 - 1 CTAs
+template <typename F>
+static bool list_grid(int count, unsigned first[], F ctas, unsigned& total) {
+    long long sum = 0;
+    for (int n = 0; n < count; ++n) {
+        first[n] = (unsigned) sum;
+        sum += ctas(n);
+        if (sum > 0x7fffffffLL) return false;
+    }
+    total = (unsigned) sum;
+    return true;
+}
+// The destination table of an output list (count == t->n <= SNNB_FRAME_LIST_MAX, checked by the caller), 256 threads per CTA, one per
+// 2 x 2 block of each image
+static int frame_out_list_view(const char* who, const snnb_tensor* t, const snnb_frame_out_list& fo, FrameOutListV& L, unsigned& grid) {
+    SNNB_REQUIRE(fo.count == t->n && fo.count >= 1 && fo.count <= SNNB_FRAME_LIST_MAX, "%s: %d images for a batch of %d", who, fo.count, t->n);
+    std::memset(&L, 0, sizeof(L));
+    L.count = fo.count;
+    for (int n = 0; n < fo.count; ++n) {
+        const snnb_frame_out_image& im = fo.images[n];
+        for (int p = 0; p < 3; ++p) L.img[n].plane[p] = im.plane[p], L.img[n].pitch[p] = im.pitch[p];
+        L.img[n].w = im.width, L.img[n].h = im.height;
+    }
+    const bool fits = list_grid(fo.count, L.first, [&](int n) { return ((long long) ((L.img[n].h + 1) / 2) * ((L.img[n].w + 1) / 2) + 255) / 256; }, grid);
+    SNNB_REQUIRE(fits, "%s: the list's output needs more than 2^31 - 1 CTAs", who);
+    return 0;
+}
+int launch_frame_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_out_list& fo) {
+    SNNB_REQUIRE((t->c == 1 || t->c == 3 || t->c == 4) && t->cp == 8 && !t->feed_only,
+                 "launch_frame_list_output: the output tensor has %d channels; frames are written from 1, 3 or 4", t->c);
+    FrameOutListV L;
+    unsigned blocks = 0;
+    if (frame_out_list_view("launch_frame_list_output", t, fo, L, blocks)) return 1;
+    const int linear = fo.linear_filter ? 1 : 0;
+    const dim3 grid(blocks), block(256);
+    switch (fo.format) {
+    case SNNB_FRAME_NV12:
+        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
+                           "frame_list_output_kernel<nv12>");
+    case SNNB_FRAME_NV21:
+        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
+                           "frame_list_output_kernel<nv21>");
+    case SNNB_FRAME_I420:
+        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
+                           "frame_list_output_kernel<i420>");
+    case SNNB_FRAME_RGBA8:
+        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
+                           "frame_list_output_kernel<rgba8>");
+    case SNNB_FRAME_P010:
+        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
+                           "frame_list_output_kernel<p010>");
+    }
+    SNNB_REQUIRE(false, "launch_frame_list_output: unknown format %d", fo.format);
+}
+int launch_luma_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_list& src, const snnb_frame_out_list& fo) {
+    SNNB_REQUIRE(t->c == 1 && t->cp == 8 && !t->feed_only && src.format != SNNB_FRAME_RGBA8,
+                 "launch_luma_list_output: the output tensor has %d channels, source format %d; luma frames are written from 1 channel with YUV chroma", t->c,
+                 src.format);
+    SNNB_REQUIRE((src.format == SNNB_FRAME_P010) == (fo.format == SNNB_FRAME_P010),
+                 "launch_luma_list_output: source format %d, out format %d; P010 pairs with P010 only", src.format, fo.format);
+    SNNB_REQUIRE(src.count == fo.count, "launch_luma_list_output: %d source images for %d out images", src.count, fo.count);
+    FrameOutListV L;
+    unsigned blocks = 0;
+    if (frame_out_list_view("launch_luma_list_output", t, fo, L, blocks)) return 1;
+    // the source chroma of each image as launch_luma_output lays it out: two planes of samples `step` samples apart
+    ChromaListV S;
+    std::memset(&S, 0, sizeof(S));
+    const int u = src.format == SNNB_FRAME_NV21 ? 1 : 0, bytes = src.format == SNNB_FRAME_P010 ? 2 : 1;
+    const int step = src.format == SNNB_FRAME_I420 ? 1 : 2;
+    for (int n = 0; n < src.count; ++n) {
+        const snnb_frame_image& im = src.images[n];
+        ChromaImageV& c = S.img[n];
+        if (src.format == SNNB_FRAME_I420) c.u = im.plane[1], c.v = im.plane[2], c.pitch_u = im.pitch[1], c.pitch_v = im.pitch[2];
+        else c.u = im.plane[1] + u * bytes, c.v = im.plane[1] + (1 - u) * bytes, c.pitch_u = c.pitch_v = im.pitch[1];
+        c.w = im.width, c.h = im.height;
+    }
+    const int linear = fo.linear_filter ? 1 : 0;
+    const dim3 grid(blocks), block(256);
+    switch (fo.format) {
+    case SNNB_FRAME_NV12:
+        return launch_done(ctx, launch_k(luma_list_output_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, view(t), L, S, step, fo.scale, fo.offset, linear),
+                           "luma_list_output_kernel<nv12>");
+    case SNNB_FRAME_NV21:
+        return launch_done(ctx, launch_k(luma_list_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), L, S, step, fo.scale, fo.offset, linear),
+                           "luma_list_output_kernel<nv21>");
+    case SNNB_FRAME_I420:
+        return launch_done(ctx, launch_k(luma_list_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), L, S, step, fo.scale, fo.offset, linear),
+                           "luma_list_output_kernel<i420>");
+    case SNNB_FRAME_P010:
+        return launch_done(ctx, launch_k(luma_list_output_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, view(t), L, S, step, fo.scale, fo.offset, linear),
+                           "luma_list_output_kernel<p010>");
+    }
+    SNNB_REQUIRE(false, "launch_luma_list_output: out format %d; luma frames are written as NV12, NV21, I420 or P010", fo.format);
+}
+int launch_segment_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_list& lo) {
+    SNNB_REQUIRE(t->c >= 1 && t->c <= 256 && t->cp % 8 == 0 && !t->feed_only,
+                 "launch_segment_list_output: the output tensor has %d channels; labels are written from 1 to 256", t->c);
+    SNNB_REQUIRE(lo.count == t->n && lo.count >= 1 && lo.count <= SNNB_FRAME_LIST_MAX, "launch_segment_list_output: %d images for a batch of %d", lo.count, t->n);
+    LabelsListV L;
+    std::memset(&L, 0, sizeof(L));
+    L.count = lo.count;
+    for (int n = 0; n < lo.count; ++n) L.img[n] = LabelsImageV {lo.images[n].plane, lo.images[n].pitch, lo.images[n].width, lo.images[n].height};
+    unsigned blocks = 0;
+    const bool fits = list_grid(lo.count, L.first, [&](int n) { return (long long) ((L.img[n].w + SEG_THREADS - 1) / SEG_THREADS) * L.img[n].h; }, blocks);
+    SNNB_REQUIRE(fits, "launch_segment_list_output: the list's labels need more than 2^31 - 1 CTAs");
+    const int linear = lo.linear_filter ? 1 : 0;
+    const dim3 grid(blocks), block(SEG_THREADS);
+    if (t->c == 1)
+        return launch_done(ctx, launch_k(segment_list_output_kernel<true>, grid, block, 0, ctx->stream, view(t), L, lo.threshold, linear),
+                           "segment_list_output_kernel<threshold>");
+    return launch_done(ctx, launch_k(segment_list_output_kernel<false>, grid, block, 0, ctx->stream, view(t), L, lo.threshold, linear),
+                       "segment_list_output_kernel<argmax>");
 }
 
 } // namespace snnb

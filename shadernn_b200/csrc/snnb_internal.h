@@ -268,9 +268,14 @@ int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const fl
                                 const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count);
 // Frame lists (snnb_model_run_frame_list / run_rois_list, checked by the caller): launch_frame_input, launch_frame_roi_input and
 // launch_roi_clear with one descriptor per image, passed to the kernel by value (fl.count <= SNNB_FRAME_LIST_MAX)
-int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t);
+int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t, bool luma);
 int launch_frame_list_roi_input(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, snnb_tensor* t);
 int launch_roi_list_clear(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes);
+// Output lists (snnb_model_transform_frame_list / transform_luma_list / segment_frame_list, checked by the caller): launch_frame_output,
+// launch_luma_output and launch_segment_output with one descriptor per image, slot n of t written to image n (count == t->n)
+int launch_frame_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_out_list& out);
+int launch_luma_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_list& src, const snnb_frame_out_list& out);
+int launch_segment_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_list& out);
 // launch_rois_from_detections with frame n's size at frame_wh[2n], frame_wh[2n + 1] (host, num_frames <= SNNB_FRAME_LIST_MAX)
 int launch_rois_from_detections_list(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows,
                                      const int* frame_wh, const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count);

@@ -55,6 +55,12 @@ NV12 on detect_frames, transform_luma and transform_frames, with each frame kern
                conversion and F.interpolate into one batch, detect_torch, rows to the host, crops as in `rois`, run_torch; alternating
                as above. The device time of each kernel of the chain from torch.profiler over 50 calls, and frame_list_input_kernel
                against frame_input_kernel on one uniform 1920x1080 batch of 16 (the cost of the per-image descriptor).
+  framelist_out (opt-in) The same sixteen streams written back: Candy 720x720 transform_frame_list in place, ESPCN 540x960 (the
+               luma part's model at a quarter of the area, so that a batch of 16 fits) transform_luma_list in place, and the U-Net of
+               `segment` (21 classes) segment_frame_list to each stream's size; each against what a user does without output lists,
+               run_frame_list with a U8 (labels: float32) output, then per stream a torch resize, conversion and pack into that stream's
+               frame (luma: each Y plane resized into one batch for run_torch, and back). And each list output kernel's device time
+               from torch.profiler over 50 calls against its batch kernel on one uniform 1920x1080 list of 16.
   card        name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -754,6 +760,80 @@ def framelist(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def framelist_out(torch, ctx, core, modelzoo, d, args):
+    import torch.nn.functional as F
+    n = len(FRAMELIST_SIZES)
+    g = torch.Generator().manual_seed(13)
+    frames = [torch.randint(16, 236, (h * 3 // 2, w), dtype=torch.uint8, generator=g).cuda() for h, w in FRAMELIST_SIZES]  # one allocation each
+    uniform = torch.randint(16, 236, (n, 1080 * 3 // 2, 1920), dtype=torch.uint8, generator=g).cuda()
+    views = [uniform[i] for i in range(n)]
+    mix = "4 x 3840x2160 + 8 x 1920x1080 + 4 x 1280x720 NV12, each its own allocation"
+    res = {}
+
+    def entry(case, list_path, today_path, fns, list_kernel, batch_kernel, list_fn, batch_fn):
+        runs, med = alternate(torch, fns, args.seconds, n, args.rounds)
+        return {"case": case, "list_path": list_path, "today_path": today_path, "list_frames_per_s_median": med["list"],
+                "today_frames_per_s_median": med["today"], "list_over_today": med["list"] / med["today"], "rounds": runs,
+                "uniform_1080p": {list_kernel: frame_kernel_us(torch, list_fn, 50, list_kernel), batch_kernel: frame_kernel_us(torch, batch_fn, 50, batch_kernel)}}
+
+    # Candy, in place
+    hw = (720, 720)
+    path, _ = modelzoo.build("candy", os.path.join(d, "listout_candy"), input_hw=hw)
+    m = core.MixedInferenceCore(ctx, path, batch=n, input_hw=hw, fuse=True, use_cuda_graph=True)
+
+    def candy_today():
+        rgb = m.run_frame_list(frames, out_dtype=torch.uint8)
+        for i, (h, w) in enumerate(FRAMELIST_SIZES):
+            frames[i].copy_(torch_rgb_to_nv12(torch, rgb[i:i + 1], (h, w))[0])
+
+    e = entry("candy %dx%d batch %d from and to %s (in place)" % (hw[0], hw[1], n, mix), "transform_frame_list(out=frames)",
+              "run_frame_list(out_dtype=uint8), then per stream F.interpolate + torch RGB -> NV12 (BT.601 limited range) + packing into the frame",
+              {"list": lambda: m.transform_frame_list(frames, out=frames), "today": candy_today}, "frame_list_output_kernel", "frame_output_kernel",
+              lambda: m.transform_frame_list(views, out=views), lambda: m.transform_frames(uniform, out=uniform))
+    res["transform"] = e
+    m.close()
+    # ESPCN, in place
+    hw = (540, 960)
+    path, _ = modelzoo.build("espcn", os.path.join(d, "listout_espcn"), input_hw=hw)
+    m = core.MixedInferenceCore(ctx, path, batch=n, input_hw=hw, fuse=True, use_cuda_graph=True)
+    kw = dict(norm=1.0 / 255.0, out_scale=255.0)
+
+    def luma_today():
+        y = torch.cat([F.interpolate(f[None, None, :h].float(), size=hw, mode="bilinear", align_corners=False) for f, (h, w) in zip(frames, FRAMELIST_SIZES)])
+        yo = m.run_torch(y.round_().to(torch.uint8).permute(0, 2, 3, 1).contiguous(), mean4=[0.0] * 4, norm4=[1.0 / 255.0] * 4, out_dtype=torch.uint8,
+                         out_scale=255.0)
+        for i, (h, w) in enumerate(FRAMELIST_SIZES):
+            up = F.interpolate(yo[i:i + 1].permute(0, 3, 1, 2).float(), size=(h, w), mode="bilinear", align_corners=False)
+            frames[i][:h].copy_(up[0, 0].round_().clamp_(0.0, 255.0).to(torch.uint8))
+
+    e = entry("espcn %dx%d batch %d from and to %s (in place)" % (hw[0], hw[1], n, mix), "transform_luma_list(out=frames)",
+              "per stream F.interpolate of the Y plane to the model's size, run_torch (uint8 in, uint8 out), per stream F.interpolate back into the "
+              "Y plane (chroma kept)", {"list": lambda: m.transform_luma_list(frames, out=frames, **kw), "today": luma_today}, "luma_list_output_kernel",
+              "luma_output_kernel", lambda: m.transform_luma_list(views, out=views, **kw), lambda: m.transform_luma(uniform, out=uniform, **kw))
+    res["luma"] = e
+    m.close()
+    # U-Net, 21 classes, labels at each stream's size
+    hw, classes = (256, 256), 21
+    path, _ = modelzoo.build("unet", os.path.join(d, "listout_unet"), input_hw=hw, classes=classes)
+    m = core.MixedInferenceCore(ctx, path, batch=n, input_hw=hw, fuse=True, use_cuda_graph=True)
+    sk = dict(mean4=[0.0] * 4, norm4=[1.0 / 255.0] * 4)
+    labels = [torch.empty((h, w), dtype=torch.uint8, device="cuda") for h, w in FRAMELIST_SIZES]
+    ulabels = torch.empty((n, 1080, 1920), dtype=torch.uint8, device="cuda")
+
+    def seg_today():
+        s = m.run_frame_list(frames, out_dtype=torch.float32, out_layout="nchw", **sk)
+        for i, (h, w) in enumerate(FRAMELIST_SIZES):
+            labels[i].copy_(F.interpolate(s[i:i + 1], size=(h, w), mode="bilinear", align_corners=False).argmax(1)[0].to(torch.uint8))
+
+    e = entry("unet %dx%d x 1 -> %d classes, batch %d, from %s to labels of each stream's size" % (hw[0], hw[1], classes, n, mix), "segment_frame_list",
+              "run_frame_list(out_dtype=float32, nchw), then per stream F.interpolate (bilinear) + argmax(1) + .to(uint8)",
+              {"list": lambda: m.segment_frame_list(frames, out=labels, **sk), "today": seg_today}, "segment_list_output_kernel", "segment_output_kernel",
+              lambda: m.segment_frame_list(views, out=[ulabels[i] for i in range(n)], **sk), lambda: m.segment_frames(uniform, out=ulabels, **sk))
+    res["segment"] = e
+    m.close()
+    return res
+
+
 def p010_surface(torch, batch, H, W, seed):
     """Random 10-bit frames as P010 words [N, H * 3 // 2, W] uint16 on the device (limited-range values, low 6 bits zero)."""
     rng = np.random.default_rng(seed)
@@ -850,7 +930,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
                     help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in), "
-                         "segment (opt-in), p010 (opt-in), framelist (opt-in)")
+                         "segment (opt-in), p010 (opt-in), framelist (opt-in), framelist_out (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -879,6 +959,8 @@ def main():
         result["segment"] = segment(torch, ctx, core, modelzoo, d, args)
     if "framelist" in parts:
         result["framelist"] = framelist(torch, ctx, core, modelzoo, d, args)
+    if "framelist_out" in parts:
+        result["framelist_out"] = framelist_out(torch, ctx, core, modelzoo, d, args)
     if "p010" in parts:
         result["p010"] = p010(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
