@@ -165,7 +165,8 @@ int snnb_graph_destroy(snnb_graph* g);
 
 /* ---- whole-model engine: dp::loadFromJsonModel + generateInferenceGraph + MixedInferenceCore ------------------- */
 typedef struct {
-    int batch;          /* images per run() on this GPU (the reference is fixed at 1, inferencegraph.h:58-64) */
+    int batch;          /* the loaded batch: images per run() on this GPU (the reference is fixed at 1, inferencegraph.h:58-64), and the most
+                         * snnb_model_set_batch may choose; storage is allocated for it */
     int input_width;    /* ShaderGenOptions::desiredInput (layeroption.h:30); 0 = use the JSON InputLayer's */
     int input_height;
     int conv_algo;      /* SNNB_ALGO_*: AUTO by default */
@@ -186,7 +187,19 @@ int snnb_model_num_inputs(const snnb_model* m);
 int snnb_model_num_outputs(const snnb_model* m);
 int snnb_model_input_dims(const snnb_model* m, int idx, int* n, int* h, int* w, int* c);
 int snnb_model_output_dims(const snnb_model* m, int idx, int* n, int* h, int* w, int* c);
-/* MixedInferenceCore::run (core.cpp:97-245), end to end with HOST buffers: H2D of the NHWC fp32 batch, forward,
+/* The model's batch: the number of images every call on this model takes, 1 <= n <= the loaded batch (snnb_model_options.batch, the
+ * default). After snnb_model_set_batch(m, n) every snnb_model_* call works on n images: host and device buffers hold n images, and
+ * nothing past image n - 1 of a caller's buffer is read or written; frame lists and output lists hold n images; run_rois fills n region
+ * slots; snnb_model_get_boxes serves the images of the last result. snnb_model_input_dims, output_dims and layer_info report n.
+ * Host-side state: it enqueues nothing and allocates nothing. The first call for a given n plans each convolution for n images (the
+ * tensor-core launch configuration: tiles, channel block, K split); use_cuda_graph models capture their forward pass at n on the first
+ * forward pass at n, after one eager pass, as at load. Every later switch to that n reuses both. Submitted tickets keep the batch they
+ * were submitted with: wait() delivers that many images whatever the model's batch is by then. The results at n are those of the same
+ * model file loaded with batch n; split-K and InstanceNorm's chunking depend on n, so they may differ from slot i of a larger batch in
+ * the last bits. snnb_model_launches_per_forward reports n's count once a forward pass at n has run (0 before).
+ * A refused call (n < 1, n > the loaded batch, a null model) changes nothing. */
+int snnb_model_set_batch(snnb_model* m, int n);
+/* MixedInferenceCore::run (core.cpp:97-245), end to end with HOST buffers: H2D of the NHWC fp32 batch (the model's batch), forward,
  * D2H of output 0 (NHWC fp32, out_capacity floats) and, for classifiers (last layer Dense/softmax), the 1-based
  * class index per image (core.cpp:228-233); classes may be NULL. Synchronous. */
 int snnb_model_run(snnb_model* m, const float* host_input_nhwc, float* host_output, size_t out_capacity, int* classes_1based);
@@ -241,7 +254,7 @@ typedef struct {
  *   inputs can be fed here, while run() / submit() feed input 0 only).
  * - outputs: outputs[j] receives model output j, for j < num_outputs <= snnb_model_num_outputs(); an entry with data == NULL is skipped,
  *   and num_outputs may be 0 (classes only).
- * - classes_1based_dev: NULL, or device int32[batch] that receives arg-max + 1 per image (core.cpp:228-233). An error for a model that
+ * - classes_1based_dev: NULL, or device int32[the model's batch] that receives arg-max + 1 per image (core.cpp:228-233). An error for a model that
  *   is not a classifier.
  * - stream: a cudaStream_t of the model's device, or NULL for the context's stream. To order against a default stream, pass
  *   cudaStreamLegacy or cudaStreamPerThread, not NULL. The call returns without waiting for the GPU: work enqueued on `stream` before
@@ -249,7 +262,7 @@ typedef struct {
  *   on the context's stream, behind two events per model (the caller's stream -> the context's stream -> the caller's stream), so calls
  *   from different streams, and calls mixed with run() / submit(), are serialised on the model's tensors. A stream that is being
  *   captured is refused: capturing this call into the caller's CUDA graph is not supported.
- * - The batch is the loaded batch. A model whose output 0 is a YOLO layer is refused: its detections come through
+ * - The batch is the model's batch (snnb_model_set_batch). A model whose output 0 is a YOLO layer is refused: its detections come through
  *   snnb_model_detect_device below, or the host paths (run() / submit() + snnb_model_get_boxes).
  * Every argument is checked on the host before anything is enqueued: null pointers, unknown dtype or layout, the input count, buffers
  * that cudaPointerGetAttributes does not report as device or managed memory of the context's device, and misaligned buffers are errors
@@ -308,7 +321,7 @@ typedef struct {
     int linear_filter;           /* as snnb_image_io */
     float mean4[4], norm4[4];    /* (x - mean4[c]) * norm4[c] on the RGBA component c */
 } snnb_frames;
-/* snnb_model_run_device / snnb_model_detect_device with `frames` (the loaded batch of them) in place of the input buffers: outputs,
+/* snnb_model_run_device / snnb_model_detect_device with `frames` (the model's batch of them) in place of the input buffers: outputs,
  * classes, rows, counts, the stream contract and the fences are exactly theirs; run_frames refuses YOLO models, detect_frames requires
  * them. Checked on the host before anything is enqueued: format and matrix, width and height >= 1, each pitch >= its row's bytes, each
  * plane device or managed memory of the context's device, a model with one input of <= 4 channels, a stream that is not capturing;
@@ -319,7 +332,7 @@ int snnb_model_run_frames(snnb_model* m, const snnb_frames* frames, const snnb_d
                           void* stream);
 int snnb_model_detect_frames(snnb_model* m, const snnb_frames* frames, float* rows_dev, int max_rows, int* counts_dev, void* stream);
 /* Image-to-image models (style transfer, super-resolution) from device frames to device frames: snnb_model_run_frames' input, the
- * forward pass, then output 0 written as the loaded batch of 8-bit frames of any size, for an encoder (NV12) or a display (RGBA8). It
+ * forward pass, then output 0 written as the model's batch of 8-bit frames of any size, for an encoder (NV12) or a display (RGBA8). It
  * replaces a U8 output followed by a resize, an RGB -> YUV conversion and a pack in the caller's own code. The reference's path is
  * the same: the output goes to an RGBA8 texture, ImageTexture::resize, then rgba8ToNv12 / rgba8ToNv21 / rgba8ToI420
  * (core/src/image.cpp:1051-1100 = libyuv ABGRToNV12 / ABGRToNV21 / ABGRToI420). Every output byte, for image n of output 0
@@ -360,7 +373,7 @@ int snnb_model_transform_frames(snnb_model* m, const snnb_frames* frames, const 
 /* Luma models (ESPCN-style super-resolution; a denoiser, deblocker or sharpener of Y) from device frames to device frames: the Y plane
  * feeds a model whose one input has 1 channel, output 0 (1 channel) becomes the Y plane of `out`, and the source chroma is resized
  * beside it, so the colour of the video is kept. It replaces a copy of the Y plane, a U8 run, a chroma resize and a pack in the
- * caller's own code. No colour conversion happens. Every byte, for image n of the loaded batch:
+ * caller's own code. No colour conversion happens. Every byte, for image n of the model's batch:
  *   1. Model input: (Y' - mean4[0]) * norm4[0], Y' = ImageTexture::resize of the Y plane to the model's size with frames.linear_filter
  *      (the taps of snnb_image_io; the byte itself at equal sizes). Bit-identical to snnb_model_submit_image fed the Y planes as an
  *      N x H x W x 1 8-bit image. frames.matrix is checked as snnb_model_run_frames checks it and not used.
@@ -417,7 +430,7 @@ int snnb_model_segment_frames(snnb_model* m, const snnb_frames* frames, int luma
 typedef struct {
     int frame, row, x, y, width, height;
 } snnb_roi;
-/* The model's loaded batch B is the number of region slots. rois_dev: device memory holding snnb_roi[B]. count_dev: NULL (all B slots
+/* The model's batch B (snnb_model_set_batch) is the number of region slots. rois_dev: device memory holding snnb_roi[B]. count_dev: NULL (all B slots
  * are used) or a device int; slots i < clamp(*count_dev, 0, B) are used. frames: an snnb_frames exactly as snnb_model_run_frames takes
  * it, holding num_frames >= 1 frames (independent of B). A used slot is valid when 0 <= frame < num_frames, width, height >= 1,
  * 0 <= x, x + width <= frames.width, 0 <= y and y + height <= frames.height; the regions live on the device, so this cannot be checked
@@ -426,7 +439,7 @@ typedef struct {
  * libyuv's RGBA8 image of the whole frame (chroma sited in frame coordinates: pixel (x, y) takes chroma sample (x / 2, y / 2)), then
  * resized as run_frames resizes a frame, with taps clamped to the edges of the region; a region of the model's size is sampled directly.
  * Slots past the count and invalid slots get an all-zero input, and every byte of their outputs and their class is zero (classes are
- * 1-based: 0 = no region). The forward pass runs on the whole batch.
+ * 1-based: 0 = no region). The forward pass runs on the model's whole batch, whatever the count.
  * Outputs, classes, the stream contract and the fences are those of snnb_model_run_frames; YOLO models are refused (no detection on
  * regions). Checked on the host before anything is enqueued: everything run_frames checks, num_frames >= 1, rois_dev (and count_dev
  * unless NULL) device or managed memory of the context's device, aligned to 4 bytes. Cost beyond run_frames: one kernel launch per
@@ -472,11 +485,11 @@ typedef struct {
     float mean4[4], norm4[4];       /* as snnb_frames */
 } snnb_frame_list;
 enum { SNNB_FRAME_LIST_MAX = 256 }; /* images per list */
-/* snnb_model_run_frames / snnb_model_detect_frames with a frame list of exactly the loaded batch of images: the model input of slot i is
+/* snnb_model_run_frames / snnb_model_detect_frames with a frame list of exactly the model's batch of images: the model input of slot i is
  * bit for bit what snnb_model_run_frames computes for a batch made only of image i, with image i's matrix (direct sampling when image i
  * has the model's size, every format, both filters). Outputs, classes, rows, counts, the stream contract and the fences are exactly
  * those of run_frames / detect_frames; run_frame_list refuses YOLO models, detect_frame_list requires them. Checked on the host before
- * anything is enqueued, each error naming the image: a known format, a non-null `images`, count == the loaded batch (<= 256); per
+ * anything is enqueued, each error naming the image: a known format, a non-null `images`, count == the model's batch (<= 256); per
  * image, width and height >= 1, a known matrix (full range with BT.601 only), each used pitch >= its row's bytes, each used plane
  * device or managed memory of the context's device (P010: even pitches, 2-byte-aligned planes); a model with one input of <= 4
  * channels and a stream that is not capturing. A plane's size cannot be checked: it must hold its image. Cost beyond the forward pass:
@@ -526,7 +539,7 @@ typedef struct {
     float threshold;                 /* as snnb_labels_out */
 } snnb_labels_list;
 /* snnb_model_transform_frames / snnb_model_transform_luma / snnb_model_segment_frames with a frame list in and an output list out, both
- * of exactly the loaded batch of images (<= SNNB_FRAME_LIST_MAX). Out image i is bit for bit what the batch call writes for image i when
+ * of exactly the model's batch of images (<= SNNB_FRAME_LIST_MAX). Out image i is bit for bit what the batch call writes for image i when
  * it is fed a batch whose every frame is input image i and writes an output of out image i's size: every rule of the batch calls holds
  * per image (quantisation, resize taps, blend, libyuv rows, the P010 steps, arg-max and threshold, pixels past an odd width or height;
  * bytes outside the rows are never written). The stream contract and the fences are those of the batch calls; a capturing stream is

@@ -292,6 +292,7 @@ SIGNATURES = {
     "snnb_model_transform_frame_list": (C.c_int, [vp, C.POINTER(FrameList), C.POINTER(FrameOutList), vp]),
     "snnb_model_transform_luma_list": (C.c_int, [vp, C.POINTER(FrameList), C.POINTER(FrameOutList), vp]),
     "snnb_model_segment_frame_list": (C.c_int, [vp, C.POINTER(FrameList), C.c_int, C.POINTER(LabelsList), vp]),
+    "snnb_model_set_batch": (C.c_int, [vp, C.c_int]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),

@@ -360,7 +360,8 @@ class MixedInferenceCore:
 
     def __init__(self, ctx, json_path, batch=1, input_hw=None, conv_algo="auto", use_cuda_graph=False, fuse=False, precision="fp32x3"):
         self.ctx = ctx
-        self.batch = int(batch)
+        self.batch = int(batch)  # the model's batch: images per call (set_batch)
+        self.max_batch = self.batch  # the loaded batch: storage is allocated for it
         opt = ModelOptions(self.batch, int(input_hw[1]) if input_hw else 0, int(input_hw[0]) if input_hw else 0, ALGO[conv_algo], int(bool(use_cuda_graph)),
                            int(bool(fuse)), PRECISION[precision])
         self.h = vp()
@@ -405,6 +406,13 @@ class MixedInferenceCore:
     @property
     def launches_per_forward(self):
         return lib().snnb_model_launches_per_forward(self.h)
+
+    def set_batch(self, n):
+        """snnb_model_set_batch: every later call takes n images, 1 <= n <= max_batch (the loaded batch). Each batch size is planned, and
+        with use_cuda_graph captured, on its first use and kept; switching back is a host-side switch. Results at n equal those of the
+        model loaded with batch n."""
+        check(lib().snnb_model_set_batch(self.h, int(n)), "snnb_model_set_batch")
+        self.batch = int(n)
 
     # -- execution --
     def run(self, images, want_classes=True):

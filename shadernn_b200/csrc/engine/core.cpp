@@ -20,8 +20,10 @@ MixedInferenceCore::~MixedInferenceCore() {
         cudaSetDevice(ctx->device);
         cudaStreamSynchronize(ctx->stream);
     }
-    if (cuGraphExec) cudaGraphExecDestroy(cuGraphExec);
-    if (cuGraph) cudaGraphDestroy(cuGraph);
+    for (auto& kv : batchPlans) {
+        if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
+        if (kv.second.graph) cudaGraphDestroy(kv.second.graph);
+    }
     for (auto* t : ownedTensors) snnb_tensor_free(t);
     if (arena) cudaFree(arena);
     if (scratchArena) cudaFree(scratchArena);
@@ -208,6 +210,7 @@ bool MixedInferenceCore::init(std::string& err) {
             snnb_tensor* in          = L->inputs[0];
             cl->plan(options.convAlgo, !noFeed && resolve(L->prevLayers[0])->isInputLayer && !in->feed_hi, options.precision,
                      ctx->sm_count); // the first stem reading an input gets its feed
+            planned.push_back(L);
             const ConvPlan& p = cl->convPlan;
             if (p.prepad_h) {
                 if (tensor_alloc(ctx, N, p.prepad_h, p.prepad_w, in->c, &cl->prepadded, twoPlanes)) {
@@ -236,6 +239,7 @@ bool MixedInferenceCore::init(std::string& err) {
                 return false;
             }
             dl->plan(options.precision, ctx->sm_count);
+            planned.push_back(L);
         }
         if ((L->typeName == "Add" || L->typeName == "Concatenate") && L->inputs.size() != 2) {
             err = L->name + ": expects exactly two inputs";
@@ -357,7 +361,7 @@ bool MixedInferenceCore::init(std::string& err) {
         return false;
     }
     if (yolo) {
-        const size_t yb = yolo->candidateBytes();
+        const size_t yb = yolo->candidateBytes(N);
         if (cudaMalloc(&yoloDev, yb) != cudaSuccess || cudaMallocHost(&yoloHost, yb) != cudaSuccess) {
             err = "cudaMalloc(YOLO candidate lists) failed";
             return false;
@@ -373,36 +377,83 @@ bool MixedInferenceCore::init(std::string& err) {
         isClassifier = last && last->output->h == 1 && last->output->w == 1 && last->output->c > 1;
     }
 
+    // ---- the loaded batch is the model's first batch: its plans are the ones made above ----
+    curBatch = N;
+    cur      = &batchPlans[N];
+    for (auto* L : planned) cur->plans.push_back(L->typeName == "Conv2D" ? static_cast<Conv2DLayer*>(L)->convPlan : static_cast<DenseLayer*>(L)->convPlan);
+
     // ---- one eager pass: counts launches and warms everything up; then optionally capture ----
     const uint64_t before = ctx->launches;
     if (enqueueForward(false)) {
         err = get_error();
         return false;
     }
-    launchesPerForward = (int) (ctx->launches - before);
+    cur->launches = launchesPerForward = (int) (ctx->launches - before);
     if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
         err = std::string("first forward pass failed: ") + cudaGetErrorString(cudaGetLastError());
         return false;
     }
-    if (options.useCudaGraph) {
-        const uint64_t keep = ctx->launches;
-        if (cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
-            err = "cudaStreamBeginCapture failed";
-            return false;
-        }
-        const int rc = enqueueForward(false);
-        cudaError_t e = cudaStreamEndCapture(ctx->stream, &cuGraph);
-        ctx->launches = keep;
-        if (rc || e != cudaSuccess) {
-            err = rc ? get_error() : "cudaStreamEndCapture failed";
-            return false;
-        }
-        if (cudaGraphInstantiate(&cuGraphExec, cuGraph, 0) != cudaSuccess) {
-            err = "cudaGraphInstantiate failed";
-            return false;
-        }
+    if (options.useCudaGraph && captureForward(*cur)) {
+        err = get_error();
+        return false;
     }
     return true;
+}
+
+// The forward pass at the model's batch captured into b's graph. Run after an eager pass at that batch: that pass made every lazily
+// allocated resource (tensor-map encoder, split-K scratch), and neither cudaMalloc nor a synchronous memset may run in a capture.
+int MixedInferenceCore::captureForward(BatchPlan& b) {
+    const uint64_t keep = ctx->launches;
+    SNNB_CUDA_OK(cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeThreadLocal));
+    const int rc        = enqueueForward(false);
+    const cudaError_t e = cudaStreamEndCapture(ctx->stream, &b.graph);
+    ctx->launches       = keep;
+    if (rc) return rc;
+    SNNB_CUDA_OK(e);
+    SNNB_CUDA_OK(cudaGraphInstantiate(&b.exec, b.graph, 0));
+    return 0;
+}
+
+// Each Conv2D and Dense layer planned for n images by the same planner and query as at load. The kernel, the pre-padded copy and the
+// feed copy were allocated and packed for the load-time plan, so they must come out the same at every n; a planner whose path choice
+// depended on n would otherwise read a copy that was never allocated.
+std::string MixedInferenceCore::makeBatchPlan(int n, BatchPlan& b) const {
+    b.plans.clear();
+    for (size_t i = 0; i < planned.size(); ++i) {
+        GenericModelLayer* L = planned[i];
+        const bool conv      = L->typeName == "Conv2D";
+        ConvQuery q          = conv ? static_cast<Conv2DLayer*>(L)->query : static_cast<DenseLayer*>(L)->query;
+        q.n                  = n;
+        const ConvPlan p     = plan_conv(q);
+        const ConvPlan& at   = batchPlans.at((int) options.batch).plans[i];
+        if (p.path != at.path || p.pad_x != at.pad_x || p.pad_y != at.pad_y || p.pad_mode != at.pad_mode || p.prepad_h != at.prepad_h ||
+            p.prepad_w != at.prepad_w || p.feed_h != at.feed_h || p.feed_w != at.feed_w || p.feed_py != at.feed_py || p.feed_px != at.feed_px)
+            return L->name + ": the plan for " + std::to_string(n) + " images (path " + std::to_string(p.path) + ", pre-padded " +
+                   std::to_string(p.prepad_h) + " x " + std::to_string(p.prepad_w) + ", feed " + std::to_string(p.feed_h) + " x " +
+                   std::to_string(p.feed_w) + ") differs from the loaded batch's (path " + std::to_string(at.path) + ", pre-padded " +
+                   std::to_string(at.prepad_h) + " x " + std::to_string(at.prepad_w) + ", feed " + std::to_string(at.feed_h) + " x " +
+                   std::to_string(at.feed_w) + ") beyond its launch configuration";
+        b.plans.push_back(p);
+    }
+    return std::string();
+}
+
+int MixedInferenceCore::setBatch(int n) {
+    SNNB_REQUIRE(n >= 1 && n <= (int) options.batch, "snnb_model_set_batch: batch %d; the model was loaded for 1 to %u images", n, options.batch);
+    auto it = batchPlans.find(n);
+    if (it == batchPlans.end()) {
+        BatchPlan b;
+        const std::string why = makeBatchPlan(n, b);
+        SNNB_REQUIRE(why.empty(), "snnb_model_set_batch: %s", why.c_str());
+        it = batchPlans.emplace(n, std::move(b)).first;
+    }
+    cur = &it->second, curBatch = n, launchesPerForward = cur->launches;
+    for (size_t i = 0; i < planned.size(); ++i) {
+        GenericModelLayer* L = planned[i];
+        (L->typeName == "Conv2D" ? static_cast<Conv2DLayer*>(L)->convPlan : static_cast<DenseLayer*>(L)->convPlan) = cur->plans[i];
+    }
+    for (auto* t : ownedTensors) t->n = n; // NHWC, image outermost: the first n images of every tensor are a prefix of its storage
+    return 0;
 }
 
 int MixedInferenceCore::enqueueForward(bool) {
@@ -426,12 +477,23 @@ int MixedInferenceCore::enqueueForward(bool) {
 }
 
 int MixedInferenceCore::forward() {
-    if (cuGraphExec) {
-        SNNB_CUDA_OK(cudaGraphLaunch(cuGraphExec, ctx->stream));
-        ctx->launches += (uint64_t) launchesPerForward;
+    if (cur->exec) {
+        SNNB_CUDA_OK(cudaGraphLaunch(cur->exec, ctx->stream));
+        ctx->launches += (uint64_t) cur->launches;
         return 0;
     }
-    return enqueueForward(false);
+    // the first forward pass at a batch size (every pass without use_cuda_graph) runs eagerly and counts its launches; with
+    // use_cuda_graph it is init's warm-up pass for that size, and the graph is captured right after it (unless the context's stream is
+    // itself being captured, by snnb_graph_capture_begin: that capture records this pass)
+    const uint64_t before = ctx->launches;
+    if (int rc = enqueueForward(false)) return rc;
+    cur->launches = launchesPerForward = (int) (ctx->launches - before);
+    if (options.useCudaGraph) {
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        SNNB_CUDA_OK(cudaStreamIsCapturing(ctx->stream, &cap));
+        if (cap == cudaStreamCaptureStatusNone) return captureForward(*cur);
+    }
+    return 0;
 }
 
 int MixedInferenceCore::setInput(int idx, const float* host) {
@@ -470,7 +532,7 @@ int MixedInferenceCore::run(const float* hostInput, float* hostOutput, size_t ca
         }
     if (classes1 && isClassifier && outIdx >= 0) {
         if (launch_argmax(ctx, outputLayers[outIdx]->output, argmaxDev)) return 1;
-        SNNB_CUDA_OK(cudaMemcpyAsync(classes1, argmaxDev, sizeof(int) * options.batch, cudaMemcpyDeviceToHost, ctx->stream));
+        SNNB_CUDA_OK(cudaMemcpyAsync(classes1, argmaxDev, sizeof(int) * curBatch, cudaMemcpyDeviceToHost, ctx->stream));
     }
     if (hostOutput && outIdx >= 0) {
         if (getOutput(outIdx, hostOutput, capacityFloats)) return 1;
@@ -478,7 +540,7 @@ int MixedInferenceCore::run(const float* hostInput, float* hostOutput, size_t ca
         SNNB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
     }
     if (classes1 && isClassifier && outIdx >= 0)
-        for (uint32_t i = 0; i < options.batch; ++i) classes1[i] += 1; // core.cpp:228-233: argmax + 1
+        for (int i = 0; i < curBatch; ++i) classes1[i] += 1; // core.cpp:228-233: argmax + 1
     return 0;
 }
 
@@ -486,10 +548,10 @@ int MixedInferenceCore::run(const float* hostInput, float* hostOutput, size_t ca
 // to the host, then the exact score formula, score sort and NMS there (identical lists, identical order: finishDecode).
 int MixedInferenceCore::decodeYolo(void* dev, void* host, bool sync) {
     if (yolo->enqueueCandidates(ctx, dev)) return 1;
-    SNNB_CUDA_OK(cudaMemcpyAsync(host, dev, yolo->headBytes(), cudaMemcpyDeviceToHost, ctx->stream)); // count + the first rows
+    SNNB_CUDA_OK(cudaMemcpyAsync(host, dev, yolo->headBytes(curBatch), cudaMemcpyDeviceToHost, ctx->stream)); // count + the first rows
     if (!sync) return 0;
     SNNB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
-    const int rc = yolo->finishDecode(host, dev, boxes);
+    const int rc = yolo->finishDecode(host, dev, curBatch, boxes);
     if (rc < 0) return yolo->decode(ctx, boxes); // an image overflowed its candidate list: all-host decode of the (still resident) heads
     return rc;
 }
@@ -508,8 +570,8 @@ int MixedInferenceCore::ensureStreaming() {
         SNNB_CUDA_OK(cudaEventCreateWithFlags(&sl.stageFree, cudaEventDisableTiming));
         SNNB_CUDA_OK(cudaEventCreateWithFlags(&sl.resultReady, cudaEventDisableTiming));
         if (yolo) {
-            SNNB_CUDA_OK(cudaMalloc(&sl.yoloDev, yolo->candidateBytes()));
-            SNNB_CUDA_OK(cudaMallocHost(&sl.yoloHost, yolo->candidateBytes()));
+            SNNB_CUDA_OK(cudaMalloc(&sl.yoloDev, yolo->candidateBytes((int) options.batch)));
+            SNNB_CUDA_OK(cudaMallocHost(&sl.yoloHost, yolo->candidateBytes((int) options.batch)));
         }
     }
     return 0;
@@ -569,7 +631,7 @@ int MixedInferenceCore::submitImpl(const void* hostInput, bool u8, const float* 
     // a small classifier result (values + classes) is written straight into mapped pinned memory by ONE kernel; wait() copies it out
     static const bool noSmall = getenv("SNNB_NO_SMALL_RESULT") != nullptr;
     const bool small = !noSmall && isClassifier && !(io && io->output_u8) && (hostOutput || classes1) &&
-                       outFloats * sizeof(float) + options.batch * sizeof(int) <= SMALL_RESULT_BYTES;
+                       outFloats * sizeof(float) + curBatch * sizeof(int) <= SMALL_RESULT_BYTES;
     if (small) {
         float* vals = static_cast<float*>(sl.smallDev);
         int* cls    = reinterpret_cast<int*>(static_cast<char*>(sl.smallDev) + outFloats * sizeof(float));
@@ -588,11 +650,12 @@ int MixedInferenceCore::submitImpl(const void* hostInput, bool u8, const float* 
     sl.classesHost = nullptr;
     if (classes1 && isClassifier) {
         if (launch_argmax(ctx, out, sl.argmax)) return 1;
-        SNNB_CUDA_OK(cudaMemcpyAsync(classes1, sl.argmax, sizeof(int) * options.batch, cudaMemcpyDeviceToHost, ctx->stream));
+        SNNB_CUDA_OK(cudaMemcpyAsync(classes1, sl.argmax, sizeof(int) * curBatch, cudaMemcpyDeviceToHost, ctx->stream));
         sl.classesHost = classes1;
     }
     if (yolo && decodeYolo(sl.yoloDev, sl.yoloHost, false)) return 1; // candidates -> pinned host, asynchronously; NMS in wait()
     SNNB_CUDA_OK(cudaEventRecord(sl.resultReady, ctx->stream));
+    sl.n    = curBatch;
     sl.busy = sl.everUsed = true;
     *ticket = nextTicket++;
     return 0;
@@ -606,14 +669,14 @@ int MixedInferenceCore::wait(int ticket) {
     if (sl.userOut) std::memcpy(sl.userOut, sl.smallHost, sl.userFloats * sizeof(float));
     if (sl.userClasses) {
         const int* cls = reinterpret_cast<const int*>(static_cast<const char*>(sl.smallHost) + sl.userFloats * sizeof(float));
-        for (uint32_t i = 0; i < options.batch; ++i) sl.userClasses[i] = cls[i] + 1; // core.cpp:228-233: argmax + 1
+        for (int i = 0; i < sl.n; ++i) sl.userClasses[i] = cls[i] + 1; // core.cpp:228-233: argmax + 1
     }
     sl.userOut = nullptr, sl.userClasses = nullptr;
     if (sl.classesHost)
-        for (uint32_t i = 0; i < options.batch; ++i) sl.classesHost[i] += 1; // core.cpp:228-233: argmax + 1
+        for (int i = 0; i < sl.n; ++i) sl.classesHost[i] += 1; // core.cpp:228-233: argmax + 1
     sl.busy = false;
     if (yolo) {
-        const int rc = yolo->finishDecode(sl.yoloHost, sl.yoloDev, boxes);
+        const int rc = yolo->finishDecode(sl.yoloHost, sl.yoloDev, sl.n, boxes);
         SNNB_REQUIRE(rc >= 0, "wait: corrupt detection candidate list");
         return rc;
     }
@@ -718,8 +781,8 @@ int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, c
             if (in.rois)
                 SNNB_REQUIRE(n >= 1 && n <= SNNB_FRAME_LIST_MAX, "%s: count %d; a list holds 1 to %d frames", api, n, (int) SNNB_FRAME_LIST_MAX);
             else
-                SNNB_REQUIRE(n == (int) options.batch && n <= SNNB_FRAME_LIST_MAX, "%s: count %d; the list must hold the model's batch of %u images (at most %d)", api,
-                             n, options.batch, (int) SNNB_FRAME_LIST_MAX);
+                SNNB_REQUIRE(n == curBatch && n <= SNNB_FRAME_LIST_MAX, "%s: count %d; the list must hold the model's batch of %d images (at most %d)", api, n,
+                             curBatch, (int) SNNB_FRAME_LIST_MAX);
         }
         const int images = in.frames ? 1 : in.list->count;
         char image[32] = "", planes[32] = "plane";
@@ -854,7 +917,7 @@ int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, con
         if (outputs[j].data && launch_device_output(ctx, outputLayers[j]->output, outputs[j])) return 1;
     if (classes1Dev && launch_argmax(ctx, outputLayers[0]->output, classes1Dev, 1)) return 1; // core.cpp:228-233: argmax + 1
     if (in.rois) { // the slots without a valid region: every output byte and the class zero
-        const int B = (int) options.batch;
+        const int B = curBatch;
         auto clear = [&](void* dst, long long slotBytes) {
             return in.list ? launch_roi_list_clear(ctx, *in.list, in.rois, in.roiCount, B, dst, slotBytes)
                            : launch_roi_clear(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, B, dst, slotBytes);
@@ -899,7 +962,11 @@ int MixedInferenceCore::detectDeviceFeed(const char* api, const DeviceFeed& in, 
     if (int rc = checkDevicePointer(api, countsDev, sizeof(int), ctx->device, "counts", 0)) return rc;
     SNNB_REQUIRE(yolo->inputs.size() == 2 && yolo->inputs[0]->c >= 18 && yolo->inputs[1]->c >= 18, "%s: %s: YOLO expects two heads of >= 18 channels", api,
                  yolo->name.c_str());
-    if (!detectScratch) SNNB_CUDA_OK(cudaMalloc(&detectScratch, yolo_detect_scratch_bytes(yolo->inputs[0], yolo->inputs[1])));
+    if (!detectScratch) { // sized for the loaded batch, whatever the model's batch is now
+        snnb_tensor h0 = *yolo->inputs[0], h1 = *yolo->inputs[1];
+        h0.n = h1.n = (int) options.batch;
+        SNNB_CUDA_OK(cudaMalloc(&detectScratch, yolo_detect_scratch_bytes(&h0, &h1)));
+    }
 
     if (enqueueDeviceForward(in, stream)) return 1;
     if (launch_yolo_detect(ctx, yolo->inputs[0], yolo->inputs[1], detectScratch, maxRows, rowsDev, countsDev)) return 1;
@@ -1004,7 +1071,7 @@ int MixedInferenceCore::transformLumaDeviceFeed(const char* api, const DeviceFee
     SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
     SNNB_REQUIRE(t->c == 1, "%s: output 0 has %d channels; the Y plane is written from exactly 1", api, t->c);
     // image i of either side: a batch is one image of `n` at its image strides, a list image is one image of its own (stride 0)
-    const int n = f ? (int) options.batch : 1;
+    const int n = f ? curBatch : 1;
     auto outExtent = [&](int i, int p, uintptr_t& b, uintptr_t& e) {
         return o ? planeExtent(oformat, o->width, o->height, o->plane[p], o->pitch[p], o->image_stride[p], n, p, b, e)
                  : planeExtent(oformat, ol->images[i].width, ol->images[i].height, ol->images[i].plane[p], ol->images[i].pitch[p], 0, 1, p, b, e);

@@ -166,7 +166,8 @@ struct Conv2DDesc : GenericConvDesc {
 class Conv2DLayer : public GenericModelLayer {
 public:
     Conv2DDesc _desc;
-    // How this layer runs (made once at load by plan(); packWeights and run follow it)
+    // How this layer runs (made once at load by plan(); packWeights and run follow it). convPlan is the plan for the model's batch:
+    // the core swaps in the plan made for each batch size (MixedInferenceCore::BatchPlan), with the path, padding and copies of this one.
     snnb::ConvQuery query;
     snnb::ConvPlan convPlan;
     // Replicate / reflect padding on the tensor path: the TMA unit can only zero-fill, so the engine materialises the
@@ -245,7 +246,8 @@ public:
     void packWeights(snnb::PackedHost& p) override;
     int run(snnb_context* ctx) override;
     snnb_tensor* flat = nullptr; // staging when the input is not 1x1
-    snnb::ConvPlan convPlan;     // its 1x1 convolution, made at load by plan() once the tensors are known
+    snnb::ConvQuery query;       // its 1x1 convolution, described at load by plan() once the tensors are known
+    snnb::ConvPlan convPlan;     // ... and planned for the model's batch
     void plan(int precision, int smCount);
     GenericModelLayer* gapSource = nullptr; // fused head: global average pool of this layer's output feeds the Dense (core.cpp, fusion 4)
 };
@@ -291,13 +293,14 @@ public:
     // (word 0 = number of candidates) + rows of 8 floats. The host copies the header and the first YOLO_HEAD_ROWS rows with every
     // submission; the (rare) rest is fetched in wait().
     static constexpr int YOLO_HEAD_ROWS = 2048;
-    int maxCand() const { return inputs.size() < 2 ? 0 : inputs[0]->n * (inputs[0]->h * inputs[0]->w + inputs[1]->h * inputs[1]->w) * 3; }
-    size_t candidateBytes() const { return 32 + (size_t) maxCand() * 8 * sizeof(float); }
-    size_t headBytes() const { return 32 + (size_t) std::min(maxCand(), YOLO_HEAD_ROWS) * 8 * sizeof(float); }
+    // sizes for `n` images: buffers are allocated for the loaded batch and used for the model's batch
+    int maxCand(int n) const { return inputs.size() < 2 ? 0 : n * (inputs[0]->h * inputs[0]->w + inputs[1]->h * inputs[1]->w) * 3; }
+    size_t candidateBytes(int n) const { return 32 + (size_t) maxCand(n) * 8 * sizeof(float); }
+    size_t headBytes(int n) const { return 32 + (size_t) std::min(maxCand(n), YOLO_HEAD_ROWS) * 8 * sizeof(float); }
     int enqueueCandidates(snnb_context* ctx, void* devBuf);
-    // host part on the downloaded buffer: exact score formula, confidence threshold, score sort, NMS (yololayer.cpp:56-164).
+    // host part on the downloaded buffer of `n` images: exact score formula, confidence threshold, score sort, NMS (yololayer.cpp:56-164).
     // Returns 0, or -1 when some image overflowed the candidate list (caller falls back to decode()).
-    int finishDecode(const void* hostBuf, const void* devBuf, std::vector<SNNModelOutputBoxes>& perImage) const;
+    int finishDecode(const void* hostBuf, const void* devBuf, int n, std::vector<SNNModelOutputBoxes>& perImage) const;
 };
 
 // -------------------------------------------------------------------------------------------------------------
@@ -375,6 +378,10 @@ public:
     int layerOutput(int layerId, float* host, size_t capacityFloats);
     int timeLayers(std::vector<float>& ms);
     int dumpOutputs(const std::string& dir);
+    // snnb_model_set_batch: every later call works on n images, 1 <= n <= options.batch, in the first n images of the loaded batch's
+    // storage. Host-side: plans n on its first use, switches to it on every later one; nothing is enqueued or allocated.
+    int setBatch(int n);
+    int batch() const { return curBatch; } // the model's batch: images per call (options.batch is the capacity)
 
     snnb_context* ctx = nullptr;
     dp::ShaderGenOptions options;
@@ -384,7 +391,7 @@ public:
     std::vector<SNNModelOutputBoxes> boxes; // per image, when the model ends in a YOLO layer
     void* arena       = nullptr;
     size_t arenaBytes = 0;
-    int launchesPerForward = 0;
+    int launchesPerForward = 0; // of the model's batch (0 until its first forward pass has counted them)
     bool isClassifier = false;
     std::vector<std::string> layerKernels; // per layer (JSON order): the kernel its last timeLayers() pass launched
 
@@ -393,8 +400,21 @@ private:
     int enqueueForward(bool countOnly);
     std::vector<snnb_tensor*> ownedTensors;
     void* scratchArena = nullptr;
-    cudaGraph_t cuGraph         = nullptr;
-    cudaGraphExec_t cuGraphExec = nullptr;
+    // What one batch size runs with: a ConvPlan per layer of `planned` (Conv2D and Dense, in that order), made by the planner for n
+    // images, and (use_cuda_graph) the forward pass captured at n after one eager pass has counted its launches and grown the split-K
+    // scratch. Made on first use and kept for the model's life; storage is the loaded batch's for every n.
+    struct BatchPlan {
+        std::vector<snnb::ConvPlan> plans;
+        int launches = 0; // kernels of one forward pass (0: not counted yet)
+        cudaGraph_t graph = nullptr;
+        cudaGraphExec_t exec = nullptr;
+    };
+    std::map<int, BatchPlan> batchPlans;
+    std::vector<dp::GenericModelLayer*> planned;
+    int curBatch = 0;
+    BatchPlan* cur = nullptr;
+    std::string makeBatchPlan(int n, BatchPlan& b) const; // "" or why the plans at n cannot run on the loaded batch's storage
+    int captureForward(BatchPlan& b);
     float* ioStage   = nullptr; // device fp32 staging for input/output conversion (stable address: graph-safe)
     size_t ioStageBytes = 0;
     int* argmaxDev   = nullptr;
@@ -421,6 +441,7 @@ private:
         size_t userFloats = 0;
         void* yoloDev = nullptr;
         void* yoloHost = nullptr;
+        int n = 0; // the model's batch when this slot's submission was made: what wait() delivers
         bool busy = false, everUsed = false;
     } slots[2];
     cudaStream_t copyStream = nullptr;
@@ -431,7 +452,7 @@ private:
     // What a device-resident call feeds the model: one snnb_device_buffer per input, or (frames != NULL) a batch of frames into input 0,
     // or (rois != NULL as well) regions of numFrames frames, one per batch slot, with roiCount (NULL: all slots) of them used, or
     // (luma) the frames' Y plane alone into a 1-channel input, or (list != NULL, in place of frames) a frame list: one descriptor per
-    // image, the loaded batch of them, or with rois its list->count (= numFrames) source frames.
+    // image, the model's batch of them, or with rois its list->count (= numFrames) source frames.
     // The input staging (and, for regions, the clearing of the slots without one) is the only step in which these entry points differ.
     struct DeviceFeed {
         const snnb_device_buffer* inputs = nullptr;

@@ -190,7 +190,8 @@ void DenseLayer::packWeights(PackedHost& p) {
 }
 void DenseLayer::plan(int precision, int smCount) {
     const snnb_tensor* x = flat ? flat : inputs[0];
-    convPlan = plan_conv(dense_query(output->n, x->c, output->c, precision, x->lo && output->lo, smCount));
+    query    = dense_query(output->n, x->c, output->c, precision, x->lo && output->lo, smCount);
+    convPlan = plan_conv(query);
 }
 int DenseLayer::run(snnb_context* ctx) {
     if (gapSource && gapSource->output && gap_dense_supported(gapSource->output, output, &weights))
@@ -361,13 +362,12 @@ int YOLOLayer::enqueueCandidates(snnb_context* ctx, void* devBuf) {
     int* counts = static_cast<int*>(devBuf);
     float* cand = reinterpret_cast<float*>(static_cast<char*>(devBuf) + 32);
     // margin below the threshold: the device's expf may differ from the host's std::exp in the last bits; the host decides
-    return launch_yolo_candidates(ctx, inputs[0], inputs[1], kConfThresh - 1e-3f, maxCand(), counts, cand);
+    return launch_yolo_candidates(ctx, inputs[0], inputs[1], kConfThresh - 1e-3f, maxCand(inputs[0]->n), counts, cand);
 }
 
-int YOLOLayer::finishDecode(const void* hostBuf, const void* devBuf, std::vector<SNNModelOutputBoxes>& perImage) const {
-    const int N     = inputs[0]->n;
+int YOLOLayer::finishDecode(const void* hostBuf, const void* devBuf, int N, std::vector<SNNModelOutputBoxes>& perImage) const {
     const int total = *static_cast<const int*>(hostBuf);
-    if (total < 0 || total > maxCand()) return -1;
+    if (total < 0 || total > maxCand(N)) return -1;
     const float* cand = reinterpret_cast<const float*>(static_cast<const char*>(hostBuf) + 32);
     if (total > YOLO_HEAD_ROWS) { // more candidates than the head copy carried: fetch the rest now (the device list is still intact)
         float* rest = const_cast<float*>(cand) + (size_t) YOLO_HEAD_ROWS * 8;

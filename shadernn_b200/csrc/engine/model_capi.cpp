@@ -65,7 +65,7 @@ int snnb_model_layer_info(const snnb_model* m, int i, char* name, int name_cap, 
     for (size_t k = 0; k < m->core->graph.sorted.size(); ++k)
         if (m->core->graph.sorted[k] == L) {
             const auto& d = m->core->graph.outputDims[k];
-            if (n) *n = (int) m->core->options.batch;
+            if (n) *n = m->core->batch();
             if (h) *h = (int) d.height;
             if (w) *w = (int) d.width;
             if (c) *c = (int) d.depth;
@@ -88,7 +88,7 @@ int snnb_model_output_dims(const snnb_model* m, int idx, int* n, int* h, int* w,
     SNNB_REQUIRE(m && idx >= 0 && idx < (int) m->core->outputLayers.size(), "snnb_model_output_dims: bad index");
     auto* L = m->core->outputLayers[idx];
     if (L->typeName == "YOLO") {
-        if (n) *n = (int) m->core->options.batch;
+        if (n) *n = m->core->batch();
         if (h) *h = 100;
         if (w) *w = 6;
         if (c) *c = 1;
@@ -197,6 +197,10 @@ int snnb_model_segment_frame_list(snnb_model* m, const snnb_frame_list* frames, 
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->segmentFrameList(frames, luma != 0, out, static_cast<cudaStream_t>(stream));
 }
+int snnb_model_set_batch(snnb_model* m, int n) {
+    SNNB_REQUIRE(m, "snnb_model_set_batch: null model");
+    return m->core->setBatch(n);
+}
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input) {
     SNNB_REQUIRE(m, "snnb_model_set_input: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
@@ -239,8 +243,7 @@ int snnb_model_layer_kernel(const snnb_model* m, int layer, char* name, int name
 
 int snnb_model_get_boxes(snnb_model* m, int n, float* rows6, int max_rows, int* count) {
     SNNB_REQUIRE(m && count, "snnb_model_get_boxes: null argument");
-    SNNB_REQUIRE(n >= 0 && n < (int) m->core->boxes.size(), "snnb_model_get_boxes: no detections for image %d (model has no YOLO layer, or run() not called)", n);
-    const auto& rows = m->core->boxes[n].rows;
+    SNNB_REQUIRE(n >= 0 && n < (int) m->core->boxes.size(), "snnb_model_get_boxes: no detections for image %d (model has no YOLO layer, or run() not called)", n);    const auto& rows = m->core->boxes[n].rows;
     int k            = 0;
     for (; k < (int) rows.size() && k < max_rows && k < 100; ++k)
         for (int j = 0; j < 6; ++j) rows6[k * 6 + j] = rows[k][j];

@@ -61,6 +61,11 @@ NV12 on detect_frames, transform_luma and transform_frames, with each frame kern
                run_frame_list with a U8 (labels: float32) output, then per stream a torch resize, conversion and pack into that stream's
                frame (luma: each Y plane resized into one batch for run_torch, and back). And each list output kernel's device time
                from torch.profiler over 50 calls against its batch kernel on one uniform 1920x1080 list of 16.
+  partial     (opt-in) Partial batches. ResNet-18 224x224 loaded at 32, run_torch (uint8 in, float32 out, device classes) at n = 1, 2, 4,
+               8, 16 and 32 images: the batch-32 model after set_batch(n), a model loaded at batch n, and the batch-32 model fed 32 images
+               of which n are used. And the `framelist` chain when only k = 4, 8, 12 or 16 of its streams have a frame:
+               detect_frame_list on the batch-16 detector after set_batch(k), against the list padded to 16 with the k frames repeated.
+               Frames/s count the frames a call needs; alternating as above.
   card        name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -923,6 +928,73 @@ def p010(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def partial(torch, ctx, core, modelzoo, d, args):
+    """Partial batches: a model loaded at its largest batch and switched with set_batch(n), against a model loaded at n and against
+    padding every call to the loaded batch. Frames/s count the n useful frames of each call."""
+    res = {}
+    # (a) ResNet-18 224x224 run_torch, loaded at 32
+    hw, big_b, mean4, norm4 = (224, 224), 32, [127.5] * 4, [1.0 / 127.5] * 4
+    path, _ = modelzoo.build("resnet18", os.path.join(d, "partial_resnet18"), input_hw=hw)
+    opts = dict(input_hw=hw, fuse=True, use_cuda_graph=True)
+    switched = core.MixedInferenceCore(ctx, path, batch=big_b, **opts)
+    padded = core.MixedInferenceCore(ctx, path, batch=big_b, **opts)
+    g = torch.Generator().manual_seed(17)
+    x = torch.randint(0, 256, (big_b,) + hw + (3,), dtype=torch.uint8, generator=g).cuda()
+    rows = []
+    for n in (1, 2, 4, 8, 16, 32):
+        switched.set_batch(n)
+        loaded = core.MixedInferenceCore(ctx, path, batch=n, **opts)
+        xn = x[:n].contiguous()
+        fns = {"set_batch": lambda: switched.run_torch(xn, mean4=mean4, norm4=norm4, want_classes=True),
+               "loaded_at_n": lambda: loaded.run_torch(xn, mean4=mean4, norm4=norm4, want_classes=True),
+               "padded_to_32": lambda: padded.run_torch(x, mean4=mean4, norm4=norm4, want_classes=True)}
+        runs, med = alternate(torch, fns, args.seconds, n, args.rounds)
+        rows.append({"n": n, "set_batch_frames_per_s_median": med["set_batch"], "loaded_at_n_frames_per_s_median": med["loaded_at_n"],
+                     "padded_frames_per_s_median": med["padded_to_32"], "set_batch_over_loaded_at_n": med["set_batch"] / med["loaded_at_n"],
+                     "set_batch_over_padded": med["set_batch"] / med["padded_to_32"], "rounds": runs})
+        loaded.close()
+    res["resnet18"] = {"case": "resnet18 224x224 loaded at batch 32, run_torch with uint8 NHWC in, float32 out and device classes; frames/s of the "
+                               "n images a call needs (padded_to_32: a batch of 32 of which n are used)", "batches": rows}
+    switched.close()
+    padded.close()
+    # (b) the framelist chain when only k of the 16 streams have a frame
+    dhw, chw, cbatch = (416, 416), (112, 112), 64
+    dbatch = len(FRAMELIST_SIZES)
+    ypath, layers = modelzoo.build("yolov3tiny", os.path.join(d, "partial_yolov3tiny"), input_hw=dhw)
+    for head in [l for l in layers if l["type"] == "Conv2D" and l["outputPlanes"] == 18]:  # all-pass heads (see `detector`)
+        head["_w"]["bias"][:] = 0
+        head["_w"]["bias"][[4, 5, 10, 11, 16, 17]] = 8.0
+    ypath = modelzoo.write_model(layers, os.path.join(d, "partial_allpass.json"), split=True)
+    det = core.MixedInferenceCore(ctx, ypath, batch=dbatch, input_hw=dhw, fuse=True, use_cuda_graph=True)
+    det_pad = core.MixedInferenceCore(ctx, ypath, batch=dbatch, input_hw=dhw, fuse=True, use_cuda_graph=True)
+    cpath, _ = modelzoo.build("resnet18", os.path.join(d, "partial_cls"), input_hw=chw)
+    cls = core.MixedInferenceCore(ctx, cpath, batch=cbatch, input_hw=chw, fuse=True, use_cuda_graph=True)
+    frames = [torch.randint(16, 236, (h * 3 // 2, w), dtype=torch.uint8, generator=g).cuda() for h, w in FRAMELIST_SIZES]
+    rows = []
+    for k in (4, 8, 12, 16):
+        det.set_batch(k)
+        # the k streams with a frame: every size class (2160p, 1080p, 720p) in the mix's proportions
+        pick = [i for j in range(dbatch // 4) for i in (j, 4 + 2 * j, 5 + 2 * j, 12 + j)][:k]
+        fk, sk = [frames[i] for i in pick], [FRAMELIST_SIZES[i] for i in pick]
+        fpad, spad = [fk[i % k] for i in range(dbatch)], [sk[i % k] for i in range(dbatch)]
+
+        def chain(m, fl, sizes):
+            r, c = m.detect_frame_list(fl, mean4=mean4, norm4=norm4)
+            regions, count = ctx.rois_from_detections(r, c, sizes, cbatch)
+            return cls.run_rois_list(fl, regions, count, mean4=mean4, norm4=norm4, want_classes=True)
+        fns = {"set_batch": lambda: chain(det, fk, sk), "padded_to_16": lambda: chain(det_pad, fpad, spad)}
+        runs, med = alternate(torch, fns, args.seconds, k, args.rounds)
+        rows.append({"k": k, "streams": sk, "set_batch_frames_per_s_median": med["set_batch"], "padded_frames_per_s_median": med["padded_to_16"],
+                     "set_batch_over_padded": med["set_batch"] / med["padded_to_16"], "rounds": runs})
+    res["framelist"] = {"case": "detect_frame_list (yolov3tiny all-pass heads 416x416 loaded at 16) -> rois_from_detections -> resnet18 112x112 "
+                                "batch 64 run_rois_list, k of the 16 streams of `framelist` with a frame; padded_to_16 repeats the k frames "
+                                "to fill the list; frames/s of the k frames", "streams": rows}
+    det.close()
+    det_pad.close()
+    cls.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
@@ -930,7 +1002,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
                     help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in), "
-                         "segment (opt-in), p010 (opt-in), framelist (opt-in), framelist_out (opt-in)")
+                         "segment (opt-in), p010 (opt-in), framelist (opt-in), framelist_out (opt-in), partial (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -963,6 +1035,8 @@ def main():
         result["framelist_out"] = framelist_out(torch, ctx, core, modelzoo, d, args)
     if "p010" in parts:
         result["p010"] = p010(torch, ctx, core, modelzoo, d, args)
+    if "partial" in parts:
+        result["partial"] = partial(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
