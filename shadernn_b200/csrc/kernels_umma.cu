@@ -18,9 +18,10 @@
 // zero-filled by the TMA unit, which is exactly the reference's constant padding (vk_conv2d.comp:168-172), and the
 // channel tail (c >= IC) is zero-filled too, so no im2col buffer and no boundary code exist anywhere.
 //
-// Roles (384 threads, persistent CTAs, one per SM): warpgroup 0 = TMA producer (one thread issues), warpgroups 1 and 2 =
-// consumers, each owning 64 of the tile's 128 rows: one m64 wgmma per K step and product term, then the epilogue of those
-// rows. The operand ring (full/empty mbarriers) is as deep as shared memory allows for the launch's n_blk, so the producer
+// Roles (384 threads, persistent CTAs, one per SM): warpgroup 0 = TMA producer (one thread issues the operand loads, one thread
+// of warp 1 the epilogue's residual loads and output stores), warpgroups 1 and 2 = consumers, each owning 64 of the tile's 128
+// rows: one m64 wgmma per K step and product term, issued in turns with the other consumer, then the epilogue arithmetic of
+// those rows. The operand ring (full/empty mbarriers) is as deep as shared memory allows for the launch's n_blk, so the producer
 // runs several K blocks ahead. Layers with few tiles split K over several CTAs (fp32 partials, last arriver reduces), or,
 // on request, use a stream-K decomposition. Also in this file: the row-window kernel for small-channel stems and the
 // TMA-staged depthwise kernel.
@@ -41,6 +42,7 @@ constexpr int UM_CONSUMERS   = 2;                          // consumer warpgroup
 constexpr int UM_THREADS     = 128 * (1 + UM_CONSUMERS);   // warpgroup 0 = producer
 constexpr int UM_EPI_THREADS = 128 * UM_CONSUMERS;
 constexpr int UM_BAR_BYTES   = 256;
+constexpr int UM_TURN_BAR    = 1;                          // named barriers 1, 2: consumer warpgroup 1's / 2's turn to issue (0 = __syncthreads)
 
 // Shared-memory carve-up of conv_umma_kernel<TERMS, NB>: [ring: STAGES x (A_hi, A_lo, B_hi, B_lo)] [staging] [barriers]. A stage
 // holds only the planes the product reads, and the ring takes whatever shared memory the staging buffer leaves (at most 8 stages).
@@ -146,8 +148,13 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// L2 prefetch of a tensor box (no shared memory, no completion to wait for)
+__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* m, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(m), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // wgmma shared-memory matrix descriptor (sm_90), K-major operand, SWIZZLE_128B:
 //   [0,14) start address >> 4 | [16,30) LBO >> 4 (= 1, unused for swizzled K-major) | [32,46) SBO >> 4 (= 1024 B: 8 rows x 128 B)
@@ -235,28 +242,68 @@ __device__ __forceinline__ void um_split2(float a, float b, uint32_t& h, uint32_
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Epilogue of one output tile, shared by both tensor-core kernels and run by the 256 consumer threads: accumulator registers
-// -> +bias (+residual) -> activation -> split-fp16 -> SHARED MEMORY (128B-swizzled for full 64-channel slabs) -> ONE TMA bulk
-// store per plane and slab. The TMA store writes full 128-byte lines and clips rows / channels that fall outside the tensor
-// by itself. The fused residual (Conv2D -> Add) comes in the same way: a TMA box load of the residual slab into the staging
-// buffer, read back by each thread at exactly the place it then overwrites.
+// Epilogue of one output tile, shared by both tensor-core kernels: accumulator registers -> +bias (+residual) -> activation ->
+// split-fp16 -> SHARED MEMORY (128B-swizzled for full 64-channel slabs) -> ONE TMA bulk store per plane and slab. The TMA store
+// writes full 128-byte lines and clips rows / channels that fall outside the tensor by itself. The fused residual (Conv2D -> Add)
+// comes in the same way: a TMA box load of the residual slab into the staging buffer, read back by each thread at exactly the
+// place it then overwrites.
+//
+// Each consumer warpgroup runs the arithmetic of its own 64 rows (disjoint in the staging buffer) on its own schedule; all TMA
+// traffic of the epilogue belongs to one STORE THREAD in the producer warpgroup, which walks the same work list. Per slab, two
+// mbarriers hand the staging buffer back and forth:
+//   stg_ready (1 arrival + residual bytes): the previous slab's store has read the buffer out, and this slab's residual (if any)
+//            has landed in it. The store thread arms it as soon as the buffer is free, so the residual load runs under the
+//            consumers' K loop rather than between their K loop and their arithmetic.
+//   stg_full  (one arrival per consumer thread): both warpgroups' rows are written; the store thread issues the slab's stores and
+//            waits for them to read the buffer out.
+// No consumer thread ever waits for a store.
 // ---------------------------------------------------------------------------------------------------------------
 struct EpiArgs {
     const CUtensorMap *o_hi64, *o_lo64, *o_hiT, *o_loT; // output maps: 64-channel slab (SWIZZLE_128B) and narrow slab (dense)
     const CUtensorMap *r_hi64, *r_lo64, *r_hiT, *r_loT; // residual maps, same geometry
     const float* bias;
     int OC, act, has_res, rows_box;
-    int has_lo;     // write (and read, for the residual) the lo plane; 0 in the fp16 storage mode
+    int has_lo;          // write (and read, for the residual) the lo plane; 0 in the fp16 storage mode
     float alpha;
-    uint32_t stg;     // staging smem (hi plane; lo plane at + UM_BLOCK_M * 128)
-    uint32_t res_bar; // mbarrier of the residual TMA load
-    bool issuer;      // the one consumer thread that issues (and later waits for) the bulk stores and residual loads
+    uint32_t stg;        // staging smem (hi plane; lo plane at + UM_BLOCK_M * 128)
+    uint32_t stg_ready;  // mbarrier: staging free (and the residual slab loaded)
+    uint32_t stg_full;   // mbarrier: staging written by every consumer thread
 };
 
-// acc: this thread's fragment of its warpgroup's 64 x NB accumulator; row0 = the tile row of its d[0] (16 w + l / 4 within the
-// warpgroup's rows), q = l % 4. SLOW_ACT: the activation is not one of the piecewise-linear ones (umma_act).
+// Store thread's side of one tile's epilogue: (oc0, c1, c2, c3) = the tile's box in the output (and residual) tensor. The staging
+// buffer is free on entry (every earlier store has been read out) and again on return.
+template <int NB>
+__device__ __forceinline__ void epilogue_store_tile(const EpiArgs& e, int oc0, int c1, int c2, int c3, uint32_t& full_phase) {
+    constexpr int W          = NB < 64 ? NB : 64;
+    constexpr bool SW        = W == 64;
+    constexpr uint32_t PITCH = SW ? 128u : (uint32_t) W * 2u;
+    const uint32_t lo_off    = UM_BLOCK_M * 128;
+    if (e.has_res) // the later slabs' residual, from L2 when their turn comes
+        for (int sl = 1; sl < NB / W; ++sl) {
+            tma_prefetch_4d(e.r_hi64, oc0 + sl * 64, c1, c2, c3);
+            if (e.has_lo) tma_prefetch_4d(e.r_lo64, oc0 + sl * 64, c1, c2, c3);
+        }
+    for (int sl = 0; sl < NB / W; ++sl) {
+        if (e.has_res) {
+            mbar_expect_tx(e.stg_ready, (e.has_lo ? 2u : 1u) * (uint32_t) e.rows_box * PITCH);
+            tma_load_4d(e.stg, SW ? e.r_hi64 : e.r_hiT, e.stg_ready, oc0 + sl * 64, c1, c2, c3);
+            if (e.has_lo) tma_load_4d(e.stg + lo_off, SW ? e.r_lo64 : e.r_loT, e.stg_ready, oc0 + sl * 64, c1, c2, c3);
+        } else {
+            mbar_arrive(e.stg_ready);
+        }
+        mbar_wait(e.stg_full, full_phase);
+        full_phase ^= 1u;
+        tma_store_4d(SW ? e.o_hi64 : e.o_hiT, e.stg, oc0 + sl * 64, c1, c2, c3);
+        if (e.has_lo) tma_store_4d(SW ? e.o_lo64 : e.o_loT, e.stg + lo_off, oc0 + sl * 64, c1, c2, c3);
+        bulk_commit();
+        bulk_wait_read0();
+    }
+}
+
+// Consumer warpgroup's side. acc: this thread's fragment of its warpgroup's 64 x NB accumulator; row0 = the tile row of its d[0]
+// (16 w + l / 4 within the warpgroup's rows), q = l % 4. SLOW_ACT: the activation is not one of the piecewise-linear ones (umma_act).
 template <int NB, bool SLOW_ACT>
-__device__ __forceinline__ void epilogue_tile_act(const EpiArgs& e, const float (&acc)[NB / 2], int oc0, int c1, int c2, int c3, int row0, int q, uint32_t& res_phase) {
+__device__ __forceinline__ void epilogue_tile_act(const EpiArgs& e, const float (&acc)[NB / 2], int oc0, int row0, int q, uint32_t& ready_phase) {
     constexpr int W      = NB < 64 ? NB : 64; // slab width in channels
     constexpr bool SW    = W == 64;            // full slab: 128-byte rows, SWIZZLE_128B
     constexpr uint32_t PITCH = SW ? 128u : (uint32_t) W * 2u;
@@ -265,18 +312,8 @@ __device__ __forceinline__ void epilogue_tile_act(const EpiArgs& e, const float 
     const uint32_t lo_off = UM_BLOCK_M * 128;
 #pragma unroll
     for (int sl = 0; sl < NB / W; ++sl) {
-        // the staging buffer is free once the previous slab's (or tile's) bulk store has finished reading it
-        if (e.issuer) bulk_wait_read0();
-        named_bar_sync(1, UM_EPI_THREADS);
-        if (e.has_res) {
-            if (e.issuer) {
-                mbar_expect_tx(e.res_bar, (e.has_lo ? 2u : 1u) * (uint32_t) e.rows_box * PITCH);
-                tma_load_4d(e.stg, SW ? e.r_hi64 : e.r_hiT, e.res_bar, oc0 + sl * 64, c1, c2, c3);
-                if (e.has_lo) tma_load_4d(e.stg + lo_off, SW ? e.r_lo64 : e.r_loT, e.res_bar, oc0 + sl * 64, c1, c2, c3);
-            }
-            mbar_wait(e.res_bar, res_phase);
-            res_phase ^= 1u;
-        }
+        mbar_wait(e.stg_ready, ready_phase);
+        ready_phase ^= 1u;
 #pragma unroll
         for (int j = 0; j < W / 8; ++j) {
             const int c = sl * 64 + 8 * j + 2 * q; // channel of the pair within the tile
@@ -311,29 +348,22 @@ __device__ __forceinline__ void epilogue_tile_act(const EpiArgs& e, const float 
             }
         }
         fence_async_smem(); // generic-proxy smem writes -> visible to the TMA (async proxy)
-        named_bar_sync(1, UM_EPI_THREADS);
-        if (e.issuer) {
-            tma_store_4d(SW ? e.o_hi64 : e.o_hiT, e.stg, oc0 + sl * 64, c1, c2, c3);
-            if (e.has_lo) tma_store_4d(SW ? e.o_lo64 : e.o_loT, e.stg + lo_off, oc0 + sl * 64, c1, c2, c3);
-            bulk_commit();
-        }
+        mbar_arrive(e.stg_full); // by every thread: a lane-0 arrive is a divergent branch that makes ptxas serialize some kernels' wgmmas
     }
 }
 
 // The transcendental activations get an epilogue of their own, chosen once per tile: inlined into every element of the unrolled loop
 // (the kernel makes no calls), their code would be strewn through the common epilogue's and more than double its size.
 template <int NB>
-__device__ __forceinline__ void epilogue_tile(const EpiArgs& e, const float (&acc)[NB / 2], int oc0, int c1, int c2, int c3, int row0, int q, uint32_t& res_phase) {
+__device__ __forceinline__ void epilogue_tile(const EpiArgs& e, const float (&acc)[NB / 2], int oc0, int row0, int q, uint32_t& ready_phase) {
     if (e.act == SNNB_ACT_NONE || e.act == SNNB_ACT_RELU || e.act == SNNB_ACT_RELU6 || e.act == SNNB_ACT_LEAKY_RELU)
-        epilogue_tile_act<NB, false>(e, acc, oc0, c1, c2, c3, row0, q, res_phase);
+        epilogue_tile_act<NB, false>(e, acc, oc0, row0, q, ready_phase);
     else
-        epilogue_tile_act<NB, true>(e, acc, oc0, c1, c2, c3, row0, q, res_phase);
+        epilogue_tile_act<NB, true>(e, acc, oc0, row0, q, ready_phase);
 }
 
-// After the last tile: the issuer's bulk stores must have completed before the CTA (and its shared memory) goes away.
-__device__ __forceinline__ void epilogue_drain(bool issuer) {
-    if (issuer) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-}
+// After the store thread's last tile: its bulk stores must have completed before the CTA (and its shared memory) goes away.
+__device__ __forceinline__ void epilogue_drain() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------------------------
 // The kernel
@@ -394,16 +424,24 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_consta
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u; // SWIZZLE_128B tiles need 1024-byte alignment
     const uint32_t stg       = smem_base + STAGES * G::STAGE_BYTES;
     const uint32_t bar_base  = stg + UM_STG_BYTES;
-    // barrier slots (8 bytes each): full[0..S), empty[S..2S), residual barrier, split-K "arrived last" flag
+    // barrier slots (8 bytes each): full[0..S), empty[S..2S), staging ready / full, split-K partials dumped / verdict, split-K
+    // "arrived last" flag
     auto full_bar  = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    const uint32_t res_bar   = bar_base + 8u * (2 * STAGES);
-    const uint32_t last_flag = bar_base + 8u * (2 * STAGES + 1);
+    const uint32_t stg_ready   = bar_base + 8u * (2 * STAGES);
+    const uint32_t stg_full    = bar_base + 8u * (2 * STAGES + 1);
+    const uint32_t dumped_bar  = bar_base + 8u * (2 * STAGES + 2);
+    const uint32_t verdict_bar = bar_base + 8u * (2 * STAGES + 3);
+    const uint32_t last_flag   = bar_base + 8u * (2 * STAGES + 4);
+    static_assert(8 * (2 * STAGES + 5) <= UM_BAR_BYTES, "barrier area");
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     pdl_trigger(); // the next kernel may start launching; it waits for this grid's completion before touching memory
     if (threadIdx.x == 0) {
-        mbar_init(res_bar, 1);
+        mbar_init(stg_ready, 1);
+        mbar_init(stg_full, UM_EPI_THREADS);
+        mbar_init(dumped_bar, UM_EPI_THREADS);
+        mbar_init(verdict_bar, 1);
         tma_prefetch_desc(&tmA_hi);
         tma_prefetch_desc(&tmA_lo);
         tma_prefetch_desc(&tmB_hi);
@@ -425,11 +463,42 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_consta
     const int total_work  = SK ? p.sk_dp + 4 * p.sk_ctas : total_tiles * p.ksplit; // one past the last work id
     auto next_work = [&](int work) { return SK ? sk_next_work(p, work, (int) blockIdx.x, (int) gridDim.x, num_kb, total_work) : work + (int) gridDim.x; };
     const int first_work = SK ? sk_first_work(p, (int) blockIdx.x, total_work) : (int) blockIdx.x;
+    EpiArgs e;
+    e.o_hi64 = &tmO_hi64, e.o_lo64 = &tmO_lo64, e.o_hiT = &tmO_hiT, e.o_loT = &tmO_loT;
+    e.r_hi64 = &tmR_hi64, e.r_lo64 = &tmR_lo64, e.r_hiT = &tmR_hiT, e.r_loT = &tmR_loT;
+    e.bias = p.bias, e.OC = p.OC, e.act = p.act, e.has_res = p.has_res, e.rows_box = p.rows_used, e.alpha = p.alpha;
+    e.has_lo = p.has_lo, e.stg = stg, e.stg_ready = stg_ready, e.stg_full = stg_full;
 
     if (wg == 0) {
-        // ===================== TMA producer (one thread) =====================
         regs_dealloc_40(); // the consumers' two accumulator sets need the registers
+        if (warp == 1) {
+            // ===================== epilogue store thread =====================
+            if (lane != 0) return;
+            uint32_t full_phase = 0, dumped_phase = 0;
+            for (int work = first_work; work < total_work; work = next_work(work)) {
+                const WorkItem wi = decode_work<SK>(p, work, total_tiles, num_kb);
+                if (wi.pieces > 1) {
+                    // every consumer thread has dumped its part of the fp32 partial tile: count this piece's arrival. The last of
+                    // the tile's pieces to arrive sums them (consumers, in piece order) and runs the epilogue; the others skip it.
+                    mbar_wait(dumped_bar, dumped_phase);
+                    dumped_phase ^= 1u;
+                    __threadfence();
+                    const int old  = atomicAdd(p.counters + wi.slot, 1);
+                    const int last = old == wi.pieces - 1;
+                    if (last) p.counters[wi.slot] = 0; // every piece has arrived: leave the counter ready for the next launch
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(last_flag), "r"(last) : "memory");
+                    mbar_arrive(verdict_bar);
+                    if (!last) continue;
+                }
+                const int m_idx = wi.tile % m_tiles, oc_idx = wi.tile / m_tiles;
+                const int bx = m_idx % p.tiles_x, by = (m_idx / p.tiles_x) % p.tiles_y, bn = m_idx / (p.tiles_x * p.tiles_y);
+                epilogue_store_tile<NB>(e, oc_idx * NB, bx * p.tw, by * p.th, bn * p.tn, full_phase);
+            }
+            epilogue_drain();
+            return;
+        }
         if (warp != 0) return;
+        // ===================== TMA producer (one thread) =====================
         const uint32_t tx_bytes = (uint32_t) G::A_PLANES * (uint32_t) p.rows_used * 128u + (uint32_t) G::B_PLANES * (uint32_t) G::B_BYTES;
         const int ks = p.ksize, cbs = p.cblocks, icp = p.ICp;
         int stage = 0;
@@ -471,15 +540,15 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_consta
     const int wq  = warp & 3;                              // warp within the warpgroup
     const int row0 = 64 * cw + 16 * wq + (lane >> 2);      // tile row of d[0]; d[2] is row0 + 8
     const int q    = lane & 3;
-    EpiArgs e;
-    e.o_hi64 = &tmO_hi64, e.o_lo64 = &tmO_lo64, e.o_hiT = &tmO_hiT, e.o_loT = &tmO_loT;
-    e.r_hi64 = &tmR_hi64, e.r_lo64 = &tmR_lo64, e.r_hiT = &tmR_hiT, e.r_loT = &tmR_loT;
-    e.bias = p.bias, e.OC = p.OC, e.act = p.act, e.has_res = p.has_res, e.rows_box = p.rows_used, e.alpha = p.alpha;
-    e.has_lo = p.has_lo, e.stg = stg, e.res_bar = res_bar, e.issuer = threadIdx.x == 128;
-    uint32_t res_phase = 0;
+    uint32_t ready_phase = 0, verdict_phase = 0;
     int stage = 0;
     uint32_t phase = 0;
     float acc[NB / 2], blk[NB / 2];
+    // The two warpgroups take turns issuing K blocks (1: block k, 2: block k, 1: block k + 1, ...), each waiting for its turn on its
+    // own named barrier and passing the turn on once its block's wgmmas are queued. So while one warpgroup drains its block
+    // (wait_group 0, promotion, stage release) or runs its epilogue, the other one's wgmmas keep the tensor cores busy. The order is
+    // seeded once and runs on across tiles and work items: both warpgroups walk the same K blocks.
+    if (cw == 1) named_bar_arrive(UM_TURN_BAR, UM_EPI_THREADS);
     for (int work = first_work; work < total_work; work = next_work(work)) {
         const WorkItem wi = decode_work<SK>(p, work, total_tiles, num_kb);
 #pragma unroll
@@ -489,6 +558,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_consta
             const uint32_t sA = smem_base + stage * G::STAGE_BYTES, sB = sA + G::A_PLANES * UM_A_BYTES;
             const uint64_t a_hi = gmma_desc_sw128(sA + cw * 64 * 128), a_lo = gmma_desc_sw128(sA + UM_A_BYTES + cw * 64 * 128);
             const uint64_t b_hi = gmma_desc_sw128(sB), b_lo = gmma_desc_sw128(sB + G::B_BYTES);
+            named_bar_sync(UM_TURN_BAR + cw, UM_EPI_THREADS); // my turn
             wg_fence();
 #pragma unroll
             for (int k = 0; k < UM_BLOCK_K / 16; ++k) {
@@ -497,16 +567,16 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_consta
                 if (TERMS >= 2) Wgmma<NB>::mma(blk, a_lo + 2u * k, b_hi + 2u * k, 1u);
             }
             wg_commit();
+            named_bar_arrive(UM_TURN_BAR + (cw ^ 1), UM_EPI_THREADS); // your turn
             wg_wait<0>(); // this K block's wgmmas have retired: its stage goes back to the producer
             __syncwarp();
             if (lane == 0) mbar_arrive(empty_bar(stage));
             acc_promote(acc, blk);
             if (++stage == STAGES) stage = 0, phase ^= 1u;
         }
-        const int m_idx = wi.tile % m_tiles, oc_idx = wi.tile / m_tiles;
-        const int bx = m_idx % p.tiles_x, by = (m_idx / p.tiles_x) % p.tiles_y, bn = m_idx / (p.tiles_x * p.tiles_y);
         if (wi.pieces > 1) {
-            // fp32 partial tile [row][NB]; the last of the tile's pieces to arrive sums them in piece order (deterministic)
+            // fp32 partial tile [row][NB]; the last of the tile's pieces to arrive sums them in piece order (deterministic). The store
+            // thread counts the arrival once all 256 consumer threads have dumped theirs, and posts the verdict in last_flag.
             float* tile_parts = p.partials + (size_t) wi.slot * (SK ? 4 : p.ksplit) * (UM_BLOCK_M * NB);
             float* mine       = tile_parts + (size_t) wi.piece * (UM_BLOCK_M * NB);
 #pragma unroll
@@ -515,14 +585,9 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_consta
                 for (int r = 0; r < 2; ++r)
                     __stcg(reinterpret_cast<float2*>(mine + (size_t) (row0 + 8 * r) * NB + 8 * j + 2 * q), make_float2(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]));
             __threadfence(); // partial tile visible device-wide before the arrival is counted
-            named_bar_sync(1, UM_EPI_THREADS);
-            if (e.issuer) {
-                const int old  = atomicAdd(p.counters + wi.slot, 1);
-                const int last = old == wi.pieces - 1;
-                if (last) p.counters[wi.slot] = 0; // every piece has arrived: leave the counter ready for the next launch
-                asm volatile("st.shared.b32 [%0], %1;" ::"r"(last_flag), "r"(last) : "memory");
-            }
-            named_bar_sync(1, UM_EPI_THREADS);
+            mbar_arrive(dumped_bar);
+            mbar_wait(verdict_bar, verdict_phase);
+            verdict_phase ^= 1u;
             int last;
             asm volatile("ld.shared.b32 %0, [%1];" : "=r"(last) : "r"(last_flag) : "memory");
             if (!last) continue;
@@ -540,9 +605,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_consta
                     acc[4 * j + 2 * r] = s.x, acc[4 * j + 2 * r + 1] = s.y;
                 }
         }
-        epilogue_tile<NB>(e, acc, oc_idx * NB, bx * p.tw, by * p.th, bn * p.tn, row0, q, res_phase);
+        epilogue_tile<NB>(e, acc, (wi.tile / m_tiles) * NB, row0, q, ready_phase);
     }
-    epilogue_drain(e.issuer);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -612,6 +676,8 @@ conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_con
     auto full_bar       = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar      = [&](int s) { return bar_base + 8u * (RW_MAX_STAGES + s); };
     const uint32_t b_bar = bar_base + 8u * (2 * RW_MAX_STAGES);
+    const uint32_t stg_ready = bar_base + 8u * (2 * RW_MAX_STAGES + 1), stg_full = bar_base + 8u * (2 * RW_MAX_STAGES + 2);
+    static_assert(8 * (2 * RW_MAX_STAGES + 3) <= RW_BAR_BYTES, "barrier area");
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     pdl_trigger();
@@ -625,6 +691,8 @@ conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_con
             mbar_init(empty_bar(s), UM_EPI_THREADS / 32);
         }
         mbar_init(b_bar, 1);
+        mbar_init(stg_ready, 1);
+        mbar_init(stg_full, UM_EPI_THREADS);
         fence_barrier_init();
     }
     __syncthreads();
@@ -632,9 +700,27 @@ conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_con
 
     const int total_tiles = p.N * p.OH * p.tiles_x;
     constexpr uint32_t B_PLANE = (uint32_t) NB * 128u; // one weight plane of a panel
+    EpiArgs e;
+    // a 64-channel slab uses the swizzled map, a narrower one the dense map: the host encodes the right one into both slots
+    e.o_hi64 = &tmO_hi, e.o_lo64 = &tmO_lo, e.o_hiT = &tmO_hi, e.o_loT = &tmO_lo;
+    e.r_hi64 = e.r_lo64 = e.r_hiT = e.r_loT = &tmO_hi;
+    e.bias = p.bias, e.OC = p.OC, e.act = p.act, e.has_res = 0, e.rows_box = UM_BLOCK_M, e.alpha = p.alpha;
+    e.has_lo = TERMS >= 2, e.stg = stg, e.stg_ready = stg_ready, e.stg_full = stg_full;
 
     if (wg == 0) {
         regs_dealloc_40();
+        if (warp == 1) {
+            // epilogue store thread (see epilogue_store_tile)
+            if (elect_one()) {
+                uint32_t full_phase = 0;
+                for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+                    const int xt = tile % p.tiles_x, oy = (tile / p.tiles_x) % p.OH, n = tile / (p.tiles_x * p.OH);
+                    epilogue_store_tile<NB>(e, 0, xt * UM_BLOCK_M, oy, n, full_phase);
+                }
+                epilogue_drain();
+            }
+            return;
+        }
         if (warp != 0) return;
         // weight panels: once per CTA, [filter row][panel][plane] (feed mode: several filter rows share one 128-byte weight row)
         if (elect_one()) {
@@ -717,13 +803,7 @@ conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_con
     const int cw   = wg - 1;
     const int row0 = 64 * cw + 16 * (warp & 3) + (lane >> 2);
     const int q    = lane & 3;
-    EpiArgs e;
-    // a 64-channel slab uses the swizzled map, a narrower one the dense map: the host encodes the right one into both slots
-    e.o_hi64 = &tmO_hi, e.o_lo64 = &tmO_lo, e.o_hiT = &tmO_hi, e.o_loT = &tmO_lo;
-    e.r_hi64 = e.r_lo64 = e.r_hiT = e.r_loT = &tmO_hi;
-    e.bias = p.bias, e.OC = p.OC, e.act = p.act, e.has_res = 0, e.rows_box = UM_BLOCK_M, e.alpha = p.alpha;
-    e.has_lo = TERMS >= 2, e.stg = stg, e.res_bar = 0, e.issuer = threadIdx.x == 128;
-    uint32_t res_phase = 0;
+    uint32_t ready_phase = 0;
     mbar_wait(b_bar, 0);
     // window descriptor of this warpgroup's 64 rows (64 pixels x 16 B further into the row segment)
     const uint64_t wdesc0 = gmma_desc_window(sA0 + (uint32_t) cw * 64u * 16u), bdesc0 = gmma_desc_sw128(sB);
@@ -749,7 +829,6 @@ conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_con
         if (++stage == RW_STAGES) stage = 0, phase ^= 1u;
     };
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int xt = tile % p.tiles_x, oy = (tile / p.tiles_x) % p.OH, n = tile / (p.tiles_x * p.OH);
 #pragma unroll
         for (int i = 0; i < NB / 2; ++i) acc[i] = 0.0f;
         if constexpr (FKS > 0) {
@@ -790,9 +869,8 @@ conv_rowwin_kernel(const __grid_constant__ CUtensorMap tmA_hi0, const __grid_con
                 finish_stage();
             }
         }
-        epilogue_tile<NB>(e, acc, 0, xt * UM_BLOCK_M, oy, n, row0, q, res_phase);
+        epilogue_tile<NB>(e, acc, 0, row0, q, ready_phase);
     }
-    epilogue_drain(e.issuer);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
