@@ -4,6 +4,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
 
@@ -728,18 +729,46 @@ static long long frameRowBytes(int format, int width, int p) {
 }
 static bool knownFrameFormat(int format) { return (format >= SNNB_FRAME_NV12 && format <= SNNB_FRAME_RGBA8) || format == SNNB_FRAME_P010; }
 
-// The planes of frames in `format`: each pitch at least its row's bytes, each plane device or managed memory of `device`; P010's
-// 16-bit samples also need even pitches and image strides and 2-byte-aligned planes.
-static int checkFramePlanes(const char* api, const char* what, int format, int width, const uint8_t* const plane[3], const int pitch[3],
-                            const long long stride[3], int device) {
-    const bool p010 = format == SNNB_FRAME_P010;
+// Image i of frames in either form, as an snnb_frames: a batch (snnb_frames, snnb_frames_out) is one description whose images lie at its
+// image strides, so it is image i for every i; a list image is a one-image description at stride 0. Only input frames have a matrix.
+template <class Batch, class List>
+static snnb_frames frameImage(const Batch* b, const List* l, int i) {
+    snnb_frames m {};
+    if (b) {
+        m.format = b->format, m.width = b->width, m.height = b->height;
+        for (int p = 0; p < 3; ++p) m.plane[p] = b->plane[p], m.pitch[p] = b->pitch[p], m.image_stride[p] = b->image_stride[p];
+    } else {
+        m.format = l->format, m.width = l->images[i].width, m.height = l->images[i].height;
+        for (int p = 0; p < 3; ++p) m.plane[p] = l->images[i].plane[p], m.pitch[p] = l->images[i].pitch[p];
+    }
+    if constexpr (std::is_same<Batch, snnb_frames>::value) m.matrix = b ? b->matrix : l->images[i].matrix;
+    return m;
+}
+static snnb_labels_image labelsImage(const snnb_labels_out* o, const snnb_labels_list* ol, int i) {
+    if (o) return {o->plane, o->pitch, o->width, o->height};
+    return ol->images[i];
+}
+// The format of frames in either form, and how many descriptions they hold
+template <class Batch, class List>
+static int frameFormat(const Batch* b, const List* l) {
+    return b ? b->format : l->format;
+}
+template <class List>
+static int frameCount(const void* b, const List* l) {
+    return b ? 1 : l->count;
+}
+
+// The planes of frame image m: each pitch at least its row's bytes, each plane device or managed memory of `device`; P010's 16-bit
+// samples also need even pitches and image strides and 2-byte-aligned planes.
+static int checkFramePlanes(const char* api, const char* what, const snnb_frames& m, int device) {
+    const bool p010 = m.format == SNNB_FRAME_P010;
     for (int p = 0; p < 3; ++p) {
-        const long long row = frameRowBytes(format, width, p);
+        const long long row = frameRowBytes(m.format, m.width, p);
         if (!row) continue;
-        SNNB_REQUIRE(pitch[p] >= row, "%s: %s %d: pitch %d is less than its row's %lld bytes", api, what, p, pitch[p], row);
-        SNNB_REQUIRE(!p010 || (pitch[p] % 2 == 0 && stride[p] % 2 == 0), "%s: %s %d: P010 pitch %d and image stride %lld must be even", api, what, p, pitch[p],
-                     stride[p]);
-        if (int rc = checkDevicePointer(api, plane[p], p010 ? 2 : 1, device, what, p)) return rc;
+        SNNB_REQUIRE(m.pitch[p] >= row, "%s: %s %d: pitch %d is less than its row's %lld bytes", api, what, p, m.pitch[p], row);
+        SNNB_REQUIRE(!p010 || (m.pitch[p] % 2 == 0 && m.image_stride[p] % 2 == 0), "%s: %s %d: P010 pitch %d and image stride %lld must be even", api, what, p,
+                     m.pitch[p], m.image_stride[p]);
+        if (int rc = checkDevicePointer(api, m.plane[p], p010 ? 2 : 1, device, what, p)) return rc;
     }
     return 0;
 }
@@ -758,13 +787,14 @@ static int checkCallerStream(const char* api, cudaStream_t stream) {
 
 // The matrix (YUV formats) and size of one frame description. `image` prefixes each message: "" for an snnb_frames batch, "image 3: "
 // for entry 3 of a frame list.
-static int checkFrameImage(const char* api, const char* image, int format, int matrix, int width, int height) {
-    if (format != SNNB_FRAME_RGBA8) {
-        const int base = matrix & ~SNNB_YUV_FULL_RANGE;
-        SNNB_REQUIRE(base == SNNB_YUV_BT601 || base == SNNB_YUV_BT709 || base == SNNB_YUV_BT2020, "%s: %sunknown YUV matrix %d", api, image, matrix);
-        SNNB_REQUIRE(base == SNNB_YUV_BT601 || !(matrix & SNNB_YUV_FULL_RANGE), "%s: %sYUV matrix %d: full range is defined for BT.601 only", api, image, matrix);
+static int checkFrameImage(const char* api, const char* image, const snnb_frames& m) {
+    if (m.format != SNNB_FRAME_RGBA8) {
+        const int base = m.matrix & ~SNNB_YUV_FULL_RANGE;
+        SNNB_REQUIRE(base == SNNB_YUV_BT601 || base == SNNB_YUV_BT709 || base == SNNB_YUV_BT2020, "%s: %sunknown YUV matrix %d", api, image, m.matrix);
+        SNNB_REQUIRE(base == SNNB_YUV_BT601 || !(m.matrix & SNNB_YUV_FULL_RANGE), "%s: %sYUV matrix %d: full range is defined for BT.601 only", api, image,
+                     m.matrix);
     }
-    SNNB_REQUIRE(width >= 1 && height >= 1, "%s: %sframe size %d x %d; width and height must be >= 1", api, image, width, height);
+    SNNB_REQUIRE(m.width >= 1 && m.height >= 1, "%s: %sframe size %d x %d; width and height must be >= 1", api, image, m.width, m.height);
     return 0;
 }
 
@@ -772,8 +802,7 @@ int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, c
     if (in.frames || in.list) {
         // one snnb_frames (its batch shares one description) or each image of a list, in run_frames' order of checks: the format,
         // each image's matrix and size, the model's input, then each image's planes
-        static const long long noStride[3] = {0, 0, 0};
-        const int format = in.frames ? in.frames->format : in.list->format;
+        const int format = frameFormat(in.frames, in.list);
         SNNB_REQUIRE(knownFrameFormat(format), "%s: unknown frame format %d", api, format);
         if (in.list) {
             SNNB_REQUIRE(in.list->images, "%s: null images", api);
@@ -784,13 +813,11 @@ int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, c
                 SNNB_REQUIRE(n == curBatch && n <= SNNB_FRAME_LIST_MAX, "%s: count %d; the list must hold the model's batch of %d images (at most %d)", api, n,
                              curBatch, (int) SNNB_FRAME_LIST_MAX);
         }
-        const int images = in.frames ? 1 : in.list->count;
+        const int images = frameCount(in.frames, in.list);
         char image[32] = "", planes[32] = "plane";
         for (int i = 0; i < images; ++i) {
             if (in.list) std::snprintf(image, sizeof(image), "image %d: ", i);
-            const int rc = in.frames ? checkFrameImage(api, image, format, in.frames->matrix, in.frames->width, in.frames->height)
-                                     : checkFrameImage(api, image, format, in.list->images[i].matrix, in.list->images[i].width, in.list->images[i].height);
-            if (rc) return rc;
+            if (int rc = checkFrameImage(api, image, frameImage(in.frames, in.list, i))) return rc;
         }
         SNNB_REQUIRE(inputLayers.size() == 1, "%s: the model has %d inputs; frames feed a model with exactly one", api, (int) inputLayers.size());
         const snnb_tensor* t = inputLayers[0]->output;
@@ -801,10 +828,7 @@ int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, c
         }
         for (int i = 0; i < images; ++i) {
             if (in.list) std::snprintf(planes, sizeof(planes), "image %d plane", i);
-            const int rc = in.frames ? checkFramePlanes(api, planes, format, in.frames->width, in.frames->plane, in.frames->pitch, in.frames->image_stride, ctx->device)
-                                     : checkFramePlanes(api, planes, format, in.list->images[i].width, in.list->images[i].plane, in.list->images[i].pitch, noStride,
-                                                        ctx->device);
-            if (rc) return rc;
+            if (int rc = checkFramePlanes(api, planes, frameImage(in.frames, in.list, i), ctx->device)) return rc;
         }
         if (in.rois) {
             SNNB_REQUIRE(in.numFrames >= 1, "%s: num_frames %d; at least one frame is required", api, in.numFrames);
@@ -822,6 +846,13 @@ int MixedInferenceCore::checkDeviceFeed(const char* api, const DeviceFeed& in, c
     return checkCallerStream(api, stream);
 }
 
+// f(*in.frames) or f(*in.list): each frame launcher has an overload for either form
+template <class Feed, class F>
+static int withFrames(const Feed& in, F&& f) {
+    if (in.list) return f(*in.list);
+    return f(*in.frames);
+}
+
 // The caller's stream -> the context's stream, the input staging and the forward pass. Called after every check has passed.
 int MixedInferenceCore::enqueueDeviceForward(const DeviceFeed& in, cudaStream_t stream) {
     if (!callerReady) SNNB_CUDA_OK(cudaEventCreateWithFlags(&callerReady, cudaEventDisableTiming));
@@ -830,14 +861,12 @@ int MixedInferenceCore::enqueueDeviceForward(const DeviceFeed& in, cudaStream_t 
         SNNB_CUDA_OK(cudaEventRecord(callerReady, stream));
         SNNB_CUDA_OK(cudaStreamWaitEvent(ctx->stream, callerReady, 0));
     }
-    if (in.rois && in.list) {
-        if (launch_frame_list_roi_input(ctx, *in.list, in.rois, in.roiCount, inputLayers[0]->output)) return 1;
-    } else if (in.rois) {
-        if (launch_frame_roi_input(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, inputLayers[0]->output)) return 1;
-    } else if (in.list) {
-        if (launch_frame_list_input(ctx, *in.list, inputLayers[0]->output, in.luma)) return 1;
-    } else if (in.frames) {
-        if (launch_frame_input(ctx, *in.frames, inputLayers[0]->output, in.luma)) return 1;
+    snnb_tensor* t = inputLayers[0]->output;
+    if (in.frames || in.list) {
+        const int rc = withFrames(in, [&](const auto& fr) {
+            return in.rois ? launch_frame_roi_input(ctx, fr, in.numFrames, in.rois, in.roiCount, t) : launch_frame_input(ctx, fr, t, in.luma);
+        });
+        if (rc) return 1;
     } else {
         for (int i = 0; i < in.numInputs; ++i)
             if (launch_device_input(ctx, in.inputs[i], inputLayers[i]->output)) return 1;
@@ -919,8 +948,7 @@ int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, con
     if (in.rois) { // the slots without a valid region: every output byte and the class zero
         const int B = curBatch;
         auto clear = [&](void* dst, long long slotBytes) {
-            return in.list ? launch_roi_list_clear(ctx, *in.list, in.rois, in.roiCount, B, dst, slotBytes)
-                           : launch_roi_clear(ctx, *in.frames, in.numFrames, in.rois, in.roiCount, B, dst, slotBytes);
+            return withFrames(in, [&](const auto& fr) { return launch_roi_clear(ctx, fr, in.numFrames, in.rois, in.roiCount, B, dst, slotBytes); });
         };
         for (int j = 0; j < numOutputs; ++j) {
             if (!outputs[j].data) continue;
@@ -976,20 +1004,16 @@ int MixedInferenceCore::detectDeviceFeed(const char* api, const DeviceFeed& in, 
 // The out frames of transform / transform_luma: one snnb_frames_out, or (ol) each image of an output list, which must hold one image per
 // frame of the input list. Each size, then each image's planes, in transform_frames' order of checks; list errors name the image.
 static int checkFramesOut(const char* api, const snnb_frames_out* o, const snnb_frame_out_list* ol, int frames, int device) {
-    static const long long noStride[3] = {0, 0, 0};
     if (ol) {
         SNNB_REQUIRE(ol->images, "%s: null out images", api);
         SNNB_REQUIRE(ol->count == frames, "%s: out count %d; the out list must hold one image per frame (%d)", api, ol->count, frames);
     }
-    const int format = o ? o->format : ol->format;
     char image[32] = "", planes[40] = "out plane";
-    for (int i = 0; i < (o ? 1 : ol->count); ++i) {
+    for (int i = 0; i < frameCount(o, ol); ++i) {
         if (ol) std::snprintf(image, sizeof(image), "image %d: ", i), std::snprintf(planes, sizeof(planes), "image %d out plane", i);
-        const int w = o ? o->width : ol->images[i].width, h = o ? o->height : ol->images[i].height;
-        SNNB_REQUIRE(w >= 1 && h >= 1, "%s: %sout frame size %d x %d; width and height must be >= 1", api, image, w, h);
-        const int rc = o ? checkFramePlanes(api, planes, format, w, o->plane, o->pitch, o->image_stride, device)
-                         : checkFramePlanes(api, planes, format, w, ol->images[i].plane, ol->images[i].pitch, noStride, device);
-        if (rc) return rc;
+        const snnb_frames m = frameImage(o, ol, i);
+        SNNB_REQUIRE(m.width >= 1 && m.height >= 1, "%s: %sout frame size %d x %d; width and height must be >= 1", api, image, m.width, m.height);
+        if (int rc = checkFramePlanes(api, planes, m, device)) return rc;
     }
     return 0;
 }
@@ -1012,27 +1036,26 @@ int MixedInferenceCore::transformFrameList(const snnb_frame_list* frames, const 
 }
 int MixedInferenceCore::transformDeviceFeed(const char* api, const DeviceFeed& in, const snnb_frames_out* o, const snnb_frame_out_list* ol, cudaStream_t stream) {
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
-    const int format = o ? o->format : ol->format;
+    const int format = frameFormat(o, ol);
     SNNB_REQUIRE(knownFrameFormat(format), "%s: unknown out frame format %d", api, format);
-    if (int rc = checkFramesOut(api, o, ol, in.list ? in.list->count : 1, ctx->device)) return rc;
+    if (int rc = checkFramesOut(api, o, ol, frameCount(in.frames, in.list), ctx->device)) return rc;
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; frames are written from an image output", api);
     const snnb_tensor* t = outputLayers[0]->output;
     SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
     SNNB_REQUIRE(t->c == 1 || t->c == 3 || t->c == 4, "%s: output 0 has %d channels; frames are written from 1 (grey), 3 (RGB) or 4 (RGBA)", api, t->c);
 
     if (enqueueDeviceForward(in, stream)) return 1;
-    if (o ? launch_frame_output(ctx, t, *o) : launch_frame_list_output(ctx, t, *ol)) return 1;
+    if (o ? launch_frame_output(ctx, t, *o) : launch_frame_output(ctx, t, *ol)) return 1;
     return fenceToCaller(stream);
 }
 
-// The bytes plane p of `n` images spans, from its first image's first byte to its last image's last row byte; false for an unused plane
-static bool planeExtent(int format, int width, int height, const uint8_t* plane, int pitch, long long stride, int n, int p, uintptr_t& begin,
-                        uintptr_t& end) {
-    const long long row = frameRowBytes(format, width, p);
+// The bytes plane p of `n` images of m spans, from its first image's first byte to its last image's last row byte; false for an unused plane
+static bool planeExtent(const snnb_frames& m, int n, int p, uintptr_t& begin, uintptr_t& end) {
+    const long long row = frameRowBytes(m.format, m.width, p);
     if (!row) return false;
-    const long long rows = p == 0 ? height : (height + 1) / 2, span = (long long) (n - 1) * stride;
-    begin = reinterpret_cast<uintptr_t>(plane) + (span < 0 ? span : 0);
-    end   = reinterpret_cast<uintptr_t>(plane) + (span > 0 ? span : 0) + (rows - 1) * pitch + row;
+    const long long rows = p == 0 ? m.height : (m.height + 1) / 2, span = (long long) (n - 1) * m.image_stride[p];
+    begin = reinterpret_cast<uintptr_t>(m.plane[p]) + (span < 0 ? span : 0);
+    end   = reinterpret_cast<uintptr_t>(m.plane[p]) + (span > 0 ? span : 0) + (rows - 1) * m.pitch[p] + row;
     return true;
 }
 
@@ -1057,51 +1080,35 @@ int MixedInferenceCore::transformLumaList(const snnb_frame_list* frames, const s
 int MixedInferenceCore::transformLumaDeviceFeed(const char* api, const DeviceFeed& in, const snnb_frames_out* o, const snnb_frame_out_list* ol,
                                                 cudaStream_t stream) {
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
-    const snnb_frames* f = in.frames;
-    const snnb_frame_list* fl = in.list;
-    const int format = f ? f->format : fl->format, oformat = o ? o->format : ol->format;
+    const int format = frameFormat(in.frames, in.list), oformat = frameFormat(o, ol);
     SNNB_REQUIRE(knownFrameFormat(oformat), "%s: unknown out frame format %d", api, oformat);
     SNNB_REQUIRE(oformat != SNNB_FRAME_RGBA8, "%s: out format RGBA8 has no Y plane; luma frames are written as NV12, NV21, I420 or P010", api);
     SNNB_REQUIRE((oformat == SNNB_FRAME_P010) == (format == SNNB_FRAME_P010),
                  "%s: frames format %d, out format %d: the bit depths differ; P010 frames are written from P010 frames only", api, format, oformat);
-    const int images = fl ? fl->count : 1;
+    const int images = frameCount(in.frames, in.list);
     if (int rc = checkFramesOut(api, o, ol, images, ctx->device)) return rc;
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; frames are written from an image output", api);
     const snnb_tensor* t = outputLayers[0]->output;
     SNNB_REQUIRE(t, "%s: output 0 (%s) has no device tensor", api, outputLayers[0]->name.c_str());
     SNNB_REQUIRE(t->c == 1, "%s: output 0 has %d channels; the Y plane is written from exactly 1", api, t->c);
-    // image i of either side: a batch is one image of `n` at its image strides, a list image is one image of its own (stride 0)
-    const int n = f ? curBatch : 1;
-    auto outExtent = [&](int i, int p, uintptr_t& b, uintptr_t& e) {
-        return o ? planeExtent(oformat, o->width, o->height, o->plane[p], o->pitch[p], o->image_stride[p], n, p, b, e)
-                 : planeExtent(oformat, ol->images[i].width, ol->images[i].height, ol->images[i].plane[p], ol->images[i].pitch[p], 0, 1, p, b, e);
-    };
-    auto srcExtent = [&](int j, int q, uintptr_t& b, uintptr_t& e) {
-        return f ? planeExtent(format, f->width, f->height, f->plane[q], f->pitch[q], f->image_stride[q], n, q, b, e)
-                 : planeExtent(format, fl->images[j].width, fl->images[j].height, fl->images[j].plane[q], fl->images[j].pitch[q], 0, 1, q, b, e);
-    };
-    auto inPlace = [&](int i) {
-        const int ow = o ? o->width : ol->images[i].width, oh = o ? o->height : ol->images[i].height;
-        const int sw = f ? f->width : fl->images[i].width, sh = f ? f->height : fl->images[i].height;
-        bool same = oformat == format && ow == sw && oh == sh;
-        for (int p = 0; p < 3 && same; ++p)
-            if (frameRowBytes(format, sw, p))
-                same = f ? o->plane[p] == f->plane[p] && o->pitch[p] == f->pitch[p] && o->image_stride[p] == f->image_stride[p]
-                         : ol->images[i].plane[p] == fl->images[i].plane[p] && ol->images[i].pitch[p] == fl->images[i].pitch[p];
-        return same;
-    };
+    // out image i against source image j: a batch spans the model's batch at its image strides, a list image itself
     char oname[24] = "", sname[24] = "";
     for (int i = 0; i < images; ++i) {
-        const bool same = inPlace(i);
+        const snnb_frames out = frameImage(o, ol, i), own = frameImage(in.frames, in.list, i);
+        bool same = out.format == own.format && out.width == own.width && out.height == own.height;
+        for (int p = 0; p < 3 && same; ++p)
+            if (frameRowBytes(format, own.width, p))
+                same = out.plane[p] == own.plane[p] && out.pitch[p] == own.pitch[p] && out.image_stride[p] == own.image_stride[p];
         for (int j = 0; j < images; ++j) {
             if (j == i && same) continue;
-            if (fl) std::snprintf(oname, sizeof(oname), "image %d ", i), std::snprintf(sname, sizeof(sname), "image %d ", j);
+            if (in.list) std::snprintf(oname, sizeof(oname), "image %d ", i), std::snprintf(sname, sizeof(sname), "image %d ", j);
+            const snnb_frames src = frameImage(in.frames, in.list, j);
             for (int p = 0; p < 3; ++p) {
                 uintptr_t ob, oe;
-                if (!outExtent(i, p, ob, oe)) continue;
+                if (!planeExtent(out, curBatch, p, ob, oe)) continue;
                 for (int q = 1; q < 3; ++q) {
                     uintptr_t sb, se;
-                    if (!srcExtent(j, q, sb, se)) continue;
+                    if (!planeExtent(src, curBatch, q, sb, se)) continue;
                     SNNB_REQUIRE(oe <= sb || se <= ob,
                                  "%s: %sout plane %d overlaps %ssource chroma plane %d; out may alias the source chroma only as the source frames themselves", api,
                                  oname, p, sname, q);
@@ -1111,7 +1118,7 @@ int MixedInferenceCore::transformLumaDeviceFeed(const char* api, const DeviceFee
     }
 
     if (enqueueDeviceForward(in, stream)) return 1;
-    if (f ? launch_luma_output(ctx, t, *f, *o) : launch_luma_list_output(ctx, t, *fl, *ol)) return 1;
+    if (o ? launch_luma_output(ctx, t, *in.frames, *o) : launch_luma_output(ctx, t, *in.list, *ol)) return 1;
     return fenceToCaller(stream);
 }
 
@@ -1139,12 +1146,12 @@ int MixedInferenceCore::segmentDeviceFeed(const char* api, const DeviceFeed& in,
         SNNB_REQUIRE(ol->count == in.list->count, "%s: out count %d; the out list must hold one image per frame (%d)", api, ol->count, in.list->count);
     }
     char image[32] = "", plane[40] = "label plane";
-    for (int i = 0; i < (o ? 1 : ol->count); ++i) {
+    for (int i = 0; i < frameCount(o, ol); ++i) {
         if (ol) std::snprintf(image, sizeof(image), "image %d: ", i), std::snprintf(plane, sizeof(plane), "image %d label plane", i);
-        const int w = o ? o->width : ol->images[i].width, h = o ? o->height : ol->images[i].height, pitch = o ? o->pitch : ol->images[i].pitch;
-        SNNB_REQUIRE(w >= 1 && h >= 1, "%s: %slabel plane size %d x %d; width and height must be >= 1", api, image, w, h);
-        SNNB_REQUIRE(pitch >= w, "%s: %slabel plane pitch %d is less than its width %d", api, image, pitch, w);
-        if (int rc = checkDevicePointer(api, o ? o->plane : ol->images[i].plane, 1, ctx->device, plane, 0)) return rc;
+        const snnb_labels_image m = labelsImage(o, ol, i);
+        SNNB_REQUIRE(m.width >= 1 && m.height >= 1, "%s: %slabel plane size %d x %d; width and height must be >= 1", api, image, m.width, m.height);
+        SNNB_REQUIRE(m.pitch >= m.width, "%s: %slabel plane pitch %d is less than its width %d", api, image, m.pitch, m.width);
+        if (int rc = checkDevicePointer(api, m.plane, 1, ctx->device, plane, 0)) return rc;
     }
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO", "%s: output 0 is a YOLO detection list; labels are written from per-pixel class scores", api);
     const snnb_tensor* t = outputLayers[0]->output;
@@ -1152,7 +1159,7 @@ int MixedInferenceCore::segmentDeviceFeed(const char* api, const DeviceFeed& in,
     SNNB_REQUIRE(t->c >= 1 && t->c <= 256, "%s: output 0 has %d channels; an 8-bit label plane is written from 1 to 256", api, t->c);
 
     if (enqueueDeviceForward(in, stream)) return 1;
-    if (o ? launch_segment_output(ctx, t, *o) : launch_segment_list_output(ctx, t, *ol)) return 1;
+    if (o ? launch_segment_output(ctx, t, *o) : launch_segment_output(ctx, t, *ol)) return 1;
     return fenceToCaller(stream);
 }
 
@@ -1233,7 +1240,7 @@ static int roisFromDetections(const char* api, snnb_context* ctx, const float* r
     if (int rc = snn::checkDevicePointer(api, count, sizeof(int), ctx->device, "count", 0)) return rc;
     if (int rc = snn::checkCallerStream(api, stream)) return rc;
     if (frameWh)
-        return snnb::launch_rois_from_detections_list(ctx, stream ? stream : ctx->stream, rows, counts, numFrames, maxRows, frameWh, *sel, rois, capacity, count);
+        return snnb::launch_rois_from_detections(ctx, stream ? stream : ctx->stream, rows, counts, numFrames, maxRows, frameWh, *sel, rois, capacity, count);
     return snnb::launch_rois_from_detections(ctx, stream ? stream : ctx->stream, rows, counts, numFrames, maxRows, fw, fh, *sel, rois, capacity, count);
 }
 int snnb::rois_from_detections(snnb_context* ctx, const float* rows, const int* counts, int numFrames, int maxRows, int fw, int fh, const snnb_roi_select* sel,

@@ -9,8 +9,10 @@
 // Semantics follow the reference's Vulkan compute shaders (cited per kernel; paths relative to the reference repo
 // core/data/assets/shaders/).
 #include <algorithm>
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include "snnb_internal.h"
 
@@ -1672,23 +1674,59 @@ __device__ __forceinline__ void store_input_pixel(const TV& t, const FeedV& f, s
     if (!f.only) store8(t.hi, t.lo, px * 8, v);
     if (f.hi) store_feed(f, px, t.H, t.W, v);
 }
+// Where batch slot n's image comes from. Each kernel takes its source as a __grid_constant__ parameter: a reference to a kernel
+// parameter that is not __grid_constant__ makes the compiler copy the parameter to local memory. frame_of(src, n) is the FrameV of image
+// n, image_of(src, n) the image's index in it, and frame_size(src, f) the size of frame f. `form` names the source in launch errors.
+// The batch's one FrameV is handed out by value: a reference to it made the YUV batch kernels 1.5-3.5 % slower (H100 SXM, 700 W).
+// snnb_frames (snnb_model_run_frames): one description, image n at its image strides
+struct FrameBatchV {
+    FrameV s;
+    static constexpr const char* form = "batch";
+};
+// Frame lists (snnb_model_run_frame_list): one FrameV per image, filled by frame_view, passed by value (26.6 KB at
+// SNNB_FRAME_LIST_MAX images; CUDA 12.1+ allows 32,764 bytes). No allocation, no host-to-device copy, nothing that must outlive the
+// launch, and a launch that a CUDA graph may capture. Indexed by a register, an entry is read from the constant bank (LDC).
+struct FrameListV {
+    FrameV img[SNNB_FRAME_LIST_MAX];
+    static constexpr const char* form = "list";
+};
+__device__ __forceinline__ FrameV frame_of(const FrameBatchV& b, int) { return b.s; }
+__device__ __forceinline__ int image_of(const FrameBatchV&, int n) { return n; }
+__device__ __forceinline__ int2 frame_size(const FrameBatchV& b, int) { return make_int2(b.s.w, b.s.h); }
+__device__ __forceinline__ const FrameV& frame_of(const FrameListV& L, int n) { return L.img[n]; }
+__device__ __forceinline__ int image_of(const FrameListV&, int) { return 0; }
+__device__ __forceinline__ int2 frame_size(const FrameListV& L, int f) { return make_int2(L.img[f].w, L.img[f].h); }
+
+// Frame sizes alone, for roi_clear_kernel and the detection rows: every frame w x h (any number of frames), or frame n's own size from
+// a table passed by value as FrameListV is (2 KB)
+struct FrameSizeV {
+    int w, h;
+    static constexpr const char* form = "batch";
+};
+struct FrameSizesV {
+    int wh[SNNB_FRAME_LIST_MAX][2];
+    static constexpr const char* form = "list";
+};
+__device__ __forceinline__ int2 frame_size(const FrameSizeV& S, int) { return make_int2(S.w, S.h); }
+__device__ __forceinline__ int2 frame_size(const FrameSizesV& S, int n) { return make_int2(S.wh[n][0], S.wh[n][1]); }
 // One thread per output pixel (C <= 4: one 8-channel group). A frame of the model's size is sampled directly, as submitImpl does.
-template <int FMT>
-__global__ void __launch_bounds__(256) frame_input_kernel(FrameV s, TV t, U8Norm q, int linear, FeedV f) {
+template <int FMT, class Src>
+__global__ void __launch_bounds__(256) frame_input_kernel(const __grid_constant__ Src src, TV t, U8Norm q, int linear, FeedV f) {
     pdl_wait();
     const size_t total = (size_t) t.N * t.H * t.W;
     const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (px >= total) return;
     const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
+    const FrameV& s   = frame_of(src, n);
     const bool direct = s.w == t.W && s.h == t.H;
     ResizeTaps r;
     if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
     else r = resize_taps(resize_pos(ox, oy, t.W, t.H, s.w, s.h), s.w, s.h, linear);
     float v[8];
-    frame_pixel<FMT>(s, n, r, linear, direct, t, q, v);
+    frame_pixel<FMT>(s, image_of(src, n), r, linear, direct, t, q, v);
     store_input_pixel(t, f, px, v);
 }
-// The kernel-side view of an snnb_frames: planes, size and libyuv's constants of its matrix; and its mean / norm
+// The kernel-side view of an snnb_frames: planes, size and libyuv's constants of its matrix
 static FrameV frame_view(const snnb_frames& fr) {
     // libyuv row_common.cc:1115-1420: YG, YGB, UB, UG, VG, VR of BT.601 (kYuvI601Constants), BT.709 (kYuvH709Constants), BT.2020
     // (kYuv2020Constants) and full-range BT.601 (kYuvJPEGConstants). The biases UB * 128 + YGB etc. are libyuv's for all four.
@@ -1702,189 +1740,6 @@ static FrameV frame_view(const snnb_frames& fr) {
     s.bb = m[2] * 128 + m[1], s.bg = m[3] * 128 + m[4] * 128 + m[1], s.br = m[5] * 128 + m[1];
     return s;
 }
-static U8Norm frame_norm(const snnb_frames& fr) {
-    U8Norm q;
-    for (int i = 0; i < 4; ++i) q.mean[i] = fr.mean4[i], q.norm[i] = fr.norm4[i];
-    return q;
-}
-int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t, bool luma) {
-    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
-    const FrameV s = frame_view(fr);
-    const U8Norm q = frame_norm(fr);
-    const int linear = fr.linear_filter ? 1 : 0;
-    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
-    if (luma) {
-        SNNB_REQUIRE(t->c == 1 && fr.format != SNNB_FRAME_RGBA8, "launch_frame_input: luma input feeds 1 channel from YUV frames (%d channels, format %d)", t->c,
-                     fr.format);
-        if (fr.format == SNNB_FRAME_P010)
-            return launch_done(ctx, launch_k(frame_input_kernel<FRAME_LUMA10>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<luma10>");
-        return launch_done(ctx, launch_k(frame_input_kernel<FRAME_LUMA>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<luma>");
-    }
-    switch (fr.format) {
-    case SNNB_FRAME_NV12:
-        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<nv12>");
-    case SNNB_FRAME_NV21:
-        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<nv21>");
-    case SNNB_FRAME_I420:
-        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<i420>");
-    case SNNB_FRAME_RGBA8:
-        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<rgba8>");
-    case SNNB_FRAME_P010:
-        return launch_done(ctx, launch_k(frame_input_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, s, view(t), q, linear, feed_view(t)), "frame_input_kernel<p010>");
-    }
-    SNNB_REQUIRE(false, "launch_frame_input: unknown format %d", fr.format);
-}
-
-// Regions of device frames (snnb_model_run_rois): batch slot n is region rois[n] of frame rois[n].frame. A used slot (n < the count)
-// is valid when its region lies inside a frame that exists; roi_slot is the one test of that, so the input kernel and the clear kernel
-// cannot disagree on which slots they serve.
-struct RoiV {
-    const snnb_roi* rois; // [N]
-    const int* count;     // nullptr: every slot is used
-    int num_frames;
-};
-__device__ __forceinline__ bool roi_slot(const RoiV& g, int slot, int N, int fw, int fh, snnb_roi& r) {
-    const int* p = reinterpret_cast<const int*>(g.rois + slot);
-    r.frame = __ldg(p), r.row = __ldg(p + 1), r.x = __ldg(p + 2), r.y = __ldg(p + 3), r.width = __ldg(p + 4), r.height = __ldg(p + 5);
-    const int used = g.count ? min(max(__ldg(g.count), 0), N) : N;
-    return slot < used && r.frame >= 0 && r.frame < g.num_frames && r.width >= 1 && r.height >= 1 && r.x >= 0 && r.y >= 0 && r.x <= fw - r.width &&
-           r.y <= fh - r.height;
-}
-// One thread per model-input pixel, as frame_input_kernel: the taps of ImageTexture::resize from a region-sized source, clamped to the
-// region, then offset to the region's origin in the frame (so chroma is sited in frame coordinates). A region of the model's size is
-// sampled directly. Invalid and unused slots get an all-zero input.
-template <int FMT>
-__global__ void __launch_bounds__(256) frame_roi_input_kernel(FrameV s, RoiV g, TV t, U8Norm q, int linear, FeedV f) {
-    pdl_wait();
-    const size_t total = (size_t) t.N * t.H * t.W;
-    const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (px >= total) return;
-    const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
-    snnb_roi roi;
-    float v[8];
-    if (roi_slot(g, n, t.N, s.w, s.h, roi)) {
-        const bool direct = roi.width == t.W && roi.height == t.H;
-        ResizeTaps r;
-        if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
-        else r = resize_taps(resize_pos(ox, oy, t.W, t.H, roi.width, roi.height), roi.width, roi.height, linear);
-        r.x0 += roi.x, r.x1 += roi.x, r.y0 += roi.y, r.y1 += roi.y;
-        frame_pixel<FMT>(s, roi.frame, r, linear, direct, t, q, v);
-    } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = 0.0f;
-    }
-    store_input_pixel(t, f, px, v);
-}
-int launch_frame_roi_input(snnb_context* ctx, const snnb_frames& fr, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t) {
-    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_roi_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
-    const FrameV s = frame_view(fr);
-    const U8Norm q = frame_norm(fr);
-    const RoiV g {rois, count, num_frames};
-    const int linear = fr.linear_filter ? 1 : 0;
-    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
-    switch (fr.format) {
-    case SNNB_FRAME_NV12:
-        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<nv12>");
-    case SNNB_FRAME_NV21:
-        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<nv21>");
-    case SNNB_FRAME_I420:
-        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<i420>");
-    case SNNB_FRAME_RGBA8:
-        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<rgba8>");
-    case SNNB_FRAME_P010:
-        return launch_done(ctx, launch_k(frame_roi_input_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, s, g, view(t), q, linear, feed_view(t)), "frame_roi_input_kernel<p010>");
-    }
-    SNNB_REQUIRE(false, "launch_frame_roi_input: unknown format %d", fr.format);
-}
-// Zeroes batch slot blockIdx.y of a caller's buffer (slot_bytes per slot, slots contiguous) when roi_slot rejects it. A slot is the
-// outermost dimension in NHWC and NCHW alike. Runs after the outputs and classes are written.
-__global__ void __launch_bounds__(256) roi_clear_kernel(RoiV g, int N, int fw, int fh, uint8_t* __restrict__ dst, long long slot_bytes) {
-    pdl_wait();
-    snnb_roi roi;
-    if (roi_slot(g, (int) blockIdx.y, N, fw, fh, roi)) return;
-    uint8_t* p = dst + (long long) blockIdx.y * slot_bytes;
-    for (long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * 16; i < slot_bytes; i += (long long) gridDim.x * blockDim.x * 16) {
-        if ((reinterpret_cast<uintptr_t>(p + i) & 15) == 0 && i + 16 <= slot_bytes) {
-            *reinterpret_cast<uint4*>(p + i) = make_uint4(0u, 0u, 0u, 0u);
-        } else {
-            for (long long k = i; k < i + 16 && k < slot_bytes; ++k) p[k] = 0;
-        }
-    }
-}
-int launch_roi_clear(snnb_context* ctx, const snnb_frames& fr, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes) {
-    SNNB_REQUIRE(batch >= 1 && batch <= 65535 && slot_bytes >= 1, "launch_roi_clear: batch %d, %lld bytes per slot", batch, slot_bytes);
-    const RoiV g {rois, count, num_frames};
-    const long long chunks = (slot_bytes + 16 * 256 - 1) / (16 * 256);
-    const dim3 grid((unsigned) std::min(chunks, 1024LL), (unsigned) batch);
-    return launch_done(ctx, launch_k(roi_clear_kernel, grid, dim3(256), 0, ctx->stream, g, batch, fr.width, fr.height, static_cast<uint8_t*>(dst), slot_bytes),
-                       "roi_clear_kernel");
-}
-
-// Frame lists (snnb_model_run_frame_list): one FrameV per image, filled by frame_view, passed by value as a __grid_constant__ kernel
-// parameter (26.6 KB at SNNB_FRAME_LIST_MAX images; CUDA 12.1+ allows 32,764 bytes). No allocation, no host-to-device copy, nothing
-// that must outlive the launch, and a launch that a CUDA graph may capture. Indexed by a register, an entry is read from the constant
-// bank (LDC). Each kernel below is its snnb_frames form with s = img[n] and image index 0, through the same frame_pixel and stores.
-struct FrameListV {
-    FrameV img[SNNB_FRAME_LIST_MAX];
-};
-template <int FMT>
-__global__ void __launch_bounds__(256) frame_list_input_kernel(const __grid_constant__ FrameListV L, TV t, U8Norm q, int linear, FeedV f) {
-    pdl_wait();
-    const size_t total = (size_t) t.N * t.H * t.W;
-    const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (px >= total) return;
-    const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
-    const FrameV& s   = L.img[n];
-    const bool direct = s.w == t.W && s.h == t.H;
-    ResizeTaps r;
-    if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
-    else r = resize_taps(resize_pos(ox, oy, t.W, t.H, s.w, s.h), s.w, s.h, linear);
-    float v[8];
-    frame_pixel<FMT>(s, 0, r, linear, direct, t, q, v);
-    store_input_pixel(t, f, px, v);
-}
-// roi_slot against the size of the region's own frame: the one validity test of frame_list_roi_input_kernel and roi_list_clear_kernel.
-// A frame index outside the list fails roi_slot's own test, so the size looked up for it does not matter.
-__device__ __forceinline__ bool roi_list_slot(const FrameListV& L, const RoiV& g, int slot, int N, snnb_roi& r) {
-    const int frame = __ldg(reinterpret_cast<const int*>(g.rois + slot));
-    const FrameV& s = L.img[min(max(frame, 0), g.num_frames - 1)];
-    return roi_slot(g, slot, N, s.w, s.h, r);
-}
-template <int FMT>
-__global__ void __launch_bounds__(256) frame_list_roi_input_kernel(const __grid_constant__ FrameListV L, RoiV g, TV t, U8Norm q, int linear, FeedV f) {
-    pdl_wait();
-    const size_t total = (size_t) t.N * t.H * t.W;
-    const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (px >= total) return;
-    const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
-    snnb_roi roi;
-    float v[8];
-    if (roi_list_slot(L, g, n, t.N, roi)) {
-        const bool direct = roi.width == t.W && roi.height == t.H;
-        ResizeTaps r;
-        if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
-        else r = resize_taps(resize_pos(ox, oy, t.W, t.H, roi.width, roi.height), roi.width, roi.height, linear);
-        r.x0 += roi.x, r.x1 += roi.x, r.y0 += roi.y, r.y1 += roi.y;
-        frame_pixel<FMT>(L.img[roi.frame], 0, r, linear, direct, t, q, v);
-    } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) v[j] = 0.0f;
-    }
-    store_input_pixel(t, f, px, v);
-}
-__global__ void __launch_bounds__(256) roi_list_clear_kernel(const __grid_constant__ FrameListV L, RoiV g, int N, uint8_t* __restrict__ dst, long long slot_bytes) {
-    pdl_wait();
-    snnb_roi roi;
-    if (roi_list_slot(L, g, (int) blockIdx.y, N, roi)) return;
-    uint8_t* p = dst + (long long) blockIdx.y * slot_bytes;
-    for (long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * 16; i < slot_bytes; i += (long long) gridDim.x * blockDim.x * 16) {
-        if ((reinterpret_cast<uintptr_t>(p + i) & 15) == 0 && i + 16 <= slot_bytes) {
-            *reinterpret_cast<uint4*>(p + i) = make_uint4(0u, 0u, 0u, 0u);
-        } else {
-            for (long long k = i; k < i + 16 && k < slot_bytes; ++k) p[k] = 0;
-        }
-    }
-}
 // The table of a list (checked by the caller: 1 <= count <= SNNB_FRAME_LIST_MAX); each entry is frame_view of the image as a one-image
 // snnb_frames, so the matrix constants come from the same code. Entries past the count stay zero and are never read.
 static void frame_list_view(const snnb_frame_list& fl, FrameListV& L) {
@@ -1897,80 +1752,181 @@ static void frame_list_view(const snnb_frame_list& fl, FrameListV& L) {
         L.img[i] = frame_view(fr);
     }
 }
-static U8Norm frame_list_norm(const snnb_frame_list& fl) {
+static U8Norm frame_norm(const float mean4[4], const float norm4[4]) {
     U8Norm q;
-    for (int i = 0; i < 4; ++i) q.mean[i] = fl.mean4[i], q.norm[i] = fl.norm4[i];
+    for (int i = 0; i < 4; ++i) q.mean[i] = mean4[i], q.norm[i] = norm4[i];
     return q;
 }
-int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t, bool luma) {
-    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_list_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
+
+// The kernel formats of a launch: every public format, the YUV ones (luma output), or the Y plane of YUV frames (FRAME_LUMA, and
+// FRAME_LUMA10 for P010)
+enum class FrameKernels { all, yuv, luma };
+// Calls launch(std::integral_constant<int, FMT>()) with FMT the kernel format of `format` and returns its result; -1 when SET has no
+// kernel for the format
+template <FrameKernels SET, class F>
+static int with_format(int format, F&& launch) {
+    using std::integral_constant;
+    if constexpr (SET == FrameKernels::luma) {
+        if (format == SNNB_FRAME_P010) return launch(integral_constant<int, FRAME_LUMA10>());
+        return launch(integral_constant<int, FRAME_LUMA>());
+    } else {
+        switch (format) {
+        case SNNB_FRAME_NV12: return launch(integral_constant<int, SNNB_FRAME_NV12>());
+        case SNNB_FRAME_NV21: return launch(integral_constant<int, SNNB_FRAME_NV21>());
+        case SNNB_FRAME_I420: return launch(integral_constant<int, SNNB_FRAME_I420>());
+        case SNNB_FRAME_P010: return launch(integral_constant<int, SNNB_FRAME_P010>());
+        case SNNB_FRAME_RGBA8:
+            if constexpr (SET == FrameKernels::all) return launch(integral_constant<int, SNNB_FRAME_RGBA8>());
+            break;
+        }
+        return -1;
+    }
+}
+static const char* format_name(int fmt) {
+    switch (fmt) {
+    case SNNB_FRAME_NV12: return "nv12";
+    case SNNB_FRAME_NV21: return "nv21";
+    case SNNB_FRAME_I420: return "i420";
+    case SNNB_FRAME_RGBA8: return "rgba8";
+    case SNNB_FRAME_P010: return "p010";
+    case FRAME_LUMA: return "luma";
+    case FRAME_LUMA10: return "luma10";
+    }
+    return "?";
+}
+// launch_done with the kernel named with its template arguments, kernel<arg0> or kernel<arg0, arg1>
+static int launch_done(snnb_context* ctx, cudaError_t launched, const char* kernel, const char* arg0, const char* arg1 = nullptr) {
+    char name[96];
+    if (arg1) std::snprintf(name, sizeof(name), "%s<%s, %s>", kernel, arg0, arg1);
+    else std::snprintf(name, sizeof(name), "%s<%s>", kernel, arg0);
+    return launch_done(ctx, launched, name);
+}
+
+template <class Src>
+static int frame_input(snnb_context* ctx, const char* who, const Src& src, int format, const U8Norm& q, int linear_filter, snnb_tensor* t, bool luma) {
+    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "%s: the input tensor has %d channels; frames feed 1 to 4", who, t->c);
+    if (luma)
+        SNNB_REQUIRE(t->c == 1 && format != SNNB_FRAME_RGBA8, "%s: luma input feeds 1 channel from YUV frames (%d channels, format %d)", who, t->c, format);
+    const int linear = linear_filter ? 1 : 0;
+    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
+    auto launch = [&](auto fmt) {
+        constexpr int FMT = decltype(fmt)::value;
+        return launch_done(ctx, launch_k(frame_input_kernel<FMT, Src>, grid, block, 0, ctx->stream, src, view(t), q, linear, feed_view(t)), "frame_input_kernel",
+                           format_name(FMT), Src::form);
+    };
+    const int rc = luma ? with_format<FrameKernels::luma>(format, launch) : with_format<FrameKernels::all>(format, launch);
+    SNNB_REQUIRE(rc >= 0, "%s: unknown format %d", who, format);
+    return rc;
+}
+int launch_frame_input(snnb_context* ctx, const snnb_frames& fr, snnb_tensor* t, bool luma) {
+    return frame_input(ctx, "launch_frame_input", FrameBatchV {frame_view(fr)}, fr.format, frame_norm(fr.mean4, fr.norm4), fr.linear_filter, t, luma);
+}
+int launch_frame_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t, bool luma) {
     SNNB_REQUIRE(fl.count == t->n && fl.count <= SNNB_FRAME_LIST_MAX, "launch_frame_list_input: %d images for a batch of %d", fl.count, t->n);
     FrameListV L;
     frame_list_view(fl, L);
-    const U8Norm q   = frame_list_norm(fl);
-    const int linear = fl.linear_filter ? 1 : 0;
-    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
-    if (luma) {
-        SNNB_REQUIRE(t->c == 1 && fl.format != SNNB_FRAME_RGBA8, "launch_frame_list_input: luma input feeds 1 channel from YUV frames (%d channels, format %d)",
-                     t->c, fl.format);
-        if (fl.format == SNNB_FRAME_P010)
-            return launch_done(ctx, launch_k(frame_list_input_kernel<FRAME_LUMA10>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)),
-                               "frame_list_input_kernel<luma10>");
-        return launch_done(ctx, launch_k(frame_list_input_kernel<FRAME_LUMA>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)),
-                           "frame_list_input_kernel<luma>");
-    }
-    switch (fl.format) {
-    case SNNB_FRAME_NV12:
-        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<nv12>");
-    case SNNB_FRAME_NV21:
-        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<nv21>");
-    case SNNB_FRAME_I420:
-        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<i420>");
-    case SNNB_FRAME_RGBA8:
-        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<rgba8>");
-    case SNNB_FRAME_P010:
-        return launch_done(ctx, launch_k(frame_list_input_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, L, view(t), q, linear, feed_view(t)), "frame_list_input_kernel<p010>");
-    }
-    SNNB_REQUIRE(false, "launch_frame_list_input: unknown format %d", fl.format);
+    return frame_input(ctx, "launch_frame_list_input", L, fl.format, frame_norm(fl.mean4, fl.norm4), fl.linear_filter, t, luma);
 }
-int launch_frame_list_roi_input(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, snnb_tensor* t) {
-    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "launch_frame_list_roi_input: the input tensor has %d channels; frames feed 1 to 4", t->c);
-    SNNB_REQUIRE(fl.count >= 1 && fl.count <= SNNB_FRAME_LIST_MAX, "launch_frame_list_roi_input: %d frames", fl.count);
+
+// Regions of device frames (snnb_model_run_rois / run_rois_list): batch slot n is region rois[n] of frame rois[n].frame. A used slot
+// (n < the count) is valid when its region lies inside a frame that exists; roi_slot is the one test of that, so the input kernel and the
+// clear kernel cannot disagree on which slots they serve.
+struct RoiV {
+    const snnb_roi* rois; // [N]
+    const int* count;     // nullptr: every slot is used
+    int num_frames;
+};
+// A frame index outside the frames fails the test, so the size looked up for it (of the nearest frame) does not matter
+template <class Src>
+__device__ __forceinline__ bool roi_slot(const Src& src, const RoiV& g, int slot, int N, snnb_roi& r) {
+    const int* p = reinterpret_cast<const int*>(g.rois + slot);
+    r.frame = __ldg(p), r.row = __ldg(p + 1), r.x = __ldg(p + 2), r.y = __ldg(p + 3), r.width = __ldg(p + 4), r.height = __ldg(p + 5);
+    const int used = g.count ? min(max(__ldg(g.count), 0), N) : N;
+    const int2 wh  = frame_size(src, min(max(r.frame, 0), g.num_frames - 1));
+    return slot < used && r.frame >= 0 && r.frame < g.num_frames && r.width >= 1 && r.height >= 1 && r.x >= 0 && r.y >= 0 && r.x <= wh.x - r.width &&
+           r.y <= wh.y - r.height;
+}
+// One thread per model-input pixel, as frame_input_kernel: the taps of ImageTexture::resize from a region-sized source, clamped to the
+// region, then offset to the region's origin in the frame (so chroma is sited in frame coordinates). A region of the model's size is
+// sampled directly. Invalid and unused slots get an all-zero input.
+template <int FMT, class Src>
+__global__ void __launch_bounds__(256) frame_roi_input_kernel(const __grid_constant__ Src src, RoiV g, TV t, U8Norm q, int linear, FeedV f) {
+    pdl_wait();
+    const size_t total = (size_t) t.N * t.H * t.W;
+    const size_t px    = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (px >= total) return;
+    const int ox = (int) (px % t.W), oy = (int) ((px / t.W) % t.H), n = (int) (px / ((size_t) t.W * t.H));
+    snnb_roi roi;
+    float v[8];
+    if (roi_slot(src, g, n, t.N, roi)) {
+        const bool direct = roi.width == t.W && roi.height == t.H;
+        ResizeTaps r;
+        if (direct) r.x0 = r.x1 = ox, r.y0 = r.y1 = oy, r.ax = r.ay = 0.0f;
+        else r = resize_taps(resize_pos(ox, oy, t.W, t.H, roi.width, roi.height), roi.width, roi.height, linear);
+        r.x0 += roi.x, r.x1 += roi.x, r.y0 += roi.y, r.y1 += roi.y;
+        frame_pixel<FMT>(frame_of(src, roi.frame), image_of(src, roi.frame), r, linear, direct, t, q, v);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) v[j] = 0.0f;
+    }
+    store_input_pixel(t, f, px, v);
+}
+template <class Src>
+static int frame_roi_input(snnb_context* ctx, const char* who, const Src& src, int format, const U8Norm& q, int linear_filter, const RoiV& g, snnb_tensor* t) {
+    SNNB_REQUIRE(t->c <= 4 && t->cp == 8, "%s: the input tensor has %d channels; frames feed 1 to 4", who, t->c);
+    const int linear = linear_filter ? 1 : 0;
+    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
+    const int rc = with_format<FrameKernels::all>(format, [&](auto fmt) {
+        constexpr int FMT = decltype(fmt)::value;
+        return launch_done(ctx, launch_k(frame_roi_input_kernel<FMT, Src>, grid, block, 0, ctx->stream, src, g, view(t), q, linear, feed_view(t)),
+                           "frame_roi_input_kernel", format_name(FMT), Src::form);
+    });
+    SNNB_REQUIRE(rc >= 0, "%s: unknown format %d", who, format);
+    return rc;
+}
+int launch_frame_roi_input(snnb_context* ctx, const snnb_frames& fr, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t) {
+    return frame_roi_input(ctx, "launch_frame_roi_input", FrameBatchV {frame_view(fr)}, fr.format, frame_norm(fr.mean4, fr.norm4), fr.linear_filter,
+                           RoiV {rois, count, num_frames}, t);
+}
+int launch_frame_roi_input(snnb_context* ctx, const snnb_frame_list& fl, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t) {
+    SNNB_REQUIRE(num_frames == fl.count && fl.count >= 1 && fl.count <= SNNB_FRAME_LIST_MAX, "launch_frame_list_roi_input: %d frames", fl.count);
     FrameListV L;
     frame_list_view(fl, L);
-    const U8Norm q   = frame_list_norm(fl);
-    const RoiV g {rois, count, fl.count};
-    const int linear = fl.linear_filter ? 1 : 0;
-    const dim3 grid((unsigned) ((t->pixels() + 255) / 256)), block(256);
-    switch (fl.format) {
-    case SNNB_FRAME_NV12:
-        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
-                           "frame_list_roi_input_kernel<nv12>");
-    case SNNB_FRAME_NV21:
-        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
-                           "frame_list_roi_input_kernel<nv21>");
-    case SNNB_FRAME_I420:
-        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
-                           "frame_list_roi_input_kernel<i420>");
-    case SNNB_FRAME_RGBA8:
-        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
-                           "frame_list_roi_input_kernel<rgba8>");
-    case SNNB_FRAME_P010:
-        return launch_done(ctx, launch_k(frame_list_roi_input_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, L, g, view(t), q, linear, feed_view(t)),
-                           "frame_list_roi_input_kernel<p010>");
-    }
-    SNNB_REQUIRE(false, "launch_frame_list_roi_input: unknown format %d", fl.format);
+    return frame_roi_input(ctx, "launch_frame_list_roi_input", L, fl.format, frame_norm(fl.mean4, fl.norm4), fl.linear_filter, RoiV {rois, count, fl.count}, t);
 }
-int launch_roi_list_clear(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes) {
-    SNNB_REQUIRE(batch >= 1 && batch <= 65535 && slot_bytes >= 1, "launch_roi_list_clear: batch %d, %lld bytes per slot", batch, slot_bytes);
-    SNNB_REQUIRE(fl.count >= 1 && fl.count <= SNNB_FRAME_LIST_MAX, "launch_roi_list_clear: %d frames", fl.count);
-    FrameListV L;
-    frame_list_view(fl, L);
-    const RoiV g {rois, count, fl.count};
+// Zeroes batch slot blockIdx.y of a caller's buffer (slot_bytes per slot, slots contiguous) when roi_slot rejects it. A slot is the
+// outermost dimension in NHWC and NCHW alike. Runs after the outputs and classes are written.
+template <class Src>
+__global__ void __launch_bounds__(256) roi_clear_kernel(const __grid_constant__ Src src, RoiV g, int N, uint8_t* __restrict__ dst, long long slot_bytes) {
+    pdl_wait();
+    snnb_roi roi;
+    if (roi_slot(src, g, (int) blockIdx.y, N, roi)) return;
+    uint8_t* p = dst + (long long) blockIdx.y * slot_bytes;
+    for (long long i = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * 16; i < slot_bytes; i += (long long) gridDim.x * blockDim.x * 16) {
+        if ((reinterpret_cast<uintptr_t>(p + i) & 15) == 0 && i + 16 <= slot_bytes) {
+            *reinterpret_cast<uint4*>(p + i) = make_uint4(0u, 0u, 0u, 0u);
+        } else {
+            for (long long k = i; k < i + 16 && k < slot_bytes; ++k) p[k] = 0;
+        }
+    }
+}
+template <class Src>
+static int roi_clear(snnb_context* ctx, const char* who, const Src& src, const RoiV& g, int batch, void* dst, long long slot_bytes) {
+    SNNB_REQUIRE(batch >= 1 && batch <= 65535 && slot_bytes >= 1, "%s: batch %d, %lld bytes per slot", who, batch, slot_bytes);
     const long long chunks = (slot_bytes + 16 * 256 - 1) / (16 * 256);
     const dim3 grid((unsigned) std::min(chunks, 1024LL), (unsigned) batch);
-    return launch_done(ctx, launch_k(roi_list_clear_kernel, grid, dim3(256), 0, ctx->stream, L, g, batch, static_cast<uint8_t*>(dst), slot_bytes),
-                       "roi_list_clear_kernel");
+    return launch_done(ctx, launch_k(roi_clear_kernel<Src>, grid, dim3(256), 0, ctx->stream, src, g, batch, static_cast<uint8_t*>(dst), slot_bytes),
+                       "roi_clear_kernel", Src::form);
+}
+int launch_roi_clear(snnb_context* ctx, const snnb_frames& fr, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes) {
+    return roi_clear(ctx, "launch_roi_clear", FrameSizeV {fr.width, fr.height}, RoiV {rois, count, num_frames}, batch, dst, slot_bytes);
+}
+int launch_roi_clear(snnb_context* ctx, const snnb_frame_list& fl, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst,
+                     long long slot_bytes) {
+    SNNB_REQUIRE(num_frames == fl.count && fl.count >= 1 && fl.count <= SNNB_FRAME_LIST_MAX, "launch_roi_list_clear: %d frames", fl.count);
+    FrameListV L;
+    frame_list_view(fl, L);
+    return roi_clear(ctx, "launch_roi_list_clear", L, RoiV {rois, count, fl.count}, batch, dst, slot_bytes);
 }
 
 // Detection rows -> regions (snnb_rois_from_detections). The rectangle of one row, every operation IEEE-rounded on its own (no FMA
@@ -1991,9 +1947,10 @@ __device__ __forceinline__ bool roi_from_row(const float* __restrict__ row, floa
 // One CTA visits rows (n, k), k < min(counts[n], max_rows), in order (frame, then row), a chunk of ROI_THREADS at a time: keep flags,
 // a block prefix sum over them, and the kept rows scattered to their rank while it is below `capacity`. Then the tail is zeroed.
 constexpr int ROI_THREADS = 1024;
+template <class Sizes>
 __global__ void __launch_bounds__(ROI_THREADS) rois_from_detections_kernel(const float* __restrict__ rows, const int* __restrict__ counts, int num_frames,
-                                                                         int max_rows, int fw, int fh, snnb_roi_select sel, snnb_roi* __restrict__ out,
-                                                                         int capacity, int* __restrict__ count_out) {
+                                                                         int max_rows, const __grid_constant__ Sizes S, snnb_roi_select sel,
+                                                                         snnb_roi* __restrict__ out, int capacity, int* __restrict__ count_out) {
     pdl_wait();
     __shared__ int warp_incl[ROI_THREADS / 32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = ROI_THREADS / 32;
@@ -2005,7 +1962,10 @@ __global__ void __launch_bounds__(ROI_THREADS) rois_from_detections_kernel(const
         bool keep = false;
         if (i < total) {
             const int n = i / max_rows, k = i - n * max_rows;
-            if (k < min(__ldg(counts + n), max_rows)) keep = roi_from_row(rows + (size_t) i * 6, (float) fw, (float) fh, sel, r);
+            if (k < min(__ldg(counts + n), max_rows)) {
+                const int2 wh = frame_size(S, n);
+                keep          = roi_from_row(rows + (size_t) i * 6, (float) wh.x, (float) wh.y, sel, r);
+            }
             r.frame = n, r.row = k;
         }
         const unsigned ballot = __ballot_sync(0xffffffffu, keep);
@@ -2029,65 +1989,24 @@ __global__ void __launch_bounds__(ROI_THREADS) rois_from_detections_kernel(const
     const int written = min(kept, capacity);
     for (int i = written + threadIdx.x; i < capacity; i += ROI_THREADS) out[i] = snnb_roi {0, 0, 0, 0, 0, 0};
     if (threadIdx.x == 0) *count_out = written;
+}
+template <class Sizes>
+static int rois_from_detections_launch(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows, const Sizes& S,
+                                       const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count) {
+    return launch_done(ctx, launch_k(rois_from_detections_kernel<Sizes>, dim3(1), dim3(ROI_THREADS), 0, stream, rows, counts, num_frames, max_rows, S, sel, rois,
+                                     capacity, count),
+                       "rois_from_detections_kernel", Sizes::form);
 }
 int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh,
                                 const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count) {
-    return launch_done(ctx, launch_k(rois_from_detections_kernel, dim3(1), dim3(ROI_THREADS), 0, stream, rows, counts, num_frames, max_rows, fw, fh, sel, rois,
-                                     capacity, count),
-                       "rois_from_detections_kernel");
+    return rois_from_detections_launch(ctx, stream, rows, counts, num_frames, max_rows, FrameSizeV {fw, fh}, sel, rois, capacity, count);
 }
-// snnb_rois_from_detections_list: rois_from_detections_kernel's scan with frame n's own size, from a table passed by value as FrameListV
-// is (2 KB).
-struct FrameSizesV {
-    int wh[SNNB_FRAME_LIST_MAX][2];
-};
-__global__ void __launch_bounds__(ROI_THREADS) rois_from_detections_list_kernel(const float* __restrict__ rows, const int* __restrict__ counts, int num_frames,
-                                                                              int max_rows, const __grid_constant__ FrameSizesV S, snnb_roi_select sel,
-                                                                              snnb_roi* __restrict__ out, int capacity, int* __restrict__ count_out) {
-    pdl_wait();
-    __shared__ int warp_incl[ROI_THREADS / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = ROI_THREADS / 32;
-    const int total = num_frames * max_rows;
-    int kept = 0; // rows kept before the current chunk (uniform over the CTA)
-    for (int c0 = 0; c0 < total; c0 += ROI_THREADS) {
-        const int i = c0 + threadIdx.x;
-        snnb_roi r;
-        bool keep = false;
-        if (i < total) {
-            const int n = i / max_rows, k = i - n * max_rows;
-            if (k < min(__ldg(counts + n), max_rows)) keep = roi_from_row(rows + (size_t) i * 6, (float) S.wh[n][0], (float) S.wh[n][1], sel, r);
-            r.frame = n, r.row = k;
-        }
-        const unsigned ballot = __ballot_sync(0xffffffffu, keep);
-        if (lane == 0) warp_incl[warp] = __popc(ballot);
-        __syncthreads();
-        if (warp == 0) {
-            int v = warp_incl[lane];
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const int u = __shfl_up_sync(0xffffffffu, v, d);
-                if (lane >= d) v += u;
-            }
-            warp_incl[lane] = v;
-        }
-        __syncthreads();
-        const int rank = kept + (warp ? warp_incl[warp - 1] : 0) + __popc(ballot & ((1u << lane) - 1u));
-        if (keep && rank < capacity) out[rank] = r;
-        kept += warp_incl[warps - 1];
-        __syncthreads(); // warp_incl is rewritten by the next chunk
-    }
-    const int written = min(kept, capacity);
-    for (int i = written + threadIdx.x; i < capacity; i += ROI_THREADS) out[i] = snnb_roi {0, 0, 0, 0, 0, 0};
-    if (threadIdx.x == 0) *count_out = written;
-}
-int launch_rois_from_detections_list(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows,
-                                     const int* frame_wh, const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count) {
+int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows,
+                                const int* frame_wh, const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count) {
     SNNB_REQUIRE(num_frames >= 1 && num_frames <= SNNB_FRAME_LIST_MAX, "launch_rois_from_detections_list: %d frames", num_frames);
     FrameSizesV S {};
     for (int n = 0; n < num_frames; ++n) S.wh[n][0] = frame_wh[2 * n], S.wh[n][1] = frame_wh[2 * n + 1];
-    return launch_done(ctx, launch_k(rois_from_detections_list_kernel, dim3(1), dim3(ROI_THREADS), 0, stream, rows, counts, num_frames, max_rows, S, sel, rois,
-                                     capacity, count),
-                       "rois_from_detections_list_kernel");
+    return rois_from_detections_launch(ctx, stream, rows, counts, num_frames, max_rows, S, sel, rois, capacity, count);
 }
 
 // Model output 0 -> device video frames (snnb_model_transform_frames), the reverse of frame_input_kernel. Each frame pixel is
@@ -2257,19 +2176,12 @@ int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_fram
     const int linear = fr.linear_filter ? 1 : 0;
     const size_t blocks = (size_t) t->n * ((fr.height + 1) / 2) * ((fr.width + 1) / 2);
     const dim3 grid((unsigned) ((blocks + 255) / 256)), block(256);
-    switch (fr.format) {
-    case SNNB_FRAME_NV12:
-        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<nv12>");
-    case SNNB_FRAME_NV21:
-        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<nv21>");
-    case SNNB_FRAME_I420:
-        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<i420>");
-    case SNNB_FRAME_RGBA8:
-        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<rgba8>");
-    case SNNB_FRAME_P010:
-        return launch_done(ctx, launch_k(frame_output_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel<p010>");
-    }
-    SNNB_REQUIRE(false, "launch_frame_output: unknown format %d", fr.format);
+    const int rc = with_format<FrameKernels::all>(fr.format, [&](auto fmt) {
+        constexpr int FMT = decltype(fmt)::value;
+        return launch_done(ctx, launch_k(frame_output_kernel<FMT>, grid, block, 0, ctx->stream, view(t), o, linear), "frame_output_kernel", format_name(FMT));
+    });
+    SNNB_REQUIRE(rc >= 0, "launch_frame_output: unknown format %d", fr.format);
+    return rc;
 }
 
 // A 1-channel model output 0 -> the Y plane of device video frames, with the source frames' chroma resampled beside it
@@ -2306,8 +2218,10 @@ __device__ __forceinline__ void chroma_texel(const FrameV& s, int step, int n, i
         v = (float) __ldg(s.plane[2] + n * s.stride[2] + (size_t) y * s.pitch[2] + (size_t) x * step);
     }
 }
-// The 2 x 2 block (bx, by) of frame pixels of image n for luma_list_output_kernel: luma_output_kernel's body below, through the same
-// helpers. It is written out twice because luma_output_kernel calling it compiles to different register allocation.
+// The 2 x 2 block (bx, by) of frame pixels of image n, i.e. one chroma sample: 4 Y bytes, then the chroma sample resized from the
+// source's chroma planes. A chroma plane of the source's size is copied. Pixels past an odd width or height are not written. P010 (from
+// P010 frames): 10-bit Y from M10 and the source's 10-bit chroma, each stored as value << 6. Shared by luma_output_kernel and
+// luma_list_output_kernel.
 template <int FMT>
 __device__ __forceinline__ void luma_out_block(const TV& t, const FrameV& s, int step, const FrameOutV& o, int n, int bx, int by, int linear) {
     constexpr bool TEN = FMT == SNNB_FRAME_P010;
@@ -2355,95 +2269,49 @@ __device__ __forceinline__ void luma_out_block(const TV& t, const FrameV& s, int
         else store_2u8(d, V, U);
     }
 }
-// One thread per 2 x 2 block of frame pixels, i.e. per chroma sample, as frame_output_kernel: 4 Y bytes, then the chroma sample resized
-// from the source's chroma planes. A chroma plane of the source's size is copied. Pixels past an odd width or height are not written.
-// P010 (from P010 frames): 10-bit Y from M10 and the source's 10-bit chroma, each stored as value << 6.
+// One thread per 2 x 2 block of frame pixels (luma_out_block), as frame_output_kernel
 template <int FMT>
 __global__ void __launch_bounds__(256) luma_output_kernel(TV t, FrameV s, int step, FrameOutV o, int linear) {
-    constexpr bool TEN = FMT == SNNB_FRAME_P010;
     pdl_wait();
     const int cw = (o.w + 1) >> 1, ch = (o.h + 1) >> 1;
     const size_t total = (size_t) t.N * ch * cw;
     const size_t gid   = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (gid >= total) return;
     const int bx = (int) (gid % cw), by = (int) ((gid / cw) % ch), n = (int) (gid / ((size_t) cw * ch));
-    const int x = 2 * bx, y = 2 * by;
-    const bool has_x1 = x + 1 < o.w, has_y1 = y + 1 < o.h;
-#pragma unroll
-    for (int dy = 0; dy < 2; ++dy) {
-        if (dy && !has_y1) break;
-        if constexpr (TEN) {
-            uint8_t* d   = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + (size_t) x * 2;
-            const int ya = luma_out_pixel<true>(t, o, n, x, y + dy, linear);
-            if (has_x1) store_2p010(d, ya, luma_out_pixel<true>(t, o, n, x + 1, y + dy, linear));
-            else *reinterpret_cast<uint16_t*>(d) = (uint16_t) (ya << 6);
-        } else {
-            uint8_t* d   = o.plane[0] + n * o.stride[0] + (size_t) (y + dy) * o.pitch[0] + x;
-            const int ya = luma_out_pixel<false>(t, o, n, x, y + dy, linear);
-            if (has_x1) store_2u8(d, ya, luma_out_pixel<false>(t, o, n, x + 1, y + dy, linear));
-            else d[0] = (uint8_t) ya;
-        }
-    }
-    const int scw = (s.w + 1) >> 1, sch = (s.h + 1) >> 1;
-    const bool direct = cw == scw && ch == sch;
-    ResizeTaps r;
-    if (direct) r.x0 = r.x1 = bx, r.y0 = r.y1 = by, r.ax = r.ay = 0.0f;
-    else r = resize_taps(resize_pos(bx, by, cw, ch, scw, sch), scw, sch, linear);
-    float u00, v00;
-    chroma_texel<TEN>(s, step, n, r.x0, r.y0, u00, v00);
-    int U = (int) u00, V = (int) v00;
-    if (linear && !direct) {
-        float u01, v01, u10, v10, u11, v11;
-        chroma_texel<TEN>(s, step, n, r.x1, r.y0, u01, v01);
-        chroma_texel<TEN>(s, step, n, r.x0, r.y1, u10, v10);
-        chroma_texel<TEN>(s, step, n, r.x1, r.y1, u11, v11);
-        U = (int) rintf(blend_rn(r, u00, u01, u10, u11)), V = (int) rintf(blend_rn(r, v00, v01, v10, v11));
-    }
-    if (TEN) {
-        store_2p010(o.plane[1] + n * o.stride[1] + (size_t) by * o.pitch[1] + (size_t) bx * 4, U, V);
-    } else if (FMT == SNNB_FRAME_I420) {
-        o.plane[1][n * o.stride[1] + (size_t) by * o.pitch[1] + bx] = (uint8_t) U;
-        o.plane[2][n * o.stride[2] + (size_t) by * o.pitch[2] + bx] = (uint8_t) V;
-    } else {
-        uint8_t* d = o.plane[1] + n * o.stride[1] + (size_t) by * o.pitch[1] + (size_t) bx * 2;
-        if (FMT == SNNB_FRAME_NV12) store_2u8(d, U, V);
-        else store_2u8(d, V, U);
-    }
+    luma_out_block<FMT>(t, s, step, o, n, bx, by, linear);
+}
+// Where luma_out_block reads the source chroma of `format` frames: U and V from planes plane[0] and plane[1] at byte offsets offset[0] and
+// offset[1], `step` samples apart along a row. I420: planes 1 and 2; NV12 / NV21 / P010: the two samples of each pair in plane 1.
+struct ChromaSource {
+    int plane[2], offset[2], step;
+};
+static ChromaSource chroma_source(int format) {
+    if (format == SNNB_FRAME_I420) return {{1, 2}, {0, 0}, 1};
+    const int u = format == SNNB_FRAME_NV21 ? 1 : 0, bytes = format == SNNB_FRAME_P010 ? 2 : 1;
+    return {{1, 1}, {u * bytes, (1 - u) * bytes}, 2};
 }
 int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames& src, const snnb_frames_out& fr) {
     SNNB_REQUIRE(t->c == 1 && t->cp == 8 && !t->feed_only && src.format != SNNB_FRAME_RGBA8,
                  "launch_luma_output: the output tensor has %d channels, source format %d; luma frames are written from 1 channel with YUV chroma", t->c, src.format);
     SNNB_REQUIRE((src.format == SNNB_FRAME_P010) == (fr.format == SNNB_FRAME_P010), "launch_luma_output: source format %d, out format %d; P010 pairs with P010 only",
                  src.format, fr.format);
-    // the source chroma as two planes of samples `step` samples apart: U and V of I420, or the two samples of an NV12 / NV21 / P010 pair
+    const ChromaSource c = chroma_source(src.format);
     FrameV s {};
-    int step = 1;
     s.w = src.width, s.h = src.height;
-    if (src.format == SNNB_FRAME_I420) {
-        for (int i = 1; i < 3; ++i) s.plane[i] = src.plane[i], s.pitch[i] = src.pitch[i], s.stride[i] = src.image_stride[i];
-    } else {
-        const int u = src.format == SNNB_FRAME_NV21 ? 1 : 0, bytes = src.format == SNNB_FRAME_P010 ? 2 : 1;
-        step = 2;
-        s.plane[1] = src.plane[1] + u * bytes, s.plane[2] = src.plane[1] + (1 - u) * bytes;
-        s.pitch[1] = s.pitch[2] = src.pitch[1], s.stride[1] = s.stride[2] = src.image_stride[1];
-    }
+    for (int i = 0; i < 2; ++i)
+        s.plane[1 + i] = src.plane[c.plane[i]] + c.offset[i], s.pitch[1 + i] = src.pitch[c.plane[i]], s.stride[1 + i] = src.image_stride[c.plane[i]];
     FrameOutV o;
     for (int i = 0; i < 3; ++i) o.plane[i] = fr.plane[i], o.pitch[i] = fr.pitch[i], o.stride[i] = fr.image_stride[i];
     o.w = fr.width, o.h = fr.height, o.scale = fr.scale, o.offset = fr.offset;
     const int linear = fr.linear_filter ? 1 : 0;
     const size_t blocks = (size_t) t->n * ((fr.height + 1) / 2) * ((fr.width + 1) / 2);
     const dim3 grid((unsigned) ((blocks + 255) / 256)), block(256);
-    switch (fr.format) {
-    case SNNB_FRAME_NV12:
-        return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<nv12>");
-    case SNNB_FRAME_NV21:
-        return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<nv21>");
-    case SNNB_FRAME_I420:
-        return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<i420>");
-    case SNNB_FRAME_P010:
-        return launch_done(ctx, launch_k(luma_output_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, view(t), s, step, o, linear), "luma_output_kernel<p010>");
-    }
-    SNNB_REQUIRE(false, "launch_luma_output: out format %d; luma frames are written as NV12, NV21, I420 or P010", fr.format);
+    const int rc = with_format<FrameKernels::yuv>(fr.format, [&](auto fmt) {
+        constexpr int FMT = decltype(fmt)::value;
+        return launch_done(ctx, launch_k(luma_output_kernel<FMT>, grid, block, 0, ctx->stream, view(t), s, c.step, o, linear), "luma_output_kernel", format_name(FMT));
+    });
+    SNNB_REQUIRE(rc >= 0, "launch_luma_output: out format %d; luma frames are written as NV12, NV21, I420 or P010", fr.format);
+    return rc;
 }
 
 // Model output 0 -> an 8-bit label plane (snnb_model_segment_frames): the fp32 scores hi + lo resampled to the plane with
@@ -2655,7 +2523,7 @@ static int frame_out_list_view(const char* who, const snnb_tensor* t, const snnb
     SNNB_REQUIRE(fits, "%s: the list's output needs more than 2^31 - 1 CTAs", who);
     return 0;
 }
-int launch_frame_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_out_list& fo) {
+int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_out_list& fo) {
     SNNB_REQUIRE((t->c == 1 || t->c == 3 || t->c == 4) && t->cp == 8 && !t->feed_only,
                  "launch_frame_list_output: the output tensor has %d channels; frames are written from 1, 3 or 4", t->c);
     FrameOutListV L;
@@ -2663,26 +2531,15 @@ int launch_frame_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb
     if (frame_out_list_view("launch_frame_list_output", t, fo, L, blocks)) return 1;
     const int linear = fo.linear_filter ? 1 : 0;
     const dim3 grid(blocks), block(256);
-    switch (fo.format) {
-    case SNNB_FRAME_NV12:
-        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
-                           "frame_list_output_kernel<nv12>");
-    case SNNB_FRAME_NV21:
-        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
-                           "frame_list_output_kernel<nv21>");
-    case SNNB_FRAME_I420:
-        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
-                           "frame_list_output_kernel<i420>");
-    case SNNB_FRAME_RGBA8:
-        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_RGBA8>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
-                           "frame_list_output_kernel<rgba8>");
-    case SNNB_FRAME_P010:
-        return launch_done(ctx, launch_k(frame_list_output_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
-                           "frame_list_output_kernel<p010>");
-    }
-    SNNB_REQUIRE(false, "launch_frame_list_output: unknown format %d", fo.format);
+    const int rc = with_format<FrameKernels::all>(fo.format, [&](auto fmt) {
+        constexpr int FMT = decltype(fmt)::value;
+        return launch_done(ctx, launch_k(frame_list_output_kernel<FMT>, grid, block, 0, ctx->stream, view(t), L, fo.scale, fo.offset, linear),
+                           "frame_list_output_kernel", format_name(FMT));
+    });
+    SNNB_REQUIRE(rc >= 0, "launch_frame_list_output: unknown format %d", fo.format);
+    return rc;
 }
-int launch_luma_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_list& src, const snnb_frame_out_list& fo) {
+int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_list& src, const snnb_frame_out_list& fo) {
     SNNB_REQUIRE(t->c == 1 && t->cp == 8 && !t->feed_only && src.format != SNNB_FRAME_RGBA8,
                  "launch_luma_list_output: the output tensor has %d channels, source format %d; luma frames are written from 1 channel with YUV chroma", t->c,
                  src.format);
@@ -2692,37 +2549,25 @@ int launch_luma_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_
     FrameOutListV L;
     unsigned blocks = 0;
     if (frame_out_list_view("launch_luma_list_output", t, fo, L, blocks)) return 1;
-    // the source chroma of each image as launch_luma_output lays it out: two planes of samples `step` samples apart
+    const ChromaSource c = chroma_source(src.format);
     ChromaListV S;
     std::memset(&S, 0, sizeof(S));
-    const int u = src.format == SNNB_FRAME_NV21 ? 1 : 0, bytes = src.format == SNNB_FRAME_P010 ? 2 : 1;
-    const int step = src.format == SNNB_FRAME_I420 ? 1 : 2;
     for (int n = 0; n < src.count; ++n) {
         const snnb_frame_image& im = src.images[n];
-        ChromaImageV& c = S.img[n];
-        if (src.format == SNNB_FRAME_I420) c.u = im.plane[1], c.v = im.plane[2], c.pitch_u = im.pitch[1], c.pitch_v = im.pitch[2];
-        else c.u = im.plane[1] + u * bytes, c.v = im.plane[1] + (1 - u) * bytes, c.pitch_u = c.pitch_v = im.pitch[1];
-        c.w = im.width, c.h = im.height;
+        S.img[n] = ChromaImageV {im.plane[c.plane[0]] + c.offset[0], im.plane[c.plane[1]] + c.offset[1], im.pitch[c.plane[0]], im.pitch[c.plane[1]], im.width,
+                                 im.height};
     }
     const int linear = fo.linear_filter ? 1 : 0;
     const dim3 grid(blocks), block(256);
-    switch (fo.format) {
-    case SNNB_FRAME_NV12:
-        return launch_done(ctx, launch_k(luma_list_output_kernel<SNNB_FRAME_NV12>, grid, block, 0, ctx->stream, view(t), L, S, step, fo.scale, fo.offset, linear),
-                           "luma_list_output_kernel<nv12>");
-    case SNNB_FRAME_NV21:
-        return launch_done(ctx, launch_k(luma_list_output_kernel<SNNB_FRAME_NV21>, grid, block, 0, ctx->stream, view(t), L, S, step, fo.scale, fo.offset, linear),
-                           "luma_list_output_kernel<nv21>");
-    case SNNB_FRAME_I420:
-        return launch_done(ctx, launch_k(luma_list_output_kernel<SNNB_FRAME_I420>, grid, block, 0, ctx->stream, view(t), L, S, step, fo.scale, fo.offset, linear),
-                           "luma_list_output_kernel<i420>");
-    case SNNB_FRAME_P010:
-        return launch_done(ctx, launch_k(luma_list_output_kernel<SNNB_FRAME_P010>, grid, block, 0, ctx->stream, view(t), L, S, step, fo.scale, fo.offset, linear),
-                           "luma_list_output_kernel<p010>");
-    }
-    SNNB_REQUIRE(false, "launch_luma_list_output: out format %d; luma frames are written as NV12, NV21, I420 or P010", fo.format);
+    const int rc = with_format<FrameKernels::yuv>(fo.format, [&](auto fmt) {
+        constexpr int FMT = decltype(fmt)::value;
+        return launch_done(ctx, launch_k(luma_list_output_kernel<FMT>, grid, block, 0, ctx->stream, view(t), L, S, c.step, fo.scale, fo.offset, linear),
+                           "luma_list_output_kernel", format_name(FMT));
+    });
+    SNNB_REQUIRE(rc >= 0, "launch_luma_list_output: out format %d; luma frames are written as NV12, NV21, I420 or P010", fo.format);
+    return rc;
 }
-int launch_segment_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_list& lo) {
+int launch_segment_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_list& lo) {
     SNNB_REQUIRE(t->c >= 1 && t->c <= 256 && t->cp % 8 == 0 && !t->feed_only,
                  "launch_segment_list_output: the output tensor has %d channels; labels are written from 1 to 256", t->c);
     SNNB_REQUIRE(lo.count == t->n && lo.count >= 1 && lo.count <= SNNB_FRAME_LIST_MAX, "launch_segment_list_output: %d images for a batch of %d", lo.count, t->n);

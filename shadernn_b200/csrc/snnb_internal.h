@@ -247,38 +247,39 @@ int launch_merge_u8(snnb_context* ctx, const snnb_tensor* t, uint8_t* dev_nhwc_u
 // Output: hi + lo as F32, __float2half_rn of it as F16, clamp(round(v * b.scale + b.offset), 0, 255) as U8. Never reads a feed copy.
 int launch_device_input(snnb_context* ctx, const snnb_device_buffer& b, snnb_tensor* t);
 int launch_device_output(snnb_context* ctx, const snnb_tensor* t, const snnb_device_buffer& b);
-// Device frames (snnb_model_run_frames, checked by the caller) -> libyuv RGBA8 per tap -> resized + normalised -> t (C <= 4). luma: the
-// Y plane of YUV frames as a 1-channel 8-bit image -> resized + normalised -> t (C = 1; snnb_model_transform_luma)
+// The device-frame launchers. Each takes a batch (snnb_frames: one description, images at its image strides) or a list (one descriptor
+// per image, passed to the kernel by value: count <= SNNB_FRAME_LIST_MAX), all checked by the caller; the two forms run one kernel
+// template (input side) or share the per-pixel code (output side).
+// Device frames (snnb_model_run_frames / run_frame_list) -> libyuv RGBA8 per tap -> resized + normalised -> t (C <= 4). luma: the Y
+// plane of YUV frames as a 1-channel 8-bit image -> resized + normalised -> t (C = 1; snnb_model_transform_luma)
 int launch_frame_input(snnb_context* ctx, const snnb_frames& f, snnb_tensor* t, bool luma);
-// t (C = 1, 3 or 4) -> 8 bits as launch_device_output's U8 -> RGBA8 -> resized -> libyuv ABGRTo* -> device frames (checked by the caller)
+int launch_frame_input(snnb_context* ctx, const snnb_frame_list& f, snnb_tensor* t, bool luma);
+// t (C = 1, 3 or 4) -> 8 bits as launch_device_output's U8 -> RGBA8 -> resized -> libyuv ABGRTo* -> device frames. A list writes slot n
+// of t to image n (count == t->n).
 int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames_out& f);
-// t (C = 1) -> 8 bits -> resized -> the Y plane of NV12 / NV21 / I420 frames; their chroma resized from src's chroma planes (checked by
-// the caller, which also keeps the out planes clear of src's chroma unless out is src itself)
+int launch_frame_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_out_list& f);
+// t (C = 1) -> 8 bits -> resized -> the Y plane of NV12 / NV21 / I420 frames; their chroma resized from src's chroma planes (the caller
+// also keeps the out planes clear of src's chroma unless out is src itself)
 int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frames& src, const snnb_frames_out& f);
-// t (C = 1 .. 256) -> scores resized to the label plane -> one byte per pixel: arg-max over C, or s >= threshold for C = 1 (checked by
-// the caller)
+int launch_luma_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_list& src, const snnb_frame_out_list& f);
+// t (C = 1 .. 256) -> scores resized to the label plane -> one byte per pixel: arg-max over C, or s >= threshold for C = 1
 int launch_segment_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_out& out);
-// Regions of device frames (snnb_model_run_rois, checked by the caller) -> t (C <= 4): slot n is rois[n] sampled as launch_frame_input
-// samples a frame of the region's size; invalid slots and slots past *count (count NULL: all used) are zero
+int launch_segment_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_list& out);
+// Regions of num_frames device frames (snnb_model_run_rois / run_rois_list; a list's count is its num_frames) -> t (C <= 4): slot n is
+// rois[n] sampled as launch_frame_input samples a frame of the region's size; invalid slots and slots past *count (count NULL: all
+// used) are zero
 int launch_frame_roi_input(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t);
+int launch_frame_roi_input(snnb_context* ctx, const snnb_frame_list& f, int num_frames, const snnb_roi* rois, const int* count, snnb_tensor* t);
 // Zeroes each of `batch` contiguous slots of slot_bytes bytes at dst whose region launch_frame_roi_input did not serve
 int launch_roi_clear(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes);
-// Detection rows -> regions (snnb_rois_from_detections, checked by the caller), one CTA on `stream`
+int launch_roi_clear(snnb_context* ctx, const snnb_frame_list& f, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst,
+                     long long slot_bytes);
+// Detection rows -> regions (snnb_rois_from_detections, checked by the caller), one CTA on `stream`: every frame fw x fh, or frame n
+// frame_wh[2n] x frame_wh[2n + 1] (host, num_frames <= SNNB_FRAME_LIST_MAX)
 int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh,
                                 const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count);
-// Frame lists (snnb_model_run_frame_list / run_rois_list, checked by the caller): launch_frame_input, launch_frame_roi_input and
-// launch_roi_clear with one descriptor per image, passed to the kernel by value (fl.count <= SNNB_FRAME_LIST_MAX)
-int launch_frame_list_input(snnb_context* ctx, const snnb_frame_list& fl, snnb_tensor* t, bool luma);
-int launch_frame_list_roi_input(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, snnb_tensor* t);
-int launch_roi_list_clear(snnb_context* ctx, const snnb_frame_list& fl, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes);
-// Output lists (snnb_model_transform_frame_list / transform_luma_list / segment_frame_list, checked by the caller): launch_frame_output,
-// launch_luma_output and launch_segment_output with one descriptor per image, slot n of t written to image n (count == t->n)
-int launch_frame_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_out_list& out);
-int launch_luma_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_frame_list& src, const snnb_frame_out_list& out);
-int launch_segment_list_output(snnb_context* ctx, const snnb_tensor* t, const snnb_labels_list& out);
-// launch_rois_from_detections with frame n's size at frame_wh[2n], frame_wh[2n + 1] (host, num_frames <= SNNB_FRAME_LIST_MAX)
-int launch_rois_from_detections_list(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows,
-                                     const int* frame_wh, const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count);
+int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows,
+                                const int* frame_wh, const snnb_roi_select& sel, snnb_roi* rois, int capacity, int* count);
 // The host-side checks of snnb_rois_from_detections, then its launch (engine/core.cpp, beside the device-feed checks)
 int rois_from_detections(snnb_context* ctx, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh, const snnb_roi_select* sel,
                          snnb_roi* rois, int capacity, int* count, cudaStream_t stream);

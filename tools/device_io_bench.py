@@ -53,8 +53,8 @@ NV12 on detect_frames, transform_luma and transform_frames, with each frame kern
                YOLOv3-tiny 416x416 batch 16 with all-pass heads detect_frame_list -> rois_from_detections with per-frame sizes ->
                ResNet-18 112x112 batch 64 run_rois_list, against what a user does without frame lists: per frame a torch NV12 -> RGB
                conversion and F.interpolate into one batch, detect_torch, rows to the host, crops as in `rois`, run_torch; alternating
-               as above. The device time of each kernel of the chain from torch.profiler over 50 calls, and frame_list_input_kernel
-               against frame_input_kernel on one uniform 1920x1080 batch of 16 (the cost of the per-image descriptor).
+               as above. The device time of each kernel of the chain from torch.profiler over 50 calls, and frame_input_kernel's list
+               form against its batch form on one uniform 1920x1080 batch of 16 (the cost of the per-image descriptor).
   framelist_out (opt-in) The same sixteen streams written back: Candy 720x720 transform_frame_list in place, ESPCN 540x960 (the
                luma part's model at a quarter of the area, so that a batch of 16 fits) transform_luma_list in place, and the U-Net of
                `segment` (21 classes) segment_frame_list to each stream's size; each against what a user does without output lists,
@@ -749,14 +749,17 @@ def framelist(torch, ctx, core, modelzoo, d, args):
         "today_frames_per_s_median": med["today"],
         "chain_over_today": med["chain"] / med["today"],
         "rounds": runs,
-        "kernels": {k: frame_kernel_us(torch, chain, 50, k) for k in ("frame_list_input_kernel", "rois_from_detections_list_kernel", "frame_list_roi_input_kernel",
-                                                                     "roi_list_clear_kernel")},
+        # the list forms of the input-side kernel templates, looked up by family: the chain runs no batch form
+        "kernels": {key: frame_kernel_us(torch, chain, 50, family) for key, family in (("frame_list_input_kernel", "frame_input_kernel"),
+                                                                                      ("rois_from_detections_list_kernel", "rois_from_detections_kernel"),
+                                                                                      ("frame_list_roi_input_kernel", "frame_roi_input_kernel"),
+                                                                                      ("roi_list_clear_kernel", "roi_clear_kernel"))},
     }}
-    # the cost of the per-image descriptor: the same uniform 1080p batch through frame_input_kernel and frame_list_input_kernel
+    # the cost of the per-image descriptor: the same uniform 1080p batch through frame_input_kernel's batch and list forms
     nv12 = torch.randint(16, 236, (dbatch, 1080 * 3 // 2, 1920), dtype=torch.uint8, generator=g).cuda()
     views = [nv12[n] for n in range(dbatch)]
     batch_kt = frame_kernel_us(torch, lambda: det.detect_frames(nv12, mean4=dmean, norm4=dnorm), 50, "frame_input_kernel")
-    list_kt = frame_kernel_us(torch, lambda: det.detect_frame_list(views, mean4=dmean, norm4=dnorm), 50, "frame_list_input_kernel")
+    list_kt = frame_kernel_us(torch, lambda: det.detect_frame_list(views, mean4=dmean, norm4=dnorm), 50, "frame_input_kernel")
     res["uniform_1080p"] = {"case": "yolov3tiny %dx%d batch %d from 1920x1080 NV12: the input kernel alone" % (dhw[0], dhw[1], dbatch),
                             "frame_input_kernel": batch_kt, "frame_list_input_kernel": list_kt,
                             "list_over_batch_time": list_kt["us_per_batch"] / batch_kt["us_per_batch"]}
