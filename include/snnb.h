@@ -61,7 +61,9 @@ int snnb_sync(snnb_context* ctx);
 void* snnb_context_stream(snnb_context* ctx);
 /* Thread-local message of the last failing call (replaces SNN_RIP / SNN_LOGE text, core/inc/snn/utils.h:57-62). */
 const char* snnb_last_error(void);
-/* Number of kernels this library has launched on the context since creation (bench.py's gpu_launches). */
+/* Number of kernels this library has launched on the context since creation (bench.py's gpu_launches). A region call whose forward pass
+ * is sized by its device-side count (snnb_model_set_count_batches) adds the selector and the forward pass at the model's batch: an upper
+ * bound, since the host cannot see which size ran. */
 uint64_t snnb_launch_count(snnb_context* ctx);
 int snnb_version(void);
 /* Default precision of per-operator convolution launches on this context (SNNB_PRECISION_FP32X3 or _FP16W; models carry
@@ -199,6 +201,23 @@ int snnb_model_output_dims(const snnb_model* m, int idx, int* n, int* h, int* w,
  * the last bits. snnb_model_launches_per_forward reports n's count once a forward pass at n has run (0 before).
  * A refused call (n < 1, n > the loaded batch, a null model) changes nothing. */
 int snnb_model_set_batch(snnb_model* m, int n);
+/* The batch sizes a region call with a device-side count may run its forward pass at. sizes: a HOST array of num_sizes (0 to 32) sizes,
+ * strictly increasing, each 1 <= sizes[i] <= the loaded batch; num_sizes == 0 clears the declaration. Once sizes are declared,
+ * snnb_model_run_rois and snnb_model_run_rois_list with a non-NULL count_dev run the forward pass at the smallest declared size >= c,
+ * c = clamp(*count_dev, 0, B) with B the model's batch (snnb_model_set_batch), or at B itself when no declared size below B is >= c
+ * (snnb_debug_count_body); c = 0 runs no forward pass. The choice is made on the device, so no call synchronises: each such call
+ * launches one CUDA graph per model batch B whose selector kernel reads the count and turns on one of its conditional (IF) nodes, each
+ * holding the forward pass at one size. Slot i < c of such a call is bit for bit what the same call writes after set_batch(s), s the
+ * size chosen; every slot >= c comes out zero, as without a declaration (the input kernel, the output conversions and the clear still run
+ * over all B slots). Calls without a count, every other entry point and submit / wait are unchanged.
+ * The graph of B is built on the first counted call at B, host-synchronously, before anything of that call is enqueued: for each of its
+ * sizes (the declared sizes below B, then B) one eager forward pass if none ran at that size yet, then its capture. A counted call while
+ * the context's stream is being captured (snnb_graph_capture_begin) is refused: a graph with conditional nodes cannot be a child graph.
+ * Requires a model loaded with use_cuda_graph and a driver with conditional graph nodes (CUDA 12.3 or later). Host-side: each size is
+ * planned as snnb_model_set_batch plans it (a size whose plan could not run on the loaded storage is refused, naming the layer), every
+ * graph built for the previous declaration is dropped (after the context's stream drains), nothing is enqueued. A refused call changes
+ * nothing, an earlier declaration included. */
+int snnb_model_set_count_batches(snnb_model* m, const int* sizes, int num_sizes);
 /* MixedInferenceCore::run (core.cpp:97-245), end to end with HOST buffers: H2D of the NHWC fp32 batch (the model's batch), forward,
  * D2H of output 0 (NHWC fp32, out_capacity floats) and, for classifiers (last layer Dense/softmax), the 1-based
  * class index per image (core.cpp:228-233); classes may be NULL. Synchronous. */
@@ -439,7 +458,8 @@ typedef struct {
  * libyuv's RGBA8 image of the whole frame (chroma sited in frame coordinates: pixel (x, y) takes chroma sample (x / 2, y / 2)), then
  * resized as run_frames resizes a frame, with taps clamped to the edges of the region; a region of the model's size is sampled directly.
  * Slots past the count and invalid slots get an all-zero input, and every byte of their outputs and their class is zero (classes are
- * 1-based: 0 = no region). The forward pass runs on the model's whole batch, whatever the count.
+ * 1-based: 0 = no region). The forward pass runs on the model's whole batch, whatever the count, unless sizes are declared with
+ * snnb_model_set_count_batches: a call with a non-NULL count_dev then runs it at the smallest declared size that holds the count.
  * Outputs, classes, the stream contract and the fences are those of snnb_model_run_frames; YOLO models are refused (no detection on
  * regions). Checked on the host before anything is enqueued: everything run_frames checks, num_frames >= 1, rois_dev (and count_dev
  * unless NULL) device or managed memory of the context's device, aligned to 4 bytes. Cost beyond run_frames: one kernel launch per
@@ -651,6 +671,10 @@ int snnb_debug_conv_launch(const int query[24], int out[59]);
  * 2 fp16w, 1 fp16; 0 on the CUDA cores), n_blk (output channels per tile), ksplit (K pieces per tile, 1 = none), stream_k (0/1),
  * fks (K steps per filter row of the row-window kernel's feed mode, 0 otherwise)}. Host-side record, no GPU work. Returns 0. */
 int snnb_debug_last_conv_variant(snnb_context* ctx, int out[6]);
+/* Diagnostics: the size snnb_model_set_count_batches' selector picks for a device-side count, evaluated on the host with the kernel's own
+ * function: the smallest of the num_sizes declared sizes (strictly increasing) that is >= c = clamp(count, 0, batch), or batch itself
+ * when none below batch is; 0 when c is 0 (no forward pass). Returns -1 for batch < 1, num_sizes < 0 or null sizes. No GPU needed. */
+int snnb_debug_count_body(const int* sizes, int num_sizes, int batch, int count);
 
 #ifdef __cplusplus
 }

@@ -293,6 +293,7 @@ SIGNATURES = {
     "snnb_model_transform_luma_list": (C.c_int, [vp, C.POINTER(FrameList), C.POINTER(FrameOutList), vp]),
     "snnb_model_segment_frame_list": (C.c_int, [vp, C.POINTER(FrameList), C.c_int, C.POINTER(LabelsList), vp]),
     "snnb_model_set_batch": (C.c_int, [vp, C.c_int]),
+    "snnb_model_set_count_batches": (C.c_int, [vp, c_int_p, C.c_int]),
     "snnb_model_set_input": (C.c_int, [vp, C.c_int, vp]),
     "snnb_model_forward": (C.c_int, [vp]),
     "snnb_model_get_output": (C.c_int, [vp, C.c_int, vp, C.c_size_t]),
@@ -318,6 +319,7 @@ SIGNATURES = {
     "snnb_debug_conv_plan": (C.c_int, [c_int_p, c_int_p]),
     "snnb_debug_conv_launch": (C.c_int, [c_int_p, c_int_p]),
     "snnb_debug_last_conv_variant": (C.c_int, [vp, c_int_p]),
+    "snnb_debug_count_body": (C.c_int, [c_int_p, C.c_int, C.c_int, C.c_int]),
 }
 
 _lib = None

@@ -414,6 +414,15 @@ class MixedInferenceCore:
         check(lib().snnb_model_set_batch(self.h, int(n)), "snnb_model_set_batch")
         self.batch = int(n)
 
+    def set_count_batches(self, sizes):
+        """snnb_model_set_count_batches: the batch sizes run_rois / run_rois_list with a count run their forward pass at, chosen on the
+        GPU from the count: the smallest declared size that holds it, or the model's batch when none below it does; a count of 0 runs no
+        forward pass. sizes: a list of ints, strictly increasing, from 1 to max_batch (use_cuda_graph models only); [] clears it."""
+        if not isinstance(sizes, (list, tuple)) or not all(isinstance(s, int) and not isinstance(s, bool) for s in sizes):
+            raise ValueError("set_count_batches: sizes must be a list of ints; got %r" % (sizes,))
+        arr = (C.c_int * max(1, len(sizes)))(*sizes)
+        check(lib().snnb_model_set_count_batches(self.h, arr, len(sizes)), "snnb_model_set_count_batches")
+
     # -- execution --
     def run(self, images, want_classes=True):
         """End to end with host buffers: returns (output0 NHWC fp32, 1-based class indices or None)."""
@@ -643,7 +652,9 @@ class MixedInferenceCore:
         CUDA tensor [batch, 6] of {frame, row, x, y, width, height} (rois_from_detections makes one); count: None (every slot is used)
         or an int32 CUDA tensor of one element (slots i < clamp(count, 0, batch) are used). Each used slot whose region lies inside an
         existing frame gets exactly what run_frames computes for that region cut out as an RGBA8 frame of its own; every other slot
-        comes out all zero, class 0. Outputs, classes and the stream contract as run_frames."""
+        comes out all zero, class 0. Outputs, classes and the stream contract as run_frames. Once sizes are declared (set_count_batches),
+        a call with a count runs the forward pass at the size the GPU picks from the count: slot i < count is then what the same call
+        gives after set_batch(that size)."""
         import torch
         if not (isinstance(rois, torch.Tensor) and rois.is_cuda and rois.dtype == torch.int32 and tuple(rois.shape) == (self.batch, 6)):
             raise ValueError("run_rois: rois must be an int32 CUDA tensor [%d, 6] (the model's batch)" % self.batch)
@@ -711,7 +722,8 @@ class MixedInferenceCore:
     def run_rois_list(self, frames, rois, count=None, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_dtype=None,
                       out_layout="nhwc", out_scale=1.0, out_offset=0.0, want_classes=False):
         """snnb_model_run_rois_list: run_rois on a list of 1 to 256 frames of mixed sizes as run_frame_list takes it. A region is valid
-        against the size of its own frame. rois, count, outputs, classes and the stream contract as run_rois."""
+        against the size of its own frame. rois, count (with the sizes of set_count_batches too), outputs, classes and the stream contract
+        as run_rois."""
         import torch
         if not (isinstance(rois, torch.Tensor) and rois.is_cuda and rois.dtype == torch.int32 and tuple(rois.shape) == (self.batch, 6)):
             raise ValueError("run_rois_list: rois must be an int32 CUDA tensor [%d, 6] (the model's batch)" % self.batch)

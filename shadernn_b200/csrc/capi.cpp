@@ -198,6 +198,13 @@ int snnb_debug_streamk_schedule(int tiles, int num_kb, int sms, int* rows, int c
     SNNB_REQUIRE(rows || capacity == 0, "snnb_debug_streamk_schedule: null buffer");
     return streamk_schedule(tiles, num_kb, sms, rows, capacity);
 }
+int snnb_debug_count_body(const int* sizes, int num_sizes, int batch, int count) {
+    if (!(sizes || num_sizes == 0) || num_sizes < 0 || batch < 1) {
+        set_error("snnb_debug_count_body: %d sizes at %p, batch %d", num_sizes, (const void*) sizes, batch);
+        return -1; // every size is >= 0
+    }
+    return count_body(sizes, num_sizes, batch, count);
+}
 int snnb_debug_last_conv_variant(snnb_context* ctx, int out[6]) {
     SNNB_REQUIRE(ctx && out, "snnb_debug_last_conv_variant: null argument");
     for (int i = 0; i < 6; ++i) out[i] = ctx->last_conv[i];

@@ -24,6 +24,7 @@ MixedInferenceCore::~MixedInferenceCore() {
     for (auto& kv : batchPlans) {
         if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
         if (kv.second.graph) cudaGraphDestroy(kv.second.graph);
+        kv.second.dropDispatch();
     }
     for (auto* t : ownedTensors) snnb_tensor_free(t);
     if (arena) cudaFree(arena);
@@ -449,11 +450,110 @@ int MixedInferenceCore::setBatch(int n) {
         it = batchPlans.emplace(n, std::move(b)).first;
     }
     cur = &it->second, curBatch = n, launchesPerForward = cur->launches;
+    useBatch(n, *cur);
+    return 0;
+}
+
+void MixedInferenceCore::useBatch(int n, const BatchPlan& b) {
     for (size_t i = 0; i < planned.size(); ++i) {
         GenericModelLayer* L = planned[i];
-        (L->typeName == "Conv2D" ? static_cast<Conv2DLayer*>(L)->convPlan : static_cast<DenseLayer*>(L)->convPlan) = cur->plans[i];
+        (L->typeName == "Conv2D" ? static_cast<Conv2DLayer*>(L)->convPlan : static_cast<DenseLayer*>(L)->convPlan) = b.plans[i];
     }
     for (auto* t : ownedTensors) t->n = n; // NHWC, image outermost: the first n images of every tensor are a prefix of its storage
+}
+
+int MixedInferenceCore::setCountBatches(const int* sizes, int numSizes) {
+    const char* api = "snnb_model_set_count_batches";
+    SNNB_REQUIRE(numSizes >= 0 && numSizes <= COUNT_BATCHES_MAX, "%s: %d sizes; 0 to %d may be declared", api, numSizes, COUNT_BATCHES_MAX);
+    SNNB_REQUIRE(sizes || numSizes == 0, "%s: null sizes", api);
+    SNNB_REQUIRE(options.useCudaGraph, "%s: the model was loaded without use_cuda_graph; the forward pass is chosen by the count inside a CUDA graph", api);
+    for (int i = 0; i < numSizes; ++i)
+        SNNB_REQUIRE(sizes[i] >= 1 && sizes[i] <= (int) options.batch && (i == 0 || sizes[i] > sizes[i - 1]),
+                     "%s: sizes[%d] = %d; sizes must be strictly increasing, from 1 to the loaded batch of %u", api, i, sizes[i], options.batch);
+    std::map<int, BatchPlan> made; // every size planned before anything changes
+    for (int i = 0; i < numSizes; ++i) {
+        if (batchPlans.count(sizes[i])) continue;
+        BatchPlan b;
+        const std::string why = makeBatchPlan(sizes[i], b);
+        SNNB_REQUIRE(why.empty(), "%s: size %d: %s", api, sizes[i], why.c_str());
+        made.emplace(sizes[i], std::move(b));
+    }
+    bool built = false;
+    for (auto& kv : batchPlans) built = built || kv.second.dispatchExec;
+    if (built) SNNB_CUDA_OK(cudaStreamSynchronize(ctx->stream)); // no dispatch graph is destroyed while a launch of it may be in flight
+    for (auto& kv : batchPlans) kv.second.dropDispatch();
+    for (auto& kv : made) batchPlans.emplace(kv.first, std::move(kv.second));
+    countSizes.assign(sizes, sizes + numSizes);
+    return 0;
+}
+
+// The dispatch graph of the model's batch B, built on the first counted region call at B, host-synchronously and before anything of that
+// call is enqueued. Bodies: each declared size below B, then B. For each, one eager pass at that size if none ran yet (it counts the
+// launches and grows the split-K scratch, which a capture cannot), then its forward pass captured into the body of an IF node. The
+// IF nodes hang in a chain after the selector; each has its own handle, reset to 0 at every launch, and the selector sets one of them.
+int MixedInferenceCore::buildDispatch(const char* api, const int* countDev) {
+    BatchPlan& top = *cur;
+    const int B    = curBatch;
+    CountBodies b;
+    for (int s : countSizes)
+        if (s < B) b.size[b.num++] = s;
+    b.size[b.num++] = B;
+    cudaGraph_t g = nullptr;
+    SNNB_CUDA_OK(cudaGraphCreate(&g, 0));
+    cudaGraphNode_t selector = nullptr;
+    const int rc = [&]() -> int {
+        for (int k = 0; k < b.num; ++k) {
+            const cudaError_t e = cudaGraphConditionalHandleCreate(&b.handle[k], g, 0, cudaGraphCondAssignDefault);
+            SNNB_REQUIRE(e == cudaSuccess, "%s: cudaGraphConditionalHandleCreate: %s", api, cudaGetErrorString(e));
+        }
+        if (count_select_add(g, &selector, countDev, b)) return 1;
+        cudaGraphNode_t prev = selector;
+        for (int k = 0; k < b.num; ++k) {
+            BatchPlan& p = batchPlans.at(b.size[k]);
+            useBatch(b.size[k], p);
+            if (!p.launches) {
+                const uint64_t before = ctx->launches;
+                if (int r = enqueueForward(false)) return r;
+                p.launches = (int) (ctx->launches - before);
+            }
+            cudaGraphNodeParams cp = {};
+            cp.type               = cudaGraphNodeTypeConditional;
+            cp.conditional.handle = b.handle[k];
+            cp.conditional.type   = cudaGraphCondTypeIf;
+            cp.conditional.size   = 1;
+            cudaGraphNode_t node  = nullptr;
+            SNNB_CUDA_OK(cudaGraphAddNode(&node, g, &prev, 1, &cp));
+            const uint64_t keep = ctx->launches;
+            SNNB_CUDA_OK(cudaStreamBeginCaptureToGraph(ctx->stream, cp.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+            const int r = enqueueForward(false);
+            cudaGraph_t body    = nullptr;
+            const cudaError_t e = cudaStreamEndCapture(ctx->stream, &body);
+            ctx->launches       = keep;
+            if (r) return r;
+            SNNB_CUDA_OK(e);
+            prev = node;
+        }
+        return 0;
+    }();
+    useBatch(B, top);
+    launchesPerForward = top.launches;
+    cudaGraphExec_t exec = nullptr;
+    cudaError_t e        = rc ? cudaSuccess : cudaStreamSynchronize(ctx->stream); // the eager passes
+    cudaGraphInstantiateParams ip = {};
+    if (!rc && e == cudaSuccess) e = cudaGraphInstantiateWithParams(&exec, g, &ip);
+    if (rc || e != cudaSuccess) {
+        cudaGraphDestroy(g);
+        if (!rc) set_error("%s: the dispatch graph at batch %d: %s (instantiation result %d)", api, B, cudaGetErrorString(e), (int) ip.result_out);
+        return rc ? rc : 1;
+    }
+    top.dispatch = g, top.dispatchExec = exec, top.selector = selector, top.bodies = b;
+    return 0;
+}
+
+int MixedInferenceCore::forwardCounted(const int* countDev) {
+    if (count_select_set(cur->dispatchExec, cur->selector, countDev, cur->bodies)) return 1;
+    SNNB_CUDA_OK(cudaGraphLaunch(cur->dispatchExec, ctx->stream));
+    ctx->launches += 1 + (uint64_t) cur->launches; // the selector and, as an upper bound, the forward pass at the model's batch
     return 0;
 }
 
@@ -871,7 +971,7 @@ int MixedInferenceCore::enqueueDeviceForward(const DeviceFeed& in, cudaStream_t 
         for (int i = 0; i < in.numInputs; ++i)
             if (launch_device_input(ctx, in.inputs[i], inputLayers[i]->output)) return 1;
     }
-    return forward();
+    return counted(in) ? forwardCounted(in.roiCount) : forward();
 }
 
 // The context's stream -> the caller's: work enqueued on `stream` from now on sees everything enqueued above.
@@ -939,6 +1039,15 @@ int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, con
     if (classes1Dev) {
         SNNB_REQUIRE(isClassifier, "%s: classes requested, but the model is not a classifier (output 0 is not 1 x 1 x C with C > 1)", api);
         if (int rc = checkDevicePointer(api, classes1Dev, sizeof(int), device, "classes", 0)) return rc;
+    }
+    if (counted(in)) {
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        SNNB_CUDA_OK(cudaStreamIsCapturing(ctx->stream, &cap));
+        SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone,
+                     "%s: the context's stream is being captured (snnb_graph_capture_begin); a call with a device-side count and declared sizes runs "
+                     "a graph with conditional nodes, which cannot become part of another graph",
+                     api);
+        if (!cur->dispatchExec && buildDispatch(api, in.roiCount)) return 1;
     }
 
     if (enqueueDeviceForward(in, stream)) return 1;

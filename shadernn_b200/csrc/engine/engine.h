@@ -382,6 +382,9 @@ public:
     // storage. Host-side: plans n on its first use, switches to it on every later one; nothing is enqueued or allocated.
     int setBatch(int n);
     int batch() const { return curBatch; } // the model's batch: images per call (options.batch is the capacity)
+    // snnb_model_set_count_batches: the sizes a region call with a device-side count runs its forward pass at (count_body). Host-side:
+    // plans each size as setBatch does and drops every dispatch graph already built; a refused call changes nothing.
+    int setCountBatches(const int* sizes, int numSizes);
 
     snnb_context* ctx = nullptr;
     dp::ShaderGenOptions options;
@@ -408,13 +411,28 @@ private:
         int launches = 0; // kernels of one forward pass (0: not counted yet)
         cudaGraph_t graph = nullptr;
         cudaGraphExec_t exec = nullptr;
+        // The dispatch graph of a region call with a device-side count at this batch (setCountBatches): the selector node, then a chain
+        // of IF nodes, one per body of `bodies`, each holding the forward pass at its size. Built on the first such call at this batch.
+        cudaGraph_t dispatch = nullptr;
+        cudaGraphExec_t dispatchExec = nullptr;
+        cudaGraphNode_t selector = nullptr;
+        snnb::CountBodies bodies;
+        void dropDispatch() {
+            if (dispatchExec) cudaGraphExecDestroy(dispatchExec);
+            if (dispatch) cudaGraphDestroy(dispatch);
+            dispatch = nullptr, dispatchExec = nullptr, selector = nullptr;
+        }
     };
     std::map<int, BatchPlan> batchPlans;
     std::vector<dp::GenericModelLayer*> planned;
     int curBatch = 0;
     BatchPlan* cur = nullptr;
+    std::vector<int> countSizes; // setCountBatches' sizes (empty: a device-side count does not size the forward pass)
     std::string makeBatchPlan(int n, BatchPlan& b) const; // "" or why the plans at n cannot run on the loaded batch's storage
+    void useBatch(int n, const BatchPlan& b);             // makes b's plans (made for n images) and n-image tensor extents current
     int captureForward(BatchPlan& b);
+    int buildDispatch(const char* api, const int* countDev); // the current batch's dispatch graph (host-synchronous)
+    int forwardCounted(const int* countDev);                 // the forward pass at count_body's size of *countDev; asynchronous
     float* ioStage   = nullptr; // device fp32 staging for input/output conversion (stable address: graph-safe)
     size_t ioStageBytes = 0;
     int* argmaxDev   = nullptr;
@@ -474,6 +492,8 @@ private:
     int transformLumaDeviceFeed(const char* api, const DeviceFeed& in, const snnb_frames_out* o, const snnb_frame_out_list* ol, cudaStream_t stream);
     int segmentDeviceFeed(const char* api, const DeviceFeed& in, const snnb_labels_out* o, const snnb_labels_list* ol, cudaStream_t stream);
     int checkDeviceFeed(const char* api, const DeviceFeed& in, cudaStream_t stream);
+    // regions with a device-side count, once sizes are declared: the forward pass is the dispatch graph's (forwardCounted)
+    bool counted(const DeviceFeed& in) const { return in.rois && in.roiCount && !countSizes.empty(); }
     int enqueueDeviceForward(const DeviceFeed& in, cudaStream_t stream);
     int fenceToCaller(cudaStream_t stream);
     void* detectScratch = nullptr; // detectDevice's per-image keys (yolo_detect_scratch_bytes), allocated on first use

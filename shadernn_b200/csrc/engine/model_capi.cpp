@@ -201,6 +201,11 @@ int snnb_model_set_batch(snnb_model* m, int n) {
     SNNB_REQUIRE(m, "snnb_model_set_batch: null model");
     return m->core->setBatch(n);
 }
+int snnb_model_set_count_batches(snnb_model* m, const int* sizes, int num_sizes) {
+    SNNB_REQUIRE(m, "snnb_model_set_count_batches: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->setCountBatches(sizes, num_sizes);
+}
 int snnb_model_set_input(snnb_model* m, int idx, const float* host_input) {
     SNNB_REQUIRE(m, "snnb_model_set_input: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));

@@ -2009,6 +2009,38 @@ int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const fl
     return rois_from_detections_launch(ctx, stream, rows, counts, num_frames, max_rows, S, sel, rois, capacity, count);
 }
 
+// The selector node of a region call's dispatch graph (snnb_model_set_count_batches): turns on the one IF body whose size count_body
+// picks for *count; the other handles keep their default of 0, and a count of 0 (or below) turns on none. The bodies' sizes are read
+// from the __grid_constant__ parameter, so indexing them makes no local copy.
+__global__ void __launch_bounds__(1) count_select_kernel(const int* __restrict__ count, const __grid_constant__ CountBodies b) {
+    const int s = count_body(b.size, b.num - 1, b.size[b.num - 1], *count);
+    for (int k = 0; k < b.num; ++k)
+        if (b.size[k] == s) {
+            cudaGraphSetConditional(b.handle[k], 1u);
+            return;
+        }
+}
+static cudaKernelNodeParams count_select_params(void** args) {
+    cudaKernelNodeParams p = {};
+    p.func         = reinterpret_cast<void*>(count_select_kernel);
+    p.gridDim      = dim3(1);
+    p.blockDim     = dim3(1);
+    p.kernelParams = args;
+    return p;
+}
+int count_select_add(cudaGraph_t g, cudaGraphNode_t* node, const int* count, const CountBodies& b) {
+    void* args[] = {&count, const_cast<CountBodies*>(&b)};
+    const cudaKernelNodeParams p = count_select_params(args);
+    SNNB_CUDA_OK(cudaGraphAddKernelNode(node, g, nullptr, 0, &p));
+    return 0;
+}
+int count_select_set(cudaGraphExec_t exec, cudaGraphNode_t node, const int* count, const CountBodies& b) {
+    void* args[] = {&count, const_cast<CountBodies*>(&b)};
+    const cudaKernelNodeParams p = count_select_params(args);
+    SNNB_CUDA_OK(cudaGraphExecKernelNodeSetParams(exec, node, &p));
+    return 0;
+}
+
 // Model output 0 -> device video frames (snnb_model_transform_frames), the reverse of frame_input_kernel. Each frame pixel is
 // ImageTexture::resize (resize_taps) of M, the model-size RGBA8 image whose texels are quant_u8 of the output's channels; then libyuv's
 // ABGRToNV12 / ABGRToNV21 / ABGRToI420 with its portable C rows (row_common.cc:423-473: RGBToY, RGBToU, RGBToV and MAKEROWY's 2 x 2

@@ -274,6 +274,28 @@ int launch_frame_roi_input(snnb_context* ctx, const snnb_frame_list& f, int num_
 int launch_roi_clear(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes);
 int launch_roi_clear(snnb_context* ctx, const snnb_frame_list& f, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst,
                      long long slot_bytes);
+// Count-sized region batches (snnb_model_set_count_batches): the forward-pass size a region call with device-side count `count` runs at,
+// given the declared sizes (strictly increasing) and the model's batch: the smallest declared size >= c, c = clamp(count, 0, batch), or
+// batch itself when no declared size below batch is; 0 when c is 0 (no forward pass). count_select_kernel runs this very function.
+__host__ __device__ inline int count_body(const int* sizes, int num_sizes, int batch, int count) {
+    const int c = count < 0 ? 0 : (count > batch ? batch : count);
+    if (c == 0) return 0;
+    for (int i = 0; i < num_sizes && sizes[i] < batch; ++i)
+        if (sizes[i] >= c) return sizes[i];
+    return batch;
+}
+constexpr int COUNT_BATCHES_MAX = 32; // declared sizes per model
+// The IF bodies of a dispatch graph: body k runs the forward pass at size[k] (the declared sizes below the batch, then the batch itself,
+// size[num - 1]) when the selector sets handle[k]
+struct CountBodies {
+    int num = 0;
+    int size[COUNT_BATCHES_MAX + 1];
+    cudaGraphConditionalHandle handle[COUNT_BATCHES_MAX + 1];
+};
+// The selector node of a dispatch graph: count_select_kernel, one thread, reading *count and setting the handle of count_body's size.
+// add: a new node of g without dependencies; set: the node of an instantiated graph pointed at another count.
+int count_select_add(cudaGraph_t g, cudaGraphNode_t* node, const int* count, const CountBodies& b);
+int count_select_set(cudaGraphExec_t exec, cudaGraphNode_t node, const int* count, const CountBodies& b);
 // Detection rows -> regions (snnb_rois_from_detections, checked by the caller), one CTA on `stream`: every frame fw x fh, or frame n
 // frame_wh[2n] x frame_wh[2n + 1] (host, num_frames <= SNNB_FRAME_LIST_MAX)
 int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const float* rows, const int* counts, int num_frames, int max_rows, int fw, int fh,

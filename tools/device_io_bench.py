@@ -66,6 +66,11 @@ NV12 on detect_frames, transform_luma and transform_frames, with each frame kern
                of which n are used. And the `framelist` chain when only k = 4, 8, 12 or 16 of its streams have a frame:
                detect_frame_list on the batch-16 detector after set_batch(k), against the list padded to 16 with the k frames repeated.
                Frames/s count the frames a call needs; alternating as above.
+  counted     (opt-in) Count-sized region batches. ResNet-18 112x112 loaded at 64 with sizes [8, 16, 32] declared, fed the 64 caller-made
+               regions of `rois` (b) with a device-side count k = 0 .. 64: run_rois against the same call on a handle with no sizes declared
+               and against a third handle after set_batch(bucket(k)), the size k selects; calls/s and the regions/s of the k used slots,
+               alternating as above. And the `framelist` chain with planted detector heads and a min_score that keeps about three boxes per
+               frame, four frame sets in turn, with and without sizes declared; the count of each frame set is reported beside the rates.
   card        name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -998,6 +1003,89 @@ def partial(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def counted(torch, ctx, core, modelzoo, d, args):
+    """Count-sized region batches: run_rois with a device-side count on a classifier with sizes declared, against the same call with none
+    declared and against set_batch(bucket(k)), the size the count selects; then the framelist chain with a few boxes per frame."""
+    H, W = 1080, 1920
+    chw, cbatch, sizes, nframes = (112, 112), 64, [8, 16, 32], 16
+    mean4, norm4 = [127.5] * 4, [1.0 / 127.5] * 4
+    cpath, _ = modelzoo.build("resnet18", os.path.join(d, "counted_resnet18"), input_hw=chw)
+    opts = dict(batch=cbatch, input_hw=chw, fuse=True, use_cuda_graph=True)
+    declared, undeclared, ceiling = (core.MixedInferenceCore(ctx, cpath, **opts) for _ in range(3))
+    declared.set_count_batches(sizes)
+    g = torch.Generator().manual_seed(7)
+    nv12 = torch.randint(16, 236, (nframes, H * 3 // 2, W), dtype=torch.uint8, generator=g).cuda()
+    rw, rh = W // 2, H // 2
+    grid = torch.tensor([(i % nframes, i, (i // nframes) % 2 * rw, (i // nframes) // 2 * rh, rw, rh) for i in range(cbatch)], dtype=torch.int32,
+                        device="cuda")
+    bucket = lambda k: min([s for s in sizes if s >= k] + [cbatch])  # noqa: E731  (k = 0: the smallest declared size, the least set_batch can do)
+    rows = []
+    for k in (0, 1, 4, 8, 16, 24, 32, 48, 64):
+        cnt = torch.tensor([k], dtype=torch.int32, device="cuda")
+        ceiling.set_batch(bucket(k))
+        cgrid = grid[:bucket(k)].contiguous()
+        fns = {"counted": lambda: declared.run_rois(nv12, grid, cnt, mean4=mean4, norm4=norm4, want_classes=True),
+               "undeclared": lambda: undeclared.run_rois(nv12, grid, cnt, mean4=mean4, norm4=norm4, want_classes=True),
+               "set_batch_bucket": lambda: ceiling.run_rois(nv12, cgrid, cnt, mean4=mean4, norm4=norm4, want_classes=True)}
+        runs, _ = alternate(torch, fns, args.seconds, 1, args.rounds)  # batch 1: frames/s are calls/s
+        med = {key: float(np.median([r[key]["frames_per_s"] for r in runs])) for key in fns}
+        rows.append({"k": k, "bucket": bucket(k), "counted_calls_per_s": med["counted"], "undeclared_calls_per_s": med["undeclared"],
+                     "set_batch_bucket_calls_per_s": med["set_batch_bucket"], "counted_regions_per_s": med["counted"] * k,
+                     "undeclared_regions_per_s": med["undeclared"] * k, "counted_over_undeclared": med["counted"] / med["undeclared"],
+                     "counted_over_set_batch_bucket": med["counted"] / med["set_batch_bucket"], "rounds": runs})
+    full = rows[-1]
+    # where the overhead at k = 64 goes: the same call with one IF body (sizes [64]) and with four (sizes [8, 16, 32] and 64 itself)
+    cnt = torch.tensor([cbatch], dtype=torch.int32, device="cuda")
+    one = core.MixedInferenceCore(ctx, cpath, **opts)
+    one.set_count_batches([cbatch])
+    fns = {"four_bodies": lambda: declared.run_rois(nv12, grid, cnt, mean4=mean4, norm4=norm4, want_classes=True),
+           "one_body": lambda: one.run_rois(nv12, grid, cnt, mean4=mean4, norm4=norm4, want_classes=True),
+           "undeclared": lambda: undeclared.run_rois(nv12, grid, cnt, mean4=mean4, norm4=norm4, want_classes=True)}
+    runs, med = alternate(torch, fns, args.seconds, 1, args.rounds)
+    one.close()
+    res = {"overhead_at_64": {"case": "k = 64: us per call over the undeclared call, with the bodies of sizes [8, 16, 32] and of sizes [64]",
+                              "four_bodies_us": 1e6 / med["four_bodies"] - 1e6 / med["undeclared"],
+                              "one_body_us": 1e6 / med["one_body"] - 1e6 / med["undeclared"], "calls_per_s_median": med, "rounds": runs}}
+    res["regions"] = {
+        "case": "resnet18 %dx%d loaded at %d, sizes %s declared; %d caller-made %dx%d regions of %d %dx%d NV12 frames, run_rois with a device count k "
+                "(+ device classes); set_batch_bucket: a third handle after set_batch(bucket(k)), the size k selects (8 for k = 0)" % (
+                    chw[0], chw[1], cbatch, sizes, cbatch, rw, rh, nframes, W, H),
+        "counts": rows,
+        "overhead_at_64_us": 1e6 / full["counted_calls_per_s"] - 1e6 / full["undeclared_calls_per_s"]}
+    # the framelist chain with planted detector heads (scores scattered around 0.35) and a min_score that keeps a few boxes per frame
+    dhw, dbatch = (416, 416), len(FRAMELIST_SIZES)
+    ypath, layers = modelzoo.build("yolov3tiny", os.path.join(d, "counted_yolov3tiny"), input_hw=dhw, seed=21)
+    for head in [l for l in layers if l["type"] == "Conv2D" and l["outputPlanes"] == 18]:
+        head["_w"]["bias"][:] = 0
+        head["_w"]["bias"][[4, 5, 10, 11]] = [-1.0, 0.0, -1.0, 0.0]
+    det = core.MixedInferenceCore(ctx, modelzoo.write_model(layers, os.path.join(d, "counted_planted.json"), split=True), batch=dbatch, input_hw=dhw,
+                                  fuse=True, use_cuda_graph=True)
+    lists = [[torch.randint(16, 236, (h * 3 // 2, w), dtype=torch.uint8, generator=g).cuda() for h, w in FRAMELIST_SIZES] for _ in range(4)]
+    r, c = det.detect_frame_list(lists[0], mean4=mean4, norm4=norm4)
+    scores = np.sort(np.concatenate([r[n, :int(c[n]), 1].cpu().numpy() for n in range(dbatch)]))[::-1]
+    min_score = float(scores[min(3 * dbatch, len(scores)) - 1])  # about three boxes per frame on the first list
+    state = {"i": 0}
+
+    def chain(m):
+        fl = lists[state["i"] % len(lists)]
+        state["i"] += 1
+        rr, cc = det.detect_frame_list(fl, mean4=mean4, norm4=norm4)
+        regions, count = ctx.rois_from_detections(rr, cc, FRAMELIST_SIZES, cbatch, min_score=min_score)
+        return m.run_rois_list(fl, regions, count, mean4=mean4, norm4=norm4, want_classes=True)
+    kept = [int(ctx.rois_from_detections(*det.detect_frame_list(fl, mean4=mean4, norm4=norm4), FRAMELIST_SIZES, cbatch, min_score=min_score)[1].item())
+            for fl in lists]
+    runs, med = alternate(torch, {"counted": lambda: chain(declared), "undeclared": lambda: chain(undeclared)}, args.seconds, dbatch, args.rounds)
+    res["framelist_chain"] = {
+        "case": "detect_frame_list (yolov3tiny planted heads %dx%d batch %d, the 16 streams of `framelist`, 4 frame sets in turn) -> "
+                "rois_from_detections (min_score %.4f) -> resnet18 %dx%d batch %d run_rois_list, sizes %s declared or not" % (
+                    dhw[0], dhw[1], dbatch, min_score, chw[0], chw[1], cbatch, sizes),
+        "regions_per_frame_set": kept, "counted_frames_per_s_median": med["counted"], "undeclared_frames_per_s_median": med["undeclared"],
+        "counted_over_undeclared": med["counted"] / med["undeclared"], "rounds": runs}
+    for m in (declared, undeclared, ceiling, det):
+        m.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
@@ -1005,7 +1093,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
                     help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in), "
-                         "segment (opt-in), p010 (opt-in), framelist (opt-in), framelist_out (opt-in), partial (opt-in)")
+                         "segment (opt-in), p010 (opt-in), framelist (opt-in), framelist_out (opt-in), partial (opt-in), counted (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -1040,6 +1128,8 @@ def main():
         result["p010"] = p010(torch, ctx, core, modelzoo, d, args)
     if "partial" in parts:
         result["partial"] = partial(torch, ctx, core, modelzoo, d, args)
+    if "counted" in parts:
+        result["counted"] = counted(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
