@@ -460,8 +460,8 @@ typedef struct {
  * Slots past the count and invalid slots get an all-zero input, and every byte of their outputs and their class is zero (classes are
  * 1-based: 0 = no region). The forward pass runs on the model's whole batch, whatever the count, unless sizes are declared with
  * snnb_model_set_count_batches: a call with a non-NULL count_dev then runs it at the smallest declared size that holds the count.
- * Outputs, classes, the stream contract and the fences are those of snnb_model_run_frames; YOLO models are refused (no detection on
- * regions). Checked on the host before anything is enqueued: everything run_frames checks, num_frames >= 1, rois_dev (and count_dev
+ * Outputs, classes, the stream contract and the fences are those of snnb_model_run_frames; YOLO models are refused (detection on regions
+ * is snnb_model_detect_rois). Checked on the host before anything is enqueued: everything run_frames checks, num_frames >= 1, rois_dev (and count_dev
  * unless NULL) device or managed memory of the context's device, aligned to 4 bytes. Cost beyond run_frames: one kernel launch per
  * output buffer and one for the classes, which clear the slots that hold no region. */
 int snnb_model_run_rois(snnb_model* m, const snnb_frames* frames, int num_frames, const snnb_roi* rois_dev, const int* count_dev,
@@ -532,6 +532,50 @@ int snnb_model_run_rois_list(snnb_model* m, const snnb_frame_list* frames, const
 int snnb_rois_from_detections_list(snnb_context* ctx, const float* rows_dev, const int* counts_dev, int num_frames, int max_rows,
                                    const int* frame_wh, const snnb_roi_select* sel, snnb_roi* rois_dev, int capacity, int* count_dev,
                                    void* stream);
+/* Detection on regions of device frames: sliced (tiled) inference on frames much larger than the detector's input, and a second
+ * detection pass on zoomed regions of a first one (snnb_model_detect_frames -> snnb_rois_from_detections with expand -> this call).
+ * Each region slot is detected as snnb_model_detect_frames detects its crop; the boxes are mapped to the frame the region lies on and
+ * merged there by one NMS per frame, all on the device.
+ *   1. Input: exactly snnb_model_run_rois (batch form) / snnb_model_run_rois_list (list form): the same slots, count, slot validity,
+ *      model input, declared count sizes (snnb_model_set_count_batches) and host checks. The model must have a YOLO output.
+ *   2. Per region: each used, valid slot's detections are exactly the rows snnb_model_detect_frames returns for that slot's model input
+ *      with max_rows = 100 (the same decode, stable score sort and NMS), in model-normalised coordinates. Unused and invalid slots
+ *      contribute nothing. The cap per region is always 100, whatever max_rows is.
+ *   3. Mapping: row {cls, score, x, y, w, h} of a slot whose region is {f, row, rx, ry, rw, rh}, on a frame of W x H, becomes
+ *      {cls, score, (rx + x * rw) / W, (ry + y * rh) / H, (w * rw) / W, (h * rh) / H}: float32, every operation rounded on its own
+ *      (no FMA), the integers converted exactly. The geometry is exact because a region is stretched to the model input without a
+ *      letterbox. Boxes are not clipped, as detect_frames does not clip them.
+ *   4. Merge, per frame f: one list of the mapped rows of every slot whose region is on f, slots in slot order and each slot's rows in
+ *      their order; std::stable_sort by descending score (equal scores: the lower slot, then the lower row first); then the greedy NMS
+ *      of the host paths (a box is dropped when a kept box of the same class overlaps it with IoU > 0.45), on the mapped boxes; the
+ *      first max_rows (1..100) kept.
+ *   5. Output: rows_dev float32 [num_frames][max_rows][6] in detect_frames' format, normalised to the frame, zero past each frame's
+ *      count; counts_dev int32 [num_frames]. A frame with no valid region gets count 0 and zero rows. The rows go straight into
+ *      snnb_rois_from_detections(_list) with the frames' sizes.
+ *   6. NMS runs per region (2), then across regions (4): the composition of detect_frames on the crop and the merge, which bounds the
+ *      merge's input at 100 rows per slot. It can differ from one NMS over every raw cell of every region in a rare chain: a box that
+ *      its own region suppresses (by a box the merge then drops) would be kept by one NMS, and could then suppress a box of another
+ *      region.
+ * Tiles for the first use come from snnb_tile_rois; append one whole-frame region {f, row, 0, 0, W, H} per frame to keep large objects
+ * that no tile holds whole.
+ * Stream contract and fences: those of snnb_model_run_device; a capturing stream is refused. Checked on the host before anything is
+ * enqueued: everything run_rois (run_rois_list) checks, a YOLO output, 1 <= max_rows <= 100, rows_dev and counts_dev device or managed
+ * memory of the context's device aligned to 4 bytes. Scratch for the loaded batch and 256 frames is allocated on the first call; a call
+ * with more frames than any before it (batch form, more than 256) waits for the context's stream before it allocates more.
+ * Cost beyond the forward pass: 7 kernel launches per call (the input, the three decode kernels over every slot, and three merge
+ * kernels: gather and map, rank sort, NMS) and one memset; a counted call also counts the selector, as snnb_launch_count describes. */
+int snnb_model_detect_rois(snnb_model* m, const snnb_frames* frames, int num_frames, const snnb_roi* rois_dev, const int* count_dev, float* rows_dev,
+                           int max_rows, int* counts_dev, void* stream);
+int snnb_model_detect_rois_list(snnb_model* m, const snnb_frame_list* frames, const snnb_roi* rois_dev, const int* count_dev, float* rows_dev, int max_rows,
+                                int* counts_dev, void* stream);
+/* The tiles of one frame for snnb_model_detect_rois, on the host (no context, no GPU): a row-major grid of regions of tile_w x tile_h
+ * (each clamped to the frame) that covers every pixel, neighbours overlapping by at least min_overlap. Along x, with W the frame width
+ * and tw the clamped tile width: nx = 1 + ceil((W - tw) / (tw - min_overlap)) columns (1 when tw = W), column i starting at
+ * i * (W - tw) / (nx - 1) in integer division (the first at 0, the last ending at W); y likewise. Region {frame, j * nx + i, x_i, y_j,
+ * tw, th} is written at rois_host[j * nx + i], and *count = nx * ny. Refused: a frame or tile size below 1, min_overlap < 0 or >= the
+ * smaller clamped tile side, null count; and a grid of more than `capacity` regions, which reports the needed count in *count and
+ * writes no region (rois_host may then be NULL). */
+int snnb_tile_rois(int frame, int frame_w, int frame_h, int tile_w, int tile_h, int min_overlap, snnb_roi* rois_host, int capacity, int* count);
 /* Output lists: the frame-writing paths with one output descriptor per image, so that each stream of a multi-stream service gets its
  * result in its own surface (its encoder's, or the decoded frame itself) at its own size. As for snnb_frame_list, the descriptors are a
  * HOST array read during the call only; they reach the kernel by value. */

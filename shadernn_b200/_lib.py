@@ -289,6 +289,9 @@ SIGNATURES = {
     "snnb_model_detect_frame_list": (C.c_int, [vp, C.POINTER(FrameList), vp, C.c_int, vp, vp]),
     "snnb_model_run_rois_list": (C.c_int, [vp, C.POINTER(FrameList), vp, vp, C.POINTER(DeviceBuffer), C.c_int, vp, vp]),
     "snnb_rois_from_detections_list": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, C.POINTER(RoiSelect), vp, C.c_int, vp, vp]),
+    "snnb_model_detect_rois": (C.c_int, [vp, C.POINTER(Frames), C.c_int, vp, vp, vp, C.c_int, vp, vp]),
+    "snnb_model_detect_rois_list": (C.c_int, [vp, C.POINTER(FrameList), vp, vp, vp, C.c_int, vp, vp]),
+    "snnb_tile_rois": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int, c_int_p]),
     "snnb_model_transform_frame_list": (C.c_int, [vp, C.POINTER(FrameList), C.POINTER(FrameOutList), vp]),
     "snnb_model_transform_luma_list": (C.c_int, [vp, C.POINTER(FrameList), C.POINTER(FrameOutList), vp]),
     "snnb_model_segment_frame_list": (C.c_int, [vp, C.POINTER(FrameList), C.c_int, C.POINTER(LabelsList), vp]),

@@ -355,6 +355,20 @@ def subpixel(ctx, x, r):
     return o.download()
 
 
+def tile_rois(frame_hw, tile_hw, min_overlap, frame=0):
+    """snnb_tile_rois: the tiles of one frame of frame_hw = (H, W) for MixedInferenceCore.detect_rois, on the host: a row-major grid of
+    tile_hw = (h, w) regions (clamped to the frame) covering every pixel, neighbours overlapping by at least min_overlap pixels. Returns
+    an int32 numpy array [k, 6] of {frame, row (the tile's index), x, y, width, height}. Append one whole-frame region
+    (frame, k, 0, 0, W, H) to keep objects larger than a tile."""
+    count = C.c_int(0)
+    args = (int(frame), int(frame_hw[1]), int(frame_hw[0]), int(tile_hw[1]), int(tile_hw[0]), int(min_overlap))
+    if lib().snnb_tile_rois(*args, None, 0, C.byref(count)) != 0 and count.value <= 0:  # a query: the grid's size, or why it is refused
+        check(1, "snnb_tile_rois")
+    out = np.zeros((count.value, 6), np.int32)
+    check(lib().snnb_tile_rois(*args, out.ctypes.data_as(vp), count.value, C.byref(count)), "snnb_tile_rois")
+    return out
+
+
 class MixedInferenceCore:
     """snn::MixedInferenceCore: create(ctx, modelFileName, options) then run(images)."""
 
@@ -747,6 +761,41 @@ class MixedInferenceCore:
         counts = torch.empty(self.batch, dtype=torch.int32, device=device)
         check(lib().snnb_model_detect_frames(self.h, C.byref(f), rows.data_ptr() or None, int(max_rows), counts.data_ptr(), self._torch_stream()),
               "snnb_model_detect_frames")
+        return rows, counts
+
+    def _region_detections(self, who, rois, count, num_frames, max_rows):
+        """detect_rois / detect_rois_list: the checked rois and count, and the (rows, counts) tensors of num_frames frames."""
+        import torch
+        if not (isinstance(rois, torch.Tensor) and rois.is_cuda and rois.dtype == torch.int32 and tuple(rois.shape) == (self.batch, 6)):
+            raise ValueError("%s: rois must be an int32 CUDA tensor [%d, 6] (the model's batch)" % (who, self.batch))
+        if count is not None and not (isinstance(count, torch.Tensor) and count.is_cuda and count.dtype == torch.int32 and count.numel() == 1):
+            raise ValueError("%s: count must be None or an int32 CUDA tensor of one element" % who)
+        device = torch.device("cuda", self.ctx.device)
+        rows = torch.empty((num_frames, max(int(max_rows), 0), 6), dtype=torch.float32, device=device)
+        counts = torch.empty(num_frames, dtype=torch.int32, device=device)
+        return rois.contiguous(), (count.data_ptr() if count is not None else None), rows, counts
+
+    def detect_rois(self, frames, rois, count=None, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, max_rows=100):
+        """snnb_model_detect_rois: detection on regions of device frames (tiles of large frames, or zoomed regions of a first pass).
+        frames, rois and count as run_rois. Each valid slot is detected as detect_frames detects its crop (100 rows at most), its boxes
+        are mapped to the frame its region lies on, and each frame's boxes are merged by one stable score sort and one NMS. Returns
+        (rows, counts) per FRAME: rows a CUDA float32 tensor [num_frames, max_rows, 6] of {class, score, x, y, w, h} normalised to the
+        frame, zero past each count, and counts a CUDA int32 tensor [num_frames]; ordered on the current torch stream, never synchronising."""
+        f, n = self._frames_any("detect_rois", frames, format, matrix, linear, mean4, norm4)
+        rois, cnt, rows, counts = self._region_detections("detect_rois", rois, count, n, max_rows)
+        check(lib().snnb_model_detect_rois(self.h, C.byref(f), n, rois.data_ptr(), cnt, rows.data_ptr() or None, int(max_rows), counts.data_ptr(),
+                                           self._torch_stream()),
+              "snnb_model_detect_rois")
+        return rows, counts
+
+    def detect_rois_list(self, frames, rois, count=None, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, max_rows=100):
+        """snnb_model_detect_rois_list: detect_rois on a list of 1 to 256 frames of mixed sizes as run_rois_list takes it; each frame's
+        boxes are normalised to its own size. Returns (rows, counts) with one entry per frame of the list."""
+        fl, images = self._frame_list("detect_rois_list", frames, format, matrix, linear, mean4, norm4)
+        rois, cnt, rows, counts = self._region_detections("detect_rois_list", rois, count, len(frames), max_rows)
+        check(lib().snnb_model_detect_rois_list(self.h, C.byref(fl), rois.data_ptr(), cnt, rows.data_ptr() or None, int(max_rows), counts.data_ptr(),
+                                                self._torch_stream()),
+              "snnb_model_detect_rois_list")
         return rows, counts
 
     def transform_frames(self, frames, format="nv12", matrix="bt601", linear=True, mean4=None, norm4=None, out_format=None, out_hw=None,

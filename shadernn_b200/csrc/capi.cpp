@@ -2,6 +2,7 @@
 // (The whole-model engine entry points live in engine/model_capi.cpp.) See include/snnb.h for the reference
 // interface each entry point replaces.
 #include <algorithm>
+#include <climits>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
@@ -144,6 +145,29 @@ int snnb_rois_from_detections_list(snnb_context* ctx, const float* rows_dev, con
     SNNB_REQUIRE(ctx, "snnb_rois_from_detections_list: null context");
     SNNB_CUDA_OK(cudaSetDevice(ctx->device));
     return rois_from_detections_list(ctx, rows_dev, counts_dev, num_frames, max_rows, frame_wh, sel, rois_dev, capacity, count_dev, static_cast<cudaStream_t>(stream));
+}
+// Tile starts along one axis of `size` pixels for tiles of t <= size with at least `ov` < t pixels of overlap: n = 1 + ceil((size - t) /
+// (t - ov)) tiles, tile i at i * (size - t) / (n - 1), so neighbours are at most t - ov apart and the last tile ends at size.
+static long long tileCount(int size, int t, int ov) { return 1 + ((long long) size - t + (t - ov) - 1) / (t - ov); }
+static int tileStart(int size, int t, long long n, long long i) { return n == 1 ? 0 : (int) (i * (size - t) / (n - 1)); }
+int snnb_tile_rois(int frame, int frame_w, int frame_h, int tile_w, int tile_h, int min_overlap, snnb_roi* rois_host, int capacity, int* count) {
+    SNNB_REQUIRE(count, "snnb_tile_rois: null count");
+    SNNB_REQUIRE(frame_w >= 1 && frame_h >= 1, "snnb_tile_rois: frame size %d x %d; width and height must be >= 1", frame_w, frame_h);
+    SNNB_REQUIRE(tile_w >= 1 && tile_h >= 1, "snnb_tile_rois: tile size %d x %d; width and height must be >= 1", tile_w, tile_h);
+    const int tw = std::min(tile_w, frame_w), th = std::min(tile_h, frame_h);
+    SNNB_REQUIRE(min_overlap >= 0 && min_overlap < std::min(tw, th), "snnb_tile_rois: min_overlap %d is outside 0..%d (the tile %d x %d, clamped to the frame)",
+                 min_overlap, std::min(tw, th) - 1, tw, th);
+    const long long nx = tileCount(frame_w, tw, min_overlap), ny = tileCount(frame_h, th, min_overlap), n = nx * ny;
+    if (n > capacity) {
+        *count = (int) std::min(n, (long long) INT_MAX);
+        SNNB_REQUIRE(false, "snnb_tile_rois: %lld x %lld = %lld tiles; capacity %d", nx, ny, n, capacity);
+    }
+    SNNB_REQUIRE(rois_host, "snnb_tile_rois: null rois");
+    for (long long j = 0; j < ny; ++j)
+        for (long long i = 0; i < nx; ++i)
+            rois_host[j * nx + i] = snnb_roi {frame, (int) (j * nx + i), tileStart(frame_w, tw, nx, i), tileStart(frame_h, th, ny, j), tw, th};
+    *count = (int) n;
+    return 0;
 }
 
 // ---- tensors ----

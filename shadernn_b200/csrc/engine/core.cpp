@@ -48,6 +48,7 @@ MixedInferenceCore::~MixedInferenceCore() {
     if (copyStream) cudaStreamDestroy(copyStream);
     if (callerReady) cudaEventDestroy(callerReady);
     if (detectScratch) cudaFree(detectScratch);
+    if (roiScratch) cudaFree(roiScratch);
     if (deviceDone) cudaEventDestroy(deviceDone);
 }
 
@@ -1018,13 +1019,28 @@ int MixedInferenceCore::runRoisList(const snnb_frame_list* frames, const snnb_ro
     return runDeviceFeed("snnb_model_run_rois_list", in, outputs, numOutputs, classes1Dev, stream);
 }
 
+// A counted region call (counted(in)): refused while the context's stream is being captured; otherwise the current batch's dispatch graph,
+// built on the first such call. Nothing to do for any other call.
+int MixedInferenceCore::prepareCounted(const char* api, const DeviceFeed& in) {
+    if (!counted(in)) return 0;
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    SNNB_CUDA_OK(cudaStreamIsCapturing(ctx->stream, &cap));
+    SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone,
+                 "%s: the context's stream is being captured (snnb_graph_capture_begin); a call with a device-side count and declared sizes runs "
+                 "a graph with conditional nodes, which cannot become part of another graph",
+                 api);
+    return !cur->dispatchExec && buildDispatch(api, in.roiCount) ? 1 : 0;
+}
+
 int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev,
                                       cudaStream_t stream) {
     // everything is validated before the first enqueue: a refused call leaves no work behind
     SNNB_REQUIRE(numOutputs >= 0 && numOutputs <= (int) outputLayers.size(), "%s: %d outputs requested, the model has %d", api, numOutputs,
                  (int) outputLayers.size());
     SNNB_REQUIRE(outputs || numOutputs == 0, "%s: null outputs", api);
-    SNNB_REQUIRE(!(in.rois && outputLayers[0]->typeName == "YOLO"), "%s: output 0 is a YOLO detection list; detection on regions is not supported", api);
+    SNNB_REQUIRE(!(in.rois && outputLayers[0]->typeName == "YOLO"),
+                 "%s: output 0 is a YOLO detection list; detection on regions is not supported by this call: use %s", api,
+                 in.list ? "snnb_model_detect_rois_list" : "snnb_model_detect_rois");
     SNNB_REQUIRE(outputLayers[0]->typeName != "YOLO",
                  "%s: output 0 is a YOLO detection list; use %s for device detections, or snnb_model_run or "
                  "snnb_model_submit / snnb_model_wait and read the boxes with snnb_model_get_boxes",
@@ -1040,15 +1056,7 @@ int MixedInferenceCore::runDeviceFeed(const char* api, const DeviceFeed& in, con
         SNNB_REQUIRE(isClassifier, "%s: classes requested, but the model is not a classifier (output 0 is not 1 x 1 x C with C > 1)", api);
         if (int rc = checkDevicePointer(api, classes1Dev, sizeof(int), device, "classes", 0)) return rc;
     }
-    if (counted(in)) {
-        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-        SNNB_CUDA_OK(cudaStreamIsCapturing(ctx->stream, &cap));
-        SNNB_REQUIRE(cap == cudaStreamCaptureStatusNone,
-                     "%s: the context's stream is being captured (snnb_graph_capture_begin); a call with a device-side count and declared sizes runs "
-                     "a graph with conditional nodes, which cannot become part of another graph",
-                     api);
-        if (!cur->dispatchExec && buildDispatch(api, in.roiCount)) return 1;
-    }
+    if (int rc = prepareCounted(api, in)) return rc;
 
     if (enqueueDeviceForward(in, stream)) return 1;
     for (int j = 0; j < numOutputs; ++j)
@@ -1093,20 +1101,79 @@ int MixedInferenceCore::detectFrameList(const snnb_frame_list* frames, float* ro
 int MixedInferenceCore::detectDeviceFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
     SNNB_REQUIRE(yolo, "%s: the model has no YOLO output; use %s", api,
                  in.list ? "snnb_model_run_frame_list" : (in.frames ? "snnb_model_run_frames" : "snnb_model_run_device"));
+    if (int rc = checkDetectOutputs(api, in, rowsDev, maxRows, countsDev, stream)) return rc;
+
+    if (enqueueDeviceForward(in, stream)) return 1;
+    if (launch_yolo_detect(ctx, yolo->inputs[0], yolo->inputs[1], detectScratch, maxRows, rowsDev, countsDev)) return 1;
+    return fenceToCaller(stream);
+}
+
+// The checks the detecting calls share once the model is known to have a YOLO output: max_rows, the feed, rows and counts, the heads;
+// then the decode's scratch (sized for the loaded batch, whatever the model's batch is now), allocated on first use.
+int MixedInferenceCore::checkDetectOutputs(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
     SNNB_REQUIRE(maxRows >= 1 && maxRows <= 100, "%s: max_rows %d is outside 1..100", api, maxRows);
     if (int rc = checkDeviceFeed(api, in, stream)) return rc;
     if (int rc = checkDevicePointer(api, rowsDev, sizeof(float), ctx->device, "rows", 0)) return rc;
     if (int rc = checkDevicePointer(api, countsDev, sizeof(int), ctx->device, "counts", 0)) return rc;
     SNNB_REQUIRE(yolo->inputs.size() == 2 && yolo->inputs[0]->c >= 18 && yolo->inputs[1]->c >= 18, "%s: %s: YOLO expects two heads of >= 18 channels", api,
                  yolo->name.c_str());
-    if (!detectScratch) { // sized for the loaded batch, whatever the model's batch is now
+    if (!detectScratch) {
         snnb_tensor h0 = *yolo->inputs[0], h1 = *yolo->inputs[1];
         h0.n = h1.n = (int) options.batch;
         SNNB_CUDA_OK(cudaMalloc(&detectScratch, yolo_detect_scratch_bytes(&h0, &h1)));
     }
+    return 0;
+}
+
+// Detection on regions: runRois' input staging and forward pass (the dispatch graph for a counted call), the device decode of every slot
+// into roiScratch (100 rows per slot, as detectFrames with max_rows 100), then the merge: each valid slot's rows mapped to its frame,
+// one stable score sort and one greedy NMS per frame, into the caller's rows and counts.
+int MixedInferenceCore::detectRois(const snnb_frames* frames, int numFrames, const snnb_roi* roisDev, const int* countDev, float* rowsDev, int maxRows,
+                                   int* countsDev, cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_detect_rois: null frames");
+    SNNB_REQUIRE(roisDev, "snnb_model_detect_rois: null rois");
+    DeviceFeed in;
+    in.frames = frames, in.rois = roisDev, in.roiCount = countDev, in.numFrames = numFrames;
+    return detectRoisFeed("snnb_model_detect_rois", in, rowsDev, maxRows, countsDev, stream);
+}
+int MixedInferenceCore::detectRoisList(const snnb_frame_list* frames, const snnb_roi* roisDev, const int* countDev, float* rowsDev, int maxRows, int* countsDev,
+                                       cudaStream_t stream) {
+    SNNB_REQUIRE(frames, "snnb_model_detect_rois_list: null frames");
+    SNNB_REQUIRE(roisDev, "snnb_model_detect_rois_list: null rois");
+    DeviceFeed in;
+    in.list = frames, in.rois = roisDev, in.roiCount = countDev, in.numFrames = frames->count;
+    return detectRoisFeed("snnb_model_detect_rois_list", in, rowsDev, maxRows, countsDev, stream);
+}
+int MixedInferenceCore::detectRoisFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream) {
+    SNNB_REQUIRE(yolo, "%s: the model has no YOLO output; use %s", api, in.list ? "snnb_model_run_rois_list" : "snnb_model_run_rois");
+    if (int rc = checkDetectOutputs(api, in, rowsDev, maxRows, countsDev, stream)) return rc;
+    if (int rc = prepareCounted(api, in)) return rc;
+    const int B             = (int) options.batch;
+    const size_t rowsBytes  = (size_t) B * 100 * 6 * sizeof(float);
+    const size_t countBytes = ((size_t) B * sizeof(int) + 255) & ~(size_t) 255;
+    const size_t mergeBytes = roi_merge_scratch_bytes(B);
+    if (in.numFrames > roiSegsCap) { // at least 256 frames; a larger call replaces the scratch once the work that reads it is done
+        if (roiScratch) {
+            SNNB_CUDA_OK(cudaStreamSynchronize(ctx->stream));
+            cudaFree(roiScratch);
+            roiScratch = nullptr, roiSegsCap = 0;
+        }
+        const int cap = std::max(in.numFrames, (int) SNNB_FRAME_LIST_MAX);
+        SNNB_CUDA_OK(cudaMalloc(&roiScratch, rowsBytes + countBytes + mergeBytes + (size_t) cap * 2 * sizeof(int)));
+        roiSegsCap = cap;
+    }
+    char* base      = static_cast<char*>(roiScratch);
+    float* slotRows = reinterpret_cast<float*>(base);
+    int* slotCounts = reinterpret_cast<int*>(base + rowsBytes);
+    void* merge     = base + rowsBytes + countBytes;
+    void* segs      = base + rowsBytes + countBytes + mergeBytes;
 
     if (enqueueDeviceForward(in, stream)) return 1;
-    if (launch_yolo_detect(ctx, yolo->inputs[0], yolo->inputs[1], detectScratch, maxRows, rowsDev, countsDev)) return 1;
+    if (launch_yolo_detect(ctx, yolo->inputs[0], yolo->inputs[1], detectScratch, 100, slotRows, slotCounts)) return 1;
+    const int rc = withFrames(in, [&](const auto& fr) {
+        return launch_roi_merge(ctx, fr, in.numFrames, in.rois, in.roiCount, curBatch, slotRows, slotCounts, merge, segs, maxRows, rowsDev, countsDev);
+    });
+    if (rc) return 1;
     return fenceToCaller(stream);
 }
 

@@ -370,6 +370,12 @@ public:
     int detectFrameList(const snnb_frame_list* frames, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
     int runRoisList(const snnb_frame_list* frames, const snnb_roi* roisDev, const int* countDev, const snnb_device_buffer* outputs, int numOutputs,
                     int* classes1Dev, cudaStream_t stream);
+    // snnb_model_detect_rois / detect_rois_list: runRois' input and forward pass, the device decode per slot, then the slots' rows mapped
+    // to their frames and merged by one NMS per frame
+    int detectRois(const snnb_frames* frames, int numFrames, const snnb_roi* roisDev, const int* countDev, float* rowsDev, int maxRows, int* countsDev,
+                   cudaStream_t stream);
+    int detectRoisList(const snnb_frame_list* frames, const snnb_roi* roisDev, const int* countDev, float* rowsDev, int maxRows, int* countsDev,
+                       cudaStream_t stream);
     // snnb_model_transform_frame_list / transform_luma_list / segment_frame_list: transformFrames / transformLuma / segmentFrames with a
     // frame list in and one output descriptor per image out
     int transformFrameList(const snnb_frame_list* frames, const snnb_frame_out_list* out, cudaStream_t stream);
@@ -486,6 +492,7 @@ private:
     // enqueued), then the fenced input staging + forward pass, the outputs or the detections, and the fence back to the caller's stream
     int runDeviceFeed(const char* api, const DeviceFeed& in, const snnb_device_buffer* outputs, int numOutputs, int* classes1Dev, cudaStream_t stream);
     int detectDeviceFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
+    int detectRoisFeed(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
     // shared by the frame-writing calls and their list forms: the feed's checks, then out's (one batch description `o`, or the output
     // list `ol`), output 0's, the forward pass, the output kernel and the fence
     int transformDeviceFeed(const char* api, const DeviceFeed& in, const snnb_frames_out* o, const snnb_frame_out_list* ol, cudaStream_t stream);
@@ -494,9 +501,17 @@ private:
     int checkDeviceFeed(const char* api, const DeviceFeed& in, cudaStream_t stream);
     // regions with a device-side count, once sizes are declared: the forward pass is the dispatch graph's (forwardCounted)
     bool counted(const DeviceFeed& in) const { return in.rois && in.roiCount && !countSizes.empty(); }
+    int prepareCounted(const char* api, const DeviceFeed& in); // a counted call's capture check and dispatch graph (host-side, before any enqueue)
+    // detectDeviceFeed's and detectRoisFeed's host checks of max_rows, the feed, rows, counts and the heads, and the decode's scratch
+    int checkDetectOutputs(const char* api, const DeviceFeed& in, float* rowsDev, int maxRows, int* countsDev, cudaStream_t stream);
     int enqueueDeviceForward(const DeviceFeed& in, cudaStream_t stream);
     int fenceToCaller(cudaStream_t stream);
     void* detectScratch = nullptr; // detectDevice's per-image keys (yolo_detect_scratch_bytes), allocated on first use
+    // detectRois' scratch, sized for the loaded batch: the per-slot rows [B][100][6] and counts [B], the merge's two row buffers
+    // (roi_merge_scratch_bytes), then one {start, length} per frame for roiSegsCap frames; allocated on first use, and again for a call
+    // with more frames than roiSegsCap
+    void* roiScratch = nullptr;
+    int roiSegsCap   = 0;
 };
 
 } // namespace snn

@@ -182,6 +182,18 @@ int snnb_model_run_rois_list(snnb_model* m, const snnb_frame_list* frames, const
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
     return m->core->runRoisList(frames, rois_dev, count_dev, outputs, num_outputs, classes_1based_dev, static_cast<cudaStream_t>(stream));
 }
+int snnb_model_detect_rois(snnb_model* m, const snnb_frames* frames, int num_frames, const snnb_roi* rois_dev, const int* count_dev, float* rows_dev,
+                           int max_rows, int* counts_dev, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_detect_rois: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->detectRois(frames, num_frames, rois_dev, count_dev, rows_dev, max_rows, counts_dev, static_cast<cudaStream_t>(stream));
+}
+int snnb_model_detect_rois_list(snnb_model* m, const snnb_frame_list* frames, const snnb_roi* rois_dev, const int* count_dev, float* rows_dev, int max_rows,
+                                int* counts_dev, void* stream) {
+    SNNB_REQUIRE(m, "snnb_model_detect_rois_list: null model");
+    SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));
+    return m->core->detectRoisList(frames, rois_dev, count_dev, rows_dev, max_rows, counts_dev, static_cast<cudaStream_t>(stream));
+}
 int snnb_model_transform_frame_list(snnb_model* m, const snnb_frame_list* frames, const snnb_frame_out_list* out, void* stream) {
     SNNB_REQUIRE(m, "snnb_model_transform_frame_list: null model");
     SNNB_CUDA_OK(cudaSetDevice(m->core->ctx->device));

@@ -966,30 +966,30 @@ __global__ void __launch_bounds__(256) yolo_rank_kernel(int cap, const int* __re
     if (i < count) sorted[(size_t) n * cap + rank] = mine;
 }
 
-// Greedy NMS of image blockIdx.x over its sorted list (nms, layers.cpp): a box is kept unless a kept box before it of the same class
-// overlaps it with IoU > 0.45, which is what the host's loop computes. The list is walked NMS_THREADS candidates at a time: each thread
-// decodes one, tests it against the boxes kept so far and records which earlier candidates of the step would suppress it; thread 0 then
-// resolves the step in order. The walk stops at max_rows kept boxes: later boxes cannot change earlier ones.
-// rows[n][max_rows][6] = {class, score, x, y, w, h}, zero past the count; out_counts[n] = the number of rows.
-__global__ void __launch_bounds__(yolo_dev::NMS_THREADS) yolo_nms_kernel(TV h0, TV h1, int cap, const int* __restrict__ counts,
-                                                                        const unsigned long long* __restrict__ sorted, int max_rows,
-                                                                        float* __restrict__ rows, int* __restrict__ out_counts) {
+// Greedy NMS of one list in descending score order, by one CTA of NMS_THREADS threads (nms, layers.cpp): a box is kept unless a kept
+// box before it of the same class overlaps it with IoU > 0.45, which is what the host's loop computes. The list is walked NMS_THREADS
+// candidates at a time: each thread fetches one (boxes(i, b): false when candidate i is not a box), tests it against the boxes kept so
+// far and records which earlier candidates of the step would suppress it; thread 0 then resolves the step in order. The walk stops at
+// max_rows kept boxes: later boxes cannot change earlier ones.
+// rows[n][max_rows][6] = {class, score, x, y, w, h}, zero past the count; out_counts[n] = the number of rows. The box source is a
+// template argument so that yolo_nms_kernel (cells decoded from the heads) and roi_merge_nms_kernel (boxes already decoded) share this
+// step; yolo_nms_kernel's machine code is the same as before the step was lifted out of it.
+template <class Boxes>
+__device__ __forceinline__ void yolo_greedy_nms(const Boxes& boxes, int count, int max_rows, int n, float* __restrict__ rows, int* __restrict__ out_counts) {
     using namespace yolo_dev;
-    pdl_wait();
     __shared__ YoloBox kept[MAX_ROWS];
     __shared__ YoloBox step[NMS_THREADS];
     __shared__ unsigned long long mask[NMS_THREADS][2];
     __shared__ int live[NMS_THREADS];
     __shared__ int nkept;
-    const int n = blockIdx.x, tid = threadIdx.x, count = counts[n];
-    const unsigned long long* s = sorted + (size_t) n * cap;
+    const int tid = threadIdx.x;
     if (tid == 0) nkept = 0;
     __syncthreads();
     for (int c0 = 0; c0 < count && nkept < max_rows; c0 += NMS_THREADS) {
         const int i = c0 + tid;
         YoloBox b {};
         bool alive = i < count;
-        if (alive) alive = yolo_decode_cell(h0, h1, n, yolo_key_scan(s[i]), true, b);
+        if (alive) alive = boxes(i, b);
         step[tid] = b;
         const int k0 = nkept;
         for (int k = 0; k < k0 && alive; ++k)
@@ -1030,6 +1030,21 @@ __global__ void __launch_bounds__(yolo_dev::NMS_THREADS) yolo_nms_kernel(TV h0, 
         r[e] = v;
     }
     if (tid == 0) out_counts[n] = nk;
+}
+// Image n's candidates: the cells of its sorted keys, decoded from the heads
+struct YoloCellBoxes {
+    TV h0, h1;
+    int n;
+    const unsigned long long* s;
+    __device__ __forceinline__ bool operator()(int i, YoloBox& b) const { return yolo_decode_cell(h0, h1, n, yolo_key_scan(s[i]), true, b); }
+};
+// Greedy NMS of image blockIdx.x over its sorted list: rows[n][max_rows][6], out_counts[n]
+__global__ void __launch_bounds__(yolo_dev::NMS_THREADS) yolo_nms_kernel(TV h0, TV h1, int cap, const int* __restrict__ counts,
+                                                                        const unsigned long long* __restrict__ sorted, int max_rows,
+                                                                        float* __restrict__ rows, int* __restrict__ out_counts) {
+    pdl_wait();
+    const int n = blockIdx.x;
+    yolo_greedy_nms(YoloCellBoxes {h0, h1, n, sorted + (size_t) n * cap}, counts[n], max_rows, n, rows, out_counts);
 }
 
 // scratch: the candidate count of every image (rounded up to 256 bytes), then the keys and the sorted keys, [N][cells per image] each
@@ -2007,6 +2022,156 @@ int launch_rois_from_detections(snnb_context* ctx, cudaStream_t stream, const fl
     FrameSizesV S {};
     for (int n = 0; n < num_frames; ++n) S.wh[n][0] = frame_wh[2 * n], S.wh[n][1] = frame_wh[2 * n + 1];
     return rois_from_detections_launch(ctx, stream, rows, counts, num_frames, max_rows, S, sel, rois, capacity, count);
+}
+
+// Detection on regions (snnb_model_detect_rois): the per-slot rows of launch_yolo_detect (max_rows 100) mapped to their frames and
+// merged by one greedy NMS per frame. Frame f's segment is the mapped rows of every valid slot on f, slots in order and each slot's rows
+// in order; the segments lie frame after frame in `seg`, so segment f starts after the rows of the valid slots on frames below f.
+// Three kernels, none with atomics: roi_merge_gather_kernel (one CTA per frame) finds its segment and fills it, roi_merge_rank_kernel
+// sorts each segment by rank as yolo_rank_kernel does, roi_merge_nms_kernel (one CTA per frame) runs yolo_greedy_nms over it.
+constexpr int MERGE_THREADS = 256;
+// Exclusive prefix sum of v over the CTA (MERGE_THREADS threads); total = the sum. sh: MERGE_THREADS / 32 ints of shared memory.
+__device__ __forceinline__ int merge_scan(int v, int* sh, int& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int incl = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= d) incl += u;
+    }
+    if (lane == 31) sh[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+        int w = lane < MERGE_THREADS / 32 ? sh[lane] : 0;
+#pragma unroll
+        for (int d = 1; d < MERGE_THREADS / 32; d <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, w, d);
+            if (lane >= d) w += u;
+        }
+        if (lane < MERGE_THREADS / 32) sh[lane] = w;
+    }
+    __syncthreads();
+    const int excl = incl - v + (warp ? sh[warp - 1] : 0);
+    total          = sh[MERGE_THREADS / 32 - 1];
+    __syncthreads(); // sh is rewritten by the next scan
+    return excl;
+}
+// Frame blockIdx.x: two walks over the N slots in order. The first sums the rows of the valid slots on lower frames (the segment's
+// start), the second places each valid slot on this frame after the ones before it and writes its rows, mapped to the frame:
+// {cls, score, (rx + x * rw) / W, (ry + y * rh) / H, (w * rw) / W, (h * rh) / H}, every operation rounded on its own.
+// segs[f] = {start, length}.
+template <class Sizes>
+__global__ void __launch_bounds__(MERGE_THREADS) roi_merge_gather_kernel(const __grid_constant__ Sizes S, RoiV g, int N, const float* __restrict__ slot_rows,
+                                                                        const int* __restrict__ slot_counts, YoloBox* __restrict__ seg,
+                                                                        int2* __restrict__ segs) {
+    using yolo_dev::MAX_ROWS;
+    pdl_wait();
+    __shared__ int sh[MERGE_THREADS / 32];
+    __shared__ int off[MERGE_THREADS], cnt[MERGE_THREADS];
+    __shared__ int4 reg[MERGE_THREADS];
+    const int f = blockIdx.x, tid = threadIdx.x;
+    const int2 wh = frame_size(S, f);
+    const float W = (float) wh.x, H = (float) wh.y;
+    int start = 0, len = 0, total;
+    for (int s0 = 0; s0 < N; s0 += MERGE_THREADS) {
+        const int s = s0 + tid;
+        snnb_roi roi;
+        const int below = s < N && roi_slot(S, g, s, N, roi) && roi.frame < f ? __ldg(slot_counts + s) : 0;
+        merge_scan(below, sh, total);
+        start += total;
+    }
+    for (int s0 = 0; s0 < N; s0 += MERGE_THREADS) {
+        const int s = s0 + tid;
+        snnb_roi roi {0, 0, 0, 0, 0, 0};
+        const int mine = s < N && roi_slot(S, g, s, N, roi) && roi.frame == f ? __ldg(slot_counts + s) : 0;
+        off[tid] = start + len + merge_scan(mine, sh, total);
+        cnt[tid] = mine;
+        reg[tid] = make_int4(roi.x, roi.y, roi.width, roi.height);
+        __syncthreads();
+        const int rows = min(MERGE_THREADS, N - s0) * MAX_ROWS;
+        for (int e = tid; e < rows; e += MERGE_THREADS) {
+            const int j = e / MAX_ROWS, k = e - j * MAX_ROWS;
+            if (k >= cnt[j]) continue;
+            const float* row = slot_rows + ((size_t) (s0 + j) * MAX_ROWS + k) * 6;
+            const int4 q   = reg[j];
+            const float rx = (float) q.x, ry = (float) q.y, rw = (float) q.z, rh = (float) q.w;
+            const float x = __ldg(row + 2), y = __ldg(row + 3), w = __ldg(row + 4), h = __ldg(row + 5);
+            seg[off[j] + k] = YoloBox {(int) __ldg(row), __ldg(row + 1), __fdiv_rn(__fadd_rn(rx, __fmul_rn(x, rw)), W), __fdiv_rn(__fadd_rn(ry, __fmul_rn(y, rh)), H),
+                                       __fdiv_rn(__fmul_rn(w, rw), W), __fdiv_rn(__fmul_rn(h, rh), H)};
+        }
+        len += total;
+        __syncthreads(); // off, cnt and reg are rewritten by the next chunk
+    }
+    if (tid == 0) segs[f] = make_int2(start, len);
+}
+// Rank sort of segment blockIdx.x (yolo_rank_kernel's): std::stable_sort by descending score over the segment == descending
+// (score, -position), yolo_key(score, position). Blocks past the segment's length exit at once.
+__global__ void __launch_bounds__(MERGE_THREADS) roi_merge_rank_kernel(const int2* __restrict__ segs, const YoloBox* __restrict__ seg, YoloBox* __restrict__ sorted) {
+    pdl_wait();
+    __shared__ unsigned long long tile[MERGE_THREADS];
+    const int2 sg = segs[blockIdx.x];
+    const int count = sg.y;
+    if ((int) (blockIdx.y * blockDim.x) >= count) return;
+    const YoloBox* b = seg + sg.x;
+    const int i      = blockIdx.y * blockDim.x + threadIdx.x;
+    const unsigned long long mine = i < count ? yolo_key(b[i].score, i) : 0ull;
+    int rank = 0;
+    for (int t0 = 0; t0 < count; t0 += MERGE_THREADS) {
+        __syncthreads();
+        if (t0 + (int) threadIdx.x < count) tile[threadIdx.x] = yolo_key(b[t0 + threadIdx.x].score, t0 + threadIdx.x);
+        __syncthreads();
+        const int m = min(MERGE_THREADS, count - t0);
+        for (int j = 0; j < m; ++j) rank += tile[j] > mine ? 1 : 0;
+    }
+    if (i < count) sorted[sg.x + rank] = b[i];
+}
+// A sorted segment's boxes, as decoded and mapped
+struct MergedBoxes {
+    const YoloBox* b;
+    __device__ __forceinline__ bool operator()(int i, YoloBox& o) const {
+        o = b[i];
+        return true;
+    }
+};
+// Greedy NMS of frame blockIdx.x's sorted segment: rows[f][max_rows][6], counts[f]
+__global__ void __launch_bounds__(yolo_dev::NMS_THREADS) roi_merge_nms_kernel(const int2* __restrict__ segs, const YoloBox* __restrict__ sorted, int max_rows,
+                                                                             float* __restrict__ rows, int* __restrict__ counts) {
+    pdl_wait();
+    const int f   = blockIdx.x;
+    const int2 sg = segs[f];
+    yolo_greedy_nms(MergedBoxes {sorted + sg.x}, sg.y, max_rows, f, rows, counts);
+}
+size_t roi_merge_scratch_bytes(int batch) { return (size_t) batch * yolo_dev::MAX_ROWS * 2 * sizeof(YoloBox); }
+template <class Sizes>
+static int roi_merge(snnb_context* ctx, const Sizes& S, const RoiV& g, int batch, const float* slot_rows, const int* slot_counts, void* scratch, int2* segs,
+                     int max_rows, float* rows, int* counts) {
+    SNNB_REQUIRE(batch >= 1 && batch <= 65535 && g.num_frames >= 1 && max_rows >= 1 && max_rows <= yolo_dev::MAX_ROWS,
+                 "launch_roi_merge: batch %d, %d frames, max_rows %d", batch, g.num_frames, max_rows);
+    auto* seg    = static_cast<YoloBox*>(scratch);
+    auto* sorted = seg + (size_t) batch * yolo_dev::MAX_ROWS;
+    const unsigned frames = (unsigned) g.num_frames;
+    if (launch_done(ctx, launch_k(roi_merge_gather_kernel<Sizes>, dim3(frames), dim3(MERGE_THREADS), 0, ctx->stream, S, g, batch, slot_rows, slot_counts, seg, segs),
+                    "roi_merge_gather_kernel", Sizes::form))
+        return 1;
+    const dim3 rank_grid(frames, (unsigned) ((batch * yolo_dev::MAX_ROWS + MERGE_THREADS - 1) / MERGE_THREADS));
+    if (launch_done(ctx, launch_k(roi_merge_rank_kernel, rank_grid, dim3(MERGE_THREADS), 0, ctx->stream, (const int2*) segs, (const YoloBox*) seg, sorted),
+                    "roi_merge_rank_kernel"))
+        return 1;
+    return launch_done(ctx, launch_k(roi_merge_nms_kernel, dim3(frames), dim3(yolo_dev::NMS_THREADS), 0, ctx->stream, (const int2*) segs, (const YoloBox*) sorted,
+                                     max_rows, rows, counts),
+                       "roi_merge_nms_kernel");
+}
+int launch_roi_merge(snnb_context* ctx, const snnb_frames& fr, int num_frames, const snnb_roi* rois, const int* count, int batch, const float* slot_rows,
+                     const int* slot_counts, void* scratch, void* segs, int max_rows, float* rows, int* counts) {
+    return roi_merge(ctx, FrameSizeV {fr.width, fr.height}, RoiV {rois, count, num_frames}, batch, slot_rows, slot_counts, scratch, static_cast<int2*>(segs), max_rows,
+                     rows, counts);
+}
+int launch_roi_merge(snnb_context* ctx, const snnb_frame_list& fl, int num_frames, const snnb_roi* rois, const int* count, int batch, const float* slot_rows,
+                     const int* slot_counts, void* scratch, void* segs, int max_rows, float* rows, int* counts) {
+    SNNB_REQUIRE(num_frames == fl.count && fl.count >= 1 && fl.count <= SNNB_FRAME_LIST_MAX, "launch_roi_list_merge: %d frames", fl.count);
+    FrameSizesV S {};
+    for (int n = 0; n < fl.count; ++n) S.wh[n][0] = fl.images[n].width, S.wh[n][1] = fl.images[n].height;
+    return roi_merge(ctx, S, RoiV {rois, count, fl.count}, batch, slot_rows, slot_counts, scratch, static_cast<int2*>(segs), max_rows, rows, counts);
 }
 
 // The selector node of a region call's dispatch graph (snnb_model_set_count_batches): turns on the one IF body whose size count_body

@@ -274,6 +274,15 @@ int launch_frame_roi_input(snnb_context* ctx, const snnb_frame_list& f, int num_
 int launch_roi_clear(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst, long long slot_bytes);
 int launch_roi_clear(snnb_context* ctx, const snnb_frame_list& f, int num_frames, const snnb_roi* rois, const int* count, int batch, void* dst,
                      long long slot_bytes);
+// Detection on regions (snnb_model_detect_rois): slot_rows [batch][100][6] and slot_counts [batch] of launch_yolo_detect (max_rows 100)
+// -> the rows of every valid slot (as launch_frame_roi_input decides validity) mapped to its frame and merged per frame by the greedy
+// NMS, into rows [num_frames][max_rows][6] (zero past the count) and counts [num_frames]. Three kernels. scratch holds
+// roi_merge_scratch_bytes(batch) bytes, segs num_frames int2 (8-byte aligned).
+size_t roi_merge_scratch_bytes(int batch);
+int launch_roi_merge(snnb_context* ctx, const snnb_frames& f, int num_frames, const snnb_roi* rois, const int* count, int batch, const float* slot_rows,
+                     const int* slot_counts, void* scratch, void* segs, int max_rows, float* rows, int* counts);
+int launch_roi_merge(snnb_context* ctx, const snnb_frame_list& f, int num_frames, const snnb_roi* rois, const int* count, int batch, const float* slot_rows,
+                     const int* slot_counts, void* scratch, void* segs, int max_rows, float* rows, int* counts);
 // Count-sized region batches (snnb_model_set_count_batches): the forward-pass size a region call with device-side count `count` runs at,
 // given the declared sizes (strictly increasing) and the model's batch: the smallest declared size >= c, c = clamp(count, 0, batch), or
 // batch itself when no declared size below batch is; 0 when c is 0 (no forward pass). count_select_kernel runs this very function.

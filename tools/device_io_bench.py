@@ -71,6 +71,13 @@ NV12 on detect_frames, transform_luma and transform_frames, with each frame kern
                and against a third handle after set_batch(bucket(k)), the size k selects; calls/s and the regions/s of the k used slots,
                alternating as above. And the `framelist` chain with planted detector heads and a min_score that keeps about three boxes per
                frame, four frame sets in turn, with and without sizes declared; the count of each frame set is reported beside the rates.
+  tiled       (opt-in) Detection on tiles of 4 x 3840x2160 NV12 frames: each frame cut by snnb_tile_rois into 960x960 tiles with at
+               least 96 px of overlap (5 x 3 = 15) plus one whole-frame region, 64 slots into YOLOv3-tiny 416x416 loaded at 64, with
+               planted heads (scores scattered around 0.35) and with all-pass heads. (a) detect_rois; (b) what a user does without it,
+               a torch NV12 -> RGB conversion, a crop + F.interpolate (bilinear) per tile, detect_torch, the rows to the host and
+               tests/_region_merge.py's merge_region_rows in numpy; (c) detect_frames on the 4 frames alone (the price of tiling). Frames/s
+               alternating as above (one warm-up call each: (b)'s merge takes seconds with all-pass heads). And, from torch.profiler
+               in a run of its own, the merge kernels' device time per call against the whole call's.
   card        name, power limit and maximum SM clock, read by nvidia-smi in the same run.
 """
 import argparse
@@ -1086,6 +1093,83 @@ def counted(torch, ctx, core, modelzoo, d, args):
     return res
 
 
+def yolo_heads(modelzoo, d, name, kind, hw):
+    """YOLOv3-tiny with planted heads (scores scattered around 0.35) or all-pass heads (every cell passes), as in `detector`."""
+    path, layers = modelzoo.build("yolov3tiny", os.path.join(d, name), input_hw=hw, **({"seed": 21} if kind == "planted" else {}))
+    for head in [l for l in layers if l["type"] == "Conv2D" and l["outputPlanes"] == 18]:
+        head["_w"]["bias"][:] = 0
+        head["_w"]["bias"][[4, 5, 10, 11] if kind == "planted" else [4, 5, 10, 11, 16, 17]] = [-1.0, 0.0, -1.0, 0.0] if kind == "planted" else 8.0
+    return modelzoo.write_model(layers, os.path.join(d, name + "_%s.json" % kind), split=True)
+
+
+def tiled(torch, ctx, core, modelzoo, d, args):
+    """Sliced detection on 2160p frames: detect_rois against the torch workaround and against detect_frames of the whole frames."""
+    import torch.nn.functional as F
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from _region_merge import merge_region_rows  # the float32 restatement of the merge that the tests hold detect_rois to
+    H, W, nframes, hw = 2160, 3840, 4, (416, 416)
+    mean4, norm4 = [127.5] * 4, [1.0 / 127.5] * 4
+    tiles = [core.tile_rois((H, W), (960, 960), 96, frame=f) for f in range(nframes)]
+    regions = np.concatenate([np.concatenate([t, [[f, len(t), 0, 0, W, H]]]) for f, t in enumerate(tiles)]).astype(np.int32)
+    batch = len(regions)
+    rois = torch.from_numpy(regions).cuda()
+    g = torch.Generator().manual_seed(11)
+    nv12 = torch.randint(16, 236, (nframes, H * 3 // 2, W), dtype=torch.uint8, generator=g).cuda()
+    mean = torch.tensor(mean4[:3], device="cuda").view(1, 3, 1, 1)
+    norm = torch.tensor(norm4[:3], device="cuda").view(1, 3, 1, 1)
+    res = {"case": "%d x %dx%d NV12, %d tiles of 960x960 (>= 96 px overlap) + 1 whole-frame region per frame: %d slots into yolov3tiny %dx%d "
+                   "loaded at %d; frames/s of the %d frames" % (nframes, W, H, len(tiles[0]), batch, hw[0], hw[1], batch, nframes)}
+    for kind in ("planted", "allpass"):
+        path = yolo_heads(modelzoo, d, "tiled_yolov3tiny", kind, hw)
+        m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=True, use_cuda_graph=True)
+        whole = core.MixedInferenceCore(ctx, path, batch=nframes, input_hw=hw, fuse=True, use_cuda_graph=True)
+
+        def workaround():
+            rgb = torch_nv12_to_rgb(torch, nv12)
+            crops = [F.interpolate(rgb[f:f + 1, :, y:y + h, x:x + w], size=hw, mode="bilinear", align_corners=False) for f, _, x, y, w, h in regions]
+            r, c = m.detect_torch(((torch.cat(crops) - mean) * norm).contiguous(), layout="nchw")
+            return merge_region_rows(r.cpu().numpy(), c.cpu().numpy(), regions, None, [(H, W)] * nframes, 100)
+        fns = {"detect_rois": lambda: m.detect_rois(nv12, rois, mean4=mean4, norm4=norm4),
+               "torch_workaround": workaround,
+               "detect_frames_whole": lambda: whole.detect_frames(nv12, mean4=mean4, norm4=norm4)}
+        for fn in fns.values():
+            fn()
+        torch.cuda.synchronize()
+        runs = [{k: timed(fn, args.seconds, nframes, torch.cuda.synchronize) for k, fn in fns.items()} for _ in range(args.rounds)]
+        med = {k: float(np.median([r[k]["frames_per_s"] for r in runs])) for k in fns}
+        counts = m.detect_rois(nv12, rois, mean4=mean4, norm4=norm4)[1].cpu().tolist()
+        # the merge kernels against the whole call, device time per call from torch.profiler
+        from torch.profiler import ProfilerActivity, profile
+        call = fns["detect_rois"]
+        for _ in range(5):
+            call()
+        torch.cuda.synchronize()
+        calls = 50
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(calls):
+                call()
+            torch.cuda.synchronize()
+        merge, total = {}, 0.0
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", None)
+            t = e.cuda_time_total if t is None else t
+            if "snnb::" not in e.key or t <= 0:
+                continue
+            total += t / calls
+            if "snnb::roi_merge_" in e.key:
+                merge[e.key.split("(")[0].replace("void ", "")] = t / calls
+        merge_us = sum(merge.values())
+        res[kind] = {"detect_rois_frames_per_s_median": med["detect_rois"], "torch_workaround_frames_per_s_median": med["torch_workaround"],
+                     "detect_frames_whole_frames_per_s_median": med["detect_frames_whole"],
+                     "detect_rois_over_torch_workaround": med["detect_rois"] / med["torch_workaround"],
+                     "detect_rois_over_detect_frames_whole": med["detect_rois"] / med["detect_frames_whole"], "boxes_per_frame": counts,
+                     "merge_kernels_us_per_call": merge, "merge_us_per_call": merge_us, "call_kernels_us_per_call": total,
+                     "merge_share_of_call": merge_us / total if total else None, "rounds": runs}
+        m.close()
+        whole.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--out", required=True)
@@ -1093,7 +1177,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--parts", default="throughput,conversions,detector,frames",
                     help="comma-separated subset of throughput, conversions, detector, frames, transform (opt-in), rois (opt-in), luma (opt-in), "
-                         "segment (opt-in), p010 (opt-in), framelist (opt-in), framelist_out (opt-in), partial (opt-in), counted (opt-in)")
+                         "segment (opt-in), p010 (opt-in), framelist (opt-in), framelist_out (opt-in), partial (opt-in), counted (opt-in), tiled (opt-in)")
     args = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -1130,6 +1214,8 @@ def main():
         result["partial"] = partial(torch, ctx, core, modelzoo, d, args)
     if "counted" in parts:
         result["counted"] = counted(torch, ctx, core, modelzoo, d, args)
+    if "tiled" in parts:
+        result["tiled"] = tiled(torch, ctx, core, modelzoo, d, args)
     text = json.dumps(result, indent=1)
     with open(os.path.join(args.out, "device_io_bench.json"), "w") as f:
         f.write(text)
