@@ -715,6 +715,12 @@ int snnb_debug_conv_launch(const int query[24], int out[59]);
  * 2 fp16w, 1 fp16; 0 on the CUDA cores), n_blk (output channels per tile), ksplit (K pieces per tile, 1 = none), stream_k (0/1),
  * fks (K steps per filter row of the row-window kernel's feed mode, 0 otherwise)}. Host-side record, no GPU work. Returns 0. */
 int snnb_debug_last_conv_variant(snnb_context* ctx, int out[6]);
+/* Diagnostics: the kernels launched on `ctx` since the last call with clear != 0 (per-operator or inside a model's forward pass; not
+ * kernels replayed by a CUDA graph), one name per line with the instantiation's template arguments, e.g. "pool_kernel<3>" or
+ * "depthwise_tma_kernel<1>"; at least the most recent 32 KB are kept. Copies at most cap - 1 bytes and a terminating NUL to buf, then
+ * empties the record if clear != 0. Host-side record, no GPU work. Returns the record's length in bytes (larger than cap - 1 when
+ * buf was too small), or -1 for a null ctx or buf or cap < 1. */
+int snnb_debug_launches(snnb_context* ctx, char* buf, int cap, int clear);
 /* Diagnostics: the size snnb_model_set_count_batches' selector picks for a device-side count, evaluated on the host with the kernel's own
  * function: the smallest of the num_sizes declared sizes (strictly increasing) that is >= c = clamp(count, 0, batch), or batch itself
  * when none below batch is; 0 when c is 0 (no forward pass). Returns -1 for batch < 1, num_sizes < 0 or null sizes. No GPU needed. */

@@ -471,13 +471,70 @@ def flatten(x):
     return y.astype(np.float64), np.zeros(y.shape)
 
 
-def upsample_nearest(x, out_hw, at=None):
-    """Nearest upsampling: output (y, x) reads input (floor(y h / oh), floor(x w / ow)) - for the integer scales of the zoo, y // s."""
+def upsample_nearest(x, out_hw, at=None, scale=None):
+    """Nearest upsampling (upsample_kernel): output column o reads input column floor(fl(o * fl(1 / scale))), the fp32 product of o
+    and the fp32 reciprocal of the layer's fp32 scale, clamped to the input (rows alike). That is the index the engine promises: it is
+    the reference's shader arithmetic (a float multiply by the inverse scale, then floor). At the integer scales it is floor(o / scale)
+    (the reciprocals of 2 and 4 are exact; fl(1/3) rounds up, and o * fl(1/3) never drops below an integer it should reach). At other
+    scales neither floor(o / scale) of the decimal scale nor that of its fp32 value is promised: at 1.7, fl(1/1.7) rounds down and
+    o = 17 reads column 9, not 10; at 1.2 the kernel agrees with the decimal scale but not with fp32(1.2) = 1.20000005 (o = 6 reads
+    column 5). scale None: out_hw / the input size (an integer scale)."""
     n, h, w, c = np.shape(x)
     oh, ow = out_hw
     ni, oy, ox = pixels(at, n, oh, ow)
-    y = gather(x, ni, (oy * h) // oh, (ox * w) // ow)
+    inv = np.float32(1) / np.float32(oh / h if scale is None else scale)
+    iy = np.clip(np.floor(oy.astype(np.float32) * inv).astype(np.int64), 0, h - 1)
+    ix = np.clip(np.floor(ox.astype(np.float32) * inv).astype(np.int64), 0, w - 1)
+    y = gather(x, ni, iy, ix)
     return shaped(y, at, n, oh, ow), shaped(np.zeros(y.shape), at, n, oh, ow)
+
+
+def bilinear_coord(o, size, scale):
+    """(X, e): the exact source coordinate (o + 0.5) / scale - 0.5 of output coordinates o clamped to [0, size - 1], and a bound of
+    the error of upsample_kernel's fp32 coordinate: inv = fl(1 / scale) errs by u / scale, offs = fl(0.5 - 0.5 inv) by
+    0.5 u / scale + u |offs|, o inv by o u / scale before its rounding (u o inv, unless contracted into the subtraction), and the
+    subtraction rounds once more (u |X|). Clamping does not increase the error."""
+    s = float(np.float32(scale))
+    offs = 0.5 - 0.5 / s
+    o = np.asarray(o, np.float64)
+    X = o / s - offs
+    e = U * (2 * o / s + 0.5 / s + abs(offs) + np.abs(X)) * SLACK
+    return np.clip(X, 0, size - 1), e
+
+
+def upsample_bilinear(x, scale, out_hw, half_out=False, at=None):
+    """Bilinear upsampling (upsample_kernel, the reference's vk_upsampling2d_bilinear): output (oy, ox) is the bilinear interpolation
+    of the input at the exact source coordinate ((oy, ox) + 0.5) / scale - 0.5, each coordinate clamped to [0, size - 1], from the
+    taps (floor, floor + 1) of each coordinate; a tap outside the input reads 0 (it only occurs at size - 1, with weight 0).
+    The kernel evaluates the interpolant at its fp32 coordinate (bilinear_coord: error e_x, e_y). The interpolant is continuous and
+    piecewise bilinear, so that moves the value by at most e_x times the largest difference of horizontal neighbours in the rows and
+    the cells the coordinate may fall in (columns floor(X) - 1 .. floor(X) + 2, rows floor(Y) - 1 .. floor(Y) + 2), plus e_y likewise.
+    Each weight is a product of two fp32 differences (x12 - sx is exact for sx >= 0.5, else one rounding): 3 u relative. The four
+    taps are accumulated from 0 in fp32 (separate or fused multiply-adds): gamma_4 sum w |t|. Then the store."""
+    n, h, w, c = np.shape(x)
+    oh, ow = out_hw
+    ni, oy, ox = pixels(at, n, oh, ow)
+    X, ex = bilinear_coord(ox, w, scale)
+    Y, ey = bilinear_coord(oy, h, scale)
+    x0, y0 = np.floor(X).astype(np.int64), np.floor(Y).astype(np.int64)
+    fx, fy = (X - x0)[:, None], (Y - y0)[:, None]
+
+    def t(yy, xx):  # outside the input: 0
+        return gather(x, ni, yy, xx)
+
+    t11, t21, t22, t12 = t(y0, x0), t(y0, x0 + 1), t(y0 + 1, x0 + 1), t(y0 + 1, x0)
+    w11, w21, w22, w12 = (1 - fx) * (1 - fy), fx * (1 - fy), fx * fy, (1 - fx) * fy
+    ref = w11 * t11 + w21 * t21 + w22 * t22 + w12 * t12
+    mag = w11 * np.abs(t11) + w21 * np.abs(t21) + w22 * np.abs(t22) + w12 * np.abs(t12)
+    dx = np.zeros((len(ni), c))
+    dy = np.zeros((len(ni), c))
+    for r in range(-1, 3):
+        for q in range(-1, 3):
+            v = t(y0 + r, x0 + q)
+            dx = np.maximum(dx, np.abs(t(y0 + r, x0 + q + 1) - v))
+            dy = np.maximum(dy, np.abs(t(y0 + r + 1, x0 + q) - v))
+    bound = (ex[:, None] * dx + ey[:, None] * dy + (3 * U + gamma(4)) * mag) * SLACK + store_bound(ref, half_out)
+    return shaped(ref, at, n, oh, ow), shaped(bound, at, n, oh, ow)
 
 
 def subpixel(x, r, half_out=False, at=None):

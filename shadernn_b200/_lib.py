@@ -322,6 +322,7 @@ SIGNATURES = {
     "snnb_debug_conv_plan": (C.c_int, [c_int_p, c_int_p]),
     "snnb_debug_conv_launch": (C.c_int, [c_int_p, c_int_p]),
     "snnb_debug_last_conv_variant": (C.c_int, [vp, c_int_p]),
+    "snnb_debug_launches": (C.c_int, [vp, C.c_char_p, C.c_int, C.c_int]),
     "snnb_debug_count_body": (C.c_int, [c_int_p, C.c_int, C.c_int, C.c_int]),
 }
 

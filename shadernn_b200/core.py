@@ -53,6 +53,22 @@ class GpuContext:
         v = list(out)
         return {"path": ["none", "simt", "igemm", "rowwin", "rowwin-feed"][v[0]], "terms": v[1], "n_blk": v[2], "ksplit": v[3], "stream_k": v[4], "fks": v[5]}
 
+    def debug_launches(self, clear=True):
+        """snnb_debug_launches: the names of the kernels launched on this context since the last clear, with their template arguments
+        (e.g. "pool_kernel<3>"), oldest first; clear=True starts a new record."""
+        cap = 1 << 16
+        while True:
+            buf = C.create_string_buffer(cap)
+            n = lib().snnb_debug_launches(self.h, buf, cap, 0)
+            check(0 if n >= 0 else 1, "snnb_debug_launches")
+            if n < cap:
+                break
+            cap = n + 1
+        names = buf.value.decode().splitlines()
+        if clear:
+            lib().snnb_debug_launches(self.h, buf, 1, 1)
+        return names
+
     @property
     def stream(self):
         return lib().snnb_context_stream(self.h)

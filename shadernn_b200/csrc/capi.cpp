@@ -234,6 +234,19 @@ int snnb_debug_last_conv_variant(snnb_context* ctx, int out[6]) {
     for (int i = 0; i < 6; ++i) out[i] = ctx->last_conv[i];
     return 0;
 }
+int snnb_debug_launches(snnb_context* ctx, char* buf, int cap, int clear) {
+    if (!ctx || !buf || cap < 1) {
+        set_error("snnb_debug_launches: context %p, buffer %p of %d bytes", (void*) ctx, (void*) buf, cap);
+        return -1;
+    }
+    const std::string& log = ctx->launch_log;
+    const size_t n         = std::min(log.size(), (size_t) cap - 1);
+    std::copy(log.data(), log.data() + n, buf);
+    buf[n] = '\0';
+    const int len = (int) log.size();
+    if (clear) ctx->launch_log.clear();
+    return len;
+}
 int snnb_tensor_planes(const snnb_tensor* t, void** hi, void** lo, int* cp) {
     SNNB_REQUIRE(t && hi && lo && cp, "snnb_tensor_planes: null argument");
     *hi = t->hi, *lo = t->lo, *cp = t->cp;

@@ -152,6 +152,8 @@ bool MixedInferenceCore::init(std::string& err) {
                 if (pool->typeName == "AveragePooling2D" && static_cast<PoolingLayer*>(pool)->isAvg && pool->nextLayers.size() == 1 && pool->prevLayers.size() == 1 &&
                     !pool->fusedAway && dimsOf(pool).width * dimsOf(pool).height == 1 && static_cast<DenseLayer*>(L)->units <= 256 &&
                     dimsOf(pool->prevLayers[0]).width * dimsOf(pool->prevLayers[0]).height >= 4 && dimsOf(pool->prevLayers[0]).depth <= 4096 &&
+                    // a head that does not fit the kernel's shared memory runs as pool + Dense: the pool must then write its tensor
+                    gap_dense_parts((int) dimsOf(pool->prevLayers[0]).depth, (int) static_cast<DenseLayer*>(L)->units) > 0 &&
                     static_cast<PoolingLayer*>(pool)->_desc.kernelSize >= dimsOf(pool->prevLayers[0]).width &&
                     static_cast<PoolingLayer*>(pool)->_desc.kernelSize >= dimsOf(pool->prevLayers[0]).height) {
                     static_cast<DenseLayer*>(L)->gapSource = pool->prevLayers[0];

@@ -429,8 +429,9 @@ int launch_depthwise(snnb_context* ctx, const ConvArgs& a) {
         const int strips      = (a.out->w + TX - 1) / TX;
         const long long total = (long long) a.out->n * a.out->h * strips * CG;
         const unsigned blocks = (unsigned) ((total + 127) / 128);
-        if (a.stride == 1) return launch_done(ctx, launch_k(depthwise_kernel<3, 1, TX>, dim3(blocks), dim3(128), 0, ctx->stream, p), "depthwise_kernel");
-        return launch_done(ctx, launch_k(depthwise_kernel<3, 2, TX>, dim3(blocks), dim3(128), 0, ctx->stream, p), "depthwise_kernel");
+        static_assert(TX == 4, "the launch names below spell TX");
+        if (a.stride == 1) return launch_done(ctx, launch_k(depthwise_kernel<3, 1, TX>, dim3(blocks), dim3(128), 0, ctx->stream, p), "depthwise_kernel<3, 1, 4>");
+        return launch_done(ctx, launch_k(depthwise_kernel<3, 2, TX>, dim3(blocks), dim3(128), 0, ctx->stream, p), "depthwise_kernel<3, 2, 4>");
     }
     const long long total = (long long) a.out->n * a.out->h * a.out->w * CG;
     return launch_done(ctx, launch_k(depthwise_generic_kernel, dim3((unsigned) ((total + 127) / 128)), dim3(128), 0, ctx->stream, p), "depthwise_generic_kernel");
@@ -651,12 +652,13 @@ __global__ void __launch_bounds__(GD_THREADS) gap_dense_kernel(TV in, TV out, co
     for (int oc = threadIdx.x; oc < out.Cp; oc += blockDim.x) store1(out.hi, out.lo, (size_t) n * out.Cp + oc, oc < out.C ? logits[oc] : 0.0f);
 }
 
-// pixel ranges per channel group, limited by the 48 KB of shared memory available without opt-in; 0 = does not fit
-static int gap_dense_parts(const snnb_tensor* in, const snnb_tensor* out) {
-    int parts = std::max(1, std::min(GD_THREADS / (in->cp >> 3), 8));
-    while (parts > 1 && (size_t) (parts * in->cp + (GD_THREADS / 32 + 1) * out->cp) * sizeof(float) > 48 * 1024) --parts;
-    return (size_t) (parts * in->cp + (GD_THREADS / 32 + 1) * out->cp) * sizeof(float) > 48 * 1024 ? 0 : parts;
+int gap_dense_parts(int in_c, int out_c) {
+    const int icp = round_up(in_c, 8), ocp = round_up(out_c, 8);
+    int parts = std::max(1, std::min(GD_THREADS / (icp >> 3), 8));
+    while (parts > 1 && (size_t) (parts * icp + (GD_THREADS / 32 + 1) * ocp) * sizeof(float) > 48 * 1024) --parts;
+    return (size_t) (parts * icp + (GD_THREADS / 32 + 1) * ocp) * sizeof(float) > 48 * 1024 ? 0 : parts;
 }
+static int gap_dense_parts(const snnb_tensor* in, const snnb_tensor* out) { return gap_dense_parts(in->cp, out->cp); }
 bool gap_dense_supported(const snnb_tensor* in, const snnb_tensor* out, const snnb_weights* w) {
     return w && w->w_f32 && in->h * in->w >= 4 && in->cp <= 4096 && out->c <= 256 && out->h * out->w == 1 && in->n == out->n && gap_dense_parts(in, out) > 0;
 }
@@ -678,11 +680,9 @@ int launch_pool(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, int 
     }
     const long long total = (long long) out->n * out->h * out->w * (out->cp >> 3);
     const dim3 grid((unsigned) ((total + 255) / 256));
-    cudaError_t e;
-    if (k == 2) e = launch_k(pool_kernel<2>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
-    else if (k == 3) e = launch_k(pool_kernel<3>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
-    else e = launch_k(pool_kernel<0>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0);
-    return launch_done(ctx, e, "pool_kernel");
+    if (k == 2) return launch_done(ctx, launch_k(pool_kernel<2>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0), "pool_kernel<2>");
+    if (k == 3) return launch_done(ctx, launch_k(pool_kernel<3>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0), "pool_kernel<3>");
+    return launch_done(ctx, launch_k(pool_kernel<0>, grid, dim3(256), 0, ctx->stream, vi, vo, k, stride, avg ? 1 : 0), "pool_kernel<0>");
 }
 
 // ------------------------------------------------------------------------------------------------------------

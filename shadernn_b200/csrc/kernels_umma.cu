@@ -1333,7 +1333,8 @@ template <int S> static int launch_depthwise_tma_s(snnb_context* ctx, const Conv
     if (ensure_smem_attr(ctx, (const void*) depthwise_tma_kernel<S>, S == 1 ? ATTR_DW1 : ATTR_DW2, T::SMEM_BYTES)) return 1;
     const long long total = (long long) p.N * p.tiles_y * p.tiles_x * p.chunks;
     const int grid        = (int) std::min<long long>(total, 2 * ctx->sm_count); // two CTAs per SM (128 registers, <= 93 KB of shared memory each)
-    return launch_done(ctx, launch_k_pdl(depthwise_tma_kernel<S>, dim3(grid), dim3(DW_THREADS), T::SMEM_BYTES, ctx->stream, tmI[0], tmI[1], p), "depthwise_tma_kernel");
+    return launch_done(ctx, launch_k_pdl(depthwise_tma_kernel<S>, dim3(grid), dim3(DW_THREADS), T::SMEM_BYTES, ctx->stream, tmI[0], tmI[1], p),
+                       S == 1 ? "depthwise_tma_kernel<1>" : "depthwise_tma_kernel<2>");
 }
 
 int launch_depthwise_tma(snnb_context* ctx, const ConvArgs& a) {

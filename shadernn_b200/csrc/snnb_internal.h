@@ -162,6 +162,9 @@ struct snnb_context {
     // stream_k, fks}; zeros before the first one
     int last_conv[6] = {0, 0, 0, 0, 0, 0};
     int precision = SNNB_PRECISION_FP32X3; // default product form of per-operator convolution launches (snnb_context_set_precision)
+    // names of the kernels launched since the last snnb_debug_launches(clear = 1), one per line; at least the most recent
+    // LAUNCH_LOG_BYTES / 2 are kept
+    std::string launch_log;
     std::vector<void*> scratch_blocks;
 };
 
@@ -180,8 +183,11 @@ namespace snnb {
 
 int ensure_stage(snnb_context* ctx, size_t bytes);
 
+constexpr size_t LAUNCH_LOG_BYTES = 64 * 1024;
+
 // Every kernel launch ends here: `launched` is the launch call's result. A failed launch (that result, else cudaGetLastError)
-// is reported under the kernel's name; a successful one is counted in ctx->launches.
+// is reported under the kernel's name; a successful one is counted in ctx->launches and its name, with the template arguments of
+// the instantiation, appended to ctx->launch_log (snnb_debug_launches).
 static inline int launch_done(snnb_context* ctx, cudaError_t launched, const char* kernel) {
     const cudaError_t e = launched != cudaSuccess ? launched : cudaGetLastError();
     if (e != cudaSuccess) {
@@ -189,6 +195,10 @@ static inline int launch_done(snnb_context* ctx, cudaError_t launched, const cha
         return 1;
     }
     ctx->launches++;
+    std::string& log = ctx->launch_log;
+    log.append(kernel).push_back('\n');
+    // past the cap, the older half goes at once (whole names): the erase's copy is paid once per ~LAUNCH_LOG_BYTES / 2 bytes of names
+    if (log.size() > LAUNCH_LOG_BYTES) log.erase(0, log.find('\n', log.size() - LAUNCH_LOG_BYTES / 2) + 1);
     return 0;
 }
 
@@ -213,6 +223,9 @@ int launch_depthwise_tma(snnb_context* ctx, const ConvArgs& a);
 int launch_pool(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, int k, int stride, bool avg);
 // global average pool -> Dense (+ activation / softmax) in one launch (small classifier heads)
 bool gap_dense_supported(const snnb_tensor* in, const snnb_tensor* out, const snnb_weights* w);
+// pixel ranges per channel group of the head for in_c input and out_c output channels, limited by the 48 KB of shared memory available
+// without opt-in; 0 = it does not fit (the engine then keeps the pool and the Dense apart)
+int gap_dense_parts(int in_c, int out_c);
 int launch_gap_dense(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, const snnb_weights* w, int act, float alpha, bool softmax);
 int launch_add(snnb_context* ctx, const snnb_tensor* a, const snnb_tensor* b, snnb_tensor* out, int act, float alpha);
 int launch_batchnorm(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out, const snnb_weights* w, int act, float alpha);

@@ -313,6 +313,10 @@ def restate(om, i, outs, kernels, precision, half, x, at=None):
     if t == "Activation":
         return exact.activation(a, act, float(l.get("leakyReluAlpha", 0.3)), half, at)
     if t == "Flatten":
+        if act == "softmax":  # flatten_kernel, then softmax_kernel in place on the stored copy
+            flat = exact.flatten(a)[0]
+            ref, bound = exact.softmax(flat.reshape(n, -1), half)
+            return ref.reshape(flat.shape), bound.reshape(flat.shape)
         if act not in ("", "linear"):
             return None
         return exact.flatten(a)
@@ -328,8 +332,8 @@ def restate(om, i, outs, kernels, precision, half, x, at=None):
         return exact.concat(a, outs[ins[1]], at)
     if t == "UpSampling2D":
         if l.get("interpolation") == "bilinear":
-            return None
-        return exact.upsample_nearest(a, shape[1:3], at)
+            return exact.upsample_bilinear(a, float(l["scaleFactor"]), shape[1:3], half, at)
+        return exact.upsample_nearest(a, shape[1:3], at, scale=float(l["scaleFactor"]))
     if t == "Pad":
         if "pads" in l:
             p = l["pads"]
