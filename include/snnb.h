@@ -220,7 +220,9 @@ int snnb_model_set_batch(snnb_model* m, int n);
 int snnb_model_set_count_batches(snnb_model* m, const int* sizes, int num_sizes);
 /* MixedInferenceCore::run (core.cpp:97-245), end to end with HOST buffers: H2D of the NHWC fp32 batch (the model's batch), forward,
  * D2H of output 0 (NHWC fp32, out_capacity floats) and, for classifiers (last layer Dense/softmax), the 1-based
- * class index per image (core.cpp:228-233); classes may be NULL. Synchronous. */
+ * class index per image (core.cpp:228-233); classes may be NULL. Synchronous.
+ * Every class index of this API (classes_1based, classes_1based_dev, snnb_argmax1) is std::max_element's index + 1, NaN scores
+ * included: 1 when score 0 is NaN or no score is a number, otherwise 1 + the first maximum of the scores that are numbers. */
 int snnb_model_run(snnb_model* m, const float* host_input_nhwc, float* host_output, size_t out_capacity, int* classes_1based);
 /* Streaming variant of snnb_model_run for serving loops: submit() enqueues the H2D copy of the batch (on a dedicated copy
  * stream, double-buffered device staging), the forward pass and the D2H copies of output 0 / class indices into the

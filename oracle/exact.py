@@ -78,14 +78,27 @@ def store_bound(y, half):
     return np.abs(y) * (2.0 ** -11 if half else 2.0 ** -22) * SLACK + 2.0 ** -25
 
 
+FP16_MAX = 65504.0
+
+
+def sat16(v):
+    """cvt.rn.satfinite.f16.f32 of fp32 values, back in float32: round to nearest even, then values past fp16's range (infinities
+    included) saturate to +-65504; NaN stays NaN."""
+    with np.errstate(over="ignore"):
+        h = np.asarray(v, np.float32).astype(np.float16).astype(np.float32)
+    return np.clip(h, np.float32(-FP16_MAX), np.float32(FP16_MAX))  # np.clip keeps NaN
+
+
 def stored(v, half):
-    """What the storage makes of fp32 values v: hi + lo (split-fp16) or fp16 alone, as float32. Saturation at +-65504 is not
-    modelled; callers keep their values inside fp16's range."""
+    """What the storage makes of fp32 values v: hi + lo (split-fp16) or fp16 alone, as float32. Both planes saturate
+    (store8's cvt.rn.satfinite): hi holds at most +-65504, lo = sat(v - hi) as well, so split-fp16 holds at most +-131008 and fp16
+    storage +-65504. NaN stays NaN."""
     v = np.asarray(v, np.float32)
-    hi = v.astype(np.float16).astype(np.float32)
+    hi = sat16(v)
     if half:
         return hi
-    return hi + (v - hi).astype(np.float16).astype(np.float32)
+    with np.errstate(invalid="ignore"):
+        return hi + sat16(v - hi)
 
 
 def act64(v, act, alpha):
@@ -552,6 +565,128 @@ def model_input(x, half, at=None):
     """The input upload (split_f32_kernel, and the stem's feed copy): fp32 -> hi + lo, or fp16 alone. Restated exactly."""
     y = stored(elementwise_operand(np.asarray(x, np.float32), at), half)
     return y.astype(np.float64), np.zeros(y.shape)
+
+
+def resize_coord(o, out, src, centre):
+    """(P, e) of output texels o along an axis of `out` texels sampling `src`: P the exact source position (o + 0.5) src / out, less
+    0.5 for the texel-centre convention of the linear filter (centre=True); e a bound of the error of resize_pos's fp32 position
+    fl(fl((o + 0.5) / out) * src) (- 0.5): the division and the product round once each (u P each), and the subtraction rounds
+    once unless the compiler contracted it with the product into an FMA (u |P - 0.5|)."""
+    o = np.asarray(o, np.float64)
+    p = (2 * o + 1) * src / (2.0 * out)
+    if not centre:
+        return p, U * 2 * p * SLACK
+    return p - 0.5, U * (2 * p + np.abs(p - 0.5)) * SLACK
+
+
+def resize_u8(images_u8, out_hw, mean4, norm4, linear, half):
+    """ImageTexture::resize (core/inc/snn/imageTexture.h:137, the sampler of shadertemplate_vk_resize.comp) of 8-bit NHWC images to
+    out_hw, then (v - mean[c & 3]) * norm[c & 3] and the store: the model input of resize_u8_kernel and frame_input_kernel (and of
+    split_u8_kernel / device_input_kernel<u8> at equal size, where every position is a texel centre). Stated from the definition,
+    not from the kernels' order of operations. Returns (ref, bound) [n, oh, ow, c].
+
+    Linear: output texel o samples the source at the exact position X = (o + 0.5) src / out - 0.5 in texel-centre units, the
+    bilinear interpolant of the texels clamped to the edge (continuous and piecewise bilinear). The kernel evaluates it at its fp32
+    position (resize_coord: error e_x, e_y), which moves the value by at most e_x times the largest difference of horizontal
+    neighbours in the rows and cells the position may fall in (columns floor(X) - 1 .. floor(X) + 2, rows floor(Y) - 1 .. floor(Y) + 2,
+    clamped), plus e_y likewise: the same argument as upsample_bilinear. The weights ax = sx - floor(sx) are exact. The blend
+    (two lerps along x, one along y, separate or fused multiply-adds; the tap differences of integers are exact) rounds by at most
+    7 u max|tap|: 2 u M for each of top and bottom, carried through the final lerp with weights (1 - ay) and ay, plus 2 u M for its
+    difference and product and u M for its sum.
+
+    Nearest: texel floor(P), P = (o + 0.5) src / out, clamped to src - 1; no blend. Where P lies within the fp32 position's error of
+    an integer k, the kernel may take k - 1 or k: ref is then the midpoint of the candidate taps' values and bound half their
+    spread (nearest_candidates gives the candidates themselves, for a check that the value is one of them); everywhere else the tap
+    is unique and the value must be bit-identical to its normalised fp32 value (the subtraction and the product are two roundings,
+    restated exactly in float32) and its store.
+
+    Normalisation (linear): (v - mean) * norm rounds twice, u |v - mean| |norm| + u |ref|, on top of |norm| times v's error. Then
+    store_bound (nothing saturates: the values stay far inside fp16's range for 8-bit inputs and sane constants)."""
+    img = np.asarray(images_u8, np.uint8)
+    n, sh, sw, c = img.shape
+    oh, ow = out_hw
+    mean = np.array([np.float32(mean4[i & 3]) for i in range(c)], np.float32)
+    norm = np.array([np.float32(norm4[i & 3]) for i in range(c)], np.float32)
+    if not linear:
+        vals = nearest_candidates(img, out_hw, mean, norm, half)
+        lo, hi = np.minimum.reduce(vals), np.maximum.reduce(vals)
+        return (lo + hi) / 2, (hi - lo) / 2
+    X, ex = resize_coord(np.arange(ow), ow, sw, centre=True)
+    Y, ey = resize_coord(np.arange(oh), oh, sh, centre=True)
+    xf, yf = np.floor(X).astype(np.int64), np.floor(Y).astype(np.int64)
+    ax, ay = (X - xf)[None, None, :, None], (Y - yf)[None, :, None, None]
+
+    def tap(dy, dx):
+        return img[:, np.clip(yf + dy, 0, sh - 1)][:, :, np.clip(xf + dx, 0, sw - 1)].astype(np.float64)
+    p00, p01, p10, p11 = tap(0, 0), tap(0, 1), tap(1, 0), tap(1, 1)
+    v = (1 - ay) * ((1 - ax) * p00 + ax * p01) + ay * ((1 - ax) * p10 + ax * p11)
+    dx = np.zeros(v.shape)
+    dy = np.zeros(v.shape)
+    for r in range(-1, 3):
+        for q in range(-1, 3):
+            t = tap(r, q)
+            dx = np.maximum(dx, np.abs(tap(r, q + 1) - t))
+            dy = np.maximum(dy, np.abs(tap(r + 1, q) - t))
+    mag = np.maximum.reduce([np.abs(p00), np.abs(p01), np.abs(p10), np.abs(p11)])
+    e_v = (ex[None, None, :, None] * dx + ey[None, :, None, None] * dy + 7 * U * mag) * SLACK
+    d = v - mean.astype(np.float64)
+    ref = d * norm.astype(np.float64)
+    bound = (np.abs(norm) * (e_v + U * np.abs(d)) + U * np.abs(ref)) * SLACK + store_bound(ref, half)
+    return ref, bound
+
+
+def nearest_candidates(images_u8, out_hw, mean, norm, half):
+    """The values the nearest filter may take at each output texel (resize_u8): the normalised, stored value of texel floor(P) along
+    each axis, or of k - 1 and k where P lies within the fp32 position's error of an integer k. Four arrays [n, oh, ow, c] (equal
+    where the tap is unique); a nearest kernel's output must equal one of them bit for bit. mean, norm: per channel, fp32."""
+    img = np.asarray(images_u8, np.uint8)
+    n, sh, sw, c = img.shape
+
+    def taps(out, src):
+        p, e = resize_coord(np.arange(out), out, src, centre=False)
+        k = np.floor(p + 0.5)
+        lo = np.minimum(np.floor(p), src - 1)
+        near = (np.abs(p - k) <= e) & (k >= 1)
+        return np.where(near, np.minimum(k, src - 1), lo).astype(np.int64), np.where(near, np.minimum(k - 1, src - 1), lo).astype(np.int64)
+    ys, xs = taps(out_hw[0], sh), taps(out_hw[1], sw)
+    mean, norm = np.asarray(mean, np.float32), np.asarray(norm, np.float32)
+    return [stored((img[:, yy][:, :, xx].astype(np.float32) - mean) * norm, half).astype(np.float64) for yy in ys for xx in xs]
+
+
+def quant_u8(v, scale, offset):
+    """quant_u8 (kernels_simt.cu: every 8-bit output) of stored values v: clamp(rint(v scale + offset), 0, 255), stated in float64 from
+    the fp32 operands, rint rounding half to even as rintf does. The kernel forms v scale + offset in fp32 (two roundings, or one where
+    the compiler contracts them into an FMA): within e = u (|v scale| + |t|) of the exact t, and exact where v scale and t are fp32
+    numbers. Where t lies within e of a half-integer, the byte may be either neighbour: ref is then the midpoint of the two candidate
+    bytes and bound 1/2; everywhere else bound = 0 and the byte must match. NaN gives 0: rintf(NaN) is NaN, fmaxf(NaN, 0) = 0.
+    Returns (ref, bound) as float64 arrays of v's shape."""
+    v = np.asarray(v, np.float32).astype(np.float64)
+    s, o = float(np.float32(scale)), float(np.float32(offset))
+    with np.errstate(invalid="ignore", over="ignore"):
+        prod = v * s  # exact in float64: two 24-bit significands
+        t = prod + o
+        exact_fp32 = (np.float32(prod).astype(np.float64) == prod) & (np.float32(t).astype(np.float64) == t)
+        e = np.where(exact_fp32, 0.0, U * (np.abs(prod) + np.abs(t)) * SLACK)
+        k = np.floor(t)
+        near = (np.abs(t - (k + 0.5)) <= e) & (e > 0)  # either neighbour of the half-integer k + 0.5
+        b0 = np.clip(np.where(near, k, np.rint(t)), 0, 255)
+        b1 = np.clip(np.where(near, k + 1, np.rint(t)), 0, 255)
+    nan = np.isnan(v)
+    b0, b1 = np.where(nan, 0.0, b0), np.where(nan, 0.0, b1)
+    return (b0 + b1) / 2, (b1 - b0) / 2
+
+
+def argmax(x):
+    """std::max_element's index over the last axis (the reference's classes, core.cpp:230-232), per image: x[..., C] -> int64 [...].
+    max_element keeps the running maximum and moves on only when it compares below a later score, so: index 0 when score 0 is NaN
+    (nothing compares above a NaN) and when no score is a number; otherwise the first maximum of the scores that are numbers (a later
+    NaN never compares above the running maximum). Returns (ref, bound) with bound 0: the index must match."""
+    x = np.asarray(x, np.float64)
+    x = x.reshape(-1, x.shape[-1]) if x.ndim > 1 else x[None]
+    num = np.where(np.isnan(x), -np.inf, x)
+    idx = np.argmax(num, axis=-1)  # the first maximum; a row of -inf and NaN only gives 0
+    idx = np.where(np.isnan(x[:, 0]), 0, idx)
+    return idx, np.zeros(idx.shape)
 
 
 def check(got, ref, bound, what):

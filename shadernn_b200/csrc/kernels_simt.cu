@@ -745,7 +745,7 @@ int launch_activation(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out
 // ------------------------------------------------------------------------------------------------------------
 // Softmax over channels, per pixel (cpulayer.h:175-191: max-subtracted, fp32). One warp per pixel.
 // Argmax over channels per image -> index of the FIRST maximum plus base_index (0 where the host adds 1 at the API,
-// core.cpp:228-233; 1 where the 1-based classes stay in device memory).
+// core.cpp:228-233; 1 where the 1-based classes stay in device memory). NaN scores: argmax_take below.
 // ------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) softmax_kernel(TV in, TV out) {
     pdl_wait();
@@ -769,24 +769,40 @@ int launch_softmax(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out) {
     return launch_done(ctx, launch_k(softmax_kernel, dim3((unsigned) ((px * 32 + 127) / 128)), dim3(128), 0, ctx->stream, view(in), view(out)), "softmax_kernel");
 }
 
+// The index is std::max_element's (the reference's core.cpp:230-232) for every input, NaN included: 0 when score 0 is NaN (no score
+// compares above it) or when no score is a number; otherwise the first maximum of the scores that are numbers (a later NaN never
+// compares above the running maximum). So the index is always in [0, C) and the + 1 of the 1-based classes cannot overflow.
+// A lane scans channels lane, lane + 32, ... in order; ARGMAX_NONE marks a lane that has seen no number yet.
+constexpr int ARGMAX_NONE = 0x7fffffff;
+__device__ __forceinline__ void argmax_take(float& best, int& bi, float v, int c) {
+    if (v == v && (bi == ARGMAX_NONE || v > best)) best = v, bi = c;
+}
+// The warp's first maximum from the lanes' (best, bi): the larger value, on ties the smaller index; lanes without a number lose.
+// lane 0 returns the image's index, nan0: score 0 is NaN.
+__device__ __forceinline__ int argmax_warp(float best, int bi, bool nan0) {
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi   = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (oi != ARGMAX_NONE && (bi == ARGMAX_NONE || ob > best || (ob == best && oi < bi))) best = ob, bi = oi;
+    }
+    return (nan0 || bi == ARGMAX_NONE) ? 0 : bi;
+}
 __global__ void __launch_bounds__(128) argmax_kernel(TV in, int* __restrict__ idx, int base_index) {
     pdl_wait();
     const int n    = (int) (((long long) blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const int lane = threadIdx.x & 31;
     if (n >= in.N) return;
     const size_t base = (size_t) n * in.H * in.W * in.Cp;
-    float best = -3.402823466e+38f;
-    int bi     = 0x7fffffff;
+    float best = 0.0f;
+    int bi     = ARGMAX_NONE;
+    bool nan0  = false;
     for (int c = lane; c < in.C; c += 32) {
-        float v = load1(in.hi, in.lo, base + c);
-        if (v > best) best = v, bi = c;
+        const float v = load1(in.hi, in.lo, base + c);
+        if (c == 0) nan0 = v != v;
+        argmax_take(best, bi, v, c);
     }
-    for (int o = 16; o > 0; o >>= 1) {
-        float ob = __shfl_xor_sync(0xffffffffu, best, o);
-        int oi   = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ob > best || (ob == best && oi < bi)) best = ob, bi = oi;
-    }
-    if (lane == 0) idx[n] = bi + base_index;
+    const int i = argmax_warp(best, bi, nan0);
+    if (lane == 0) idx[n] = i + base_index;
 }
 // Classifier result in one launch: fp32 values of a 1x1xC tensor and/or the arg-max per image, written wherever the pointers point -
 // the streaming path hands in MAPPED PINNED HOST memory, so a small result needs no device->host copy commands at all.
@@ -796,20 +812,18 @@ __global__ void __launch_bounds__(128) result_small_kernel(TV in, float* __restr
     const int lane = threadIdx.x & 31;
     if (n >= in.N) return;
     const size_t base = (size_t) n * in.Cp; // H = W = 1
-    float best = -3.402823466e+38f;
-    int bi     = 0x7fffffff;
+    float best = 0.0f;
+    int bi     = ARGMAX_NONE;
+    bool nan0  = false;
     for (int c = lane; c < in.C; c += 32) {
         const float v = load1(in.hi, in.lo, base + c);
         if (values) values[(size_t) n * in.C + c] = v;
-        if (v > best) best = v, bi = c;
+        if (c == 0) nan0 = v != v;
+        argmax_take(best, bi, v, c);
     }
     if (!idx) return;
-    for (int o = 16; o > 0; o >>= 1) { // same order as argmax_kernel: the larger value, on ties the smaller index
-        float ob = __shfl_xor_sync(0xffffffffu, best, o);
-        int oi   = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ob > best || (ob == best && oi < bi)) best = ob, bi = oi;
-    }
-    if (lane == 0) idx[n] = bi;
+    const int i = argmax_warp(best, bi, nan0); // argmax_kernel's scan and reduction, so the two agree on every input
+    if (lane == 0) idx[n] = i;
 }
 int launch_result_small(snnb_context* ctx, const snnb_tensor* in, float* values, int* idx) {
     SNNB_REQUIRE(in->h == 1 && in->w == 1, "launch_result_small: a 1x1 tensor is expected");
