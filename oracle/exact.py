@@ -737,3 +737,286 @@ def instancenorm(x, gamma_c, beta_c, act="", alpha=0.0, half_out=False, at=None)
     ref = act64(pre, act, alpha)
     bound = act_bound(pre, e_pre, ref, act, alpha) * SLACK + store_bound(ref, half_out)
     return shaped(ref, at, n, h, w), shaped(bound, at, n, h, w)
+
+
+# ---- YOLO decode, score order and NMS (yolo_select / yolo_rank / yolo_nms kernels; layers.cpp decodeCell, iou, nms) ------------
+# Two statements of the same decode. yolo_contract is the float32 arithmetic the kernels promise (kernels_simt.cu, snnb.h): every
+# + - * / one IEEE-rounded fp32 operation in the host's order, no FMA, exp = (float) exp((double) x), > against 0.35f and 0.45f,
+# std::max / std::min as written, keys ordered by (score bits, -scan). The device must match it bit for bit. yolo_define is the
+# mathematical decode in float64 with a bound on every value, from first-order propagation of u = 2^-24 per operation and one fp32
+# ulp per exp (so glibc's expf on the host path is covered too); yolo_decisions uses it to check the contract's threshold, order and
+# suppression decisions wherever the float64 margin exceeds the bound, and never decides one inside it.
+YOLO_SCALE = (32, 16)
+YOLO_ANCHORS = (10, 14, 23, 27, 37, 58, 81, 82, 135, 169, 344, 319)
+YOLO_MASKS = (3, 4, 5, 1, 2, 3)
+YOLO_CONF, YOLO_IOU = np.float32(0.35), np.float32(0.45)
+FLT_MAX = np.float32(3.402823466e+38)
+F32_OVERFLOW = (2.0 - 2.0 ** -24) * 2.0 ** 127  # the smallest real that rounds to +inf in fp32
+EXP_REL, EXP_ABS = 2.0 ** -23, 2.0 ** -149     # one fp32 ulp of an exp: relative, and at fp32's subnormals
+
+
+def yolo_cells(h0, h1, pitch=(None, None)):
+    """The six values of every (cell, anchor) of two heads [N, gh, gw, C], C >= 18, in the kernels' scan order (head, gy, gx, gc).
+    pitch: the channel pitch each head is read with (default its C). Returns a dict of d [N, S, 6] float32 and, per scan index, yi,
+    gx, gy, gc, gw, gh (int64 [S])."""
+    d, meta = [], {k: [] for k in ("yi", "gx", "gy", "gc", "gw", "gh")}
+    for yi, h in enumerate((h0, h1)):
+        h = np.asarray(h, np.float32)
+        n, gh, gw, c = h.shape
+        p = pitch[yi] or c
+        cell = np.repeat(np.arange(gh * gw), 3)
+        gc = np.tile(np.arange(3), gh * gw)
+        flat = h.reshape(n, -1)
+        d.append(flat[:, (cell * p + gc * 6)[:, None] + np.arange(6)])
+        for k, v in (("yi", np.full(cell.size, yi)), ("gx", cell % gw), ("gy", cell // gw), ("gc", gc), ("gw", np.full(cell.size, gw)),
+                     ("gh", np.full(cell.size, gh))):
+            meta[k].append(v)
+    out = {k: np.concatenate(v).astype(np.int64) for k, v in meta.items()}
+    out["d"] = np.concatenate(d, axis=1)
+    return out
+
+
+def exp_cr(x):
+    """(float) exp((double) x) of fp32 values, and a flag where exp(x) lies within 4 double ulps of an fp32 rounding midpoint: there
+    numpy's float64 exp does not decide the correctly rounded result, so either neighbour is right."""
+    with np.errstate(over="ignore", invalid="ignore", under="ignore"):
+        y = np.exp(np.asarray(x, np.float32).astype(np.float64))
+        r = y.astype(np.float32)
+        up, dn = np.nextafter(r, np.float32(np.inf)), np.nextafter(r, np.float32(0))
+        r64 = r.astype(np.float64)
+        gap = np.minimum(np.abs(y - (r64 + up.astype(np.float64)) / 2), np.where(dn != r, np.abs(y - (r64 + dn.astype(np.float64)) / 2), np.inf))
+        near = np.isfinite(r) & np.isfinite(up) & (gap <= 4 * np.spacing(np.abs(y)))
+    return r, near
+
+
+def yolo_score32(d4, d5, exp=exp_cr):
+    """prob = 1.f / ((1.f + exp(-d4) * (1.f + exp(-maxLogit)))) in fp32, maxLogit = d5 > -3.402823466e+38f ? d5 : -3.402823466e+38f.
+    Returns (score, near flag of exp(-d4), near flag of exp(-maxLogit))."""
+    f = np.float32
+    d4, d5 = np.asarray(d4, f), np.asarray(d5, f)
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        ml = np.where(d5 > -FLT_MAX, d5, -FLT_MAX)
+        e4, n4 = exp(-d4)
+        e5, n5 = exp(-ml)
+        return (f(1) / (f(1) + e4 * (f(1) + e5))).astype(f), n4, n5
+
+
+def yolo_decode32(c, exp=exp_cr):
+    """decodeCell in fp32 for every cell of yolo_cells(...) c: returns cls [N, S] int64, score [N, S], box [N, S, 4] = (x, y, w, h)
+    float32 (evaluated everywhere; meaningful where score > 0.35f) and near [N, S], the exp_cr flag over the exps the cell evaluates."""
+    f = np.float32
+    d = c["d"]
+    score, n4, n5 = yolo_score32(d[..., 4], d[..., 5], exp)
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        a = np.array(YOLO_ANCHORS, f)[np.array(YOLO_MASKS)[c["gc"] + 3 * c["yi"]][:, None] * 2 + np.arange(2)]
+        net = (np.array(YOLO_SCALE)[c["yi"]][:, None] * np.stack([c["gw"], c["gh"]], 1)).astype(f)
+        g = np.stack([c["gx"], c["gy"]], 1).astype(f)
+        s0, n0 = exp(-d[..., 0:2])
+        cxy = (g + f(1) / (f(1) + s0)) / np.stack([c["gw"], c["gh"]], 1).astype(f)
+        e2, n2 = exp(d[..., 2:4])
+        wh = e2 * a / net
+        box = np.concatenate([cxy - wh / f(2), wh], axis=-1).astype(f)
+    passed = score > YOLO_CONF
+    near = n4 | n5 | (passed & (n0.any(-1) | n2.any(-1)))
+    return np.zeros(score.shape, np.int64), score.astype(f), box, near
+
+
+def yolo_iou32(a, b):
+    """iou (layers.cpp) of boxes a and b [..., 4], broadcast, in fp32: std::max(p, q) = p < q ? q : p, std::min(p, q) = q < p ? q : p."""
+    ax, ay, aw, ah = (a[..., k] for k in range(4))
+    bx, by, bw, bh = (b[..., k] for k in range(4))
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        ix0, iy0 = np.where(ax < bx, bx, ax), np.where(ay < by, by, ay)
+        ax1, bx1, ay1, by1 = ax + aw, bx + bw, ay + ah, by + bh
+        ix1, iy1 = np.where(bx1 < ax1, bx1, ax1), np.where(by1 < ay1, by1, ay1)
+        r = ((ix1 - ix0) * (iy1 - iy0)) / ((aw * ah + bw * bh) - (ix1 - ix0) * (iy1 - iy0))
+    return np.where((ix1 < ix0) | (iy1 < iy0), np.float32(0), r).astype(np.float32)
+
+
+def yolo_nms32(box, cls, max_rows):
+    """Greedy NMS of a score-ordered list (yolo_greedy_nms, nms): a box is kept unless a kept box before it of the same class has
+    IoU > 0.45 with it, up to max_rows kept boxes. Returns the kept positions."""
+    alive = np.ones(len(box), bool)
+    kept, i = [], 0
+    while len(kept) < max_rows:
+        nxt = np.flatnonzero(alive[i:])
+        if not nxt.size:
+            break
+        i += int(nxt[0])
+        kept.append(i)
+        alive[i + 1:] &= ~((yolo_iou32(box[i], box[i + 1:]) > YOLO_IOU) & (cls[i + 1:] == cls[i]))
+        i += 1
+    return np.array(kept, np.int64)
+
+
+def yolo_contract(h0, h1, max_rows=100):
+    """The device decode of two heads [N, gh, gw, C] (C >= 18, any two grids): netW = 32 gw, netH = 32 gh on head 0 and 16 gw, 16 gh
+    on head 1. Returns (rows [N, max_rows, 6] float32 {class, score, x, y, w, h} zero past the count, counts [N], near [N, S] (an exp of
+    the cell within reach of an fp32 midpoint: exp_cr), paths): paths[n] = {"order": the passing scan indices stable-sorted by
+    descending score, "kept": the kept positions in that order}, for yolo_decisions."""
+    c = yolo_cells(h0, h1)
+    cls, score, box, near = yolo_decode32(c)
+    n = score.shape[0]
+    rows, counts, paths = np.zeros((n, max_rows, 6), np.float32), np.zeros(n, np.int64), []
+    for i in range(n):
+        p = np.flatnonzero(score[i] > YOLO_CONF)
+        o = p[np.argsort(-score[i, p], kind="stable")]
+        kept = yolo_nms32(box[i, o], cls[i, o], max_rows)
+        k = o[kept]
+        rows[i, :len(k), 0], rows[i, :len(k), 1], rows[i, :len(k), 2:] = cls[i, k], score[i, k], box[i, k]
+        counts[i] = len(k)
+        paths.append({"order": o, "kept": kept})
+    return rows, counts, near, paths
+
+
+def _f32_range(v, e):
+    """A float64 value v +- e as fp32 makes it: past fp32's range it rounds to +-inf, exactly when the whole interval lies past it,
+    unbounded when it straddles the edge. Non-finite values are exact (what they came from was); a NaN bound is unbounded. Finite
+    values gain 2^-150, the absolute error of an operation rounded into fp32's subnormals (u |v| only holds above them)."""
+    a = np.abs(v)
+    with np.errstate(invalid="ignore"):
+        over = (a == np.inf) | (a - e >= F32_OVERFLOW)
+        strad = ~over & (a + e >= F32_OVERFLOW)
+    v = np.where(over, np.copysign(np.inf, v), v)
+    e = np.where(np.isfinite(v), np.where(strad | np.isnan(e), np.inf, e + 2.0 ** -150), 0.0)
+    return v, e
+
+
+def yolo_define(h0, h1):
+    """The YOLO decode in float64 for every cell of two heads: score = 1 / (1 + e^-d4 (1 + e^-d5)) (the reference's parenthesisation,
+    d5 the max logit as the kernels take it: NaN gives -FLT_MAX), x = (gx + sigma(d0)) / gw - w / 2, y likewise, w = e^d2 bw / netW,
+    h = e^d3 bh / netH. Returns dict of [N, S] float64 arrays score, x, y, w, h, their bounds e_score ... e_h, and the operands
+    (d4, maxLogit) that decide the score. A bound covers any fp32 evaluation that rounds each operation once (u = 2^-24 |result|) and
+    takes each exp within one fp32 ulp (EXP_REL |y| + EXP_ABS), to first order (SLACK); x and y carry absolute bounds, as cx - w / 2
+    can cancel. Values past fp32's range are +-inf (_f32_range)."""
+    c = yolo_cells(h0, h1)
+    d = c["d"].astype(np.float64)
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore", under="ignore"):
+        def ex(x):
+            y = np.exp(x)
+            return _f32_range(y, EXP_REL * y + EXP_ABS)
+
+        def add1(v, e):
+            return _f32_range(1.0 + v, e + U * (1.0 + v))
+
+        def recip(v, e):
+            r = 1.0 / v
+            return _f32_range(r, e / (v * v) + U * np.abs(r))
+
+        ml = np.where(d[..., 5] > -float(FLT_MAX), d[..., 5], -float(FLT_MAX))
+        e4, ee4 = ex(-d[..., 4])
+        p, ep = add1(*ex(-ml))
+        q, eq = _f32_range(e4 * p, e4 * ep + p * ee4 + U * e4 * p)
+        score, e_score = recip(*add1(q, eq))
+        out = {"score": score, "e_score": e_score * SLACK, "d4": c["d"][..., 4], "maxlogit": ml}
+        for k, (dv, g, gs) in enumerate(((d[..., 0], c["gx"], c["gw"]), (d[..., 1], c["gy"], c["gh"]))):
+            sig, esig = recip(*add1(*ex(-dv)))
+            b, eb = _f32_range(g + sig, esig + U * np.abs(g + sig))
+            cen, ecen = _f32_range(b / gs, eb / gs + U * np.abs(b / gs))
+            anchor = np.array(YOLO_ANCHORS, np.float64)[np.array(YOLO_MASKS)[c["gc"] + 3 * c["yi"]] * 2 + k]
+            net = np.array(YOLO_SCALE)[c["yi"]] * gs
+            t, et = ex(d[..., 2 + k])
+            m, em = _f32_range(t * anchor, et * anchor + U * t * anchor)
+            wv, ew = _f32_range(m / net, em / net + U * m / net)
+            xv, exv = _f32_range(cen - wv / 2, ecen + ew / 2 + U * np.abs(cen - wv / 2))
+            out["xy"[k]], out["e_" + "xy"[k]] = xv, exv * SLACK
+            out["wh"[k]], out["e_" + "wh"[k]] = wv, ew * SLACK
+    return out
+
+
+def yolo_iou64(a, ea, b, eb):
+    """iou of float64 boxes a, b [..., 4] (x, y, w, h) with per-coordinate bounds ea, eb, taking std::max / std::min as written (so a
+    NaN or infinity selects as it does in fp32). Returns (iou, bound): the bound covers the boxes anywhere within their bounds and the
+    fp32 evaluation's roundings; max and min move by at most the larger of their operands' errors. ref takes a negative overlap as
+    empty (inter 0); the bound on inter uses the overlaps' magnitudes, so it also covers an fp32 evaluation that finds a small positive
+    overlap where the float64 one is empty, or the reverse. Where an overlap is certainly negative, both return 0 and the bound is 0."""
+    ax, ay, aw, ah = (a[..., k] for k in range(4))
+    bx, by, bw, bh = (b[..., k] for k in range(4))
+    eax, eay, eaw, eah = (ea[..., k] for k in range(4))
+    ebx, eby, ebw, ebh = (eb[..., k] for k in range(4))
+    with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
+        def side(p0, e0, ps, es, q0, f0, qs, fs):
+            lo = np.where(p0 < q0, q0, p0)
+            e_lo = np.maximum(e0, f0)
+            p1, q1 = p0 + ps, q0 + qs
+            e_p1, e_q1 = e0 + es + U * np.abs(p1), f0 + fs + U * np.abs(q1)
+            hi = np.where(q1 < p1, q1, p1)
+            e_hi = np.maximum(e_p1, e_q1)
+            s = hi - lo
+            return s, e_hi + e_lo + U * np.abs(s)
+
+        iw, e_iw = side(ax, eax, aw, eaw, bx, ebx, bw, ebw)
+        ih, e_ih = side(ay, eay, ah, eah, by, eby, bh, ebh)
+        zero = (iw < 0) | (ih < 0)
+        inter = np.where(zero, 0.0, iw * ih)
+        e_inter = np.abs(iw) * e_ih + np.abs(ih) * e_iw + e_iw * e_ih + U * inter
+        A, B = aw * ah, bw * bh
+        eA, eB = aw * eah + ah * eaw + U * A, bw * ebh + bh * ebw + U * B
+        den = A + B - inter
+        e_den = eA + eB + U * np.abs(A + B) + e_inter + U * np.abs(den)
+        iou = inter / den
+        e = e_inter / np.abs(den) + np.abs(inter) * e_den / (den * den) + U * np.abs(iou)
+        e = np.where(np.isfinite(iou), np.where(np.isnan(e), np.inf, e), 0.0)
+        e = np.where((iw < -e_iw) | (ih < -e_ih), 0.0, e)  # fp32 takes the same empty branch
+    return np.where(zero, 0.0, iou), e * SLACK
+
+
+def yolo_decisions(h0, h1, paths, max_rows, defn=None, contract=None):
+    """Every decision on the contract's path (yolo_contract's paths), classified against yolo_define: certain where the float64 margin
+    exceeds its bound, inside-bound otherwise. Decisions: the threshold of every cell (a NaN score is a certain rejection), the order
+    of each adjacent pair of the sorted list (two cells with the same d4 and max logit tie in any evaluation: a certain tie, broken by
+    the scan) and every IoU test of a kept box against a later candidate up to where the walk stops. Returns one dict per image:
+    certain / inside counts per kind, wrong (certain decisions the contract made the other way, as (kind, detail)) and first_uncertain:
+    the first row whose presence or place may depend on an inside-bound decision (the count when none does)."""
+    defn = yolo_define(h0, h1) if defn is None else defn
+    cls, score32, box32, _ = yolo_decode32(yolo_cells(h0, h1)) if contract is None else contract
+    box64 = np.stack([defn[k] for k in "xywh"], -1)
+    ebox = np.stack([defn["e_" + k] for k in "xywh"], -1)
+    res = []
+    for n, path in enumerate(paths):
+        o, kept = path["order"], path["kept"]
+        r = {"certain": {"threshold": 0, "order": 0, "suppress": 0}, "inside": {"threshold": 0, "order": 0, "suppress": 0}, "wrong": []}
+        kept_before = np.concatenate([[0], np.cumsum(np.isin(np.arange(len(o)), kept))])  # kept rows before sorted position p
+        first = len(kept)
+        s64, es = defn["score"][n], defn["e_score"][n]
+        passed = score32[n] > YOLO_CONF
+        margin = s64 - float(YOLO_CONF)
+        nan = np.isnan(s64)
+        sure = nan | (np.abs(margin) > es)
+        r["certain"]["threshold"], r["inside"]["threshold"] = int(sure.sum()), int((~sure).sum())
+        bad = sure & (passed != (margin > es))
+        r["wrong"] += [("threshold", int(s)) for s in np.flatnonzero(bad)]
+        if (~sure).any():  # where an undecided cell would sort: after every passing score above its bound
+            so = score32[n, o].astype(np.float64)
+            for s in np.flatnonzero(~sure):
+                first = min(first, int(kept_before[int(np.sum(so > s64[s] + es[s]))]))
+        if len(o) > 1:
+            a, b = o[:-1], o[1:]
+            m = s64[a] - s64[b]
+            tie = (defn["d4"][n, a] == defn["d4"][n, b]) & (defn["maxlogit"][n, a] == defn["maxlogit"][n, b])
+            sure = tie | (np.abs(m) > es[a] + es[b])
+            r["certain"]["order"], r["inside"]["order"] = int(sure.sum()), int((~sure).sum())
+            # no certain inversion between any two positions: s64[j] - e[j] <= min over i < j of s64[i] + e[i]
+            lo = np.minimum.accumulate(s64[o] + es[o])[:-1]
+            inv = (s64[b] - es[b] > lo) | (tie & (b < a)) | (sure & ~tie & (m < 0))
+            r["wrong"] += [("order", int(p)) for p in np.flatnonzero(inv)]
+            if (~sure).any():
+                first = min(first, int(kept_before[int(np.flatnonzero(~sure)[0])]))
+        stop = int(kept[-1]) + 1 if len(kept) == max_rows else len(o)
+        for k in kept:
+            j = np.arange(k + 1, stop)
+            j = j[cls[n, o[j]] == cls[n, o[k]]]
+            if not j.size:
+                continue
+            iou, e = yolo_iou64(box64[n, o[k]], ebox[n, o[k]], box64[n, o[j]], ebox[n, o[j]])
+            got = yolo_iou32(box32[n, o[k]], box32[n, o[j]]) > YOLO_IOU
+            m = iou - float(YOLO_IOU)
+            sure = np.isnan(iou) | (np.abs(m) > e)
+            r["certain"]["suppress"] += int(sure.sum())
+            r["inside"]["suppress"] += int((~sure).sum())
+            r["wrong"] += [("suppress", (int(k), int(q))) for q in j[sure & (got != (m > e))]]
+            if (~sure).any():
+                first = min(first, int(kept_before[int(j[~sure][0])]))
+        r["first_uncertain"] = first
+        res.append(r)
+    return res

@@ -9,7 +9,7 @@ accumulates with depth, so the bounds are those of one layer's arithmetic.
   device's SM count. The engine never asks for stream-K, so those cases run in a child process with SNNB_SK=1, which makes the
   planner consider it.
 - Whole zoo models in fp32x3, fp16w and fp16, fused and unfused, and on the CUDA-core convolution: every layer with a tensor of
-  its own is restated (only YOLO's host decode is not).
+  its own is restated. The YOLO decode has its own table in test_detect_exact_gpu.py.
 """
 import json
 import os
