@@ -699,13 +699,14 @@ def check(got, ref, bound, what):
     return ratio, bad
 
 
-def instancenorm(x, gamma_c, beta_c, act="", alpha=0.0, half_out=False, at=None):
+def instancenorm(x, gamma_c, beta_c, act="", alpha=0.0, half_out=False, at=None, eps=1e-5):
     """InstanceNorm (instnorm_*_kernel): per (image, channel) mean and biased variance over H W of d = x - x[first pixel], summed in
     fp32 (sum d with adds, sum d^2 with FMAs, any order: gamma_{HW+2}); m = S1 / HW, var = max(S2 / HW - m^2, 0), mean = x0 + m,
     rstd = 1 / sqrtf(var + 1e-5) (correctly rounded sqrt and division), y = (x - mean) * (gamma rstd) + beta, then the activation.
     ref evaluates the same formula in float64 with the exact mean and variance. The bound follows each rounding: e_m of m,
     e_var of the variance, e_r of rstd by the mean value theorem on (v + eps)^-1/2 over [v + eps - e_var, v + eps], then the
-    elementwise part. The statistics always cover the whole plane; at only chooses the output pixels evaluated."""
+    elementwise part. The statistics always cover the whole plane; at only chooses the output pixels evaluated. eps: the kernels' is
+    1e-5 (another value states a different layer, for the converter's checks)."""
     n, h, w, c = np.shape(x)
     hw = h * w
     g = np.asarray(gamma_c, np.float32).astype(np.float64)
@@ -723,10 +724,10 @@ def instancenorm(x, gamma_c, beta_c, act="", alpha=0.0, half_out=False, at=None)
     e_m = e_s1 / hw + U * np.abs(m)
     e_mean = e_m + U * np.abs(mu)
     e_var = (e_s2 / hw + U * s2 / hw) + 2 * np.abs(m) * e_m + e_m * e_m + U * m * m + U * (np.abs(var) + 1e-30)
-    v = var + 1e-5
+    v = var + eps
     r = 1.0 / np.sqrt(v)
     r_lo = 1.0 / np.sqrt(np.maximum(v - e_var * SLACK, 1e-30))
-    e_r = 0.5 * r_lo ** 3 * e_var * SLACK + 2.5 * U * r_lo + U * 1e-5 * 0.5 * r_lo ** 3
+    e_r = 0.5 * r_lo ** 3 * e_var * SLACK + 2.5 * U * r_lo + U * eps * 0.5 * r_lo ** 3
     mul = g * r
     e_mul = np.abs(g) * e_r + U * np.abs(mul) * SLACK
     ni, oy, ox = pixels(at, n, h, w)

@@ -201,6 +201,69 @@ def load_onnx(path):
 # ----------------------------------------------------------------------------------------------------------------
 # ONNX graph -> SNN layer list (modelzoo.Builder dicts: JSON keys + "_w" / "_bn")
 # ----------------------------------------------------------------------------------------------------------------
+def _engine_conv_size(n, k, s, lo, hi):
+    """Output size of one axis by the engine's Conv2D rule (layers.cpp, Conv2DLayer): fp32 scale 1 / s and translation
+    1 + (lo + hi - k) / s (one less pad for an even k), the translation clamped at 0, the sum truncated."""
+    f = np.float32
+    t = f(1) + (f(lo + hi - (1 if k % 2 == 0 else 0)) - f(k)) / f(s)
+    return int(f(f(1) / f(s) * f(n)) + max(f(0), t))
+
+
+def _engine_pool_size(n, k, s):
+    """Output size of one axis by the engine's "valid" pool rule (layers.cpp, PoolingLayer): translation 1 - k / s clamped at 0."""
+    f = np.float32
+    return int(f(f(1) / f(s) * f(n)) + max(f(0), f(1) - f(k) / f(s)))
+
+
+def _sizes_agree(engine, onnx, k, s):
+    """True when the engine's size rule gives ONNX's output size at every input size from k on (both are periodic in s)."""
+    return all(engine(n) == onnx(n) for n in range(k, k + 8 * s + 8))
+
+
+# what the engine evaluates (src_coord in kernels_simt.cu) for each ONNX Pad mode; "wrap" has no counterpart
+_PAD_MODE = {"constant": "constant", "reflect": "reflect", "edge": "replicate"}
+_ENGINE_EPS_IN = np.float32(1e-5)  # InstanceNorm: the kernel's epsilon (kernels_simt.cu, instancenorm)
+_ENGINE_EPS_BN = np.float32(1e-3)  # BatchNorm: the reader's epsilon (pack.cpp)
+
+
+def _bn_fold_eps(bn, eps):
+    """A node's BatchNorm epsilon, written for a reader that uses 1e-3: gamma scaled by sqrt(var + 1e-3) / sqrt(var + eps) in float64
+    and rounded once. Writing var + eps - 1e-3 instead would cancel catastrophically for var + eps far below 1e-3 (and go negative)."""
+    var = bn["moving_variance"].astype(np.float64)
+    r = np.sqrt(var + float(_ENGINE_EPS_BN)) / np.sqrt(var + float(np.float32(eps)))
+    bn["gamma"] = (bn["gamma"].astype(np.float64) * r).astype(np.float32)
+    return bn
+
+
+def _pad_mode(nd):
+    mode = nd["attr"].get("mode", "constant")
+    if mode not in _PAD_MODE:
+        raise ValueError("Pad %s: mode %r is not supported (constant, reflect and edge are)" % (nd["name"], mode))
+    return _PAD_MODE[mode]
+
+
+def _nearest_src(o, n, scale, ctm, nearest_mode):
+    """The input index ONNX Resize's nearest mode reads for output index o (input size n, scale), in float64."""
+    out = int(np.floor(n * scale))
+    if ctm in ("half_pixel", "pytorch_half_pixel"):
+        x = (o + 0.5) / scale - 0.5 if (ctm == "half_pixel" or out > 1) else 0.0
+    elif ctm == "asymmetric":
+        x = o / scale
+    elif ctm == "align_corners":
+        x = o * (n - 1) / (out - 1) if out > 1 else 0.0
+    else:
+        return None
+    if nearest_mode == "floor":
+        i = np.floor(x)
+    elif nearest_mode == "ceil":
+        i = np.ceil(x)
+    elif nearest_mode == "round_prefer_ceil":
+        i = np.floor(x + 0.5)
+    else:  # round_prefer_floor
+        i = np.ceil(x - 0.5)
+    return int(min(max(i, 0), n - 1))
+
+
 _ACT = {"Relu": "relu", "Clip": "relu6", "LeakyRelu": "leakyRelu", "Tanh": "tanh", "Sigmoid": "sigmoid"}
 _FUSIBLE_INTO = ("Conv2D", "DepthwiseConv2D", "Add", "InstanceNormalization", "Dense")
 
@@ -240,17 +303,67 @@ def convert_graph(g, input_hw=None, fold_pads=True):
             raise ValueError("Pad %s: only spatial pads of an NCHW tensor are supported (%s)" % (nd["name"], p))
         return [int(p[2]), int(p[6]), int(p[3]), int(p[7])]  # T, B, L, R  (ONNX order: x1_begin.. x4_begin, x1_end.. x4_end)
 
+    def pad_value(nd):
+        v = nd["attr"].get("value", 0.0)
+        if len(nd["input"]) > 2 and nd["input"][2]:
+            v = float(np.asarray(init[nd["input"][2]]).ravel()[0])
+        return float(v)
+
+    def conv_geometry(nd):
+        """(k, stride, group, [T, B, L, R]) of a Conv node; refuses the attributes the engine has no form for."""
+        a = nd["attr"]
+        kh, kw = np.shape(init[nd["input"][1]])[2:]
+        if kh != kw:
+            raise ValueError("Conv %s: non-square kernels are not representable (kernel_size is one number)" % nd["name"])
+        st = [int(v) for v in a.get("strides", [1, 1])]
+        if st[0] != st[1]:
+            raise ValueError("Conv %s: strides %s differ between the axes (strides is one number)" % (nd["name"], st))
+        if any(int(v) != 1 for v in a.get("dilations", [1, 1])):
+            raise ValueError("Conv %s: dilations %s are not supported" % (nd["name"], a["dilations"]))
+        if a.get("auto_pad", "NOTSET") != "NOTSET":
+            raise ValueError("Conv %s: auto_pad %s is not supported (write explicit pads)" % (nd["name"], a["auto_pad"]))
+        p = [int(v) for v in a.get("pads", [0, 0, 0, 0])]  # ONNX: [t, l, b, r]
+        return int(kh), st[0], int(a.get("group", 1)), [p[0], p[2], p[1], p[3]]
+
+    def foldable(tblr, mode, conv):
+        """Whether a Pad may become `conv`'s own padding: the consumer must apply it as the engine's convolution would (see conv_padding)."""
+        k, s, group, own = conv_geometry(conv)
+        if any(own) or k == 1:
+            return False
+        if group > 1:  # the depthwise kernels pad with zeros only, the same amount on every side
+            return mode == "constant" and len(set(tblr)) == 1
+        return tblr[0] == tblr[2] and tblr[1] == tblr[3]
+
+    def conv_padding(nd, k, s, group, tblr):
+        """The engine hands the kernels (T, L) as (column, row) offsets and sizes both axes of a Conv2D from T + B, a depthwise's width from
+        T + L and its height from B + R (layers.cpp). Padding is written only in forms where that is ONNX's padding: the same on both axes
+        (T == L, B == R; every side alike for a depthwise), none on a 1x1, and a Conv2D's size rule giving ONNX's size."""
+        t, b, l, r = tblr
+        if k == 1 and any(tblr):
+            raise ValueError("Conv %s: pads %s on a 1x1 convolution are not supported" % (nd["name"], tblr))
+        if group > 1 and len(set(tblr)) != 1:
+            raise ValueError("Conv %s: depthwise pads [T, B, L, R] = %s must be equal on every side" % (nd["name"], tblr))
+        if t != l or b != r:
+            raise ValueError("Conv %s: pads [T, B, L, R] = %s differ between the axes" % (nd["name"], tblr))
+        if group == 1 and fold_pads and not _sizes_agree(lambda n: _engine_conv_size(n, k, s, t, b), lambda n: (n + t + b - k) // s + 1, k, s):
+            raise ValueError("Conv %s: pads [T, B, L, R] = %s with kernel %d, stride %d: the engine's output size differs from ONNX's" % (nd["name"], tblr, k, s))
+        return [[t, b], [l, r]] if any(tblr) else "valid"
+
     for nd in nodes:
         op, a = nd["op"], nd["attr"]
         out = nd["output"][0]
         x = nd["input"][0] if nd["input"] else None
         if op == "Pad":
-            mode = a.get("mode", "constant")
+            mode = _pad_mode(nd)
             tblr = pads_of(nd)
+            if mode == "constant" and pad_value(nd) != 0.0:
+                raise ValueError("Pad %s: constant value %g is not supported (only 0)" % (nd["name"], pad_value(nd)))
             users = consumers.get(out, [])
-            if fold_pads and len(users) == 1 and users[0]["op"] == "Conv" and not any(users[0]["attr"].get("pads", [0, 0, 0, 0])):
+            if fold_pads and len(users) == 1 and users[0]["op"] == "Conv" and foldable(tblr, mode, users[0]):
                 pending_pad[out] = (x, tblr, mode)
                 continue
+            if tblr[0] != tblr[2]:  # pad_kernel places the input at (T, L) as (column, row)
+                raise ValueError("Pad %s: pads [T, B, L, R] = %s need T == L" % (nd["name"], tblr))
             i = src(x)
             d = {"type": "Pad", "name": nd["name"] or "pad_%d" % len(layers), "inputPlanes": planes[i], "outputPlanes": planes[i],
                  "pads": [0, 0, tblr[0], tblr[2], 0, 0, tblr[1], tblr[3]], "mode": mode}
@@ -259,16 +372,11 @@ def convert_graph(g, input_hw=None, fold_pads=True):
         elif op == "Conv":
             wt = np.asarray(init[nd["input"][1]], np.float32)
             oc, icg, kh, kw = wt.shape
-            if kh != kw:
-                raise ValueError("Conv %s: non-square kernels are not representable (kernel_size is one number)" % nd["name"])
-            stride = int(a.get("strides", [1, 1])[0])
-            group = int(a.get("group", 1))
-            pad = [int(v) for v in a.get("pads", [0, 0, 0, 0])]  # ONNX: [t, l, b, r]
-            padding = [[pad[0], pad[2]], [pad[1], pad[3]]] if any(pad) else "valid"
+            kh, stride, group, tblr = conv_geometry(nd)
             mode = None
             if x in pending_pad:
                 x, tblr, mode = pending_pad.pop(x)
-                padding = [[tblr[0], tblr[1]], [tblr[2], tblr[3]]]
+            padding = conv_padding(nd, kh, stride, group, tblr)
             i = src(x)
             bias = np.asarray(init[nd["input"][2]], np.float32) if len(nd["input"]) > 2 else None
             if group > 1:
@@ -281,13 +389,16 @@ def convert_graph(g, input_hw=None, fold_pads=True):
                 d = {"type": "Conv2D", "name": nd["name"] or "conv2d_%d" % len(layers), "inputPlanes": int(icg), "outputPlanes": int(oc), "kernel_size": int(kh),
                      "strides": stride, "padding": padding, "activation": "linear", "useBias": "True" if bias is not None else "False",
                      "useBatchNormalization": "False", "_w": {"kernel": wt.copy()}}
-            if mode and mode != "constant":
-                d["mode"] = mode
+            if isinstance(padding, list) and group == 1:
+                d["mode"] = mode or "constant"  # the reader requires a mode beside [[t, b], [l, r]] (modelparser.cpp)
             if bias is not None:
                 d["_w"]["bias"] = bias.copy()
             produced[out] = add(d, [i])
             planes[produced[out]] = int(oc)
         elif op == "InstanceNormalization":
+            eps = a.get("epsilon", 1e-5)
+            if np.float32(eps) != _ENGINE_EPS_IN:
+                raise ValueError("InstanceNormalization %s: epsilon %g is not supported (the engine's is 1e-5)" % (nd["name"], eps))
             i = src(x)
             d = {"type": "InstanceNormalization", "name": nd["name"] or "instance_norm_%d" % len(layers), "inputPlanes": planes[i], "outputPlanes": planes[i],
                  "epsilon": float(a.get("epsilon", 1e-5)), "activation": "linear",
@@ -299,8 +410,8 @@ def convert_graph(g, input_hw=None, fold_pads=True):
             L = layers[i]
             bn = {"gamma": np.asarray(init[nd["input"][1]], np.float32).copy(), "beta": np.asarray(init[nd["input"][2]], np.float32).copy(),
                   "moving_mean": np.asarray(init[nd["input"][3]], np.float32).copy(), "moving_variance": np.asarray(init[nd["input"][4]], np.float32).copy()}
-            # the reader hard-codes eps = 1e-3 (vk_conv2d.comp:282): fold the node's own epsilon into the written variance
-            bn["moving_variance"] = (bn["moving_variance"] + np.float32(a.get("epsilon", 1e-5)) - np.float32(1e-3)).astype(np.float32)
+            # the reader hard-codes eps = 1e-3 (vk_conv2d.comp:282): fold the node's own epsilon into the written gamma
+            bn = _bn_fold_eps(bn, a.get("epsilon", 1e-5))
             if L["type"] in ("Conv2D", "DepthwiseConv2D") and L.get("activation", "linear") == "linear" and len(consumers.get(x, [])) == 1:
                 L["useBatchNormalization"] = "True"  # batchNormalization.py:35-42: merged into the producer
                 L["_bn"] = bn
@@ -311,6 +422,11 @@ def convert_graph(g, input_hw=None, fold_pads=True):
                 produced[out] = add(d, [i])
                 planes[produced[out]] = planes[i]
         elif op in _ACT:
+            if op == "Clip":
+                lo = a.get("min", float(np.asarray(init[nd["input"][1]]).ravel()[0]) if len(nd["input"]) > 1 and nd["input"][1] else None)
+                hi = a.get("max", float(np.asarray(init[nd["input"][2]]).ravel()[0]) if len(nd["input"]) > 2 and nd["input"][2] else None)
+                if (lo, hi) != (0.0, 6.0):
+                    raise ValueError("Clip %s: min %s / max %s are not supported (only 0 / 6, relu6)" % (nd["name"], lo, hi))
             i = src(x)
             L = layers[i]
             act = _ACT[op]
@@ -321,6 +437,8 @@ def convert_graph(g, input_hw=None, fold_pads=True):
                 produced[out] = i
             else:
                 d = {"type": "Activation", "name": nd["name"] or "activation_%d" % len(layers), "inputPlanes": planes[i], "outputPlanes": planes[i], "activation": act}
+                if act == "leakyRelu":
+                    d["leakyReluAlpha"] = float(a.get("alpha", 0.01))
                 produced[out] = add(d, [i])
                 planes[produced[out]] = planes[i]
         elif op == "Add":
@@ -335,18 +453,48 @@ def convert_graph(g, input_hw=None, fold_pads=True):
                 sc = [float(v) for v in init[sname].ravel()]
             if not (len(sc) == 4 and sc[0] == 1 and sc[1] == 1 and sc[2] == sc[3] and sc[2] >= 1):
                 raise ValueError("%s %s: only uniform spatial up-scaling is supported (%s)" % (op, nd["name"], sc))
+            scale, mode = float(sc[2]), a.get("mode", "nearest")
+            # Upsample (opset 7-9) samples at o / scale (asymmetric) and nearest takes the floor; Resize defaults to half_pixel and round_prefer_floor
+            ctm = a.get("coordinate_transformation_mode", "half_pixel") if op == "Resize" else "asymmetric"
+            nearest_mode = a.get("nearest_mode", "round_prefer_floor") if op == "Resize" else "floor"
+            if mode == "linear":
+                # upsample_kernel samples at (o + 0.5) / scale - 0.5, clamped to the input: half_pixel (pytorch_half_pixel for outputs > 1 pixel);
+                # at scale 1 every mode samples the input pixels themselves
+                if scale != 1 and ctm not in ("half_pixel", "pytorch_half_pixel"):
+                    raise ValueError("%s %s: linear with coordinate_transformation_mode %s is not supported (half_pixel is)" % (op, nd["name"], ctm))
+            elif mode == "nearest":
+                # upsample_kernel reads floor(o * fl(1 / scale)): ONNX's index at integer scales, for the modes checked here
+                if scale != int(scale):
+                    raise ValueError("%s %s: nearest at the non-integer scale %g is not supported" % (op, nd["name"], scale))
+                inv = np.float32(1) / np.float32(scale)
+                for n in range(1, 9):
+                    for o in range(int(n * scale)):
+                        if _nearest_src(o, n, scale, ctm, nearest_mode) != min(int(np.floor(np.float32(o) * inv)), n - 1):
+                            raise ValueError("%s %s: nearest with coordinate_transformation_mode %s and nearest_mode %s is not supported" % (
+                                op, nd["name"], ctm, nearest_mode))
+            else:
+                raise ValueError("%s %s: mode %s is not supported (nearest and linear are)" % (op, nd["name"], mode))
             i = src(x)
             d = {"type": "UpSampling2D", "name": nd["name"] or "up_sampling2d_%d" % len(layers), "inputPlanes": planes[i], "outputPlanes": planes[i],
-                 "scaleFactor": float(sc[2]) if sc[2] != int(sc[2]) else int(sc[2]), "interpolation": "bilinear" if a.get("mode", "nearest") == "linear" else "nearest"}
+                 "scaleFactor": scale if scale != int(scale) else int(scale), "interpolation": "bilinear" if mode == "linear" else "nearest"}
             produced[out] = add(d, [i])
             planes[produced[out]] = planes[i]
         elif op in ("MaxPool", "AveragePool"):
             i = src(x)
-            k = int(a["kernel_shape"][0])
-            s = int(a.get("strides", [k, k])[0])
-            p = [int(v) for v in a.get("pads", [0, 0, 0, 0])]
+            ks = [int(v) for v in a["kernel_shape"]]
+            st = [int(v) for v in a.get("strides", [1, 1])]  # ONNX's default stride is 1
+            k, s = ks[0], st[0]
+            if ks[0] != ks[1] or st[0] != st[1]:
+                raise ValueError("%s %s: kernel_shape %s / strides %s differ between the axes" % (op, nd["name"], ks, st))
+            if any(int(v) for v in a.get("pads", [0, 0, 0, 0])) or a.get("auto_pad", "NOTSET") not in ("NOTSET", "VALID"):
+                # the engine's pools never pad the top or left, and clip windows at the bottom and right (maxpool2dVulkan.cpp:57-60)
+                raise ValueError("%s %s: pads %s are not supported (write a Pad node)" % (op, nd["name"], a.get("pads", a.get("auto_pad"))))
+            if int(a.get("ceil_mode", 0)) or any(int(v) != 1 for v in a.get("dilations", [1, 1])):
+                raise ValueError("%s %s: ceil_mode / dilations are not supported" % (op, nd["name"]))
+            if not _sizes_agree(lambda n: _engine_pool_size(n, k, s), lambda n: (n - k) // s + 1, k, s):
+                raise ValueError("%s %s: kernel_shape %d with strides %d: the engine's output size differs from ONNX's" % (op, nd["name"], k, s))
             d = {"type": "MaxPooling2D" if op == "MaxPool" else "AveragePooling2D", "name": nd["name"] or "pool_%d" % len(layers), "inputPlanes": planes[i],
-                 "outputPlanes": planes[i], "padding": "same" if any(p) else "valid"}
+                 "outputPlanes": planes[i], "padding": "valid"}
             if op == "MaxPool":
                 d["pool"], d["strides"] = [k, k], s
             else:
@@ -364,6 +512,8 @@ def convert_graph(g, input_hw=None, fold_pads=True):
             raise NotImplementedError("ONNX op %s (%s) is not supported by this converter" % (op, nd["name"]))
     if pending_pad:
         raise ValueError("Pad nodes left unfolded: %s" % list(pending_pad))
+    for t, j in produced.items():  # the graph tensor each layer's output stands for (the last node merged into it); not written
+        layers[j]["_onnx"] = t
     return layers
 
 
@@ -380,11 +530,41 @@ def convert(onnx_path, out_dir, input_hw=None, split=True, fold_pads=True):
 # ----------------------------------------------------------------------------------------------------------------
 # torch-CPU evaluation of the ONNX graph ITSELF (no conversion involved): the ground truth the converted model is held to
 # ----------------------------------------------------------------------------------------------------------------
-def torch_eval(g, x_nhwc):
+def _resize_axis(torch, x, axis, scale, ctm, linear, nearest_mode):
+    """ONNX Resize along one axis of x (output size floor(n * scale)), written from the operator's definition."""
+    n = x.shape[axis]
+    out = int(np.floor(n * scale))
+    if linear:
+        o = np.arange(out, dtype=np.float64)
+        if ctm == "align_corners":
+            c = o * (n - 1) / (out - 1) if out > 1 else np.zeros(out)
+        elif ctm == "asymmetric":
+            c = o / scale
+        elif ctm == "pytorch_half_pixel" and out == 1:
+            c = np.zeros(out)
+        else:  # half_pixel
+            c = (o + 0.5) / scale - 0.5
+        c = np.clip(c, 0, n - 1)
+        i0 = np.floor(c).astype(np.int64)
+        i1 = np.minimum(i0 + 1, n - 1)
+        shape = [1] * x.dim()
+        shape[axis] = out
+        f = torch.from_numpy(c - i0).to(x.dtype).reshape(shape)
+        return x.index_select(axis, torch.from_numpy(i0)) * (1 - f) + x.index_select(axis, torch.from_numpy(i1)) * f
+    idx = [_nearest_src(o, n, scale, ctm, nearest_mode) for o in range(out)]
+    return x.index_select(axis, torch.tensor(idx, dtype=torch.int64))
+
+
+def torch_eval(g, x_nhwc, dtype=None, return_all=False, feeds=None):
+    """The graph's output (NHWC) for NHWC input x, evaluated node by node with torch on the CPU in `dtype` (default float32).
+    return_all: a dict of every tensor, NCHW, instead. feeds: {tensor name: NHWC value} to start from instead of x (the nodes of g
+    then need only those)."""
     import torch
     import torch.nn.functional as F
-    init = {k: torch.from_numpy(np.array(v)) for k, v in g["init"].items() if v.dtype.kind == "f"}
-    vals = {g["inputs"][0][0]: torch.from_numpy(np.ascontiguousarray(x_nhwc, dtype=np.float32)).permute(0, 3, 1, 2).contiguous()}
+    dt = dtype or torch.float32
+    init = {k: torch.from_numpy(np.array(v)).to(dt) for k, v in g["init"].items() if v.dtype.kind == "f"}
+    start = feeds if feeds is not None else {g["inputs"][0][0]: x_nhwc}
+    vals = {k: torch.from_numpy(np.ascontiguousarray(v)).to(dt).permute(0, 3, 1, 2).contiguous() for k, v in start.items()}
     with torch.no_grad():
         for nd in g["nodes"]:
             op, a = nd["op"], nd["attr"]
@@ -393,7 +573,8 @@ def torch_eval(g, x_nhwc):
                 p = a.get("pads")
                 if p is None:
                     p = [int(v) for v in g["init"][nd["input"][1]].ravel()]
-                y = F.pad(x, (int(p[3]), int(p[7]), int(p[2]), int(p[6])), mode=a.get("mode", "constant"))
+                mode = {"constant": "constant", "reflect": "reflect", "edge": "replicate"}[a.get("mode", "constant")]
+                y = F.pad(x, (int(p[3]), int(p[7]), int(p[2]), int(p[6])), mode=mode)
             elif op == "Conv":
                 p = [int(v) for v in a.get("pads", [0, 0, 0, 0])]
                 xx = F.pad(x, (p[1], p[3], p[0], p[2])) if any(p) else x
@@ -406,7 +587,9 @@ def torch_eval(g, x_nhwc):
             elif op == "Relu":
                 y = F.relu(x)
             elif op == "Clip":
-                y = torch.clamp(x, 0.0, 6.0)
+                lo = a.get("min", float(g["init"][nd["input"][1]].ravel()[0]) if len(nd["input"]) > 1 and nd["input"][1] else -np.inf)
+                hi = a.get("max", float(g["init"][nd["input"][2]].ravel()[0]) if len(nd["input"]) > 2 and nd["input"][2] else np.inf)
+                y = torch.clamp(x, lo, hi)
             elif op == "LeakyRelu":
                 y = F.leaky_relu(x, float(a.get("alpha", 0.01)))
             elif op == "Tanh":
@@ -420,15 +603,20 @@ def torch_eval(g, x_nhwc):
                 if sc is None:
                     sname = nd["input"][2] if op == "Resize" and len(nd["input"]) > 2 else nd["input"][1]
                     sc = [float(v) for v in g["init"][sname].ravel()]
-                y = F.interpolate(x, scale_factor=float(sc[2]), mode="nearest")
+                linear = a.get("mode", "nearest") == "linear"
+                ctm = a.get("coordinate_transformation_mode", "half_pixel") if op == "Resize" else "asymmetric"
+                nearest_mode = a.get("nearest_mode", "round_prefer_floor") if op == "Resize" else "floor"
+                y = _resize_axis(torch, _resize_axis(torch, x, 2, float(sc[2]), ctm, linear, nearest_mode), 3, float(sc[3]), ctm, linear, nearest_mode)
             elif op == "MaxPool":
-                y = F.max_pool2d(x, int(a["kernel_shape"][0]), int(a.get("strides", a["kernel_shape"])[0]))
+                y = F.max_pool2d(x, int(a["kernel_shape"][0]), int(a.get("strides", [1, 1])[0]))
             elif op == "AveragePool":
-                y = F.avg_pool2d(x, int(a["kernel_shape"][0]), int(a.get("strides", a["kernel_shape"])[0]))
+                y = F.avg_pool2d(x, int(a["kernel_shape"][0]), int(a.get("strides", [1, 1])[0]))
             elif op == "Concat":
                 y = torch.cat([vals[t] for t in nd["input"]], dim=1)
             else:
                 raise NotImplementedError("torch_eval: ONNX op %s" % op)
             vals[nd["output"][0]] = y
+    if return_all:
+        return vals
     out_name = g["outputs"][0][0] if g["outputs"] else g["nodes"][-1]["output"][0]
     return vals[out_name].permute(0, 2, 3, 1).contiguous().numpy()

@@ -258,13 +258,16 @@ def restate(om, i, outs, kernels, precision, half, x, at=None):
     if t == "InputLayer":
         return exact.model_input(x, half, at)
     outs = list(outs)
-    for j in ins:  # a constant Pad folded into its consumer: zero padding composes, so restate it as a tensor (pure data movement)
+    for j in ins:
+        # a Pad without a tensor in a fused run, restated as a tensor (pure data movement): a constant Pad folded into its consumer (zero
+        # padding composes), or one the engine kept but the walker does not read back. A reflect / replicate Pad folded into a Conv2D is
+        # restated by restate_conv from the Pad's input.
         p = om.layers[j]
-        if outs[j] is None and om.type_of(p) == "Pad" and p.get("mode", "constant") in ("constant", ""):
+        if outs[j] is None and om.type_of(p) == "Pad" and (p.get("mode", "constant") in ("constant", "") or not pad_folded(om, j)):
             up = int(p["inputId"][0])
             if outs[up] is not None:
                 o = om._offsets(p, 0, False) if "pads" not in p else [int(p["pads"][2]), int(p["pads"][6]), int(p["pads"][3]), int(p["pads"][7])]
-                outs[j] = exact.pad(outs[up], o[0], o[2], kernels["shapes"][j][1:3])[0]
+                outs[j] = exact.pad(outs[up], o[0], o[2], kernels["shapes"][j][1:3], p.get("mode", "constant") or "constant")[0]
     if t == "Add" and any(outs[j] is None for j in ins):
         # a Conv2D fused into this Add: its epilogue adds the other operand and applies the Add's activation
         j = [j for j in ins if outs[j] is None][0]
@@ -346,12 +349,32 @@ def restate(om, i, outs, kernels, precision, half, x, at=None):
     return None
 
 
+def pad_folded(om, j):
+    """Whether the engine's fusion folds Pad layer j into its consumer's gather (core.cpp, pass 1): one consumer, a Conv2D with k > 1
+    and no padding of its own, or a depthwise behind a constant Pad."""
+    users = [l for l in om.layers if j in [int(v) for v in l.get("inputId", [])][:int(l.get("numInputs", 0))]]
+    if len(users) != 1:
+        return False
+    u = users[0]
+    t = om.type_of(u)
+    k = int(u.get("kernel_size", 1))
+    own = u.get("padding")
+    zero = own in ("valid", "none") or (not isinstance(own, str) and not any(om._offsets(u, k)))
+    return zero and ((t == "Conv2D" and k > 1) or (t == "SeparableConv2D" and om.layers[j].get("mode", "constant") in ("constant", "")))
+
+
 def restate_conv(om, j, outs, kernels, precision, half, act, alpha, residual=None, shape_of=None, at=None):
     l = om.layers[j]
     k, s = int(l["kernel_size"]), int(l["strides"])
     src = [int(v) for v in l["inputId"]][0]
     x = outs[src]
     px, py, mode = conv_params(l, k)
+    p = om.layers[src]
+    if x is None and om.type_of(p) == "Pad" and k > 1:
+        # a Pad fused into this convolution (core.cpp, pass 1): the kernels read the Pad's input at the Pad's (T, L) offsets, in its mode
+        x = outs[int(p["inputId"][0])]
+        o = om._offsets(p, 0, False) if "pads" not in p else [int(p["pads"][2]), int(p["pads"][6]), int(p["pads"][3]), int(p["pads"][7])]
+        px, py, mode = o[0], o[2], p.get("mode", "constant") or "constant"
     if x is None:
         return None
     kern = conv_kernel(kernels["names"][j])
@@ -362,9 +385,18 @@ def restate_conv(om, j, outs, kernels, precision, half, act, alpha, residual=Non
 
 
 def teacher_forced(ctx, name, hw, batch, model_dir, precision, fuse, conv_algo="auto", **kw):
-    from shadernn_b200._lib import SnnbError
+    """A zoo model built by modelzoo.Builder, on its synthetic input, through teacher_forced_model."""
     path, _ = modelzoo.build(name, model_dir, input_hw=hw, **kw)
     x = modelzoo.synthetic_input(name, batch, hw)
+    return teacher_forced_model(ctx, path, x, batch, hw, precision, fuse, conv_algo, label=name)[0]
+
+
+def teacher_forced_model(ctx, path, x, batch, hw, precision, fuse, conv_algo="auto", label=None):
+    """Every layer of the model file `path` with a tensor of its own, run on the NHWC input x, held to its restatement fed the engine's
+    outputs of its producers. Fails on any layer outside its bound or without a restatement. Returns (worst |err| / bound, layers
+    checked, kernels: the kernel names and output shapes per layer)."""
+    from shadernn_b200._lib import SnnbError
+    name = label or os.path.basename(path)
     om = oracle.Model(path)
     m = core.MixedInferenceCore(ctx, path, batch=batch, input_hw=hw, fuse=fuse, conv_algo=conv_algo, precision=precision)
     try:
@@ -407,7 +439,7 @@ def teacher_forced(ctx, name, hw, batch, model_dir, precision, fuse, conv_algo="
     print("%-12s %4dx%-4d batch %2d %-6s fuse=%d %-4s: %3d layers, worst |err|/bound %.3g%s" % (
         name, hw[0], hw[1], batch, precision, int(fuse), conv_algo, checked, worst, (" (not restated: %s)" % ", ".join(skipped)) if skipped else ""))
     assert not skipped, "layers without a restatement: %s" % skipped
-    return worst
+    return worst, checked, kernels
 
 
 ZOO = [("resnet18", (64, 64), 2, {}), ("mobilenetv2", (64, 64), 2, {"classes": 100}), ("yolov3tiny", (128, 128), 1, {}),
