@@ -113,10 +113,16 @@ int snnb_weights_free(snnb_weights* w);
 
 /* ---- operator launches (one call == one RenderPass::run, core/src/ic2/renderpass.h:64) ------------------------- */
 /* Conv2D k x k incl. 1x1 (shadertemplate_vk_conv2d.comp:148-347, vk_conv2d_1x1.comp:68-211). `residual` (may be
- * NULL) is added before the activation: the fused form of Conv2D -> Add(+act) (vk_add.comp:41-90). */
+ * NULL) is added before the activation: the fused form of Conv2D -> Add(+act) (vk_add.comp:41-90). Output pixel (oy, ox) reads input
+ * row oy * stride + ky - pad_y and column ox * stride + kx - pad_x; out->h and out->w are the caller's, so they imply the bottom and right
+ * padding. The plan is made at each launch: the context's precision as it stands then, may_prepad = may_feed = 0 (so under AUTO
+ * replicate and reflect run on CUDA cores, and a forced tensor path on them is refused), and the row window only when the weights were
+ * packed for this launch's (stride, pad_x). A forced tensor path (SNNB_ALGO_TCGEN05*) the shape cannot take is refused. */
 int snnb_conv2d_launch(snnb_context* ctx, const snnb_conv_desc* d, const snnb_weights* w, const snnb_tensor* in, const snnb_tensor* residual,
                        snnb_tensor* out);
-/* Depthwise k x k (shadertemplate_vk_depthwise.comp:64-139). */
+/* Depthwise k x k (shadertemplate_vk_depthwise.comp:64-139). Zero padding only: d->pad_mode must be SNNB_PAD_NONE or SNNB_PAD_CONSTANT
+ * (replicate and reflect are refused; pad one with snnb_pad_launch first). The output size is the caller's: out->h and out->w imply the
+ * bottom and right padding, as for snnb_conv2d_launch. */
 int snnb_depthwise_launch(snnb_context* ctx, const snnb_conv_desc* d, const snnb_weights* w, const snnb_tensor* in, snnb_tensor* out);
 /* MaxPooling2D / AveragePooling2D (vk_maxpool2d.comp:42-71, vk_avgpool2d.comp:42-69; window origin o*stride). */
 int snnb_maxpool_launch(snnb_context* ctx, int kernel, int stride, const snnb_tensor* in, snnb_tensor* out);
@@ -132,7 +138,7 @@ int snnb_activation_launch(snnb_context* ctx, int activation, float leaky_alpha,
 int snnb_dense_launch(snnb_context* ctx, const snnb_weights* w, int activation, float leaky_alpha, const snnb_tensor* in, snnb_tensor* out);
 /* Softmax over channels per pixel (cpulayer.h:175-191) and classifier index argmax+1 (core.cpp:228-233), per image. */
 int snnb_softmax_launch(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out);
-int snnb_argmax1(snnb_context* ctx, const snnb_tensor* in, int* host_idx_1based); /* synchronous; in: [N,1,1,C] */
+int snnb_argmax1(snnb_context* ctx, const snnb_tensor* in, int* host_idx_1based); /* synchronous; in: [N,1,1,C], any other H or W is refused */
 /* Flatten in HWC order (cpulayer.h:94-115): [N,H,W,C] -> [N,1,1,H*W*C]. */
 int snnb_flatten_launch(snnb_context* ctx, const snnb_tensor* in, snnb_tensor* out);
 /* Concatenate along channels (vk_concat.comp:39-52). */

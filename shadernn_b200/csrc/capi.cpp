@@ -403,6 +403,9 @@ int snnb_depthwise_launch(snnb_context* ctx, const snnb_conv_desc* d, const snnb
     SNNB_REQUIRE(ctx && d && w && in && out, "snnb_depthwise_launch: null argument");
     SNNB_REQUIRE(w->kind == 2 && in->c == w->in_ch && out->c == in->c && d->kernel == w->kernel, "snnb_depthwise_launch: weights/tensor mismatch");
     SNNB_REQUIRE(in->n == out->n, "snnb_depthwise_launch: batch mismatch");
+    // the depthwise kernels clip the window to the input, which is zero padding; replicate or reflect would silently read zeros
+    SNNB_REQUIRE(d->pad_mode == SNNB_PAD_NONE || d->pad_mode == SNNB_PAD_CONSTANT, "snnb_depthwise_launch: pad_mode %d; depthwise pads with zeros only (NONE or CONSTANT)",
+                 d->pad_mode);
     ConvArgs a {in, nullptr, out, w, d->kernel, d->stride, d->pad_x, d->pad_y, SNNB_PAD_CONSTANT, d->activation, d->leaky_alpha};
     return launch_depthwise(ctx, a);
 }
@@ -461,6 +464,8 @@ int snnb_dense_launch(snnb_context* ctx, const snnb_weights* w, int act, float a
 }
 int snnb_argmax1(snnb_context* ctx, const snnb_tensor* in, int* host_idx) {
     SNNB_REQUIRE(ctx && in && host_idx, "snnb_argmax1: null argument");
+    // argmax_kernel scans the channels of pixel 0 of each image
+    SNNB_REQUIRE(in->h == 1 && in->w == 1, "snnb_argmax1: input is %dx%d per image; it must be [N,1,1,C]", in->h, in->w);
     if (ensure_stage(ctx, sizeof(int) * in->n)) return 1;
     int* dev = reinterpret_cast<int*>(ctx->stage_dev);
     if (launch_argmax(ctx, in, dev)) return 1;
